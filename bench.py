@@ -12,12 +12,15 @@ One "step" = one full pass of the workload over one batch:
             ByT5/CLIP embeddings (L=128), re-randomised weights (paella_b200/synth.py)
   sample64  configs[3]: bs=16, 64x64 latents, 12 steps, + CLIP-image conditioning (unconditional side without it)
   vqgan     configs[4]: f4 VQGAN encode -> indices -> decode_indices round trip, bs=256/GPU, 256x256 images
-Prints ONE JSON line (rank 0).
+Prints ONE JSON line (rank 0).  --dump-outputs DIR writes what the last timed step returned (rank 0) as DIR/<name>.npy:
+sample* -> tokens.npy (the sampled token ids as float64, exact), vqgan -> images_sample.npy (a fixed, seeded sample of the
+decoded fp32 images).  Weights, inputs and the sampler's seed depend only on the arguments, so two builds run with the
+same arguments can be compared output for output.
 
   value     images/s with the inputs already resident in HBM
   e2e       images/s through the public API with HOST (pinned) inputs: H2D of the step's inputs and D2H of its result
             inside the timed region, every step
-  roofline  tcgen05 GEMM family: algorithmic FLOPs of one step / summed CUDA-event durations of its launches,
+  roofline  wgmma GEMM family: algorithmic FLOPs of one step / summed CUDA-event durations of its launches,
             measured live by one extra profiled step after the timed region (events on the launching stream)
   cpu_baseline        the unmodified reference (baseline/_ref; oracle port if absent) on a bounded sample, rank 0, N=1 only
   torch_cuda_baseline the unmodified reference on the same GPU (fp32 w/ cuDNN TF32 default, and torch.autocast fp16)
@@ -90,7 +93,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tflops": 1400.0, "src": "fallback"}
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "src": "H100 SXM data sheet (dense fp16, 700 W)"}
 
 
 class ClockSampler:
@@ -130,22 +133,6 @@ class ClockSampler:
         reasons = [n for i, n in enumerate(names) if any(len(r) > 3 + i and r[3 + i].lower().startswith("active") for r in self.rows)]
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
                 "samples": len(sm)}
-
-
-def ncu_traffic():
-    """DRAM bytes per launch of the dominant (GEMM) kernels from the committed `ncu --set full` capture: the
-    launch-weighted mean over the main-path shapes of one forward (bench.py cannot run ncu itself)."""
-    for name in ("r02_ncu_traffic.json", "r01_ncu_traffic.json"):
-        path = os.path.join(ROOT, "profiles", name)
-        try:
-            ks = json.load(open(path))["kernels"]
-            n = sum(k["launches_per_forward"] for k in ks)
-            mean = sum(k["launches_per_forward"] * k["dram_bytes"] for k in ks) / n
-            alg = sum(k["launches_per_forward"] * k["algorithmic_bytes"] for k in ks) / n
-            return mean, f"profiles/{name} (launch-weighted mean of {len(ks)} shapes; algorithmic {alg / 1e6:.0f} MB)"
-        except (OSError, KeyError, ValueError, ZeroDivisionError):
-            continue
-    return None, None
 
 
 def build_model(device):
@@ -322,6 +309,28 @@ def _child_json(extra, timeout):
 
 
 # ---------------------------------------------------------------------------------------------- our arm
+DUMP_LIMIT = 64 << 20          # bytes of .npy data per dump
+DUMP_SAMPLE = 1 << 22          # elements kept of a larger output (a fixed, seeded choice)
+
+
+def dump_outputs(d, workload, out):
+    """What the timed path returned in its last step -> d/<name>.npy: sample tokens in full (float64 holds every id exactly),
+    decoded images as a seeded sample of DUMP_SAMPLE elements when the whole tensor would exceed DUMP_LIMIT."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    if workload == "vqgan":
+        a = out.detach().float().reshape(-1)
+        name = "images"
+        if a.numel() * 4 > DUMP_LIMIT:
+            pick = torch.from_numpy(np.random.default_rng(0).choice(a.numel(), DUMP_SAMPLE, replace=False)).to(a.device)
+            a, name = a[pick], "images_sample"
+            np.save(os.path.join(d, "images_sample_index.npy"), pick.cpu().numpy().astype(np.float64))
+        np.save(os.path.join(d, f"{name}.npy"), a.cpu().numpy().astype(np.float32))
+    else:
+        np.save(os.path.join(d, "tokens.npy"), out.detach().cpu().numpy().astype(np.float64))
+    log(f"outputs of the last timed step written to {d}")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -333,6 +342,8 @@ def main():
     ap.add_argument("--ref-batch", type=int, default=1)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-cuda-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32/float64, <= 64 MB)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -417,15 +428,19 @@ def main():
             assert len(set(sums)) == 1, f"cross-rank token checksum mismatch (weights differ between ranks?): {sums}"
             extra["cross_rank_token_checksum"] = {"value": sums[0], "ranks_agree": world}
 
-    def timed(fn, steps):
+    last = {}
+
+    def timed(fn, steps, keep=False):
         if world > 1:
             dist.barrier()
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            r = fn()
         e1.record()
+        if keep and steps > 0:
+            last["out"] = r
         torch.cuda.synchronize()
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
         if world > 1:
@@ -440,8 +455,10 @@ def main():
     log(f"timing {args.steps} steps (HBM-resident inputs)")
     launches0 = L.pb200_launch_count()
     with ClockSampler(local_rank) as clk:
-        ms = timed(step_resident, args.steps)
+        ms = timed(step_resident, args.steps, keep=True)
     launches = L.pb200_launch_count() - launches0
+    if args.dump_outputs and rank == 0 and "out" in last:
+        dump_outputs(args.dump_outputs, args.workload, last.pop("out"))
     log(f"  {ms / args.steps:.1f} ms/step; timing {args.steps} steps end to end (host inputs)")
     for _ in range(2):
         step_e2e()
@@ -480,7 +497,6 @@ def main():
     gemm_n = sum(prof[k]["launches"] for k in tensor_tags)
     total_ms = sum(v["ms"] for v in prof.values())
     achieved = gemm_fl / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
-    traffic, traffic_src = ncu_traffic() if args.workload == "sample" else (None, None)
 
     def fam(k, v):
         tensor = k in tensor_tags or k == "fused_sampler"
@@ -488,10 +504,9 @@ def main():
         peak = pk["tflops"] if tensor else pk["hbm_gbs"]
         return {"ms": round(v["ms"], 3), "launches": v["launches"], "rate": rate, "unit": "TFLOP/s" if tensor else "GB/s",
                 "frac": (rate / peak if rate else None), "bound": "alu(philox)" if k == "fused_sampler" else ("tensor" if tensor else "hbm")}
-    roofline = {"bound": "tensor", "kernel": "gemm_f16_cg2_kernel / gemm_f16_kernel (tcgen05 GEMM family)", "achieved": achieved,
-                "peak": pk["tflops"], "unit": "TFLOP/s", "frac": achieved / pk["tflops"], "traffic": traffic,
-                "traffic_source": traffic_src,
-                "peak_source": pk["src"] + " bf16 sustained", "launches_per_step": gemm_n,
+    roofline = {"bound": "tensor", "kernel": "gemm_f16_kernel (wgmma GEMM family)", "achieved": achieved,
+                "peak": pk["tflops"], "unit": "TFLOP/s", "frac": achieved / pk["tflops"],
+                "peak_source": pk["src"], "launches_per_step": gemm_n,
                 "avg_launch_ms": gemm_ms / max(gemm_n, 1), "share_of_step": gemm_ms / total_ms if total_ms else None,
                 "families": {k: fam(k, v) for k, v in prof.items()}}
 
@@ -504,7 +519,7 @@ def main():
            "data": "synthetic",
            "config": {"workload": w["desc"], "baseline_config": w["baseline_config"], "batch_per_gpu": B, "global_batch": B * world,
                       "parallelism": f"batch-shard x{world}, 1 weight broadcast",
-                      "l2": "inputs larger than L2 (weights + activations per step far exceed 126 MB)"},
+                      "l2": "inputs larger than L2 (weights + activations per step far exceed 50 MB)"},
            "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                    "ms_per_step": ms_e2e / args.steps, "copies": e2e_note},
            "gpu_launches": int(launches), "clocks": clk.summary(), "roofline": roofline}

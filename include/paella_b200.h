@@ -1,4 +1,4 @@
-/* paella_b200 — C ABI of the B200-native Paella hot path.
+/* paella_b200 — C ABI of the Paella hot path, native to the H100 (sm_90a).
  *
  * The reference (dome272/Paella @ e1ab72b) has no FFI layer: its boundary is the
  * Python class surface (SURVEY.md §8b).  This header is the C ABI the Python
@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define PB200_ABI_VERSION 2
+#define PB200_ABI_VERSION 3      /* 3: pb200_vq_mlp_fused removed */
 
 const char* pb200_last_error(void);
 int pb200_abi_version(void);
@@ -88,7 +88,7 @@ int pb200_vq_nearest(const float* x, int64_t n, int c, const float* codebook, in
 int pb200_vq_gather(const int64_t* idx, int64_t n, const float* codebook, int k, int c, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Tensor-core GEMM (tcgen05, TMA-fed, TMEM accumulators): C[M,N] = A[M,K] . W[N,K]^T (+epilogue)
+ * Tensor-core GEMM (wgmma, TMA-fed, register accumulators): C[M,N] = A[M,K] . W[N,K]^T (+epilogue)
  * A, W: fp16 row-major (K contiguous), K % 8 == 0.  Used by every 1x1-conv / Linear of the path;
  * exported for unit tests.
  * ------------------------------------------------------------------------------------------ */
@@ -135,7 +135,7 @@ typedef struct pb200_gemm_epilogue {
     float* ln_mean_out;        /* F16_LN: fp32 [M] true row mean (shift + mean of the shifted row), or NULL */
     const void* a_scale;       /* RESID / RESID_LN: fp16 [M / rows_per_sample, a_scale_ld] per-(sample, k) factors multiplied into
                                   the A operand on its way to the tensor core (GlobalResponseNorm folded into the GEMM that
-                                  consumes it: A'[m,k] = A[m,k] * a_scale[m / rows_per_sample, k]), or NULL.  Needs M > 128,
+                                  consumes it: A'[m,k] = A[m,k] * a_scale[m / rows_per_sample, k]), or NULL.  Needs
                                   K % 64 == 0 and rows_per_sample dividing 128 (>= 16) or a multiple of 128 */
     int64_t a_scale_ld;
 } pb200_gemm_epilogue;
@@ -143,8 +143,8 @@ typedef struct pb200_gemm_epilogue {
 int pb200_gemm_f16(const void* a, int64_t lda, const void* w, int64_t ldw, int64_t m, int64_t n, int64_t k,
                    const pb200_gemm_epilogue* epi, void* stream);
 /* Host-side tile plan pb200_gemm_f16 would use for an [m,k] x [n,k]^T problem on `sm_count` multiprocessors (0 = the
- * current device, or 148 without one): BLOCK_N, whether the 2-SM (cta_group::2) kernel runs it, and the column width
- * of the narrow tail tiles (0 = none).  Pure arithmetic, no device work. */
+ * current device, or 132 without one): BLOCK_N; two_sm and tail_block_n are always 0 on sm_90a (one CTA per tile, every
+ * tile BLOCK_N wide).  Pure arithmetic, no device work. */
 int pb200_gemm_plan(int64_t m, int64_t n, int64_t k, int sm_count, int* block_n, int* two_sm, int* tail_block_n);
 
 /* ------------------------------------------------------------------------------------------
@@ -313,12 +313,6 @@ int64_t pb200_vqgan_resblock_workspace_bytes(int batch, int h, int w, int c);
 int pb200_vqgan_resblock(float* x_nhwc, int batch, int h, int w, int c, const float* dw_w9, const float* dw_bias,
                          const void* w1_f16, const float* b1, const void* w2_f16, const float* b2, const float* gammas_host,
                          void* workspace, int64_t workspace_bytes, void* stream);
-
-/* Experiment kept for the record (measured slower than the two GEMMs, see csrc/vq_mlp.cu): the ResBlock MLP in one tcgen05
- * kernel, x[rows, c] += alpha * (GELU(a16 W1^T + b1) W2^T + b2) with the 4c-wide hidden kept in TMEM / shared memory.
- * c in {384, 192}, rows >= 256.  The codec uses it only with PB200_VQ_MLP_FUSED=1. */
-int pb200_vq_mlp_fused(const void* a16, int64_t rows, int c, const void* w1_f16, const float* b1, const void* w2_f16,
-                       const float* b2, float* x, float alpha, void* stream);
 
 /* Output forms of the decoder's last kernel (out_block: 1x1 conv + PixelShuffle, ref/src/vqgan.py:86-89), fused with what
  * the reference's callers do next (ref/src_distributed/train.py:168-171 `decode_indices(x).clamp(0, 1)`, then

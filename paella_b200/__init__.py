@@ -1,4 +1,4 @@
-"""paella_b200 — B200-native (sm_100a) implementation of Paella's sampling hot path.
+"""paella_b200 — H100-native (sm_90a) implementation of Paella's sampling hot path.
 
 Python mirror of the reference's class surface (``Paella``, ``sample``, ``VQModel`` ...) over the
 C ABI in ``include/paella_b200.h`` (``libpaella_b200.so``, hand-written CUDA).  No CPU fallback.

@@ -114,7 +114,6 @@ SIGNATURES = {
     "pb200_vqgan_decode_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int64,
                                       c_void_p]),
     "pb200_vqgan_sync_params": (c_int, [c_void_p, c_void_p]),
-    "pb200_vq_mlp_fused": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p]),
     "pb200_vqgan_resblock_workspace_bytes": (c_int64, [c_int, c_int, c_int, c_int]),
     "pb200_vqgan_resblock": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p, POINTER(c_float), c_void_p, c_int64, c_void_p]),
@@ -142,7 +141,7 @@ def lib() -> ctypes.CDLL:
             fn = getattr(l, name)        # AttributeError here = header/library mismatch
             fn.restype = res
             fn.argtypes = args
-        if l.pb200_abi_version() != 2:
+        if l.pb200_abi_version() != 3:
             raise PaellaB200Error("libpaella_b200.so ABI version mismatch")
         _lib = l
     return _lib

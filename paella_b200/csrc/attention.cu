@@ -4,9 +4,10 @@
 //
 // At the reference's shapes this op is HBM/latency bound, not tensor bound: <=256 queries x <=1032 keys x 16
 // heads x hd 80 per sample is ~1% of a forward's FLOPs (SURVEY.md §8a R7), and one (sample, head) problem is far
-// smaller than a tcgen05 tile.  So: one CTA per (64 queries, head, sample), flash-style online softmax over
-// 64-key chunks, fp16 mma.sync m16n8k16 with fp32 accumulation, K/V staged in padded shared memory and read
-// with ldmatrix.  The projections around it (QKV, out_proj) are the tcgen05 GEMMs in gemm.cu.
+// smaller than a 128-row GEMM tile.  So: one CTA per (64 queries, head, sample), flash-style online softmax over
+// 64-key chunks.  head_dim 80 runs the wgmma + TMA kernel of attention_wg.cu; this file's kernel (fp16 mma.sync
+// m16n8k16 with fp32 accumulation, K/V staged in padded shared memory and read with ldmatrix) every other head dim.
+// The projections around it (QKV, out_proj) are the wgmma GEMMs in gemm.cu.
 #include "attention.cuh"
 
 namespace pb {
@@ -39,10 +40,8 @@ constexpr int ATT_BN = 64;   // keys per chunk
 constexpr float NEG_BIG = -1e30f;
 
 // One CTA per (64 queries, head, sample); each warp owns 16 queries and walks the keys in 64-key chunks
-// (double-buffered cp.async).  Tried on B200 and dropped, twice: splitting the KEYS over the warps for the <= 16-query
-// levels -- (a) whole chunks per warp, all chunks resident: 20.7 vs 19.6 ms per bench step (the extra shared memory costs
-// a resident CTA); (b) the 16-key groups of every chunk per warp, same loads: 19.9 vs 19.5 ms.  Those launches are bound
-// by the K/V load latency (86 MB of conditioning K/V per launch), not by the one busy warp.
+// (double-buffered cp.async).  It runs every head dim other than 80 (csrc/attention_wg.cu), and head_dim 80 with
+// PB200_ATTN_MMA_SYNC=1.
 template <int HD>
 __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
     constexpr int LDS = HD + 8;           // padded row: (HD+8)*2 bytes is an odd multiple of 16 -> conflict-free ldmatrix
@@ -89,8 +88,8 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
             cp_async16(smem_u32(sV + r * LDS + cc * 8), vs, nbytes);
         }
     };
-    // Q rides in the same cp.async group as the first K/V chunk (a register-staged Q load cost 5 serialised global
-    // round trips before anything else could start: 22% of the kernel's stall samples in ncu)
+    // Q rides in the same cp.async group as the first K/V chunk (a register-staged Q load costs 5 serialised global
+    // round trips before anything else can start)
     for (int c = tid; c < QROWS * CPR; c += 128) {
         const int r = c / CPR, cc = c - r * CPR;
         const bool ok = q0 + r < p.P;
@@ -246,9 +245,7 @@ int launch_attention(const AttnParams& p, cudaStream_t st) {
     PB_CHECK(p.E % 8 == 0, "attention: E must be a multiple of 8");
     if (p.B == 0 || p.P == 0) return 0;
     {
-        int rc = launch_attention_tt(p, st);
-        if (rc >= 0) return rc;
-        rc = launch_attention_tc(p, st);
+        const int rc = launch_attention_wgmma(p, st);
         if (rc >= 0) return rc;
     }
     // algorithmic bytes: q, self k/v, out once; conditioning k/v once per sample

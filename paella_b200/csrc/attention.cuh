@@ -16,13 +16,11 @@ struct AttnParams {
     const float* attn_w;   // optional post-softmax weights for the last n_w keys ...
     int n_w;
     int w_batch;           // ... of samples [0, w_batch)
-    int n_slots = 0;       // blocks of S_max rows in ckv (0: B); only bounds the TMA of the tcgen05 kernel
+    int n_slots = 0;       // blocks of S_max rows in ckv (0: B)
 };
 
-// Dispatch: the tcgen05/TMEM kernel (attention_tc.cu) for head_dim 80 and query counts that tile by 64 (or <= 64), the
-// mma.sync kernel below for every other shape (tiny test configs, odd head dims, very long key lists).
+// Dispatch: the wgmma + TMA kernel (attention_wg.cu) for head_dim 80, the mma.sync kernel (attention.cu) for other head dims
 int launch_attention(const AttnParams& p, cudaStream_t st);
-int launch_attention_tc(const AttnParams& p, cudaStream_t st);      // 0 launched, 1 error, -1 shape not handled
-int launch_attention_tt(const AttnParams& p, cudaStream_t st);      // transposed (keys on M = 128) variant for <= 64 queries: same codes
+int launch_attention_wgmma(const AttnParams& p, cudaStream_t st);      // 0 launched, 1 error, -1 shape not handled
 
 }  // namespace pb

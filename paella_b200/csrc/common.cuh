@@ -1,4 +1,4 @@
-// Shared device/host helpers for the paella_b200 CUDA library (sm_100a only).
+// Shared device/host helpers for the paella_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -90,7 +90,7 @@ TraceBuf trace_begin(const char* kernel);
 int trace_end(const char* kernel, TraceBuf t, const char* const* role_names, const char* const* event_names);
 
 // ---------------------------------------------------------------- small device helpers
-// Lets a dependent kernel launched with programmatic stream serialization (the tcgen05 GEMMs, see ptx.cuh) start its
+// Lets a dependent kernel launched with programmatic stream serialization (the wgmma GEMMs, see ptx.cuh) start its
 // prologue while this kernel's last CTAs are still running.  No effect otherwise.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
@@ -174,7 +174,7 @@ __device__ __forceinline__ float u32_to_uniform(uint32_t x) {
 
 // Tensor.exponential_(1) CUDA branch (ATen/core/TransformationHelper.h:129-146): -log(u), with
 // log(u) replaced by -eps/2 when u >= 1 - eps/2.  `at::log` on the device is the fast __logf
-// (ATen/NumericUtils.h:149-160) — measured on the B200: using logf() here flips ~1e-4 of the draws.
+// (ATen/NumericUtils.h:149-160); using logf() here flips ~1e-4 of the draws.
 __device__ __forceinline__ float torch_exponential1(float u) {
     const float lg = (u >= 1.0f - 1.1920928955078125e-07f / 2.0f) ? -(1.1920928955078125e-07f / 2.0f) : __logf(u);
     return -1.0f * lg;

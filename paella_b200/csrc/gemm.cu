@@ -1,22 +1,20 @@
-// tcgen05 GEMM for every Linear / 1x1-conv / patchify contraction on the path:
-//     C[M,N] = A[M,K] . W[N,K]^T   (fp16 operands, fp32 accumulation in TMEM)  + fused epilogue
+// wgmma GEMM for every Linear / 1x1-conv / patchify contraction on the path:
+//     C[M,N] = A[M,K] . W[N,K]^T   (fp16 operands, fp32 accumulation in registers)  + fused epilogue
 // Replaces the cuBLAS/cuDNN calls behind nn.Linear / nn.Conv2d(k=1) / Conv2d(k=2,s=2) /
 // ConvTranspose2d(k=2,s=2) in ref/src/modules.py (ResBlock :49-55, AttnBlock :71-74, embedding :130-134,
 // resamplers :153-156,172-175, clf/out_mapper :179-187) and ref/src/vqgan.py (ResBlock :16-20).
 //
-// Two persistent, warp-specialised kernels share the epilogues:
-//   gemm_f16_cg2_kernel   2-SM tiles (cluster of 2, tcgen05.mma.cta_group::2, M256 x N{128,256}); the default for M > 128
-//   gemm_f16_kernel       1-SM tiles (M128 x N{64,128,256}); small M, and the im2col-free convolutions (AMODE 1/2)
-// Roles inside a CTA (64 + 32*E threads, E = 8 or 16 epilogue warps):
-//   warp 0   : TMA producer  - cp.async.bulk.tensor loads of the 128x64 A tile and of this CTA's share of the W tile,
-//              128B-swizzled, into a 4-8 stage shared-memory ring guarded by full/empty mbarriers
-//   warp 1   : MMA issuer    - one thread issues tcgen05.mma (K=16) x4 per stage into one of two TMEM accumulators;
-//              tcgen05.commit (multicast to both CTAs of a pair) releases the stage / publishes the accumulator
-//   warps 2+ : epilogue      - tcgen05.ld 32x32b (lane = row, registers = 32 columns), fused bias / GELU + GRN statistic /
-//              residual + FiLM / LayerNorm fold / un-patchify / NCHW transpose; the chunk is transposed inside the warp so
-//              that every store instruction writes whole 128-byte lines; overlaps the next tile's MMAs (second accumulator)
-// Scheduling: tile width from a tensor / L2-fabric cycle model (gemm_pick_block_n), narrow tail tiles for the leftover
-// of the last wave (gemm_tail_block_n), programmatic dependent launch so the prologue overlaps the previous kernel.
+// One persistent, warp-specialised kernel (gemm_f16_kernel), M128 x N{64,128,256} tiles, 384 threads:
+//   warpgroup 0    : TMA producer  - one thread issues cp.async.bulk.tensor loads of the 128x64 A tile and the BLOCK_N x 64
+//                    W tile, 128B-swizzled, into a 3-8 stage shared-memory ring guarded by full/empty mbarriers; the
+//                    warpgroup hands its registers to the MMA warpgroups (setmaxnreg)
+//   warpgroups 1,2 : MMA + epilogue - each issues wgmma m64nNk16 (4 per stage) for its 64 rows of the tile, keeps one
+//                    k-block in flight and releases the previous stage; then the fused epilogue (bias / GELU + GRN statistic /
+//                    residual + FiLM / LayerNorm fold / un-patchify / NCHW transpose) through a shared-memory slab that turns
+//                    the accumulator fragment into row-per-lane chunks, transposed inside the warp so that every store
+//                    instruction writes whole 128-byte lines.  The producer runs ahead into the next tile meanwhile.
+// Scheduling: tile width from a tensor / L2 cycle model (gemm_pick_block_n), programmatic dependent launch so the prologue
+// overlaps the previous kernel.
 #include "gemm.cuh"
 #include <type_traits>
 
@@ -136,10 +134,9 @@ int make_tmap_f16_nd(CUtensorMap* tm, const void* ptr, int rank, const int64_t* 
 
 // ------------------------------------------------------------------ epilogue
 // Global operands of a 32-column chunk that do not depend on the accumulator (the fp32 residual row segment).  They
-// are fetched BEFORE the wait on the accumulator: out may alias resid (the model updates x in place), so inside the
-// store loop the compiler must order every load after the previous store -- 8 dependent L2 round trips per chunk,
-// which made the K=1280 out-projection epilogue-bound (73 us for 27 GFLOP).  Preloaded, the latency hides behind
-// the tile's main loop.
+// are fetched for the whole chunk BEFORE its store loop: out may alias resid (the model updates x in place), so inside
+// the store loop the compiler must order every load after the previous store -- 8 dependent L2 round trips per chunk
+// instead of 8 independent loads in flight together.
 template <int MODE>
 struct EpiPre {};
 template <>
@@ -153,9 +150,8 @@ struct EpiPre<PB200_EPI_RESID_LN_F32> {
     float shift = 0.f;                 // this lane's row: the shift subtracted before the fp16 copy and the statistics
 };
 
-// Coalescing.  tcgen05.ld hands every lane one ROW of the chunk (32 consecutive columns), so a direct 16-byte store
-// per lane touches 32 different 128-byte lines per instruction and the LSU serialises them (measured: the fp32
-// epilogue of the 8192x1280x1280 out-projection took 2x its main loop).  The chunk is therefore transposed inside the
+// Coalescing.  The epilogue hands every lane one ROW of the chunk (32 consecutive columns), so a direct 16-byte store
+// per lane touches 32 different 128-byte lines per instruction and the LSU serialises them.  The chunk is therefore transposed inside the
 // warp with xor-butterfly shuffles first:
 //   fp32: 8x8 transpose of float4 items in 8-lane groups -> lane (a,b) item i = row 8a+i, columns 4b..4b+3
 //         (a store instruction then writes 4 full 128-byte lines);
@@ -199,7 +195,7 @@ template <int MODE>
 __device__ __forceinline__ void epilogue_preload(const pb200_gemm_epilogue& ep, int M, int N, int row, int col0,
                                                  EpiPre<MODE>& pre, int lane, bool first_chunk) {
     if constexpr (MODE == PB200_EPI_F16_LN) {
-        if (first_chunk && row < M) {      // row statistics -> (mean, rstd), before the wait on the accumulator
+        if (first_chunk && row < M) {      // row statistics -> (mean, rstd), once per tile
             const longlong2 st = *reinterpret_cast<const longlong2*>(ep.ln_stat + 2 * (int64_t)row);
             const float inv_c = 1.0f / (float)ep.ln_c;
             const float mean = (float)st.x * (1.0f / 1048576.0f) * inv_c;
@@ -447,67 +443,59 @@ __device__ __forceinline__ void epilogue_finish(const pb200_gemm_epilogue& ep, i
 // AMODE 0: A is a [M,K] matrix.  AMODE 1/2: A rows are gathered by TMA straight from an NHWC fp16 activation
 // (im2col-free convolution): a 128-row tile is a th x tw patch of the output grid and k-block kb selects a filter
 // tap and a 64-channel slice; out-of-image taps are zero-filled by the TMA unit (the conv's zero padding).
-template <int BLOCK_N, int MODE, int AMODE>
-__global__ void __launch_bounds__(gemm_threads(BLOCK_N), 1)
+// ASCALE (GlobalResponseNorm folded into the A operand, ref/src/modules.py:37-40 + :53): the A tile is multiplied in shared
+// memory, between TMA and MMA, by a per-(sample, k) fp16 factor  s[b, k] = 1 + gamma[k] * Nx[b, k]  -- GEMM2 of a ResBlock then
+// computes (h * s) W2^T + (W2 beta + b2) = GRN(h) W2^T + b2 without the separate read-modify-write pass over the 4c-wide hidden.
+// The [samples x 64] slice of s lands in the stage beside A and W; each MMA warpgroup rescales its own 64 rows in place (one
+// HMUL2 rounding, the fp16 product), fences the generic->async proxy and only then issues its wgmma.
+template <int BLOCK_N, int MODE, int AMODE, bool ASCALE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                const pb200_gemm_epilogue ep, const ConvGeom geom, int M, int N, int K) {
-    using L = GemmSmem<BLOCK_N>;
+                const __grid_constant__ CUtensorMap tm_s, const pb200_gemm_epilogue ep, const ConvGeom geom, int M, int N,
+                int K) {
+    using L = GemmSmem<BLOCK_N, ASCALE>;
+    constexpr int NSUB = BLOCK_N > 128 ? 2 : 1;          // a 256-wide tile is issued as two n128 wgmma per k-step
+    constexpr int SUBN = BLOCK_N / NSUB;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
     const uint32_t bar_base = smem_base + L::STAGES * L::STAGE_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (L::STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * L::STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * L::STAGES + 2 + s); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * L::STAGES + 4);
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+    float* epi_stage = reinterpret_cast<float*>(smem_gen + L::STAGES * L::STAGE_BYTES + 256);
 
-    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
     const int lane = threadIdx.x & 31;
     const int n_tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
     const int n_tiles_m = AMODE == 0 ? (M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M : geom.batch * geom.tiles_y * geom.tiles_x;
     const int n_kb = (K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
-    // Optional 2-CTA cluster (launch attribute): the two CTAs take M-tiles 2p and 2p+1 of the same N-tile and each
-    // loads only HALF of the W tile, multicasting it into both CTAs' shared memory — the SM<-L2 traffic per FLOP
-    // drops by a third (ncu: the single-CTA kernel saturates the L2->SM fabric at ~13 TB/s).
-    const uint32_t csize = ptx::cluster_nctarank();
-    const uint32_t crank = ptx::cluster_ctarank();
-    const int n_units = ((n_tiles_m + (int)csize - 1) / (int)csize) * n_tiles_n;     // work units = (M-tile group, N-tile)
-    const int unit0 = blockIdx.x / csize, unit_step = gridDim.x / csize;
+    const int n_units = n_tiles_m * n_tiles_n;
+    const int P = ep.rows_per_sample;
+    const int ns = ASCALE ? (P >= GEMM_BLOCK_M ? 1 : GEMM_BLOCK_M / P) : 0;      // samples in a 128-row tile
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tm_a);
         ptx::prefetch_tensormap(&tm_b);
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < L::STAGES; ++s) {
-                ptx::mbar_init(full_bar(s), 1);
-                ptx::mbar_init(empty_bar(s), csize);        // every CTA of the cluster must have drained the stage
-            }
-            for (int s = 0; s < 2; ++s) {
-                ptx::mbar_init(tfull_bar(s), 1);
-                ptx::mbar_init(tempty_bar(s), gemm_epi_warps(BLOCK_N));       // one arrival per epilogue warp
-            }
-            ptx::fence_barrier_init();
+        for (int s = 0; s < L::STAGES; ++s) {
+            ptx::mbar_init(full_bar(s), 1);
+            ptx::mbar_init(empty_bar(s), GEMM_CONSUMERS);      // one arrival per MMA warpgroup
         }
-        __syncwarp();
-        ptx::tmem_alloc(tmem_slot, L::TMEM_COLS);
-        ptx::tmem_relinquish();
+        ptx::fence_barrier_init();
     }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    if (csize > 1) ptx::cluster_sync();          // peer barriers are initialised before anything can signal them
-    const uint32_t tmem_base = *tmem_slot_ptr;
+    // everything above overlapped the tail of the previous kernel (programmatic dependent launch); its results are
+    // read from here on
+    ptx::griddep_launch();
+    ptx::griddep_wait();
 
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (ptx::elect_one()) {
+    if (wg == 0) {
+        // ===================== TMA producer (one elected thread of warp 0) =====================
+        ptx::setmaxnreg_dec<40>();
+        if (threadIdx.x < 32 && ptx::elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int unit = unit0; unit < n_units; unit += unit_step) {
-                const int mt = (unit / n_tiles_n) * (int)csize + (int)crank;
+            for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
+                const int mt = unit / n_tiles_n;
                 const int m_idx = mt * GEMM_BLOCK_M;
                 const int n_idx = (unit % n_tiles_n) * BLOCK_N;
                 int cb = 0, cy0 = 0, cx0 = 0;
@@ -519,7 +507,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
                 }
                 for (int kb = 0; kb < n_kb; ++kb) {
                     ptx::mbar_wait(empty_bar(stage), phase ^ 1);
-                    ptx::mbar_arrive_expect_tx(full_bar(stage), L::STAGE_BYTES);
+                    ptx::mbar_arrive_expect_tx(full_bar(stage), (uint32_t)(L::A_BYTES + L::B_BYTES + ns * GEMM_BLOCK_K * 2));
                     const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
                     if (AMODE == 0) {
                         ptx::tma_load_2d(&tm_a, full_bar(stage), sa, kb * GEMM_BLOCK_K, m_idx);
@@ -539,67 +527,92 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
                         const int ox = geom.px == 0 ? (tx == 0 ? 0 : -1) : (tx == 0 ? 1 : 0);
                         ptx::tma_load_4d(&tm_a, full_bar(stage), sa, cc * 64, cx0 + ox, cy0 + oy, cb);
                     }
-                    if (csize == 1) {          // the W map's box is half a tile (BLOCK_N/2 rows): two loads
-                        ptx::tma_load_2d(&tm_b, full_bar(stage), sa + L::A_BYTES, kb * GEMM_BLOCK_K, n_idx);
-                        ptx::tma_load_2d(&tm_b, full_bar(stage), sa + L::A_BYTES + L::B_BYTES / 2, kb * GEMM_BLOCK_K,
-                                         n_idx + BLOCK_N / 2);
-                    } else {   // my half of the W tile, written into both CTAs' stage (same offsets, same barrier slot)
-                        ptx::tma_load_2d_mcast(&tm_b, full_bar(stage), sa + L::A_BYTES + crank * (L::B_BYTES / 2),
-                                               kb * GEMM_BLOCK_K, n_idx + (int)crank * (BLOCK_N / 2), (uint16_t)0x3);
-                    }
+                    // the W map's box is half a tile (BLOCK_N/2 rows): two loads
+                    ptx::tma_load_2d(&tm_b, full_bar(stage), sa + L::A_BYTES, kb * GEMM_BLOCK_K, n_idx);
+                    ptx::tma_load_2d(&tm_b, full_bar(stage), sa + L::A_BYTES + L::B_BYTES / 2, kb * GEMM_BLOCK_K,
+                                     n_idx + BLOCK_N / 2);
+                    if (ASCALE)
+                        ptx::tma_load_2d(&tm_s, full_bar(stage), sa + L::A_BYTES + L::B_BYTES, kb * GEMM_BLOCK_K, m_idx / P);
                     if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc = ptx::umma_idesc_f16(GEMM_BLOCK_M, BLOCK_N, 0);
+    } else {
+        // ===================== MMA + epilogue: warpgroup cw owns rows [64 cw, 64 cw + 64) of every tile =====================
+        ptx::setmaxnreg_inc<232>();
+        const int cw = wg - 1;
+        const int tid = threadIdx.x & 127;
+        const int wq = tid >> 5;                 // warp of the warpgroup: wgmma rows [16 wq, 16 wq + 16)
+        float* stage_rows = epi_stage + cw * 64 * GEMM_EPI_STRIDE;
+        float acc[NSUB][SUBN / 2];
         int stage = 0;
         uint32_t phase = 0;
-        int iter = 0;
-        for (int unit = unit0; unit < n_units; unit += unit_step, ++iter) {
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ptx::mbar_wait(tempty_bar(as), aphase ^ 1);
-            ptx::tc_fence_after();
-            const uint32_t tmem_d = tmem_base + as * BLOCK_N;
-            for (int kb = 0; kb < n_kb; ++kb) {
-                ptx::mbar_wait(full_bar(stage), phase);
-                ptx::tc_fence_after();
-                if (ptx::elect_one()) {
-                    const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
-                    const uint64_t da = ptx::umma_desc_kmajor_sw128(sa);
-                    const uint64_t db = ptx::umma_desc_kmajor_sw128(sa + L::A_BYTES);
-#pragma unroll
-                    for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
-                        // advance 16 elements (32 bytes) along K inside the 128-byte swizzle atom: +2 in (addr>>4)
-                        ptx::umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                    }
-                    if (csize == 1) ptx::umma_commit(empty_bar(stage));  // smem stage reusable once these MMAs retire
-                    else ptx::umma_commit_mcast(empty_bar(stage), (uint16_t)0x3);   // ... in both CTAs of the pair
-                    if (kb == n_kb - 1) ptx::umma_commit(tfull_bar(as)); // accumulator complete
-                }
-                __syncwarp();
-                if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else {
-        // ===================== epilogue =====================
-        const int q = warp & 3;                 // TMEM lane quarter this warp may read
-        const int half = (warp - 2) >> 2;       // which half of the tile's columns (two warps share a quarter)
-        constexpr int COLS_PER_WARP = BLOCK_N / (gemm_epi_warps(BLOCK_N) / 4);
-        int iter = 0;
-        for (int unit = unit0; unit < n_units; unit += unit_step, ++iter) {
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            const int mt = (unit / n_tiles_n) * (int)csize + (int)crank;
+        for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
+            const int mt = unit / n_tiles_n;
             const int m_idx = mt * GEMM_BLOCK_M;
             const int n_idx = (unit % n_tiles_n) * BLOCK_N;
-            int row = m_idx + q * 32 + lane;
+            int prev = 0;
+            for (int kb = 0; kb < n_kb; ++kb) {
+                ptx::mbar_wait(full_bar(stage), phase);
+                const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
+                if (ASCALE) {
+                    // thread = half a row: chunks [4 (tid & 1), +4) of row 64 cw + tid / 2; logical 16-byte chunk j of row r
+                    // sits at j ^ (r & 7) (128-byte swizzle)
+                    const int r = cw * 64 + (tid >> 1);
+                    const int sl = P >= GEMM_BLOCK_M ? 0 : min(r / P, ns - 1);
+                    uint8_t* sg = smem_gen + stage * L::STAGE_BYTES;
+                    uint4* arow = reinterpret_cast<uint4*>(sg + r * 128);
+                    const uint4* srow = reinterpret_cast<const uint4*>(sg + L::A_BYTES + L::B_BYTES + sl * 128);
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const int j = (tid & 1) * 4 + jj;
+                        uint4 av = arow[j ^ (r & 7)];
+                        const uint4 sv = srow[j];
+                        __half2* a2 = reinterpret_cast<__half2*>(&av);
+                        const __half2* s2 = reinterpret_cast<const __half2*>(&sv);
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) a2[e] = __hmul2(a2[e], s2[e]);
+                        arow[j ^ (r & 7)] = av;
+                    }
+                    ptx::fence_proxy_async_smem();       // the rescaled rows must be visible to the tensor core's async proxy
+                    ptx::bar_sync(1 + cw, 128);
+                }
+                const uint64_t da = ptx::wgmma_desc_kmajor_sw128(sa + (uint32_t)cw * (64 * 128));
+                const uint64_t db = ptx::wgmma_desc_kmajor_sw128(sa + L::A_BYTES);
+                ptx::wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
+                    // advance 16 elements (32 bytes) along K inside the 128-byte swizzle atom: +2 in (addr>>4)
+                    const uint32_t accum = (kb | k) != 0 ? 1u : 0u;
+#pragma unroll
+                    for (int s = 0; s < NSUB; ++s) {
+                        const uint64_t dbs = db + (uint64_t)((s * SUBN * 128) >> 4) + 2 * k;
+                        if constexpr (SUBN == 64) ptx::wgmma_m64n64k16(acc[s], da + 2 * k, dbs, accum);
+                        else ptx::wgmma_m64n128k16(acc[s], da + 2 * k, dbs, accum);
+                    }
+                }
+                ptx::wgmma_commit();
+                if (kb > 0) {              // the previous k-block's MMAs have retired: its stage goes back to the producer
+                    ptx::wgmma_wait<1>();
+                    if (tid == 0) ptx::mbar_arrive(empty_bar(prev));
+                }
+                prev = stage;
+                if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
+            }
+            ptx::wgmma_wait<0>();
+            if (tid == 0) ptx::mbar_arrive(empty_bar(prev));
+#pragma unroll
+            for (int s = 0; s < NSUB; ++s) ptx::fence_regs(acc[s]);
+
+            // ---- epilogue.  The accumulator fragment (thread = rows 16 wq + lane/4 (+8), column pairs) goes through shared
+            // memory in 64-column slabs so that the epilogue sees what it is written for: lane = row, 32 consecutive columns.
+            // Warp wq takes rows [32 (wq & 1), +32) of the warpgroup's 64 and columns [32 (wq >> 1), +32) of the slab.
+            const int rl = (wq & 1) * 32 + lane;               // row of the warpgroup's 64
+            const int r = cw * 64 + rl;                         // row of the 128-row tile
+            int row = m_idx + r;
             if (AMODE != 0) {   // tile row r = (ly, lx) of a th x tw patch -> output pixel row of the NHWC result
                 const int cb = mt / (geom.tiles_y * geom.tiles_x);
                 const int rr = mt - cb * geom.tiles_y * geom.tiles_x;
-                const int r = q * 32 + lane;
                 const int gy = (rr / geom.tiles_x) * geom.th + r / geom.tw;
                 const int gx = (rr % geom.tiles_x) * geom.tw + r % geom.tw;
                 row = (gy < geom.gh && gx < geom.gw)
@@ -607,298 +620,53 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
                           : M;      // M = B*oh*ow: out of range -> masked
             }
             EpiPre<MODE> pre;
-            if (n_idx + half * COLS_PER_WARP < N) epilogue_preload<MODE>(ep, M, N, row, n_idx + half * COLS_PER_WARP, pre, lane, true);
-            ptx::mbar_wait(tfull_bar(as), aphase);
-            ptx::tc_fence_after();
 #pragma unroll 1
-            for (int c = half * COLS_PER_WARP; c < (half + 1) * COLS_PER_WARP; c += 32) {
-                if (n_idx + c >= N) break;
-                if (c != half * COLS_PER_WARP) epilogue_preload<MODE>(ep, M, N, row, n_idx + c, pre, lane, false);
-                float v[32];
-                ptx::tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BLOCK_N + c), v);
-                epilogue_chunk<MODE>(ep, M, N, row, n_idx + c, v, lane, pre);
+            for (int c64 = 0; c64 < BLOCK_N / 64; ++c64) {
+                if (n_idx + c64 * 64 >= N) break;
+                // the 32 registers of slab c64 (compile-time indices: one case per slab), each written once
+                auto scatter = [&](auto slab) {
+                    constexpr int C = decltype(slab)::value;
+                    constexpr int S = (C * 64) / SUBN, I0 = ((C * 64) % SUBN) / 2;
+#pragma unroll
+                    for (int i = 0; i < 32; ++i)
+                        stage_rows[(wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1)) * GEMM_EPI_STRIDE + (i >> 2) * 8 + 2 * (lane & 3) + (i & 1)] =
+                            acc[S][I0 + i];
+                };
+                switch (c64) {
+                    case 0: scatter(std::integral_constant<int, 0>{}); break;
+                    case 1: if constexpr (BLOCK_N > 64) scatter(std::integral_constant<int, (BLOCK_N > 64 ? 1 : 0)>{}); break;
+                    case 2: if constexpr (BLOCK_N > 128) scatter(std::integral_constant<int, (BLOCK_N > 128 ? 2 : 0)>{}); break;
+                    default: if constexpr (BLOCK_N > 128) scatter(std::integral_constant<int, (BLOCK_N > 128 ? 3 : 0)>{}); break;
+                }
+                ptx::bar_sync(1 + cw, 128);
+                const int col0 = n_idx + c64 * 64 + (wq >> 1) * 32;
+                if (col0 < N) {
+                    float v[32];
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) v[j] = stage_rows[rl * GEMM_EPI_STRIDE + (wq >> 1) * 32 + j];
+                    epilogue_preload<MODE>(ep, M, N, row, col0, pre, lane, c64 == 0);
+                    epilogue_chunk<MODE>(ep, M, N, row, col0, v, lane, pre);
+                }
+                ptx::bar_sync(1 + cw, 128);                     // the slab buffer is rewritten next
             }
             epilogue_finish<MODE>(ep, M, row, pre);
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(tempty_bar(as));
         }
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (csize > 1) ptx::cluster_sync();          // the peer may still be multicasting into / signalling this CTA
-    if (warp == 1) ptx::tmem_dealloc(tmem_base, L::TMEM_COLS);
 }
 
-// ------------------------------------------------------------------ 2-SM kernel (cta_group::2)
-// A CTA pair (cluster of 2 on one TPC) computes a 256 x BLOCK_N tile with ONE tcgen05.mma.cta_group::2 stream issued
-// by the leader CTA: each CTA stages its own 128 rows of A and only its HALF of the W tile (BLOCK_N/2 rows); the
-// tensor cores of both SMs read both halves.  Per SM this halves the W bytes pulled from L2 and the W bytes read
-// from shared memory per MMA (ncu on the 1-SM kernel: L2->SM fabric at ~13 TB/s and, for BLOCK_N=128, the
-// 128 B/clk shared-memory port are the limiters).  Accumulators: each CTA's TMEM holds its 128 rows x BLOCK_N.
-//   full[s]   (leader)  : 2 arrivals (both producers) + the bytes of both CTAs' TMA loads (cta_group::2 loads
-//                         complete_tx on the leader's barrier)
-//   empty[s]  (each CTA): tcgen05.commit.cta_group::2 multicast from the leader's MMA thread
-//   tfull[a]  (each CTA): same commit, when a tile's last k-block has been issued
-//   tempty[a] (leader)  : one arrival per epilogue warp of BOTH CTAs (the peer arrives remotely)
-// ASCALE (GlobalResponseNorm folded into the A operand, ref/src/modules.py:37-40 + :53): the A tile is multiplied in shared
-// memory, between TMA and MMA, by a per-(sample, k) fp16 factor  s[b, k] = 1 + gamma[k] * Nx[b, k]  -- GEMM2 of a ResBlock then
-// computes (h * s) W2^T + (W2 beta + b2) = GRN(h) W2^T + b2 without the separate read-modify-write pass over the 4c-wide hidden.
-// Four extra warps per CTA (one thread per row) transform every stage: the A tile and the [samples x 64] slice of s land on
-// a CTA-local barrier (afull), the transform warps rescale the swizzled rows in place, fence the generic->async proxy and arrive
-// on the leader's ready[s]; the MMA thread waits for full[s] (both W halves) and ready[s] (both CTAs' A tiles transformed).
-constexpr int GEMM_ASCALE_WARPS = 4;         // one thread per row of the 128-row A tile
-constexpr int GEMM_ASCALE_BYTES = 1024;        // up to 8 samples x 64 factors per 128-row tile and k-block
-template <int BLOCK_N, int MODE, bool ASCALE>
-__global__ void __launch_bounds__(gemm_threads(BLOCK_N) + (ASCALE ? 32 * GEMM_ASCALE_WARPS : 0), 1)
-gemm_f16_cg2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                    const __grid_constant__ CUtensorMap tm_b_tail, const __grid_constant__ CUtensorMap tm_s,
-                    const pb200_gemm_epilogue ep, int M, int N, int K, int n_main, int tail_bn) {
-    constexpr int A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
-    constexpr int BH_BYTES = (BLOCK_N / 2) * GEMM_BLOCK_K * 2;       // this CTA's half of the W tile
-    constexpr int STAGE_BYTES = A_BYTES + BH_BYTES + (ASCALE ? GEMM_ASCALE_BYTES : 0);
-    constexpr int STAGES = BLOCK_N >= 256 ? 6 : 8;
-    constexpr int TMEM_COLS = BLOCK_N >= 256 ? 512 : 256;
-    constexpr int EW = gemm_epi_warps(BLOCK_N);
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t bar_base = smem_base + STAGES * STAGE_BYTES;
-    auto full_bar = [&](int s) { return bar_base + 8u * s; };
-    auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-    auto afull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 6 + s); };          // ASCALE: this CTA's A + factors landed
-    auto ready_bar = [&](int s) { return bar_base + 8u * (3 * STAGES + 6 + s); };          // ASCALE (leader): both A tiles rescaled
-    const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-    uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
-    const int lane = threadIdx.x & 31;
-    const uint32_t crank = ptx::cluster_ctarank();
-    const bool leader = crank == 0;
-    const int n_tiles_n = (N + BLOCK_N - 1) / BLOCK_N;
-    const int n_pairs_m = (M + 2 * GEMM_BLOCK_M - 1) / (2 * GEMM_BLOCK_M);
-    // Work units.  Units [0, n_main) are full 256 x BLOCK_N pair tiles.  With a tail (tail_bn > 0) the remaining pair
-    // tiles -- the ones that would form a mostly idle last wave -- are cut into BLOCK_N / tail_bn narrower tiles of
-    // tail_bn columns, so the last wave is short and (nearly) full instead (8192 x 1280: 160 tiles on 74 SM pairs =
-    // 2.16 waves ran as 3; with the 12 leftover tiles split 4 ways it runs as 2 + a quarter-width wave).
-    const int n_big = n_pairs_m * n_tiles_n;
-    const int tail_split = tail_bn > 0 ? BLOCK_N / tail_bn : 1;
-    const int n_units = tail_bn > 0 ? n_main + (n_big - n_main) * tail_split : n_big;
-    const int unit0 = blockIdx.x >> 1, unit_step = gridDim.x >> 1;
-    struct Unit { int m_pair, n0, width; };
-    auto decode = [&](int u) {
-        Unit r;
-        int big = u, sub = 0;
-        r.width = BLOCK_N;
-        if (u >= n_main && tail_bn > 0) {
-            const int v = u - n_main;
-            big = n_main + v / tail_split;
-            sub = v - (v / tail_split) * tail_split;
-            r.width = tail_bn;
-        }
-        r.m_pair = big / n_tiles_n;
-        r.n0 = (big - r.m_pair * n_tiles_n) * BLOCK_N + sub * r.width;
-        if (r.n0 >= N) r.width = 0;           // a sub-tile entirely past the last column: every role skips it
-        return r;
-    };
-    const int n_kb = (K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tensormap(&tm_a);
-        ptx::prefetch_tensormap(&tm_b);
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < STAGES; ++s) {
-                ptx::mbar_init(full_bar(s), 2);
-                ptx::mbar_init(empty_bar(s), 1);
-            }
-            for (int s = 0; s < 2; ++s) {
-                ptx::mbar_init(tfull_bar(s), 1);
-                ptx::mbar_init(tempty_bar(s), 2 * EW);
-            }
-            if (ASCALE) {
-                for (int s = 0; s < STAGES; ++s) {
-                    ptx::mbar_init(afull_bar(s), 1);
-                    ptx::mbar_init(ready_bar(s), 2 * GEMM_ASCALE_WARPS);
-                }
-            }
-            ptx::fence_barrier_init();
-        }
-        __syncwarp();
-        ptx::tmem_alloc_cg2(tmem_slot, TMEM_COLS);
-        ptx::tmem_relinquish_cg2();
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::tc_fence_after();
-    ptx::cluster_sync();
-    const uint32_t tmem_base = *tmem_slot_ptr;
-    // everything above overlapped the tail of the previous kernel (programmatic dependent launch); its results are
-    // read from here on
-    ptx::griddep_launch();
-    ptx::griddep_wait();
-
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs) =====================
-        if (ptx::elect_one()) {
-            int stage = 0;
-            uint32_t phase = 0;
-            const uint32_t leader_full0 = ptx::mapa(full_bar(0), 0);      // leader's full[0] in cluster address space
-            for (int unit = unit0; unit < n_units; unit += unit_step) {
-                const Unit un = decode(unit);
-                if (un.width == 0) continue;
-                const int m_idx = un.m_pair * (2 * GEMM_BLOCK_M) + (int)crank * GEMM_BLOCK_M;
-                const int n_idx = un.n0 + (int)crank * (un.width / 2);
-                const bool narrow = un.width != BLOCK_N;
-                const uint32_t tx = 2u * (uint32_t)((ASCALE ? 0 : A_BYTES) + (un.width / 2) * GEMM_BLOCK_K * 2);
-                const int P = ep.rows_per_sample;
-                const int ns = ASCALE ? (P >= GEMM_BLOCK_M ? 1 : GEMM_BLOCK_M / P) : 0;      // samples in this CTA's 128 rows
-                for (int kb = 0; kb < n_kb; ++kb) {
-                    ptx::mbar_wait(empty_bar(stage), phase ^ 1);
-                    const uint32_t lfull = leader_full0 + 8u * stage;
-                    if (leader) ptx::mbar_arrive_expect_tx(full_bar(stage), tx);
-                    else ptx::mbar_arrive_cluster(lfull);
-                    const uint32_t sa = smem_base + stage * STAGE_BYTES;
-                    if (ASCALE) {       // A and its factors complete on this CTA's own barrier: the transform warps wait there
-                        ptx::mbar_arrive_expect_tx(afull_bar(stage), (uint32_t)(A_BYTES + ns * GEMM_BLOCK_K * 2));
-                        ptx::tma_load_2d(&tm_a, afull_bar(stage), sa, kb * GEMM_BLOCK_K, m_idx);
-                        ptx::tma_load_2d(&tm_s, afull_bar(stage), sa + A_BYTES + BH_BYTES, kb * GEMM_BLOCK_K, m_idx / P);
-                    } else {
-                        ptx::tma_load_2d_cg2(&tm_a, lfull, sa, kb * GEMM_BLOCK_K, m_idx);
-                    }
-                    ptx::tma_load_2d_cg2(narrow ? &tm_b_tail : &tm_b, lfull, sa + A_BYTES, kb * GEMM_BLOCK_K, n_idx);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (leader CTA only) =====================
-        if (leader) {
-            constexpr uint32_t idesc_full = ptx::umma_idesc_f16(2 * GEMM_BLOCK_M, BLOCK_N, 0);
-            const uint32_t idesc_tail = ptx::umma_idesc_f16(2 * GEMM_BLOCK_M, tail_bn > 0 ? tail_bn : BLOCK_N, 0);
-            int stage = 0;
-            uint32_t phase = 0;
-            int iter = 0;
-            for (int unit = unit0; unit < n_units; unit += unit_step) {
-                const Unit un = decode(unit);
-                if (un.width == 0) continue;
-                const uint32_t idesc = un.width == BLOCK_N ? idesc_full : idesc_tail;
-                const int as = iter & 1;
-                const uint32_t aphase = (iter >> 1) & 1;
-                ptx::mbar_wait(tempty_bar(as), aphase ^ 1);
-                ptx::tc_fence_after();
-                const uint32_t tmem_d = tmem_base + as * BLOCK_N;
-                for (int kb = 0; kb < n_kb; ++kb) {
-                    ptx::mbar_wait(full_bar(stage), phase);
-                    if (ASCALE) ptx::mbar_wait(ready_bar(stage), phase);
-                    ptx::tc_fence_after();
-                    if (ptx::elect_one()) {
-                        const uint32_t sa = smem_base + stage * STAGE_BYTES;
-                        const uint64_t da = ptx::umma_desc_kmajor_sw128(sa);
-                        const uint64_t db = ptx::umma_desc_kmajor_sw128(sa + A_BYTES);
-#pragma unroll
-                        for (int k = 0; k < GEMM_BLOCK_K / 16; ++k)
-                            ptx::umma_f16_cg2(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                        ptx::umma_commit_cg2_mcast(empty_bar(stage), (uint16_t)0x3);
-                        if (kb == n_kb - 1) ptx::umma_commit_cg2_mcast(tfull_bar(as), (uint16_t)0x3);
-                    }
-                    __syncwarp();
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-                ++iter;
-            }
-        }
-    } else if (ASCALE && warp >= 2 + EW) {
-        // ===================== A-operand transform (both CTAs, own 128 rows) =====================
-        const int r = (warp - 2 - EW) * 32 + lane;          // this thread's row of the 128-row tile
-        const int P = ep.rows_per_sample;
-        const int ns = P >= GEMM_BLOCK_M ? 1 : GEMM_BLOCK_M / P;
-        const int sl = P >= GEMM_BLOCK_M ? 0 : min(r / P, ns - 1);          // factor row = sample of this row inside the tile
-        const uint32_t leader_ready0 = ptx::mapa(ready_bar(0), 0);
-        uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int unit = unit0; unit < n_units; unit += unit_step) {
-            const Unit un = decode(unit);
-            if (un.width == 0) continue;
-            for (int kb = 0; kb < n_kb; ++kb) {
-                ptx::mbar_wait(afull_bar(stage), phase);
-                uint8_t* sa = smem_gen + stage * STAGE_BYTES;
-                uint4* arow = reinterpret_cast<uint4*>(sa + r * 128);
-                const uint4* srow = reinterpret_cast<const uint4*>(sa + A_BYTES + BH_BYTES + sl * 128);
-                uint4 av[8], sv[8];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {                // logical 16-byte chunk j sits at j ^ (r & 7) (128B swizzle)
-                    av[j] = arow[j ^ (r & 7)];
-                    sv[j] = srow[j];
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    __half2* a2 = reinterpret_cast<__half2*>(&av[j]);
-                    const __half2* s2 = reinterpret_cast<const __half2*>(&sv[j]);
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) a2[e] = __hmul2(a2[e], s2[e]);
-                    arow[j ^ (r & 7)] = av[j];
-                }
-                ptx::fence_proxy_async_smem();       // the rescaled tile must be visible to the tensor core's async proxy
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive_cluster(leader_ready0 + 8u * stage);
-                if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-        }
-    } else if (warp < 2 + EW) {
-        // ===================== epilogue (both CTAs, own 128 rows) =====================
-        const int q = warp & 3;
-        const int slice = (warp - 2) >> 2;
-        constexpr int COLS_PER_WARP = BLOCK_N / (EW / 4);
-        const uint32_t leader_tempty0 = ptx::mapa(tempty_bar(0), 0);
-        int iter = 0;
-        for (int unit = unit0; unit < n_units; unit += unit_step) {
-            const Unit un = decode(unit);
-            if (un.width == 0) continue;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            ++iter;
-            const int m_idx = un.m_pair * (2 * GEMM_BLOCK_M) + (int)crank * GEMM_BLOCK_M;
-            const int n_idx = un.n0;
-            const int row = m_idx + q * 32 + lane;
-            const int c_end = min((slice + 1) * COLS_PER_WARP, un.width);      // a narrow tile leaves the upper slices idle
-            EpiPre<MODE> pre;
-            if (slice * COLS_PER_WARP < c_end && n_idx + slice * COLS_PER_WARP < N)
-                epilogue_preload<MODE>(ep, M, N, row, n_idx + slice * COLS_PER_WARP, pre, lane, true);
-            ptx::mbar_wait(tfull_bar(as), aphase);
-            ptx::tc_fence_after();
-#pragma unroll 1
-            for (int c = slice * COLS_PER_WARP; c < c_end; c += 32) {
-                if (n_idx + c >= N) break;
-                if (c != slice * COLS_PER_WARP) epilogue_preload<MODE>(ep, M, N, row, n_idx + c, pre, lane, false);
-                float v[32];
-                ptx::tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BLOCK_N + c), v);
-                epilogue_chunk<MODE>(ep, M, N, row, n_idx + c, v, lane, pre);
-            }
-            epilogue_finish<MODE>(ep, M, row, pre);
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive_cluster(leader_tempty0 + 8u * as);
-        }
-    }
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::cluster_sync();
-    if (warp == 1) ptx::tmem_dealloc_cg2(tmem_base, TMEM_COLS);
-}
-
-template <int BLOCK_N, int MODE, bool ASCALE = false>
-static int launch_cg2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tb_tail, int tail_bn,
-                      const pb200_gemm_epilogue& ep, int M, int N, int K, cudaStream_t st) {
-    constexpr int STAGES = BLOCK_N >= 256 ? 6 : 8;
-    constexpr int SMEM = STAGES * (GEMM_BLOCK_M * 128 + (BLOCK_N / 2) * 128 + (ASCALE ? GEMM_ASCALE_BYTES : 0)) + 1024 + 512;
+// ------------------------------------------------------------------ dispatch
+template <int BLOCK_N, int MODE, int AMODE = 0, bool ASCALE = false>
+static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const pb200_gemm_epilogue& ep, int M, int N, int K,
+                      cudaStream_t st, const ConvGeom* geom = nullptr) {
+    using L = GemmSmem<BLOCK_N, ASCALE>;
     static DeviceOnce attr_set;
     if (attr_set.first()) {
-        PB_CUDA(cudaFuncSetAttribute(gemm_f16_cg2_kernel<BLOCK_N, MODE, ASCALE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+        PB_CUDA(cudaFuncSetAttribute(gemm_f16_kernel<BLOCK_N, MODE, AMODE, ASCALE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     L::SMEM_BYTES));
     }
+    ConvGeom g;
+    memset(&g, 0, sizeof(g));
+    if (geom) g = *geom;
     CUtensorMap ts = ta;            // placeholder when unused
     if (ASCALE) {
         const int P = ep.rows_per_sample;
@@ -906,92 +674,22 @@ static int launch_cg2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtens
         const int64_t samples = ((int64_t)M + P - 1) / P;
         PB_TRY(make_tmap_f16_2d_box(&ts, ep.a_scale, samples, K, ep.a_scale_ld, GEMM_BLOCK_K, ns, 0));
     }
-    const int n_big = ceil_div(M, 2 * GEMM_BLOCK_M) * ceil_div(N, BLOCK_N);
-    const int max_pairs = sm_count() / 2;
-    if (!tb_tail || tail_bn <= 0 || tail_bn >= BLOCK_N || BLOCK_N % tail_bn != 0) { tail_bn = 0; tb_tail = &tb; }
-    const int n_main = tail_bn ? (n_big / max_pairs) * max_pairs : n_big;      // the complete waves
-    const int n_units = n_main + (n_big - n_main) * (tail_bn ? BLOCK_N / tail_bn : 1);
-    const int grid = 2 * (n_units < max_pairs ? n_units : max_pairs);
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(gemm_threads(BLOCK_N) + (ASCALE ? 32 * GEMM_ASCALE_WARPS : 0));
-    cfg.dynamicSmemBytes = SMEM;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    static const bool pdl = getenv("PB200_NO_PDL") == nullptr;      // A/B knob
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl ? 2 : 1;
-    PB_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_cg2_kernel<BLOCK_N, MODE, ASCALE>, ta, tb, *tb_tail, ts, ep, M, N, K, n_main, tail_bn));
-    PB_LAUNCH_CHECK();
-    return 0;
-}
-
-template <int BLOCK_N>
-static int launch_cg2_mode(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* tb_tail, int tail_bn,
-                           const pb200_gemm_epilogue& ep, int M, int N, int K, cudaStream_t st) {
-    if (ep.a_scale) {       // GlobalResponseNorm folded into the A operand: the two residual epilogues only
-        if (ep.mode == PB200_EPI_RESID_F32) return launch_cg2<BLOCK_N, PB200_EPI_RESID_F32, true>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        if (ep.mode == PB200_EPI_RESID_LN_F32) return launch_cg2<BLOCK_N, PB200_EPI_RESID_LN_F32, true>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        PB_CHECK(false, "gemm: a_scale is only built for the RESID epilogues (mode %d)", ep.mode);
-    }
-    switch (ep.mode) {
-        case PB200_EPI_F16: return launch_cg2<BLOCK_N, PB200_EPI_F16>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        case PB200_EPI_F32: return launch_cg2<BLOCK_N, PB200_EPI_F32>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        case PB200_EPI_GELU_F16: return launch_cg2<BLOCK_N, PB200_EPI_GELU_F16>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        case PB200_EPI_RESID_F32: return launch_cg2<BLOCK_N, PB200_EPI_RESID_F32>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        case PB200_EPI_UNPATCH_F32: return launch_cg2<BLOCK_N, PB200_EPI_UNPATCH_F32>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        case PB200_EPI_NCHW_F32: return launch_cg2<BLOCK_N, PB200_EPI_NCHW_F32>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        case PB200_EPI_RESID_LN_F32: return launch_cg2<BLOCK_N, PB200_EPI_RESID_LN_F32>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-        case PB200_EPI_F16_LN: return launch_cg2<BLOCK_N, PB200_EPI_F16_LN>(ta, tb, tb_tail, tail_bn, ep, M, N, K, st);
-    }
-    PB_CHECK(false, "gemm: unknown epilogue mode %d", ep.mode);
-    return 1;
-}
-
-// ------------------------------------------------------------------ dispatch
-template <int BLOCK_N, int MODE, int AMODE = 0>
-static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const pb200_gemm_epilogue& ep, int M, int N, int K,
-                      cudaStream_t st, const ConvGeom* geom = nullptr) {
-    using L = GemmSmem<BLOCK_N>;
-    static DeviceOnce attr_set;
-    if (attr_set.first()) {
-        PB_CUDA(cudaFuncSetAttribute(gemm_f16_kernel<BLOCK_N, MODE, AMODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     L::SMEM_BYTES));
-    }
-    ConvGeom g;
-    memset(&g, 0, sizeof(g));
-    if (geom) g = *geom;
     const int tiles_m = AMODE == 0 ? ceil_div(M, GEMM_BLOCK_M) : g.batch * g.tiles_y * g.tiles_x;
-    const int tiles_n = ceil_div(N, BLOCK_N);
-    // pairs of CTAs (one cluster) share the W tile through TMA multicast when there are >= 2 M-tiles
-    // (measured on B200: no gain — the L2 already de-duplicates the two SMs' unicast requests for the same W tile, as
-    // B300_MICROARCH.md predicts for clusters <= 4 — so the TMA-multicast pairing is opt-in: PB200_MCAST=1)
-    static const bool use_mcast = getenv("PB200_MCAST") != nullptr;
-    const int csize = (AMODE == 0 && tiles_m >= 2 && use_mcast) ? 2 : 1;
-    const int n_units = ceil_div(tiles_m, csize) * tiles_n;
-    const int max_clusters = sm_count() / csize;
-    const int grid = csize * (n_units < max_clusters ? n_units : max_clusters);
+    const int n_units = tiles_m * ceil_div(N, BLOCK_N);
+    const int grid = n_units < sm_count() ? n_units : sm_count();
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(gemm_threads(BLOCK_N));
+    cfg.blockDim = dim3(GEMM_THREADS);
     cfg.dynamicSmemBytes = L::SMEM_BYTES;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = csize;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
+    static const bool pdl = getenv("PB200_NO_PDL") == nullptr;      // A/B knob
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    PB_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_kernel<BLOCK_N, MODE, AMODE>, ta, tb, ep, g, M, N, K));
+    cfg.numAttrs = pdl ? 1 : 0;
+    PB_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_kernel<BLOCK_N, MODE, AMODE, ASCALE>, ta, tb, ts, ep, g, M, N, K));
     PB_LAUNCH_CHECK();
     return 0;
 }
@@ -1022,6 +720,11 @@ int gemm_conv_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, 
 template <int BLOCK_N>
 static int launch_mode(const CUtensorMap& ta, const CUtensorMap& tb, const pb200_gemm_epilogue& ep, int M, int N, int K,
                        cudaStream_t st) {
+    if (ep.a_scale) {       // GlobalResponseNorm folded into the A operand: the two residual epilogues only
+        if (ep.mode == PB200_EPI_RESID_F32) return launch_cfg<BLOCK_N, PB200_EPI_RESID_F32, 0, true>(ta, tb, ep, M, N, K, st);
+        if (ep.mode == PB200_EPI_RESID_LN_F32) return launch_cfg<BLOCK_N, PB200_EPI_RESID_LN_F32, 0, true>(ta, tb, ep, M, N, K, st);
+        PB_CHECK(false, "gemm: a_scale is only built for the RESID epilogues (mode %d)", ep.mode);
+    }
     switch (ep.mode) {
         case PB200_EPI_F16: return launch_cfg<BLOCK_N, PB200_EPI_F16>(ta, tb, ep, M, N, K, st);
         case PB200_EPI_F32: return launch_cfg<BLOCK_N, PB200_EPI_F32>(ta, tb, ep, M, N, K, st);
@@ -1041,81 +744,43 @@ static thread_local int g_plan_sms = 0;
 static int plan_sm_count() {
     if (g_plan_sms > 0) return g_plan_sms;
     const int s = sm_count();
-    return s > 0 ? s : 148;
-}
-
-static bool gemm_use_cg2(int64_t M) {
-    // The 2-SM kernel takes every problem with more than one 128-row tile (1243 vs 1095 TFLOP/s on 8192x3840x1280 once
-    // its producer stopped issuing MEMBAR.ALL.GPU per k-block, profiles/r01_cg2_gemm_notes.md); PB200_NO_CG2 disables it.
-    static const bool off = getenv("PB200_NO_CG2") != nullptr;
-    return !off && M > GEMM_BLOCK_M && plan_sm_count() % 2 == 0;
+    return s > 0 ? s : 132;
 }
 
 bool gemm_can_scale_a(int64_t M, int64_t N, int64_t K, int rows_per_sample) {
+    (void)M; (void)N;
     const int P = rows_per_sample;
-    if (P <= 0 || !gemm_use_cg2(M) || K % GEMM_BLOCK_K != 0) return false;
-    if (!(P >= GEMM_BLOCK_M ? P % GEMM_BLOCK_M == 0 : (GEMM_BLOCK_M % P == 0 && GEMM_BLOCK_M / P <= 8))) return false;
-    // 256-wide tiles only: a k-block of a 128-wide tile lasts 256 tensor cycles, less than the rescale of its A tile took with two
-    // transform warps (PB200_GRN_FOLD_128=1 lets 128-wide tiles fold too: experiment knob for the four-warp version)
-    static const bool allow128 = getenv("PB200_GRN_FOLD_128") != nullptr;
-    const int bn = gemm_pick_block_n(M, N, K);
-    return bn == 256 || (allow128 && bn == 128);
+    if (P <= 0 || K % GEMM_BLOCK_K != 0) return false;
+    return P >= GEMM_BLOCK_M ? P % GEMM_BLOCK_M == 0 : (GEMM_BLOCK_M % P == 0 && GEMM_BLOCK_M / P <= 8);
 }
 
-int gemm_pick_block_n(int64_t M, int64_t N, int64_t K, bool allow_cg2) {
-    // Cycle model per candidate BLOCK_N (measured anchors on B200, profiles/r01_cg2_gemm_notes.md):
-    //   tensor   : waves x k-blocks x 4 MMAs x (BLOCK_N/2 cycles per 128-row MMA)
-    //   L2->SM   : all tiles' operand bytes / ~6300 B/clk (the fabric saturates at ~13 TB/s): per k-block a CTA pulls
-    //              its 128x64 A tile and BLOCK_N x 64 of W (1-SM kernel) or half of that W (2-SM kernel)
-    //   per tile : ~2500 cycles of fill/drain + epilogue tail
-    // and pick the minimum.  The 2-SM kernel's work unit is a 256-row pair tile on sm_count/2 pairs.
+int gemm_pick_block_n(int64_t M, int64_t N, int64_t K) {
+    // Cycle model per candidate BLOCK_N, from the H100 SXM data sheet (not calibrated by measurement):
+    //   tensor   : waves x k-blocks x 128 x BLOCK_N x 64 MACs at ~2048 fp16 MACs per clock and SM (989 TFLOP/s, 132 SMs)
+    //   L2->SM   : all tiles' operand bytes (per k-block the 128x64 A tile and BLOCK_N x 64 of W) at ~3000 B/clk
+    //   per tile : ~2000 cycles of fill/drain + the epilogue, which does not overlap the main loop
+    // and pick the minimum.
     static const int force = getenv("PB200_FORCE_BN") ? atoi(getenv("PB200_FORCE_BN")) : 0;   // experiments only
     if (force == 64 || force == 128 || force == 256) return force;
     const int sms = plan_sm_count();
-    const bool cg2 = allow_cg2 && gemm_use_cg2(M);
     const long n_kb = K > 0 ? (long)ceil_div(K, GEMM_BLOCK_K) : 16;
     const int cands[3] = {256, 128, 64};
     int best = 128;
     double best_cost = 1e30;
-    for (int i = 0; i < (cg2 ? 2 : 3); ++i) {
+    for (int i = 0; i < 3; ++i) {
         const int bn = cands[i];
-        const long units = (long)ceil_div(M, cg2 ? 2 * GEMM_BLOCK_M : GEMM_BLOCK_M) * ceil_div(N, bn);
-        const long workers = cg2 ? sms / 2 : sms;
-        const long waves = (units + workers - 1) / workers;
-        const double mma = (double)waves * n_kb * 4.0 * (bn / 2.0);
-        const double bytes_per_kb = (cg2 ? 2.0 : 1.0) * 16384.0 + bn * 128.0;
-        const double l2 = (double)units * n_kb * bytes_per_kb / 6300.0;
-        const double cost = (mma > l2 ? mma : l2) + waves * 2500.0;
+        const long units = (long)ceil_div(M, GEMM_BLOCK_M) * ceil_div(N, bn);
+        const long waves = (units + sms - 1) / sms;
+        const double mma = (double)waves * n_kb * 4.0 * bn;
+        const double l2 = (double)units * n_kb * (16384.0 + bn * 128.0) / 3000.0;
+        const double cost = (mma > l2 ? mma : l2) + waves * (2000.0 + 4.0 * bn);
         if (cost < best_cost) { best_cost = cost; best = bn; }
     }
     return best;
 }
 
-int gemm_tail_block_n(int64_t M, int64_t N, int block_n) {
-    // Worth it when the leftover tiles are a small part of a wave: cut them so that the last wave is full but narrow.
-    // A narrow tile costs more per column than a full one (A is re-read per tile: the L2->SM fabric model of
-    // gemm_pick_block_n), hence the 0.55 / 0.45 weights; measured on 8192 x 1280 x {1280, 5120}.
-    static const int force = getenv("PB200_GEMM_TAIL") ? atoi(getenv("PB200_GEMM_TAIL")) : -1;   // 0 disables, 64/128 force
-    if (!gemm_use_cg2(M) || block_n != 256) return 0;
-    const long workers = plan_sm_count() / 2;
-    const long n_big = (long)ceil_div(M, 2 * GEMM_BLOCK_M) * ceil_div(N, block_n);
-    const long rem = n_big % workers;
-    if (n_big < workers || rem == 0) return 0;
-    if (force >= 0) return (force == 64 || force == 128) ? force : 0;
-    double best = 1.0;                 // cost of running the leftover as one more full wave
-    int pick = 0;
-    const int cand[2] = {128, 64};
-    const double weight[2] = {0.55, 0.45};
-    for (int i = 0; i < 2; ++i) {
-        const long sub = rem * (block_n / cand[i]);
-        const double cost = (double)((sub + workers - 1) / workers) * weight[i];
-        if (cost < best - 0.15) { best = cost; pick = cand[i]; }
-    }
-    return pick;
-}
-
 int gemm_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, const pb200_gemm_epilogue& ep, int64_t M,
-                int64_t N, int64_t K, cudaStream_t st, const GemmTail* tail) {
+                int64_t N, int64_t K, cudaStream_t st) {
     PB_CHECK(M > 0 && N > 0 && K > 0, "gemm: empty problem");
     PB_CHECK(N % 8 == 0, "gemm: N=%lld must be a multiple of 8", (long long)N);
     PB_CHECK(ep.out != nullptr, "gemm: null output");
@@ -1131,17 +796,11 @@ int gemm_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, const
         ep.mode == PB200_EPI_NCHW_F32)
         PB_CHECK(ep.rows_per_sample > 0, "gemm: rows_per_sample required");
     if (ep.a_scale)
-        PB_CHECK(gemm_can_scale_a(M, N, K, ep.rows_per_sample) && block_n >= 128 && ep.a_scale_ld % 8 == 0 && ((uintptr_t)ep.a_scale & 15) == 0,
-                 "gemm: a_scale needs the 2-SM kernel (M > 128), rows_per_sample dividing or divided by 128, K %% 64 == 0");
+        PB_CHECK(gemm_can_scale_a(M, N, K, ep.rows_per_sample) && ep.a_scale_ld % 8 == 0 && ((uintptr_t)ep.a_scale & 15) == 0,
+                 "gemm: a_scale needs rows_per_sample dividing or divided by 128, K %% 64 == 0");
     static const char* kTags[8] = {"gemm_f16", "gemm_f32", "gemm_gelu_sqsum", "gemm_resid", "gemm_unpatch", "gemm_nchw",
                                    "gemm_resid", "gemm_f16"};
     ProfScope prof(ep.mode >= 0 && ep.mode < 8 ? kTags[ep.mode] : "gemm", 2.0 * (double)M * (double)N * (double)K, st);
-    if (gemm_use_cg2(M) && block_n >= 128) {
-        const int tbn = tail ? tail->bn : 0;
-        const CUtensorMap* ttb = tail ? tail->tb : nullptr;
-        if (block_n == 256) return launch_cg2_mode<256>(ta, tb, ttb, tbn, ep, (int)M, (int)N, (int)K, st);
-        return launch_cg2_mode<128>(ta, tb, ttb, tbn, ep, (int)M, (int)N, (int)K, st);
-    }
     switch (block_n) {
         case 64: return launch_mode<64>(ta, tb, ep, (int)M, (int)N, (int)K, st);
         case 128: return launch_mode<128>(ta, tb, ep, (int)M, (int)N, (int)K, st);
@@ -1155,12 +814,10 @@ int gemm_f16(const void* a, int64_t lda, const void* w, int64_t ldw, int64_t M, 
              const pb200_gemm_epilogue& ep, cudaStream_t st) {
     PB_CHECK(K % 8 == 0, "gemm: K=%lld must be a multiple of 8", (long long)K);
     const int bn = gemm_pick_block_n(M, N, K);
-    CUtensorMap ta, tb, tbt;
+    CUtensorMap ta, tb;
     PB_TRY(make_tmap_f16_2d(&ta, a, M, K, lda, GEMM_BLOCK_M));
     PB_TRY(make_tmap_f16_2d(&tb, w, N, K, ldw, bn / 2));      // W box = half a tile (see the producer)
-    GemmTail tail{gemm_tail_block_n(M, N, bn), &tbt};
-    if (tail.bn) PB_TRY(make_tmap_f16_2d(&tbt, w, N, K, ldw, tail.bn / 2));
-    return gemm_launch(ta, tb, bn, ep, M, N, K, st, tail.bn ? &tail : nullptr);
+    return gemm_launch(ta, tb, bn, ep, M, N, K, st);
 }
 
 }  // namespace pb
@@ -1170,8 +827,8 @@ extern "C" int pb200_gemm_plan(int64_t m, int64_t n, int64_t k, int sm_count, in
     pb::g_plan_sms = sm_count > 0 ? sm_count : 0;
     const int bn = pb::gemm_pick_block_n(m, n, k);
     *block_n = bn;
-    *two_sm = pb::gemm_use_cg2(m) && bn >= 128 ? 1 : 0;
-    *tail_block_n = pb::gemm_tail_block_n(m, n, bn);
+    *two_sm = 0;            // Hopper has no 2-SM MMA: every tile is one CTA's
+    *tail_block_n = 0;      // ... and every tile is BLOCK_N wide
     pb::g_plan_sms = 0;
     return 0;
 }

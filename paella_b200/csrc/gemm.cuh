@@ -1,4 +1,4 @@
-// Internal interface of the tcgen05 GEMM (see gemm.cu).
+// Internal interface of the wgmma GEMM (see gemm.cu).
 #pragma once
 #include "common.cuh"
 #include "paella_b200.h"
@@ -8,19 +8,22 @@ namespace pb {
 
 constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;     // 64 fp16 = one 128-byte swizzle row
-// Epilogue warps: several per TMEM lane quarter, each taking a slice (>= 32 columns) of the tile's columns.  The
-// epilogue is a latency-bound instruction stream (ncu: IPC 1.4 with 8 warps), so it gets as many warps as columns allow.
-constexpr int gemm_epi_warps(int block_n) { return block_n >= 128 ? 16 : 8; }
-constexpr int gemm_threads(int block_n) { return 64 + 32 * gemm_epi_warps(block_n); }   // + TMA warp + MMA warp
+constexpr int GEMM_CONSUMERS = 2;    // MMA warpgroups, 64 rows of the tile each
+constexpr int GEMM_THREADS = 128 * (1 + GEMM_CONSUMERS);      // + the producer warpgroup
+constexpr int GEMM_EPI_STRIDE = 65;  // fp32 row stride of the epilogue slab (odd: the row-per-lane reads are conflict-free)
+constexpr int GEMM_EPI_BYTES = GEMM_CONSUMERS * 64 * GEMM_EPI_STRIDE * 4;
+constexpr int GEMM_ASCALE_BYTES = 1024;        // up to 8 samples x 64 factors per 128-row tile and k-block
+constexpr int SMEM_PER_BLOCK_MAX = 232448;     // 227 KB: the opt-in limit of one block on sm_90
 
-template <int BLOCK_N>
+template <int BLOCK_N, bool ASCALE = false>
 struct GemmSmem {
     static constexpr int A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
     static constexpr int B_BYTES = BLOCK_N * GEMM_BLOCK_K * 2;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = BLOCK_N >= 256 ? 4 : (BLOCK_N >= 128 ? 6 : 8);
-    static constexpr int TMEM_COLS = BLOCK_N >= 256 ? 512 : (BLOCK_N >= 128 ? 256 : 128);   // 2 accumulators
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
+    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES + (ASCALE ? GEMM_ASCALE_BYTES : 0);
+    static constexpr int FIXED = GEMM_EPI_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
+    static constexpr int FIT = (SMEM_PER_BLOCK_MAX - FIXED) / STAGE_BYTES;
+    static constexpr int STAGES = FIT > 8 ? 8 : FIT;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED;
 };
 
 // 2-D fp16 tensor map over a row-major [rows, cols] matrix with leading dimension ld (elements):
@@ -54,33 +57,20 @@ struct ConvGeom {
 int gemm_conv_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, const pb200_gemm_epilogue& ep,
                      const ConvGeom& geom, int64_t N, int64_t K, cudaStream_t st);
 
-// BLOCK_N that minimises a tensor / L2-fabric cycle model of the launch (see gemm.cu); allow_cg2=false for the
-// conv (TMA-gather) variants, which run on the 1-SM kernel
-int gemm_pick_block_n(int64_t M, int64_t N, int64_t K = 0, bool allow_cg2 = true);
-// whether gemm_launch can take ep.a_scale for this problem (2-SM kernel, sample rows aligned with the 128-row tiles)
+// BLOCK_N that minimises a tensor / L2 cycle model of the launch (see gemm.cu)
+int gemm_pick_block_n(int64_t M, int64_t N, int64_t K = 0);
+// whether gemm_launch can take ep.a_scale for this problem (sample rows aligned with the 128-row tiles, K % 64 == 0)
 bool gemm_can_scale_a(int64_t M, int64_t N, int64_t K, int rows_per_sample);
 
-// Narrow tiles for the leftover of the last wave (2-SM kernel, BLOCK_N 256): 0 = none, else 64 or 128; tb = tensor map of
-// W with box rows bn / 2.
-struct GemmTail {
-    int bn;
-    const CUtensorMap* tb;
-};
-int gemm_tail_block_n(int64_t M, int64_t N, int block_n);
-
+// tb: tensor map of W with box rows block_n / 2
 int gemm_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, const pb200_gemm_epilogue& ep, int64_t M,
-                int64_t N, int64_t K, cudaStream_t st, const GemmTail* tail = nullptr);
+                int64_t N, int64_t K, cudaStream_t st);
 
 // convenience: builds both tensor maps and launches
 int gemm_f16(const void* a, int64_t lda, const void* w, int64_t ldw, int64_t M, int64_t N, int64_t K,
              const pb200_gemm_epilogue& ep, cudaStream_t st);
 
-// Fused MLP of the codec ResBlock (vq_mlp.cu): x[M, C] += alpha * (GELU(a16 W1^T + b1) W2^T + b2), hidden kept on chip.
-// 0 = launched, 1 = error, -1 = shape not handled (C not in {384, 192} or M < 256): the caller runs the two GEMMs instead.
-int launch_vq_mlp_fused(const __half* a16, int64_t M, int C, const __half* w1, const float* b1, const __half* w2, const float* b2,
-                        float* x, float alpha, cudaStream_t st);
-
-// In-warp 8x8 transpose of float4 items (xor-butterfly shuffles): tcgen05.ld hands lane l row l of a 32-column chunk; afterwards
+// In-warp 8x8 transpose of float4 items (xor-butterfly shuffles): the epilogue hands lane l row l of a 32-column chunk; afterwards
 // item i of lane (a, b) = row 8a + i, columns 4b..4b+3, so one store instruction writes four full 128-byte lines.
 __device__ __forceinline__ void transpose8x8_f4(float (&v)[32], int lane) {
 #pragma unroll

@@ -137,8 +137,8 @@ template <int NV, bool SKIP>
 __global__ void __launch_bounds__(128) dwconv_ln_kernel(const float* __restrict__ x, const float* __restrict__ skip,
                                                         const float* __restrict__ wp, const float* __restrict__ bias,
                                                         int B, int h, int w, int c, int k, __half* __restrict__ out) {
-    // one CTA = a 2x2 patch of positions of one sample (4 warps, small CTAs for occupancy: measured on B200, 16-warp
-    // 4x4 patches were 18% slower); the four 3x3 halos overlap so half of the tap rows come from L1
+    // one CTA = a 2x2 patch of positions of one sample (4 warps, small CTAs for occupancy); the four 3x3 halos overlap so
+    // half of the tap rows come from L1
     pdl_launch_dependents();
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int pw = (w + 1) >> 1, ph = (h + 1) >> 1;
@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(128) dwconv_ln_kernel(const float* __restrict_
 
 // ------------------------------------------------------------------ depthwise 3x3 conv + LayerNorm (thread per 4 channels)
 // The warp-per-position kernel above issues 9 activation + 9 weight loads per position and float4 chunk and is bound
-// by LSU/L1 issue (measured 40 us at 8192 x 1280, HBM ideal 10 us).  Here a thread owns 4 output channels of a
+// by LSU/L1 issue, not by HBM.  Here a thread owns 4 output channels of a
 // 2-row x 8-column patch of positions: it walks the patch's 4 x 10 input halo once (2.5 loads per output instead of
 // 18), keeps the 16 accumulators in registers, and the CTA (c/4 threads) then reduces the LayerNorm statistics of
 // its 16 positions through shared memory.  Tap order per output is (ky, kx) ascending, as in the kernel above.
@@ -545,8 +545,7 @@ int launch_vq_front_fused(const float* x, int B, int h, int w, int c, const floa
     const int64_t grid = (int64_t)B * ceil_div(h, DW_PH) * ceil_div(w, DW_PW);
     PB_CHECK(grid < (1ll << 31), "vq_front: grid too large");
     const int threads = ceil_div(c / 4, 32) * 32;
-    // 3 CTAs of 96 threads per SM at 168 registers; capping at 128 registers for a fourth CTA spilled 376 B per thread and measured
-    // 6.25 vs 5.73 ms per bs=64 round trip (profiles/r02j_*)
+    // 3 CTAs of 96 threads per SM at 168 registers (capping at 128 registers for a fourth CTA spills)
     if (threads <= 64)
         vq_front_patch_kernel<64, 6><<<(unsigned)grid, threads, 0, st>>>(x, stats_scratch, w9, bias, 1.0f + gam[0], gam[1], gam[2], 1.0f + gam[3], gam[4], B, h, w, c, x_out, a16);
     else
@@ -574,8 +573,7 @@ int launch_dwconv_ln(const float* x, const float* skip, const float* w_packed, c
     PB_CHECK(c % 8 == 0, "dwconv: c=%d must be a multiple of 8", c);
     PB_CHECK(k % 2 == 1, "dwconv: kernel_size %d must be odd", k);
     static const bool old_kernel = getenv("PB200_DWCONV_WARP") != nullptr;      // A/B knob
-    // measured (ncu, B200): the patch kernel wins at 8192 x 1280 (32.6 vs 39.6 us) and loses at 32768 x 640
-    // (99 vs 62 us: 152 registers x 160 threads leaves 15% occupancy), so it takes the wide levels only
+    // the patch kernel takes the wide levels only: at 640 channels its 152 registers x 160 threads leave 15% occupancy
     static const bool patch_all = getenv("PB200_DWCONV_PATCH") != nullptr;
     if (k == 3 && c <= 2560 && !old_kernel && (patch_all || (c > 640 && w >= DW_PW)))
         return dwconv3_patch_launch(x, skip, w_packed, bias, B, h, w, c, out, st);

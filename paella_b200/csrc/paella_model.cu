@@ -185,9 +185,7 @@ struct pb200_paella {
         const CUtensorMap *ta, *tb;
         PB_TRY(tmap(A, M, K, lda, GEMM_BLOCK_M, &ta));
         PB_TRY(tmap(w<__half>(w_off), N, K, K, bn / 2, &tb));     // W box = half a tile
-        GemmTail tail{gemm_tail_block_n(M, N, bn), nullptr};
-        if (tail.bn) PB_TRY(tmap(w<__half>(w_off), N, K, K, tail.bn / 2, &tail.tb));
-        return gemm_launch(*ta, *tb, bn, ep, M, N, K, st, tail.bn ? &tail : nullptr);
+        return gemm_launch(*ta, *tb, bn, ep, M, N, K, st);
     }
 };
 
@@ -761,9 +759,8 @@ int pb200_paella_features(pb200_paella* m, const int64_t* tokens, const float* r
                 PB_TRY(m->gemm(ws.a16, ch, M, ch, b.w1, 4 * (int64_t)ch, e1, st));
                 // GlobalResponseNorm: folded into GEMM2's A operand where its tiles line up with the samples (multipliers only,
                 // shift pushed into the bias), else applied to the hidden in place
-                // Measured on B200 (profiles/r02_ab_notes.md): the fold removes the 168 MB GRN pass (-12.4 ms per bench step) but the
-                // in-place rescale adds 32 KB of shared-memory traffic per k-block to a 2-SM main loop whose operand reads already
-                // use ~3/4 of the 128 B/clk port: GEMM2 61 -> 89 us per level-1 launch (+17 ms per step).  Net loss: opt-in.
+                // The fold removes the stand-alone GRN pass over the 4c-wide hidden but makes each MMA warpgroup rescale its A
+                // rows in shared memory before every k-block's wgmma; DESIGN.md section 5.1 has the A/B on the bench step.
                 static const bool fold_on = getenv("PB200_GRN_FOLD") != nullptr;
                 const bool fold_grn = fold_on && gemm_can_scale_a(M, ch, 4 * (int64_t)ch, P);
                 __half* grn_s16 = reinterpret_cast<__half*>(ws.grn_mult);

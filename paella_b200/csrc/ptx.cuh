@@ -1,4 +1,4 @@
-// Inline-PTX wrappers for the Blackwell (sm_100a) async machinery: mbarrier, TMA, tcgen05/TMEM.
+// Inline-PTX wrappers for the Hopper (sm_90a) async machinery: mbarrier, TMA, wgmma.
 #pragma once
 #include "common.cuh"
 
@@ -48,35 +48,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     }
 }
 
-// Same with a suspend-time hint on try_wait (the form CUTLASS's ClusterBarrier::wait uses, 0x989680 ticks): the warp sleeps in
-// hardware until the phase flips instead of re-issuing the poll -- for kernels whose waiting roles share an SM sub-partition with
-// busy compute warps (attention_tt.cu: the polls of the MMA / TMA warps cost the softmax warps beside them issue slots).
-__device__ __forceinline__ bool mbar_try_wait_hint(uint32_t bar, uint32_t parity, uint32_t ticks) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "selp.b32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity), "r"(ticks)
-        : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_hint(uint32_t bar, uint32_t parity) {
-    if (mbar_try_wait(bar, parity)) return;
-    const uint64_t t0 = globaltimer_ns();
-    uint32_t spins = 0;
-    while (!mbar_try_wait_hint(bar, parity, 0x989680u)) {
-        if ((++spins & 0x3f) == 0 && globaltimer_ns() - t0 > 4000000000ull) {   // 4 s
-            printf("paella_b200: mbarrier wait timed out (block %d thread %d bar %u parity %u)\n", blockIdx.x,
-                   threadIdx.x, bar, parity);
-            __trap();
-        }
-    }
-}
-
 // One elected lane of a converged warp (elect.sync): unlike `lane == 0`, the compiler knows the guarded region runs in exactly one
-// thread, so single-thread instructions (tcgen05.mma / commit, TMA) are emitted straight instead of inside an ELECT / BRA.U.ANY
+// thread, so single-thread instructions (wgmma issue bookkeeping, TMA) are emitted straight instead of inside an ELECT / BRA.U.ANY
 // "uniformisation" loop each.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
@@ -84,41 +57,13 @@ __device__ __forceinline__ bool elect_one() {
     return pred != 0;
 }
 
-// ------------------------------------------------------------------ thread-block clusters
-__device__ __forceinline__ uint32_t cluster_nctarank() {
-    uint32_t v;
-    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(v));
-    return v;
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t v;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(v));
-    return v;
-}
+// ------------------------------------------------------------------ programmatic dependent launch
 // Programmatic dependent launch: a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start
-// (block scheduling, barrier / TMEM setup) while its predecessor in the stream is still draining; it must execute
+// (block scheduling, barrier setup) while its predecessor in the stream is still draining; it must execute
 // griddep_wait() before touching anything the predecessor wrote.  griddep_launch() in a kernel lets its dependent start
 // early.  Both are no-ops when the launch carries no such dependency.
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void griddep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-__device__ __forceinline__ void cluster_sync() {     // all threads of all CTAs of the cluster
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// shared::cluster address of `smem_addr` (a shared::cta address of this CTA's window) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa(uint32_t smem_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-    return r;
-}
-// arrive on an mbarrier anywhere in the cluster (address from mapa)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-    // default (.release.cta) semantics as in CUTLASS' ClusterBarrier::arrive(cta_id): with an explicit
-    // .release.cluster ptxas emits MEMBAR.ALL.GPU per arrive, which throttled the peer CTA's TMA producer to one
-    // stage per ~1800 cycles (ncu source view, profiles/r01_cg2_gemm_notes.md)
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
-}
 
 // ------------------------------------------------------------------ TMA
 __device__ __forceinline__ void prefetch_tensormap(const void* tmap) {
@@ -128,24 +73,6 @@ __device__ __forceinline__ void tma_load_2d(const void* tmap, uint32_t bar, uint
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
-        : "memory");
-}
-// same box written to the same shared-memory offset of every CTA in cta_mask; each destination CTA's mbarrier (same
-// offset) receives the complete_tx
-__device__ __forceinline__ void tma_load_2d_mcast(const void* tmap, uint32_t bar, uint32_t smem_dst, int c0, int c1,
-                                                  uint16_t cta_mask) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
-        : "memory");
-}
-// 2-SM form: data lands in THIS CTA's shared memory, the transaction bytes are credited to `cluster_bar`
-// (the leader CTA's mbarrier, a shared::cluster address)
-__device__ __forceinline__ void tma_load_2d_cg2(const void* tmap, uint32_t cluster_bar, uint32_t smem_dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(cluster_bar), "r"(c0), "r"(c1)
         : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(const void* tmap, uint32_t bar, uint32_t smem_dst, int c0, int c1, int c2,
@@ -162,125 +89,6 @@ __device__ __forceinline__ void tma_load_5d(const void* tmap, uint32_t bar, uint
         "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
         ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
         : "memory");
-}
-
-// ------------------------------------------------------------------ tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {   // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {    // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] . B[smem]^T, single-CTA, kind::f16 (fp16/bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// mbarrier arrives when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// ... and the arrival is delivered to the barrier at the same offset in every CTA of cta_mask
-__device__ __forceinline__ void umma_commit_mcast(uint32_t bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"(cta_mask) : "memory");
-}
-// ---- cta_group::2 (a CTA pair drives one 256-row MMA; issued by the leader CTA only)
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t smem_dst, uint32_t ncols) {   // same warp id in both CTAs
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_cg2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_cg2(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_cg2_mcast(uint32_t bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets lane (base_lane + t), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// 32 lanes x 64 consecutive fp32 columns (one wait for 64 values: the softmax reads its S row in 64-column pieces)
-__device__ __forceinline__ void tmem_ld_32x64(uint32_t taddr, float (&v)[64]) {
-    uint32_t r[64];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x64.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]), "=r"(r[32]),
-          "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]), "=r"(r[37]), "=r"(r[38]), "=r"(r[39]), "=r"(r[40]),
-          "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]), "=r"(r[46]), "=r"(r[47]), "=r"(r[48]),
-          "=r"(r[49]), "=r"(r[50]), "=r"(r[51]), "=r"(r[52]), "=r"(r[53]), "=r"(r[54]), "=r"(r[55]), "=r"(r[56]),
-          "=r"(r[57]), "=r"(r[58]), "=r"(r[59]), "=r"(r[60]), "=r"(r[61]), "=r"(r[62]), "=r"(r[63])
-        : "r"(taddr)
-        : "memory");
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 64; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// 16 lanes x 64 consecutive fp32 columns in the mma C-fragment arrangement (cute SM100_TMEM_LOAD_16dp256b8x): thread t holds
-// lane t/4 (registers 4n, 4n+1) and lane t/4 + 8 (registers 4n+2, 4n+3), columns 8n + 2(t%4) + {0, 1}, n = 0..7 -- all 32
-// threads carry data of a 16-lane (M = 64) accumulator slice, where the 32x32b shape leaves lanes 16..31 idle
-__device__ __forceinline__ void tmem_ld_16x256b_x8(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.16x256b.x8.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
 }
 
 // named barrier among `nthreads` threads (a subset of the CTA's warps)
@@ -300,75 +108,96 @@ __device__ __forceinline__ float ex2_approx(float x) {
     return y;
 }
 
-// 32 lanes x 16 consecutive fp32 columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// Shared-memory matrix descriptors (cute/arch/mma_sm100_desc.hpp SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout type [61,64): 2 = SWIZZLE_128B, 6 = SWIZZLE_32B).  All tiles here are dense
-// [rows][128 B] or [rows][32 B] as TMA writes them:
-//   K-major  (rows = M/N index, the row holds K):    8-row groups are SBO = 8 * row bytes apart
-//   MN-major (rows = K index, the row holds M/N):    8-row (K) groups are SBO = 8 * row bytes apart; one row = one MN block
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t layout_type) {
+// ------------------------------------------------------------------ wgmma (Hopper warpgroup MMA)
+// Shared-memory matrix descriptor of a K-major operand tile stored as rows of 128 bytes (64 fp16) with the 128-byte swizzle
+// TMA writes (CU_TENSOR_MAP_SWIZZLE_128B): start address >> 4 [0,14), LBO (unused for swizzled K-major) [16,30),
+// SBO = 8 rows * 128 B = 1024 [32,46), layout type 1 = SWIZZLE_128B [62,64).  The tile base must be 1024-byte aligned; a
+// K step of 16 elements (32 bytes) inside the swizzle atom is +2 on the descriptor.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;                           // LBO (unused by the dense single-block tiles above)
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)layout_type << 61;
-    return d;
-}
-// MN-major operand spanning several 64-element (128-byte) swizzle atoms along M/N: lbo_bytes = distance between the atoms' tiles
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-    uint64_t d = umma_desc(smem_addr, 1024, 2);
-    d &= ~((uint64_t)0x3FFF << 16);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    return d;
-}
-// same with 32-element (64-byte) swizzle atoms: canonical layout ((8,4,m),(8,k)):((1,8,LBO),(32,SBO)), SBO = 8 rows * 64 B
-__device__ __forceinline__ uint64_t umma_desc_mn_sw64(uint32_t smem_addr, uint32_t lbo_bytes) {
-    uint64_t d = umma_desc(smem_addr, 512, 4);
-    d &= ~((uint64_t)0x3FFF << 16);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    return d;
-}
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) { return umma_desc(smem_addr, 1024, 2); }
-__device__ __forceinline__ uint64_t umma_desc_sw32(uint32_t smem_addr) { return umma_desc(smem_addr, 256, 6); }
-
-// Shared-memory matrix descriptor for a K-major operand tile stored as rows of 128 bytes
-// (64 fp16) with the 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B):
-//   start address >>4 | LBO (unused for swizzled K-major) | SBO = 8 rows * 128 B = 1024 | version 1 | SWIZZLE_128B
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+    d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
+    return d;
+}
+// Register fences around a batch of wgmma: fence before the first (the accumulator registers were written by ordinary
+// instructions), commit closes the batch into a group, wait<N> blocks until at most N groups are still in flight.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x 64] (+)= A[smem 64 x 16] . B[smem 64 x 16]^T, both K-major (descriptors), fp16 in, fp32 accumulate in registers
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+// D[64 x 80] (+)= A[smem 64 x 16] . B[smem 80 x 16]^T, both K-major (descriptors), fp16 in, fp32 accumulate in registers
+__device__ __forceinline__ void wgmma_m64n80k16(float (&d)[40], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %42, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, "
+        "%40, %41, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+// D[64 x 128] (+)= A[smem 64 x 16] . B[smem 128 x 16]^T, both K-major (descriptors), fp16 in, fp32 accumulate in registers
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+// D[64 x 80] (+)= A[registers 64 x 16] . B[smem 80 x 16]^T: A in the accumulator fragment arrangement (per warp 16 rows:
+// a[0] = rows lane/4, k 2(lane%4)+{0,1}; a[1] = rows +8; a[2], a[3] = the same at k + 8), two fp16 per register
+__device__ __forceinline__ void wgmma_m64n80k16_rs(float (&d)[40], const uint32_t (&a)[4], uint64_t desc_b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, "
+        "{%40, %41, %42, %43}, %44, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b));
+}
+// K-major operand tile stored as rows of 32 bytes (16 fp16) with the 32-byte swizzle (CU_TENSOR_MAP_SWIZZLE_32B):
+// SBO = 8 rows * 32 B = 256, layout type 3 = SWIZZLE_32B; one 16-element K step per tile
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_sw32(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(256 >> 4) << 32;
+    d |= (uint64_t)3 << 62;
     return d;
 }
 
-// Instruction descriptor with explicit operand major-ness (0 = K-major, 1 = MN-major), fp16 inputs, fp32 accumulate
-__host__ __device__ constexpr uint32_t umma_idesc_f16_major(int m, int n, int a_mn_major, int b_mn_major) {
-    return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(n >> 3) << 17) |
-           ((uint32_t)(m >> 4) << 24);
-}
-
-// Instruction descriptor, kind::f16: D fp32, A/B fp16 (fmt 0) or bf16 (fmt 1), both K-major, M x N tile.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n, int ab_fmt) {
-    return (1u << 4) | ((uint32_t)ab_fmt << 7) | ((uint32_t)ab_fmt << 10) | ((uint32_t)(n >> 3) << 17) |
-           ((uint32_t)(m >> 4) << 24);
-}
+// Register budget of a warp-specialised kernel: the producer warpgroup gives registers back, the MMA warpgroups take them.
+// ptxas allocates the code after setmaxnreg.inc against the raised limit (its -v line reports the launch value, 168 at 384
+// threads): without these the 256-wide GEMM tiles spill 0.8-1 KB per thread.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 }  // namespace ptx
 }  // namespace pb

@@ -9,10 +9,10 @@
 //                                                  exponential_() would hand to element (row, k)
 // which equals argmax_k softmax(l/T)_k / q_k (what torch computes) up to fp32 rounding of near-ties.
 //
-// One CTA per 128 token rows, 320 threads:
-//   warp 0     TMA: the 128 x c_out A tile once (resident), then W tiles [128 labels x 64] through a 6-deep ring
-//   warp 1     tcgen05.mma issuer: 128x128 accumulators, double-buffered in TMEM
-//   warps 2-9  epilogue: tcgen05.ld (thread = token row), Philox4x32-10 per element, running arg-max in registers
+// One CTA per 128 token rows, 384 threads:
+//   warpgroup 0     TMA: the 128 x c_out A tile once (resident), then W tiles [128 labels x 64] through a 6-deep ring
+//   warpgroups 1,2  wgmma m64n128k16 for 64 token rows each (accumulators in registers), then per element Philox4x32-10 and
+//                   a running arg-max per row in registers; the quad of threads sharing a row is reduced at the end
 #include <cstdlib>
 
 #include "gemm.cuh"
@@ -23,60 +23,46 @@ namespace pb {
 constexpr int SMP_BN = 128;
 constexpr int SMP_STAGES = 6;
 constexpr int SMP_MAX_KB = 4;                 // c_out <= 256
-constexpr int SMP_EPI_WARPS = 16;             // 4 per TMEM lane quarter: Philox is a long dependent chain, hide it with warps
-constexpr int SMP_THREADS = 64 + 32 * SMP_EPI_WARPS;
-constexpr int SMP_COLS_PER_WARP = SMP_BN / (SMP_EPI_WARPS / 4);
+constexpr int SMP_THREADS = 384;              // producer warpgroup + 2 MMA warpgroups
 constexpr int SMP_A_BYTES = 128 * 64 * 2;     // one k-block of the A tile
 constexpr int SMP_W_BYTES = SMP_BN * 64 * 2;
-constexpr int SMP_SMEM = SMP_MAX_KB * SMP_A_BYTES + SMP_STAGES * SMP_W_BYTES + 1024 + 256 + (SMP_EPI_WARPS / 4) * 128 * 8;
+constexpr int SMP_SMEM = SMP_MAX_KB * SMP_A_BYTES + SMP_STAGES * SMP_W_BYTES + 1024 + 256;
+
+// keeps (v, i) if it wins: larger value, or equal value and smaller label (torch's first maximum)
+__device__ __forceinline__ void argmax_merge(float& bv, int& bi, float ov, int oi) {
+    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+}
 
 __global__ void __launch_bounds__(SMP_THREADS, 1)
 fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, int R, int NL,
                      int Kc, float inv_t, TorchPhilox rng, int64_t* __restrict__ out) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
     const uint32_t a_base = smem_base;
     const uint32_t w_base = smem_base + SMP_MAX_KB * SMP_A_BYTES;
     const uint32_t bar_base = w_base + SMP_STAGES * SMP_W_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (SMP_STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * SMP_STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * SMP_STAGES + 2 + s); };
-    const uint32_t a_bar = bar_base + 8u * (2 * SMP_STAGES + 4);
-    const uint32_t tmem_slot = bar_base + 8u * (2 * SMP_STAGES + 5);
-    uint8_t* tail = smem_gen + (bar_base - smem_base) + 256;
-    float* best_v = reinterpret_cast<float*>(tail);                // [slices-1][128] candidates of the other column slices
-    int* best_i = reinterpret_cast<int*>(tail + (SMP_EPI_WARPS / 4) * 128 * 4);
+    const uint32_t a_bar = bar_base + 8u * (2 * SMP_STAGES);
 
-    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
     const int lane = threadIdx.x & 31;
     const int n_kb = (Kc + 63) / 64;
     const int n_chunks = (NL + SMP_BN - 1) / SMP_BN;
     const int m_idx = blockIdx.x * 128;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tm_a);
         ptx::prefetch_tensormap(&tm_w);
+        for (int s = 0; s < SMP_STAGES; ++s) { ptx::mbar_init(full_bar(s), 1); ptx::mbar_init(empty_bar(s), 2); }
+        ptx::mbar_init(a_bar, 1);
+        ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < SMP_STAGES; ++s) { ptx::mbar_init(full_bar(s), 1); ptx::mbar_init(empty_bar(s), 1); }
-            for (int s = 0; s < 2; ++s) { ptx::mbar_init(tfull_bar(s), 1); ptx::mbar_init(tempty_bar(s), SMP_EPI_WARPS); }
-            ptx::mbar_init(a_bar, 1);
-            ptx::fence_barrier_init();
-        }
-        __syncwarp();
-        ptx::tmem_alloc(tmem_slot, 256);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *reinterpret_cast<uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
-    if (warp == 0) {
-        if (ptx::elect_one()) {
+    if (wg == 0) {
+        ptx::setmaxnreg_dec<40>();
+        if (threadIdx.x < 32 && ptx::elect_one()) {
             ptx::mbar_arrive_expect_tx(a_bar, n_kb * SMP_A_BYTES);
             for (int kb = 0; kb < n_kb; ++kb) ptx::tma_load_2d(&tm_a, a_bar, a_base + kb * SMP_A_BYTES, kb * 64, m_idx);
             int stage = 0;
@@ -89,123 +75,80 @@ fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
                     if (++stage == SMP_STAGES) { stage = 0; phase ^= 1; }
                 }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = ptx::umma_idesc_f16(128, SMP_BN, 0);
+    } else {
+        ptx::setmaxnreg_inc<232>();
+        const int cw = wg - 1;                   // token rows [64 cw, 64 cw + 64) of the tile
+        const int tid = threadIdx.x & 127;
+        const int wq = tid >> 5;
+        // this thread's two rows (wgmma fragment: rows 16 wq + lane/4 and + 8, column pairs 8n + 2 (lane % 4))
+        const int row0 = m_idx + cw * 64 + wq * 16 + (lane >> 2);
+        float bv[2] = {-INFINITY, -INFINITY};
+        int bi[2] = {0x7fffffff, 0x7fffffff};
+        float acc[SMP_BN / 2];
         ptx::mbar_wait(a_bar, 0);
         int stage = 0;
         uint32_t phase = 0;
         for (int ch = 0; ch < n_chunks; ++ch) {
-            const int as = ch & 1;
-            ptx::mbar_wait(tempty_bar(as), ((ch >> 1) & 1) ^ 1);
-            ptx::tc_fence_after();
+            int prev = 0;
             for (int kb = 0; kb < n_kb; ++kb) {
                 ptx::mbar_wait(full_bar(stage), phase);
-                ptx::tc_fence_after();
-                if (ptx::elect_one()) {
-                    const uint64_t da = ptx::umma_desc_kmajor_sw128(a_base + kb * SMP_A_BYTES);
-                    const uint64_t db = ptx::umma_desc_kmajor_sw128(w_base + stage * SMP_W_BYTES);
+                const uint64_t da = ptx::wgmma_desc_kmajor_sw128(a_base + kb * SMP_A_BYTES + cw * (64 * 128));
+                const uint64_t db = ptx::wgmma_desc_kmajor_sw128(w_base + stage * SMP_W_BYTES);
+                ptx::wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        ptx::umma_f16(tmem_base + as * SMP_BN, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                    ptx::umma_commit(empty_bar(stage));
-                    if (kb == n_kb - 1) ptx::umma_commit(tfull_bar(as));
+                for (int k = 0; k < 4; ++k) ptx::wgmma_m64n128k16(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+                ptx::wgmma_commit();
+                if (kb > 0) {
+                    ptx::wgmma_wait<1>();
+                    if (tid == 0) ptx::mbar_arrive(empty_bar(prev));
                 }
-                __syncwarp();
+                prev = stage;
                 if (++stage == SMP_STAGES) { stage = 0; phase ^= 1; }
             }
-        }
-    } else {
-        const int q = warp & 3;                  // TMEM lane quarter
-        const int half = (warp - 2) >> 2;        // which slice of the chunk's 128 columns
-        const int row_in_tile = q * 32 + lane;
-        const int row = m_idx + row_in_tile;
-        const bool row_ok = row < R;
-        float bv = -INFINITY;
-        int bidx = 0;
-        for (int ch = 0; ch < n_chunks; ++ch) {
-            const int as = ch & 1;
-            ptx::mbar_wait(tfull_bar(as), (ch >> 1) & 1);
-            ptx::tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < SMP_COLS_PER_WARP; c += 32) {
-                const int col0 = ch * SMP_BN + half * SMP_COLS_PER_WARP + c;
-                float v[32];
-                ptx::tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * SMP_BN + half * SMP_COLS_PER_WARP + c), v);
-                if (row_ok && col0 < NL) {
-                    const uint64_t e0 = (uint64_t)row * (uint64_t)NL + (uint64_t)col0;
-                    uint64_t j = e0 / rng.stride;
-                    uint32_t tid = (uint32_t)(e0 - j * rng.stride);
+            ptx::wgmma_wait<0>();
+            if (tid == 0) ptx::mbar_arrive(empty_bar(prev));
+            ptx::fence_regs(acc);
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const uint4 r4 = torch_philox_call(rng, tid, j >> 2);
-                        const uint32_t ln = (uint32_t)(j & 3);
-                        const uint32_t bits = ln == 0 ? r4.x : ln == 1 ? r4.y : ln == 2 ? r4.z : r4.w;
-                        const float qv = torch_exponential1(u32_to_uniform(bits));
-                        const float gum = fmaf(v[i], inv_t, -__logf(qv));
-                        if (col0 + i < NL && gum > bv) { bv = gum; bidx = col0 + i; }
-                        if (++tid == rng.stride) { tid = 0; ++j; }
-                    }
+            for (int i = 0; i < SMP_BN / 2; ++i) {
+                const int rr = (i >> 1) & 1;
+                const int row = row0 + 8 * rr;
+                const int col = ch * SMP_BN + (i >> 2) * 8 + 2 * (lane & 3) + (i & 1);
+                if (row < R && col < NL) {
+                    const float qv = torch_exponential1(u32_to_uniform(torch_philox_u32(rng, (uint64_t)row * (uint64_t)NL + (uint64_t)col)));
+                    const float gum = fmaf(acc[i], inv_t, -__logf(qv));
+                    if (gum > bv[rr]) { bv[rr] = gum; bi[rr] = col; }      // columns of a row arrive in increasing order
                 }
             }
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(tempty_bar(as));
         }
-        // combine the column slices of each row
-        constexpr int NS = SMP_EPI_WARPS / 4;
-        if (half > 0) { best_v[(half - 1) * 128 + row_in_tile] = bv; best_i[(half - 1) * 128 + row_in_tile] = bidx; }
-        asm volatile("bar.sync 1, %0;" ::"n"(32 * SMP_EPI_WARPS) : "memory");
-        if (half == 0 && row_ok) {
+        // combine the four threads of each row
 #pragma unroll
-            for (int s = 0; s < NS - 1; ++s) {
-                const float ov = best_v[s * 128 + row_in_tile];
-                const int oi = best_i[s * 128 + row_in_tile];
-                if (ov > bv || (ov == bv && oi < bidx)) { bv = ov; bidx = oi; }
-            }
-            out[row] = bidx;
+        for (int rr = 0; rr < 2; ++rr) {
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1)
+                argmax_merge(bv[rr], bi[rr], __shfl_xor_sync(0xffffffffu, bv[rr], o), __shfl_xor_sync(0xffffffffu, bi[rr], o));
+            const int row = row0 + 8 * rr;
+            if ((lane & 3) == 0 && row < R) out[row] = bi[rr];
         }
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) ptx::tmem_dealloc(tmem_base, 256);
 }
 
 // =====================================================================================================================
 // Shared-Philox variant.  torch's generator hands element (row, label) the lane (row / rs) % 4 of curand4 call number
-// row / (4 rs) of thread (row % rs) * NL + label, rs = stride / NL (37 on a B200 for 8192 labels): the four rows
+// row / (4 rs) of thread (row % rs) * NL + label, rs = stride / NL (33 on a 132-SM H100 for 8192 labels): the four rows
 // r, r+rs, r+2rs, r+3rs of a 4rs-row block share ONE Philox4x32-10 evaluation per label.  To use all four outputs in
 // one thread the product is computed TRANSPOSED — D[label, token] = W[labels, K] . F[tokens, K]^T — with the token
-// tile ordered (jj, g) -> row 4rs*i + rs*g + jj0 + jj (a 4-D TMA box, g innermost).  A thread then owns one label of
-// each 128-label chunk (TMEM lane) and 20 token columns = 5 Philox calls, keeps a running arg-max per column over the
-// 64 chunks in registers, and the 128 lanes are reduced once at the end.  ~2.9x fewer instructions per logit.
+// tile ordered (jj, g) -> row 4rs*i + rs*g + jj0 + jj (a 4-D TMA box, g innermost).  Each MMA warpgroup takes 64 labels of a
+// 128-label chunk (wgmma m64n80k16); in the fragment a thread holds two of the four g of a (label, jj) pair, so neighbouring
+// threads swap halves: afterwards a thread owns one label and all four g of 10 jj = 10 Philox calls for 40 logits, keeps a
+// running arg-max per token column over the 64 chunks in registers, and the labels are reduced once at the end.
 constexpr int SH_JJ = 20;                      // jj slots per task
-constexpr int SH_N = 4 * SH_JJ;                // token columns per MMA tile (UMMA N = 80)
-constexpr int SH_EPI_WARPS = 16;
-constexpr int SH_THREADS = 64 + 32 * SH_EPI_WARPS;
+constexpr int SH_N = 4 * SH_JJ;                // token columns per MMA tile (wgmma N = 80)
+constexpr int SH_THREADS = 384;
 constexpr int SH_STAGES = 6;
 constexpr int SH_F_BYTES = SH_N * 128;         // one k-block of the token tile
 constexpr int SH_W_BYTES = 128 * 128;          // 128 labels x 64 halves
-constexpr int SH_SMEM = SMP_MAX_KB * SH_F_BYTES + SH_STAGES * SH_W_BYTES + 1024 + 256 + 4 * SH_N * 8;
-
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-    ptx::tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_x4(uint32_t taddr, float* v) {
-    uint32_t r[4];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(taddr) : "memory");
-    ptx::tmem_ld_wait();
-#pragma unroll
-    for (int i = 0; i < 4; ++i) v[i] = __uint_as_float(r[i]);
-}
+constexpr int SH_RED_WARPS = 8;                // MMA warps, one reduction row each
+constexpr int SH_SMEM = SMP_MAX_KB * SH_F_BYTES + SH_STAGES * SH_W_BYTES + 1024 + 256 + SH_RED_WARPS * SH_N * 8;
 
 __global__ void __launch_bounds__(SH_THREADS, 1)
 fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __grid_constant__ CUtensorMap tm_w, int R, int NL,
@@ -218,43 +161,30 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
     const uint32_t bar_base = w_base + SH_STAGES * SH_W_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (SH_STAGES + s); };
-    auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * SH_STAGES + s); };
-    auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * SH_STAGES + 2 + s); };
-    const uint32_t f_bar = bar_base + 8u * (2 * SH_STAGES + 4);
-    const uint32_t tmem_slot = bar_base + 8u * (2 * SH_STAGES + 5);
+    const uint32_t f_bar = bar_base + 8u * (2 * SH_STAGES);
     uint8_t* tail = smem_gen + (bar_base - smem_base) + 256;
-    float* red_v = reinterpret_cast<float*>(tail);                    // [4 quarters][SH_N]
-    int* red_i = reinterpret_cast<int*>(tail + 4 * SH_N * 4);
+    float* red_v = reinterpret_cast<float*>(tail);                    // [8 warps][SH_N]
+    int* red_i = reinterpret_cast<int*>(tail + SH_RED_WARPS * SH_N * 4);
 
-    const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
     const int lane = threadIdx.x & 31;
     const int n_kb = (Kc + 63) / 64;
     const int n_chunks = (NL + 127) / 128;
     const int blk = blockIdx.x / tasks_per_block;                      // 4rs-row block = Philox call index
     const int jj0 = (blockIdx.x - blk * tasks_per_block) * SH_JJ;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tm_f);
         ptx::prefetch_tensormap(&tm_w);
+        for (int s = 0; s < SH_STAGES; ++s) { ptx::mbar_init(full_bar(s), 1); ptx::mbar_init(empty_bar(s), 2); }
+        ptx::mbar_init(f_bar, 1);
+        ptx::fence_barrier_init();
     }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < SH_STAGES; ++s) { ptx::mbar_init(full_bar(s), 1); ptx::mbar_init(empty_bar(s), 1); }
-            for (int s = 0; s < 2; ++s) { ptx::mbar_init(tfull_bar(s), 1); ptx::mbar_init(tempty_bar(s), SH_EPI_WARPS); }
-            ptx::mbar_init(f_bar, 1);
-            ptx::fence_barrier_init();
-        }
-        __syncwarp();
-        ptx::tmem_alloc(tmem_slot, 256);
-        ptx::tmem_relinquish();
-    }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *reinterpret_cast<uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
-    if (warp == 0) {
-        if (ptx::elect_one()) {
+    if (wg == 0) {
+        ptx::setmaxnreg_dec<40>();
+        if (threadIdx.x < 32 && ptx::elect_one()) {
             ptx::mbar_arrive_expect_tx(f_bar, n_kb * SH_F_BYTES);
             for (int kb = 0; kb < n_kb; ++kb) ptx::tma_load_4d(&tm_f, f_bar, f_base + kb * SH_F_BYTES, kb * 64, 0, jj0, blk);
             int stage = 0;
@@ -267,99 +197,101 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
                     if (++stage == SH_STAGES) { stage = 0; phase ^= 1; }
                 }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = ptx::umma_idesc_f16(128, SH_N, 0);
+    } else {
+        ptx::setmaxnreg_inc<232>();
+        const int cw = wg - 1;                       // labels [64 cw, 64 cw + 64) of each chunk
+        const int tid = threadIdx.x & 127;
+        const int wq = tid >> 5;
+        const int q = lane & 3;
+        const bool odd = (q & 1) != 0;
+        // after the swap: this thread's label of the chunk, and jj = jj0 + 2 n + (q >> 1) for n = 0..9, all four g
+        const int l = cw * 64 + wq * 16 + (lane >> 2) + (odd ? 8 : 0);
+        float bv[SH_N / 2];
+        int bi[SH_N / 2];
+#pragma unroll
+        for (int i = 0; i < SH_N / 2; ++i) { bv[i] = -INFINITY; bi[i] = 0x7fffffff; }
+        float acc[SH_N / 2];
         ptx::mbar_wait(f_bar, 0);
         int stage = 0;
         uint32_t phase = 0;
         for (int ch = 0; ch < n_chunks; ++ch) {
-            const int as = ch & 1;
-            ptx::mbar_wait(tempty_bar(as), ((ch >> 1) & 1) ^ 1);
-            ptx::tc_fence_after();
+            int prev = 0;
             for (int kb = 0; kb < n_kb; ++kb) {
                 ptx::mbar_wait(full_bar(stage), phase);
-                ptx::tc_fence_after();
-                if (ptx::elect_one()) {
-                    const uint64_t da = ptx::umma_desc_kmajor_sw128(w_base + stage * SH_W_BYTES);     // labels = M
-                    const uint64_t db = ptx::umma_desc_kmajor_sw128(f_base + kb * SH_F_BYTES);        // tokens = N
+                const uint64_t da = ptx::wgmma_desc_kmajor_sw128(w_base + stage * SH_W_BYTES + cw * (64 * 128));   // labels = M
+                const uint64_t db = ptx::wgmma_desc_kmajor_sw128(f_base + kb * SH_F_BYTES);                        // tokens = N
+                ptx::wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                        ptx::umma_f16(tmem_base + as * 128, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                    ptx::umma_commit(empty_bar(stage));
-                    if (kb == n_kb - 1) ptx::umma_commit(tfull_bar(as));
+                for (int k = 0; k < 4; ++k) ptx::wgmma_m64n80k16(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+                ptx::wgmma_commit();
+                if (kb > 0) {
+                    ptx::wgmma_wait<1>();
+                    if (tid == 0) ptx::mbar_arrive(empty_bar(prev));
                 }
-                __syncwarp();
+                prev = stage;
                 if (++stage == SH_STAGES) { stage = 0; phase ^= 1; }
             }
-        }
-    } else {
-        const int q = warp & 3;                      // TMEM lane quarter -> labels 32q..32q+31 of the chunk
-        const int sub = (warp - 2) >> 2;             // token columns [sub*20, sub*20+20): jj = sub*5 .. sub*5+4
-        const int l = q * 32 + lane;
-        float bv[SH_JJ];
-        int bi[SH_JJ];
-#pragma unroll
-        for (int i = 0; i < SH_JJ; ++i) { bv[i] = -INFINITY; bi[i] = 0x7fffffff; }
-        for (int ch = 0; ch < n_chunks; ++ch) {
-            const int as = ch & 1;
-            ptx::mbar_wait(tfull_bar(as), (ch >> 1) & 1);
-            ptx::tc_fence_after();
-            float v[SH_JJ];
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * 128 + sub * SH_JJ);
-            tmem_ld_x16(taddr, v);
-            tmem_ld_x4(taddr + 16, v + 16);
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(tempty_bar(as));      // accumulator copied to registers: MMA may reuse it
+            ptx::wgmma_wait<0>();
+            if (tid == 0) ptx::mbar_arrive(empty_bar(prev));
+            ptx::fence_regs(acc);
             const int label = ch * 128 + l;
-            if (label < NL) {
 #pragma unroll
-                for (int c4 = 0; c4 < SH_JJ / 4; ++c4) {
-                    const int jj = jj0 + sub * (SH_JJ / 4) + c4;
+            for (int n = 0; n < SH_N / 8; ++n) {
+                // fragment: acc[4n + {0,1}] = (label row lane/4, g = 2 (q & 1) + {0,1}), acc[4n + {2,3}] = (row + 8, same g)
+                const float s0 = odd ? acc[4 * n + 0] : acc[4 * n + 2];
+                const float s1 = odd ? acc[4 * n + 1] : acc[4 * n + 3];
+                const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1);
+                const float r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+                float v[4];
+                v[0] = odd ? r0 : acc[4 * n + 0];
+                v[1] = odd ? r1 : acc[4 * n + 1];
+                v[2] = odd ? acc[4 * n + 2] : r0;
+                v[3] = odd ? acc[4 * n + 3] : r1;
+                if (label < NL) {
+                    const int jj = jj0 + 2 * n + (q >> 1);
                     const uint4 r4 = torch_philox_call(rng, (uint64_t)jj * (uint64_t)NL + (uint64_t)label, (uint64_t)blk);
                     const uint32_t bits[4] = {r4.x, r4.y, r4.z, r4.w};
 #pragma unroll
                     for (int g = 0; g < 4; ++g) {
                         const float qv = torch_exponential1(u32_to_uniform(bits[g]));
-                        const float gum = fmaf(v[c4 * 4 + g], inv_t, -__logf(qv));
-                        if (gum > bv[c4 * 4 + g]) { bv[c4 * 4 + g] = gum; bi[c4 * 4 + g] = label; }
+                        const float gum = fmaf(v[g], inv_t, -__logf(qv));
+                        if (gum > bv[4 * n + g]) { bv[4 * n + g] = gum; bi[4 * n + g] = label; }
                     }
                 }
             }
         }
-        // reduce over the 32 labels of this warp, then over the 4 quarters through shared memory
+        // reduce over the labels of this warp (lanes with the same q >> 1 hold the same token columns), then over the 8 warps
 #pragma unroll
-        for (int i = 0; i < SH_JJ; ++i) {
+        for (int i = 0; i < SH_N / 2; ++i) {
 #pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(0xffffffffu, bv[i], o);
-                const int oi = __shfl_xor_sync(0xffffffffu, bi[i], o);
-                if (ov > bv[i] || (ov == bv[i] && oi < bi[i])) { bv[i] = ov; bi[i] = oi; }
+            for (int o = 1; o <= 16; o <<= 1) {
+                if (o == 2) continue;
+                argmax_merge(bv[i], bi[i], __shfl_xor_sync(0xffffffffu, bv[i], o), __shfl_xor_sync(0xffffffffu, bi[i], o));
             }
         }
-        if (lane == 0) {
+        const int w8 = cw * 4 + wq;
+        if (lane == 0 || lane == 2) {
 #pragma unroll
-            for (int i = 0; i < SH_JJ; ++i) { red_v[q * SH_N + sub * SH_JJ + i] = bv[i]; red_i[q * SH_N + sub * SH_JJ + i] = bi[i]; }
+            for (int n = 0; n < SH_N / 8; ++n)
+#pragma unroll
+                for (int g = 0; g < 4; ++g) {
+                    const int c = (2 * n + (q >> 1)) * 4 + g;       // token column = jj_local * 4 + g
+                    red_v[w8 * SH_N + c] = bv[4 * n + g];
+                    red_i[w8 * SH_N + c] = bi[4 * n + g];
+                }
         }
-        asm volatile("bar.sync 1, %0;" ::"n"(32 * SH_EPI_WARPS) : "memory");
-        const int t = threadIdx.x - 64;
+        ptx::bar_sync(1, 256);
+        const int t = threadIdx.x - 128;
         if (t < SH_N) {
             float best = red_v[t];
             int besti = red_i[t];
 #pragma unroll
-            for (int qq = 1; qq < 4; ++qq) {
-                const float ov = red_v[qq * SH_N + t];
-                const int oi = red_i[qq * SH_N + t];
-                if (ov > best || (ov == best && oi < besti)) { best = ov; besti = oi; }
-            }
+            for (int w = 1; w < SH_RED_WARPS; ++w) argmax_merge(best, besti, red_v[w * SH_N + t], red_i[w * SH_N + t]);
             const int jj = jj0 + t / 4, g = t & 3;
             const int64_t row = (int64_t)blk * 4 * rs + (int64_t)g * rs + jj;
             if (jj < rs && row < R) out[row] = besti;
         }
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 1) ptx::tmem_dealloc(tmem_base, 256);
 }
 
 int64_t fused_sampler_rows_padded(int64_t R, int NL) {

@@ -2,7 +2,7 @@
 //   VQModel blocks / parameter names   ref/src/vqgan.py:45-89
 //   encode / decode / decode_indices   ref/src/vqgan.py:91-107
 //   ResBlock                           ref/src/vqgan.py:6-42
-// The MLPs of the ResBlocks are the tcgen05 GEMMs of gemm.cu; Conv2d(k4,s2,p1) and ConvTranspose2d(k4,s2,p1) are
+// The MLPs of the ResBlocks are the wgmma GEMMs of gemm.cu; Conv2d(k4,s2,p1) and ConvTranspose2d(k4,s2,p1) are
 // the same kernel with an im2col-free TMA gather of the A operand (ConvGeom); the 12/4-channel 1x1 convs at the
 // image / latent ends are CUDA-core kernels (K or N of 4..12 cannot fill a tensor-core tile).
 #include <cstring>
@@ -417,7 +417,7 @@ static void vq_plan(const pb200_vqgan* m, int B, int H, int W, uint8_t* base, in
 // The part of a codec ResBlock (ref/src/vqgan.py:36-42) before its MLP: x' = x + g2 * dw3x3(pad(LN(x)(1+g0)+g1)), then
 // a16 = fp16(LN(x')(1+g3)+g4).  x: NHWC fp32 [B,h,w,c].  *resid = where x' lives: `tmp32` on the fused path (one patch kernel +
 // a statistics pre-pass, ops.cu::launch_vq_front_fused; `scratch` = B*h*w float2), x itself (updated in place) on the three-launch
-// path that narrow widths (tiny test codecs) and in_place = true (the fused-MLP experiment) take.
+// path that narrow widths (tiny test codecs) and in_place = true take.
 static int resblock_front(float* x, int B, int h, int w, int c, const float* dw_w9, const float* dw_b, const float* gam,
                           float* tmp32, __half* a16, void* scratch, bool in_place, const float** resid, cudaStream_t st) {
     const int64_t M = (int64_t)B * h * w;
@@ -440,15 +440,9 @@ static int resblock_front(float* x, int B, int h, int w, int c, const float* dw_
 static int run_resblock(pb200_vqgan* m, const VqResBlock& rb, float* x, int B, int h, int w, VqWs& ws, cudaStream_t st) {
     const int c = rb.c;
     const int64_t M = (int64_t)B * h * w;
-    static const bool fused = getenv("PB200_VQ_MLP_FUSED") != nullptr;      // experiment knob: see vq_mlp.cu (measured slower)
     const float* resid = x;
     // (h16 is idle until GEMM1 writes it: it lends its first bytes to the row statistics)
-    PB_TRY(resblock_front(x, B, h, w, c, m->w<float>(rb.dw_w), m->w<float>(rb.dw_b), rb.gam, ws.tmp32, ws.a16, ws.h16, fused, &resid, st));
-    if (fused) {    // Linear -> GELU -> Linear -> x + g5 * (.) in one kernel, the 4c hidden never leaves the SM
-        const int rc = launch_vq_mlp_fused(ws.a16, M, c, m->w<__half>(rb.w1), m->w<float>(rb.b1), m->w<__half>(rb.w2), m->w<float>(rb.b2), x,
-                                           rb.gam[5], st);
-        if (rc >= 0) return rc;
-    }
+    PB_TRY(resblock_front(x, B, h, w, c, m->w<float>(rb.dw_w), m->w<float>(rb.dw_b), rb.gam, ws.tmp32, ws.a16, ws.h16, false, &resid, st));
     pb200_gemm_epilogue e1 = vepi(PB200_EPI_GELU_F16, m->w<float>(rb.b1), ws.h16, 4 * c);
     PB_TRY(m->gemm(ws.a16, c, M, c, rb.w1, 4 * (int64_t)c, e1, st));
     pb200_gemm_epilogue e2 = vepi(PB200_EPI_RESID_F32, m->w<float>(rb.b2), x, c);
@@ -495,15 +489,6 @@ int pb200_vqgan_resblock(float* x_nhwc, int batch, int h, int w, int c, const fl
     pb200_gemm_epilogue e2 = vepi(PB200_EPI_RESID_F32, b2, x_nhwc, c);
     e2.resid = resid; e2.ldr = c; e2.alpha = gammas_host[5];
     return gemm_f16(h16, 4 * (int64_t)c, w2_f16, 4 * (int64_t)c, M, c, 4 * (int64_t)c, e2, st);
-}
-
-int pb200_vq_mlp_fused(const void* a16, int64_t rows, int c, const void* w1_f16, const float* b1, const void* w2_f16, const float* b2,
-                       float* x, float alpha, void* stream) {
-    PB_CHECK(a16 && w1_f16 && b1 && w2_f16 && b2 && x, "vq_mlp_fused: null pointer");
-    const int rc = launch_vq_mlp_fused(reinterpret_cast<const __half*>(a16), rows, c, reinterpret_cast<const __half*>(w1_f16), b1,
-                                       reinterpret_cast<const __half*>(w2_f16), b2, x, alpha, (cudaStream_t)stream);
-    PB_CHECK(rc >= 0, "vq_mlp_fused: built for c in {384, 192} and rows >= 256 only (got c=%d, rows=%lld)", c, (long long)rows);
-    return rc;
 }
 
 int pb200_vqgan_create(const pb200_vqgan_config* cfg, pb200_vqgan** out) {
@@ -625,7 +610,7 @@ int pb200_vqgan_encode(pb200_vqgan* m, const float* img, int batch, int img_h, i
         g.tiles_x = ceil_div(w1, g.tw); g.tiles_y = ceil_div(h1, g.th);
         g.oh = h1; g.ow = w1; g.sy = 1; g.sx = 1; g.py = 0; g.px = 0;
         const int64_t N = c1, K = 16 * (int64_t)m->cpad0;
-        const int bn = gemm_pick_block_n((int64_t)B * g.tiles_x * g.tiles_y * 128, N, K, false);
+        const int bn = gemm_pick_block_n((int64_t)B * g.tiles_x * g.tiles_y * 128, N, K);
         CUtensorMap ta;
         const int64_t dims[5] = {2 * (int64_t)c0, w0 / 2, 2, h0 / 2, B};
         const int64_t strides[4] = {2 * (int64_t)c0 * 2, (int64_t)w0 * c0 * 2, 2 * (int64_t)w0 * c0 * 2, (int64_t)h0 * w0 * c0 * 2};
@@ -699,7 +684,7 @@ int pb200_vqgan_decode_ex(pb200_vqgan* m, const int64_t* indices, const float* l
         g.tiles_x = ceil_div(w1, g.tw); g.tiles_y = ceil_div(h1, g.th);
         g.oh = h0; g.ow = w0; g.sy = 2; g.sx = 2;
         const int64_t N = c0, K = 4 * (int64_t)m->cpad1;
-        const int bn = gemm_pick_block_n((int64_t)B * g.tiles_x * g.tiles_y * 128, N, K, false);
+        const int bn = gemm_pick_block_n((int64_t)B * g.tiles_x * g.tiles_y * 128, N, K);
         CUtensorMap ta;
         const int64_t dims[4] = {c1, w1, h1, B};
         const int64_t strides[3] = {(int64_t)c1 * 2, (int64_t)w1 * c1 * 2, (int64_t)h1 * w1 * c1 * 2};

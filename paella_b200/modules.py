@@ -2,7 +2,7 @@
 
 Same class names, constructor kwargs, attribute names and state-dict keys as the reference, so
 ``load_state_dict(paella_v3.pt)`` and ``paella_inference.ipynb`` work unchanged — but ``forward`` runs the
-hand-written sm_100a kernels behind the C ABI (include/paella_b200.h).  The ``torch.nn`` layers created
+hand-written sm_90a kernels behind the C ABI (include/paella_b200.h).  The ``torch.nn`` layers created
 here are PARAMETER HOLDERS ONLY (they give the reference's key names and initialisation); none of their
 ``forward`` methods is ever called, and there is no PyTorch or CPU fallback.
 """

@@ -36,7 +36,7 @@ def philox_row_chunks(rows: int, k: int, elem_bytes: int = 4):
     INT32_MAX, i.e. > 2^29 fp32 elements) into halves, first half first, recursively (ATen TensorIterator::split /
     SplitUntil32Bit, DistributionTemplates.h:132-138); every sub-kernel takes its own Philox offset from the generator --
     and the ROOT call has already taken one for the whole tensor before it notices that it must split (it computes its
-    execution policy and calls philox_cuda_state first; measured on B200: a 2^30-element draw advances the offset by
+    execution policy and calls philox_cuda_state first: a 2^30-element draw advances the offset by
     inc(2^30) + 2 inc(2^29)), see ``skip_philox_for_split``.  bs=64 at 32x32x8192 is exactly 2^29 elements (one kernel);
     larger batches split -- mirrored here so the draws stay bit-identical to torch.multinomial's."""
     lim = 2 ** 31 - 1

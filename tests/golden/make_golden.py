@@ -10,6 +10,9 @@ restatement (oracle/vqgan_oracle.py) and is NOT what these fixtures pin — the
 fixtures record the conv stacks' pre-quantisation latents and decoder outputs.
 
 Outputs (small, committed):  tests/golden/paella_tiny.npz, vqgan_tiny.npz, sample_tiny.npz
+    python tests/golden/make_golden.py --default
+writes tests/golden/default_ref.npz: the reference-default denoiser's logits and the f4 VQGAN's conv-stack outputs (the
+latents in full, seeded samples of the rest), on the inputs tests/test_oracle_vs_reference.py rebuilds.
 """
 import importlib.util
 import os
@@ -187,5 +190,41 @@ def main():
     print("vqgan_tiny.npz:", {k: v.shape for k, v in vo_.items() if not k.startswith("sd:")})
 
 
+DEFAULT_SAMPLE = 4096          # logits kept of the 8192 x 32 x 32 output
+DECODED_SAMPLE = 2048          # decoded values kept of the 3 x 64 x 64 image
+
+
+def default_inputs(modules, vqgan):
+    """The reference-default denoiser and VQGAN (torch.manual_seed(0) initialisation + rerandomize_) and their inputs; `modules`
+    / `vqgan` are the reference's module files or this package's mirrors, which initialise identically."""
+    from paella_b200.synth import synthetic_conditioning
+    torch.manual_seed(0)
+    m = modules.Paella(byt5_embd=2560).eval()
+    rerandomize_(m.state_dict(), seed=0)
+    cond, _ = synthetic_conditioning(1, 16, with_clip_image=True)
+    x = torch.randint(0, 8192, (1, 32, 32), generator=torch.Generator().manual_seed(1))
+    r = torch.tensor([0.6])
+    torch.manual_seed(0)
+    vq = vqgan.VQModel().eval()
+    rerandomize_(vq.state_dict(), seed=4)
+    img = torch.rand(1, 3, 64, 64, generator=torch.Generator().manual_seed(7))
+    idx = torch.randint(0, 8192, (1, 16, 16), generator=torch.Generator().manual_seed(8))
+    rng = np.random.default_rng(0)
+    pick = rng.choice(8192 * 32 * 32, DEFAULT_SAMPLE, replace=False)
+    pick_dec = rng.choice(3 * 64 * 64, DECODED_SAMPLE, replace=False)
+    return m, cond, x, r, vq, img, idx, (pick, pick_dec)
+
+
+def default_size():
+    ref_modules, _, _, ref_vqgan, _ = load_reference()
+    with torch.no_grad():
+        m, cond, x, r, vq, img, idx, (pick, pick_dec) = default_inputs(ref_modules, ref_vqgan)
+        logits = m(x, r, cond["byt5"], clip=cond["clip"], clip_image=cond["clip_image"])
+        lat = vq.down_blocks(vq.in_block(img))
+        dec = vq.decode_indices(idx)
+    np.savez_compressed(os.path.join(HERE, "default_ref.npz"), logits=logits.reshape(-1)[pick].numpy(),
+                        logits_std=np.float32(logits.std()), latents=lat.numpy(), decoded=dec.reshape(-1)[pick_dec].numpy())
+
+
 if __name__ == "__main__":
-    main()
+    default_size() if "--default" in sys.argv[1:] else main()

@@ -31,7 +31,7 @@ def test_ctypes_table_mirrors_header():
     from paella_b200 import _lib
     assert sorted(_lib.SIGNATURES) == _header_functions()
     l = _lib.lib()
-    assert l.pb200_abi_version() == 2
+    assert l.pb200_abi_version() == 3
     assert l.pb200_last_error() is not None
 
 
@@ -106,8 +106,8 @@ def test_load_conditional_models_reads_reference_checkpoint_layout(tmp_path):
 
 
 def test_gemm_tile_plan_on_a_148_sm_part():
-    """Host-side tile planner (pure arithmetic, no device work): which kernel / BLOCK_N / tail width the bench
-    workload's GEMM shapes get on a 148-SM B200 (DESIGN.md §3)."""
+    """Host-side tile planner on a part with more SMs than the H100 (pure arithmetic, no device work): the bench
+    workload's GEMM shapes keep their 256-wide one-CTA tiles, and small problems still get narrow tiles."""
     import ctypes
     from paella_b200 import _lib
     L = _lib.lib()
@@ -116,22 +116,37 @@ def test_gemm_tile_plan_on_a_148_sm_part():
         bn, two, tail = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
         _lib.check(L.pb200_gemm_plan(m, n, k, sms, ctypes.byref(bn), ctypes.byref(two), ctypes.byref(tail)), "gemm_plan")
         return bn.value, two.value, tail.value
-    # level-1 MLP GEMM2 / out-projection: 160 pair tiles on 74 SM pairs = 2 waves + 12 -> narrow tail tiles
-    assert plan(8192, 1280, 5120) == (256, 1, 128)
-    assert plan(8192, 1280, 1280) == (256, 1, 128)
-    # level-1 MLP GEMM1: 640 tiles = 8 waves + 48: a tail wave would not be shorter -> none
-    assert plan(8192, 5120, 1280) == (256, 1, 0)
-    # QKV projection: 480 tiles = 6 waves + 36 -> 72 half-width tiles
-    assert plan(8192, 3840, 1280) == (256, 1, 128)
-    # a single 128-row tile stays on the 1-SM kernel
-    bn, two, tail = plan(64, 1280, 1280)
-    assert two == 0 and tail == 0 and bn in (64, 128, 256)
+    assert plan(8192, 1280, 5120) == (256, 0, 0)
+    assert plan(8192, 1280, 1280) == (256, 0, 0)
+    assert plan(8192, 5120, 1280) == (256, 0, 0)
+    assert plan(8192, 3840, 1280) == (256, 0, 0)
+    assert plan(64, 1280, 1280) == (64, 0, 0)
+    assert plan(300, 640, 64) == (64, 0, 0)
+
+
+def test_gemm_tile_plan_on_a_132_sm_part():
+    """Host-side tile planner (pure arithmetic, no device work): the BLOCK_N the bench workload's GEMM shapes get on a
+    132-SM H100 (DESIGN.md section 3).  Every tile is one CTA's and BLOCK_N wide on sm_90a."""
+    import ctypes
+    from paella_b200 import _lib
+    L = _lib.lib()
+
+    def plan(m, n, k, sms=132):
+        bn, two, tail = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        _lib.check(L.pb200_gemm_plan(m, n, k, sms, ctypes.byref(bn), ctypes.byref(two), ctypes.byref(tail)), "gemm_plan")
+        return bn.value, two.value, tail.value
+    # level-1 MLP GEMMs, out-projection and QKV projection: 256-wide tiles
+    assert plan(8192, 1280, 5120) == (256, 0, 0)
+    assert plan(8192, 1280, 1280) == (256, 0, 0)
+    assert plan(8192, 5120, 1280) == (256, 0, 0)
+    assert plan(8192, 3840, 1280) == (256, 0, 0)
+    # a single 128-row tile with a short N: narrow tiles spread it over more SMs
+    assert plan(64, 1280, 1280) == (64, 0, 0)
     # every answer is a legal configuration, on any SM count
-    for sms in (148, 132, 74):
+    for sms in (148, 132, 66):
         for m, n, k in [(8192, 1280, 5120), (300, 640, 64), (32768, 2560, 640), (2048, 1280, 1280), (12032, 512, 256)]:
             bn, two, tail = plan(m, n, k, sms)
-            assert bn in (64, 128, 256) and two in (0, 1) and tail in (0, 64, 128)
-            assert tail == 0 or (two == 1 and bn == 256)
+            assert bn in (64, 128, 256) and two == 0 and tail == 0
 
 
 def test_product_never_imports_oracle():

@@ -1,6 +1,8 @@
 """Attention core (ref/src/modules.py:12-19, ref/utils/alter_attention.py:19-36) through the C ABI (pb200_attention) against an
-fp32 torch restatement on the same fp16-rounded q/k/v: the tcgen05/TMEM kernel (head_dim 80, csrc/attention_tc.cu) on the
-shapes of BASELINE configs 2 and 4, the mma.sync kernel on everything else, and the two kernels against each other."""
+fp32 torch restatement on the same fp16-rounded q/k/v: the shapes of BASELINE configs 2 and 4, the shapes with ragged or
+shared conditioning and ring wrap-around, and other head dims.  head_dim 80 runs the wgmma + TMA kernel (csrc/attention_wg.cu) by
+default; PB200_ATTN_MMA_SYNC=1 (child process) sends it to the flash-style mma.sync kernel (csrc/attention.cu), which every
+other head dim runs, so both kernels stay covered on every shape."""
 import json
 import os
 import subprocess
@@ -80,7 +82,7 @@ def _run(B, P, S, H, hd, self_attn, varlen, weighted, seed=0):
 TC_CASES = [
     (4, 64, 132, 16, 80, True, False, False),      # BASELINE config 2, level 1: 196 keys, 2 S accumulators, 2 K/V stages
     (3, 16, 132, 16, 80, True, True, False),       # config 2, level 2: 16 queries in a 64-row tile
-    (2, 256, 136, 16, 80, True, True, False),      # config 4, level 1: 392 keys -> mma.sync by default, attention_tc with PB200_ATTN_TC_WIDE
+    (2, 256, 136, 16, 80, True, True, False),      # config 4, level 1: 392 keys
     (2, 64, 136, 16, 80, True, False, True),       # config 4, level 2 + attn_weights
     (5, 64, 20, 4, 80, False, True, False),        # cross-attention only, short ragged conditioning
     (2, 128, 7, 2, 80, True, False, False),        # two query tiles, odd conditioning length
@@ -88,7 +90,7 @@ TC_CASES = [
 ]
 
 
-# shapes of the transposed kernel (csrc/attention_tt.cu: <= 64 queries, <= 256 keys, no attn_weights) beyond those in TC_CASES
+# <= 64 queries, <= 256 keys, no attn_weights: ragged key tiles, one key tile, the 256-key edge, many units
 TT_CASES = [
     (6, 64, 100, 4, 80, True, True, False),        # ragged: some samples end inside key tile 0 (tile 1 fully masked), some in tile 1
     (3, 32, 12, 2, 80, True, False, False),        # one key tile (48 keys), 32 queries in the 64-wide N
@@ -99,37 +101,37 @@ TT_CASES = [
 
 @pytest.mark.parametrize("case", TC_CASES + TT_CASES)
 def test_tcgen05_attention_vs_fp32_reference(case):
-    """The default dispatch: attention_tt for <= 64 queries / <= 256 keys without attn_weights, attention_tc otherwise."""
+    """The default dispatch on every head_dim-80 shape of the workloads: the wgmma + TMA kernel."""
     mx, rms, _ = _run(*case)
-    _log({"kernel": "tcgen05", "case": case, "max_abs": mx, "rms": rms})
+    _log({"kernel": "wgmma", "case": case, "max_abs": mx, "rms": rms})
     assert mx < 4e-3 and rms < 4e-4, (case, mx, rms)      # outputs are O(1): fp16 P and fp16 output rounding
 
 
 def test_tcgen05_row_major_kernel_on_the_transposed_kernels_shapes():
-    """PB200_ATTN_NO_TT=1 (child process) sends every head_dim-80 shape to attention_tc.cu: it stays covered on the shapes the
-    transposed kernel normally takes."""
+    """PB200_ATTN_MMA_SYNC=1 (child process) sends every head_dim-80 shape to the mma.sync kernel: the second kernel stays
+    covered on the shapes the wgmma kernel normally takes."""
     here = os.path.dirname(os.path.abspath(__file__))
-    cases = [c for c in TC_CASES + TT_CASES if not c[7]]       # incl. the > 256-key shape (PB200_ATTN_TC_WIDE), mma.sync by default
+    cases = [c for c in TC_CASES + TT_CASES if not c[7]]
     code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import test_gpu_attention as t\n"
             "for c in %r:\n    mx, rms, _ = t._run(*c); print('RES', mx, rms)") % (os.path.dirname(here), here, cases)
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=dict(os.environ, PB200_ATTN_NO_TT="1", PB200_ATTN_TC_WIDE="1"))
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=dict(os.environ, PB200_ATTN_MMA_SYNC="1"))
     assert r.returncode == 0, r.stderr[-2000:]
     res = [tuple(float(x) for x in l.split()[1:]) for l in r.stdout.splitlines() if l.startswith("RES")]
     assert len(res) == len(cases)
     for c, (mx, rms) in zip(cases, res):
-        _log({"kernel": "tcgen05-rowmajor", "case": c, "max_abs": mx, "rms": rms})
+        _log({"kernel": "mma.sync", "case": c, "max_abs": mx, "rms": rms})
         assert mx < 4e-3 and rms < 4e-4, (c, mx, rms)
 
 
 @pytest.mark.parametrize("case", [(2, 64, 9, 4, 16, True, False, False), (2, 16, 20, 4, 32, True, True, True),
                                   (2, 100, 30, 2, 64, True, False, False), (3, 64, 132, 16, 80, True, True, False)])
 def test_mma_sync_attention_vs_fp32_reference(case):
-    """Other head dims / query counts run the mma.sync kernel; with PB200_ATTN_LEGACY=1 (child process) so does head_dim 80."""
+    """Other head dims run the mma.sync kernel; with PB200_ATTN_MMA_SYNC=1 (child process) so does head_dim 80."""
     if case[4] == 80:
         code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import test_gpu_attention as t; "
                 "mx, rms, _ = t._run(*%r); print(mx, rms)") % (os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                                                                os.path.dirname(os.path.abspath(__file__)), case)
-        r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=dict(os.environ, PB200_ATTN_LEGACY="1"))
+        r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=dict(os.environ, PB200_ATTN_MMA_SYNC="1"))
         assert r.returncode == 0, r.stderr[-2000:]
         mx, rms = (float(x) for x in r.stdout.split()[-2:])
     else:

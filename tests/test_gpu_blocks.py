@@ -64,7 +64,7 @@ def test_resblock_standalone(c, skip, hw, B):
     assert got.shape == x.shape and got.dtype == torch.float32
     mx, rms = _errs(got, want)
     _log("resblock", {"c": c, "skip": skip, "hw": hw, "max_abs": mx, "rms": rms})
-    assert mx < 6e-3 and rms < 1.2e-3, (mx, rms)         # measured <= 2.0e-3 / 3.9e-4 (profiles/r01_block_parity.jsonl)
+    assert mx < 6e-3 and rms < 1.2e-3, (mx, rms)
 
 
 def test_feedforward_standalone():
@@ -76,7 +76,7 @@ def test_feedforward_standalone():
     got = blk.to(DEV)(x.to(DEV))
     mx, rms = _errs(got, want)
     _log("feedforward", {"max_abs": mx, "rms": rms})
-    assert mx < 6e-3 and rms < 1.2e-3, (mx, rms)         # measured <= 2.0e-3 / 3.9e-4 (profiles/r01_block_parity.jsonl)
+    assert mx < 6e-3 and rms < 1.2e-3, (mx, rms)
 
 
 def test_timestep_standalone():
@@ -107,7 +107,7 @@ def test_attnblock_standalone(c, nhead, hw, S, self_attn, weighted):
     got = blk(x.to(DEV), kv.to(DEV), **({"attn_weights": aw.to(DEV)} if weighted else {}))
     mx, rms = _errs(got, want)
     _log("attnblock", {"c": c, "hw": hw, "S": S, "self_attn": self_attn, "weighted": weighted, "max_abs": mx, "rms": rms})
-    assert mx < 2.5e-3 and rms < 6e-4, (mx, rms)         # measured <= 8.5e-4 / 1.9e-4 (profiles/r01_block_parity.jsonl)
+    assert mx < 2.5e-3 and rms < 6e-4, (mx, rms)
 
 
 def test_attention2d_standalone():
@@ -126,7 +126,7 @@ def test_attention2d_standalone():
         blk = blk.cpu()
         mx, rms = _errs(got, want)
         _log("attention2d", {"self_attn": self_attn, "max_abs": mx, "rms": rms})
-        assert mx < 1.4e-3 and rms < 3e-4, (mx, rms)         # measured <= 4.4e-4 / 1.0e-4
+        assert mx < 1.4e-3 and rms < 3e-4, (mx, rms)
 
 
 @pytest.mark.parametrize("affine,eps", [(False, 1e-6), (True, 1e-5)])

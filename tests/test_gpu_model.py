@@ -5,8 +5,7 @@
 Tolerances: the CUDA path rounds GEMM operands to fp16 (fp32 accumulate, fp32 residual stream).  Emulating
 exactly that rounding in the oracle (oracle.paella_oracle.mm_f16_operands) moves the default model's logits
 (std 0.18) by 8e-4 max / 1.4e-4 rms; the kernels add fp16 storage of the MLP hidden, q/k/v and softmax
-weights.  Bounds below are <= 3x what was measured on B200 (profiles/r01_model_parity_final.jsonl): default 1.008 B model
-7.4e-4 / 1.3e-4 (max-abs / rms; logit std 0.177) -> 2.5e-3 / 4e-4; tiny golden model 2.7e-3 / 4.2e-4 -> 7e-3 / 1.2e-3.
+weights.  Bounds below (max-abs / rms): default 1.008 B model (logit std 0.177) 2.5e-3 / 4e-4; tiny golden model 7e-3 / 1.2e-3.
 """
 import json
 import os
@@ -81,7 +80,7 @@ def test_tiny_r_and_c_embeddings_match_reference_golden(tiny):
     assert ce.shape == tuple(g["c_embed"].shape)
     mx, rms = _errs(ce, t(g["c_embed"]))
     _log("tiny_c_embed", {"max_abs": mx, "rms": rms})
-    assert mx < 3.5e-3 and rms < 9e-4          # measured 1.26e-3 / 3.0e-4
+    assert mx < 3.5e-3 and rms < 9e-4
     ce2 = m.gen_c_embeddings(t(g["byt5"]).to(DEV), None, [t(g["clip_image"]).to(DEV)] * 2)
     assert ce2.shape == (2, 5 + 8, cfg["c_cond"])
 

@@ -115,7 +115,7 @@ def test_cfg1_default_sample_vs_oracle_per_step_with_margin_audit(default_model)
             nb, gap = _margin_audit(flat, temp, qs[i], want, got)
             bound = 2 * (abs(cfg) + abs(1 - cfg)) * MAX_ABS_D / temp
             per_step.append({"step": i, "T": temp, "agree": agree, "mismatches": nb, "worst_gap": gap, "gap_bound": bound})
-            assert agree >= 0.99, per_step[-1]          # measured: 99.5 % at the T = 0.2 step, 99.9-100 % elsewhere; every mismatch audited below
+            assert agree >= 0.99, per_step[-1]
             assert gap <= bound, per_step[-1]
             worst_gap, n_bad = max(worst_gap, gap), n_bad + nb
             state = want
@@ -176,7 +176,7 @@ def test_vq_indices_vs_torchtools_addmm_form_with_margin_audit():
     addmm(|c|^2 + |x|^2, x, c^T, alpha=-2) -> first minimum), not vs an oracle that copies the kernel's fma order.  The two
     evaluate the same real-valued distance with different fp32 roundings, so exact equality is not implied; every disagreement
     must be a tie within the rounding noise of the expanded form (a sum of ~6 fp32 roundings per entry, two entries):
-    |d_a - d_b| <= 4 ulp(|x|^2 + |c|^2) (measured on B200: 0.74 ulp worst, 6 mismatches in 350 000 vectors)."""
+    |d_a - d_b| <= 4 ulp(|x|^2 + |c|^2)."""
     from oracle import vqgan_oracle as vo
     from paella_b200 import ops
     g = torch.Generator().manual_seed(5)

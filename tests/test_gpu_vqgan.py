@@ -118,7 +118,7 @@ def test_f4_roundtrip_vs_oracle(f4):
     assert lat_err < 2e-2
     assert agree > 0.98 and worst < 5e-2
     # north_star: decoded RGB within 1e-3 abs of fp32.  fp16 operands + fp32 accumulation predict 8.4e-4 max on this
-    # input (oracle with fp16-rounded operands); measured on B200: 7.4e-4 (profiles/r01_vqgan_parity.jsonl).
+    # input (oracle with fp16-rounded operands).
     assert dec_err < 1e-3
 
 

@@ -1,11 +1,9 @@
 """Static checks on the SASS of the built library (cuobjdump; no GPU needed).
 
-  * the tensor-core / TMA kernels really are Blackwell-native: tcgen05.mma (UTCHMMA), TMA tensor loads (UTMALDG) and
-    TMEM loads (LDTM) in every GEMM variant, the fused sampler and both tcgen05 attention kernels (VERDICT r1: the attention core
-    was an mma.sync kernel);
+  * the tensor-core / TMA kernels really are Hopper-native: warpgroup MMA (HGMMA) fed by TMA tensor loads (UTMALDG) in every
+    GEMM variant, both fused sampler kernels and the head_dim-80 attention core, no mma.sync (HMMA) among them;
   * no `ELECT ... BRA.U.ANY` uniformisation loop around a single-thread instruction: the single-thread regions are entered through
-    elect.sync (ptx::elect_one), see DESIGN.md section 3 -- with `lane == 0` nvcc wraps every tcgen05.mma / commit / TMA issue in
-    such a loop (~110 cycles per 50-cycle MMA in the attention kernel's timeline).
+    elect.sync (ptx::elect_one), see DESIGN.md section 3 -- with `lane == 0` nvcc wraps every TMA issue in such a loop.
 """
 import collections
 import os
@@ -39,18 +37,32 @@ def census():
     return counts
 
 
-def _kernels(census, needle):
-    return {k: v for k, v in census.items() if needle in k}
+def _kernels(census, pattern):
+    return {k: v for k, v in census.items() if re.search(pattern, k)}
 
 
-@pytest.mark.parametrize("needle", ["gemm_f16_cg2_kernel", "gemm_f16_kernel", "fused_sampler", "attention_tt_kernel", "attention_tc_kernel",
-                                    "vq_mlp_fused_kernel"])
-def test_tensor_core_kernels_are_tcgen05_and_tma(census, needle):
+# the tensor-core kernels, one parameter per family of template instances (mangled names:
+# gemm_f16_kernel<BLOCK_N, MODE, AMODE, ASCALE> = gemm_f16_kernelILi<BLOCK_N>ELi<MODE>ELi<AMODE>ELb<ASCALE>E)
+WGMMA_VARIANTS = [
+    pytest.param(r"gemm_f16_kernelILi64E", id="gemm_f16_kernel_bn64"),
+    pytest.param(r"gemm_f16_kernelILi128E", id="gemm_f16_kernel_bn128"),
+    pytest.param(r"gemm_f16_kernelILi256E", id="gemm_f16_kernel_bn256"),
+    pytest.param(r"gemm_f16_kernelILi\d+ELi\d+ELi1E", id="gemm_f16_kernel_conv_k4s2"),
+    pytest.param(r"gemm_f16_kernelILi\d+ELi\d+ELi2E", id="gemm_f16_kernel_convT_k4s2"),
+    pytest.param(r"gemm_f16_kernelILi\d+ELi\d+ELi0ELb1E", id="gemm_f16_kernel_a_scale"),
+    pytest.param(r"fused_sampler_kernel", id="fused_sampler_kernel"),
+    pytest.param(r"fused_sampler_shared_kernel", id="fused_sampler_shared_kernel"),
+    pytest.param(r"attention_wgmma_kernel", id="attention_wgmma_kernel"),
+]
+
+
+@pytest.mark.parametrize("needle", WGMMA_VARIANTS)
+def test_tensor_core_kernels_are_wgmma_and_tma(census, needle):
     ks = _kernels(census, needle)
     assert ks, f"no kernel matching {needle} in the library"
     for name, c in ks.items():
-        assert c["UTCHMMA"] > 0 and c["UTMALDG"] > 0 and c["LDTM"] > 0, (name, dict(c))
-        assert c["HMMA"] == 0, f"{name}: mma.sync instructions in a tcgen05 kernel"
+        assert c["HGMMA"] > 0 and c["UTMALDG"] > 0, (name, dict(c))
+        assert c["HMMA"] == 0, f"{name}: mma.sync instructions in a wgmma kernel"
 
 
 def test_attention_fallback_is_the_only_mma_sync_kernel(census):
@@ -58,10 +70,11 @@ def test_attention_fallback_is_the_only_mma_sync_kernel(census):
     assert hmma and all("attention_kernel" in k for k in hmma), hmma
 
 
-@pytest.mark.parametrize("needle", ["gemm_f16_cg2_kernel", "gemm_f16_kernel", "fused_sampler", "attention_tt_kernel", "attention_tc_kernel",
-                                    "vq_mlp_fused_kernel"])
+@pytest.mark.parametrize("needle", ["gemm_f16_kernel", "fused_sampler"] + WGMMA_VARIANTS)
 def test_single_thread_regions_have_no_uniformisation_loops(census, needle):
-    for name, c in _kernels(census, needle).items():
+    ks = _kernels(census, needle)
+    assert ks, f"no kernel matching {needle} in the library"
+    for name, c in ks.items():
         # a handful remain around mbarrier arrivals / trace hooks guarded by `lane == 0`; none may sit on an MMA or TMA issue path:
         # far fewer loops than tensor-core + TMA instructions
-        assert c["BRA.U.ANY"] <= 2, (name, c["BRA.U.ANY"], c["UTCHMMA"], c["UTMALDG"])
+        assert c["BRA.U.ANY"] <= 2, (name, c["BRA.U.ANY"], c["HGMMA"], c["UTMALDG"])

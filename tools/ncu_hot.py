@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Top stall lines of one kernel in an ncu report (SASS view): python tools/ncu_hot.py rep kernel-id-filter [N]
-   e.g. python tools/ncu_hot.py gpurun_out/x.ncu-rep ::regex:dwconv3:3 25"""
+   e.g. python tools/ncu_hot.py x.ncu-rep ::regex:dwconv3:3 25"""
 import csv
 import io
 import subprocess

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarise `ncu --set full` reports: python tools/ncu_summary.py a.ncu-rep [b.ncu-rep ...] > profiles/x.md"""
+"""Summarise `ncu --set full` reports: python tools/ncu_summary.py a.ncu-rep [b.ncu-rep ...] > x.md"""
 import csv
 import io
 import subprocess

@@ -1,9 +1,9 @@
 #!/bin/bash
-# compute-sanitizer over the hand-rolled mbarrier / TMEM / TMA kernels (python launched DIRECTLY under the tool; attach mode
-# is what failed in round 1).  Small shapes only: the tools run kernels 10-100x slower.
-#   bash tools/sanitize.sh <tag>  ->  gpurun_out/<tag>_memcheck.log, <tag>_racecheck.log, <tag>_synccheck.log
-TAG=${1:-r2}
-O=gpurun_out
+# compute-sanitizer over the hand-rolled mbarrier / TMA / wgmma kernels (python launched DIRECTLY under the tool, not in
+# attach mode).  Small shapes only: the tools run kernels 10-100x slower.
+#   bash tools/sanitize.sh <tag> [outdir]  ->  <outdir>/<tag>_memcheck.log, <tag>_racecheck.log, <tag>_synccheck.log
+TAG=${1:-san}
+O=${2:-/tmp/paella_sanitize}
 mkdir -p $O
 cat > /tmp/san_case.py <<'PY'
 import os, sys, math, torch
@@ -11,7 +11,7 @@ sys.path.insert(0, os.getcwd()); sys.path.insert(0, os.path.join(os.getcwd(), "t
 from paella_b200 import _lib, ops
 DEV = "cuda"
 g = torch.Generator(device=DEV).manual_seed(0)
-# tcgen05 GEMMs: 1-SM and 2-SM kernels, GELU+sqsum, RESID (+a_scale), LN fold
+# wgmma GEMMs: every tile width, GELU+sqsum, RESID (+a_scale), LN fold
 for (M, N, K) in [(128, 128, 64), (300, 136, 128), (512, 256, 128)]:
     a = torch.randn(M, K, device=DEV, generator=g).half(); w = (torch.randn(N, K, device=DEV, generator=g) / math.sqrt(K)).half()
     bias = torch.randn(N, device=DEV, generator=g)
@@ -19,14 +19,14 @@ for (M, N, K) in [(128, 128, 64), (300, 136, 128), (512, 256, 128)]:
     o16 = torch.zeros(M, N, device=DEV, dtype=torch.float16); sq = torch.zeros(max(1, M // 4), N, device=DEV, dtype=torch.int64)
     ops.gemm_f16(a, w, _lib.EPI_GELU_F16, o16, bias=bias, sqsum=sq, rows_per_sample=4)
     x = torch.randn(M, N, device=DEV, generator=g); ops.gemm_f16(a, w, _lib.EPI_RESID_F32, x, bias=bias, resid=x)
-M, N, K, P = 2048, 1280, 640, 16          # a shape the planner puts on 256-wide 2-SM tiles (the a_scale path)
+M, N, K, P = 2048, 1280, 640, 16          # the a_scale path
 a = torch.randn(M, K, device=DEV, generator=g).half(); w = (torch.randn(N, K, device=DEV, generator=g) / math.sqrt(K)).half()
 x = torch.randn(M, N, device=DEV, generator=g); s = (1 + 0.3 * torch.randn(M // P, K, device=DEV, generator=g)).half()
 ops.gemm_f16(a, w, _lib.EPI_RESID_F32, x, bias=None, resid=x, rows_per_sample=P, a_scale=s)
-# attention: tcgen05 kernel (head_dim 80) and mma.sync kernel
+# attention: wgmma kernel (head_dim 80) and mma.sync kernel
 import test_gpu_attention as ta
-print("attn tc", ta._run(2, 64, 20, 2, 80, True, True, False)[:2])
-print("attn tc P=16", ta._run(2, 16, 12, 2, 80, True, False, True)[:2])
+print("attn wgmma", ta._run(2, 64, 20, 2, 80, True, True, False)[:2])
+print("attn wgmma P=16", ta._run(2, 16, 12, 2, 80, True, False, True)[:2])
 print("attn mma", ta._run(2, 16, 12, 2, 32, True, True, False)[:2])
 # codec ResBlock front (row statistics + patch kernel), partial patches
 from paella_b200.vqgan import ResBlock

@@ -1,12 +1,11 @@
 #!/usr/bin/env python
-"""Census of the Blackwell-specific SASS mnemonics per kernel of the built library (cuobjdump -sass; no GPU needed):
-   python tools/sass_census.py > profiles/r01_sass_census.md"""
+"""Census of the tensor-core / TMA / synchronisation SASS mnemonics per kernel of the built library (cuobjdump -sass; no GPU
+needed):  python tools/sass_census.py > sass_census.md"""
 import collections
 import re
 import subprocess
 
-KEYS = ["UTCHMMA", "UTCHMMA.2CTA", "UTMALDG", "UTMALDG.MULTICAST", "UTCBAR", "LDTM", "UTCATOMSWS", "SYNCS", "HMMA", "LDSM", "LDGSTS",
-        "ACQBULK", "PREEXIT", "REDG", "ATOMG", "MUFU", "SHFL"]
+KEYS = ["HGMMA", "WARPGROUP", "UTMALDG", "SYNCS", "HMMA", "LDSM", "LDGSTS", "ACQBULK", "PREEXIT", "REDG", "ATOMG", "MUFU", "SHFL"]
 out = subprocess.run(["cuobjdump", "-sass", "paella_b200/libpaella_b200.so"], capture_output=True, text=True).stdout
 fn, counts = None, collections.OrderedDict()
 for line in out.splitlines():
@@ -25,14 +24,10 @@ for line in out.splitlines():
         base = op.split(".")[0]
         if base in KEYS:
             counts[fn][base] += 1
-        if base == "UTCHMMA" and ".2CTA" in op:
-            counts[fn]["UTCHMMA.2CTA"] += 1
-        if base == "UTMALDG" and "MULTICAST" in op:
-            counts[fn]["UTMALDG.MULTICAST"] += 1
-print("# SASS census of `paella_b200/libpaella_b200.so` (sm_100a)\n")
-print("`cuobjdump -sass`, static instruction counts per kernel.  UTCHMMA = tcgen05.mma (`.2CTA` = cta_group::2), UTMALDG = TMA")
-print("tensor load, LDTM = tcgen05.ld (TMEM -> registers), UTCBAR = tcgen05.commit, SYNCS = mbarrier ops, ACQBULK / PREEXIT =")
-print("griddepcontrol.wait / launch_dependents, HMMA/LDSM/LDGSTS = mma.sync / ldmatrix / cp.async (attention core).\n")
+print("# SASS census of `paella_b200/libpaella_b200.so` (sm_90a)\n")
+print("`cuobjdump -sass`, static instruction counts per kernel.  HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / commit /")
+print("wait, UTMALDG = TMA tensor load, SYNCS = mbarrier ops, ACQBULK / PREEXIT = griddepcontrol.wait / launch_dependents,")
+print("HMMA/LDSM/LDGSTS = mma.sync / ldmatrix / cp.async (the mma.sync attention kernel).\n")
 cols = [k for k in KEYS if any(c[k] for c in counts.values())]
 print("| kernel | instr | " + " | ".join(cols) + " |")
 print("|---|---:|" + "---:|" * len(cols))

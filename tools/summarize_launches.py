@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Aggregate an `ncu --metrics gpu__time_duration.sum --csv` launch list by kernel -> markdown table.
-usage: python tools/summarize_launches.py gpurun_out/launches_r01.csv profiles/r01_launches_summary.md "title" """
+usage: python tools/summarize_launches.py launches.csv launches_summary.md "title" """
 import collections
 import csv
 import re
