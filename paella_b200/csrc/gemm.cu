@@ -291,15 +291,20 @@ __device__ __forceinline__ void epilogue_chunk(const pb200_gemm_epilogue& ep, in
                 for (int j = 0; j < 32; ++j) v[j] = (row_ok && col0 + j < N) ? v[j] * v[j] : 0.f;
             }
             if ((P & 31) == 0) {
-                // transpose-reduce over the warp's 32 rows: lane j ends with the column-(col0+j) sum
+                // transpose-reduce over the warp's 32 rows: lane j ends with the column-(col0+j) sum.  The loops have
+                // fixed trip counts so that they unroll completely: with `o >>= 1` nvcc kept a rolled loop that indexes v[]
+                // at run time, which put v[] in local memory (a 128-byte stack frame, STL/LDL in every chunk).
 #pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
+                for (int step = 0; step < 5; ++step) {
+                    const int o = 16 >> step;
+                    const bool up = (lane & o) != 0;
 #pragma unroll
-                    for (int i = 0; i < o; ++i) {
-                        const bool up = (lane & o) != 0;
-                        const float send = up ? v[i] : v[i + o];
-                        const float keep = up ? v[i + o] : v[i];
-                        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+                    for (int i = 0; i < 16; ++i) {
+                        if (i < o) {
+                            const float send = up ? v[i] : v[i + o];
+                            const float keep = up ? v[i + o] : v[i];
+                            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+                        }
                     }
                 }
                 const int row0 = row - lane;
@@ -311,16 +316,20 @@ __device__ __forceinline__ void epilogue_chunk(const pb200_gemm_epilogue& ep, in
                 // (~30 shuffles and 32/P atomics per lane instead of 32 x log2(P) shuffles and 32 atomics)
                 auto grouped = [&](auto pc) {
                     constexpr int PP = decltype(pc)::value;
+                    constexpr int LOG_PP = PP == 16 ? 4 : PP == 8 ? 3 : PP == 4 ? 2 : 1;
 #pragma unroll
-                    for (int o = PP / 2; o > 0; o >>= 1) {
+                    for (int step = 0; step < LOG_PP; ++step) {       // fixed trip counts: see the branch above
+                        const int o = (PP / 2) >> step;
                         const bool up = (lane & o) != 0;
 #pragma unroll
                         for (int j = 0; j < 32 / PP; ++j)
 #pragma unroll
-                            for (int i = 0; i < o; ++i) {
-                                const float send = up ? v[j * PP + i] : v[j * PP + i + o];
-                                const float keep = up ? v[j * PP + i + o] : v[j * PP + i];
-                                v[j * PP + i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+                            for (int i = 0; i < PP / 2; ++i) {
+                                if (i < o) {
+                                    const float send = up ? v[j * PP + i] : v[j * PP + i + o];
+                                    const float keep = up ? v[j * PP + i + o] : v[j * PP + i];
+                                    v[j * PP + i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
+                                }
                             }
                     }
                     const int grow = row - (lane & (PP - 1));          // first row of this lane's sample
@@ -759,7 +768,8 @@ int gemm_pick_block_n(int64_t M, int64_t N, int64_t K) {
     //   tensor   : waves x k-blocks x 128 x BLOCK_N x 64 MACs at ~2048 fp16 MACs per clock and SM (989 TFLOP/s, 132 SMs)
     //   L2->SM   : all tiles' operand bytes (per k-block the 128x64 A tile and BLOCK_N x 64 of W) at ~3000 B/clk
     //   per tile : ~2000 cycles of fill/drain + the epilogue, which does not overlap the main loop
-    // and pick the minimum.
+    // and pick the minimum.  tools/gemm_sweep.py measures the per-tile term of 256-wide tiles at 4-22 us (8-40 k cycles)
+    // depending on the epilogue; it has not been measured for the narrower widths, so the model keeps its data-sheet constants.
     static const int force = getenv("PB200_FORCE_BN") ? atoi(getenv("PB200_FORCE_BN")) : 0;   // experiments only
     if (force == 64 || force == 128 || force == 256) return force;
     const int sms = plan_sm_count();

@@ -35,14 +35,19 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
     return t;
 }
 // Wait with a watchdog: a pipeline bug must trap (kernel error) instead of hanging the GPU.
+// The release build traps without a message.  printf is a call to vprintf, and ptxas serialises every wgmma of a kernel that
+// contains a function call (warning C7510: each MMA waits for the previous one to retire; the GEMM main loop ran 10-20 %
+// slower, the fused samplers and the wgmma attention too).  Build with -DPB200_MBAR_DEBUG to name the barrier.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     const uint64_t t0 = globaltimer_ns();
     uint32_t spins = 0;
     while (!mbar_try_wait(bar, parity)) {
         if ((++spins & 0x3ff) == 0 && globaltimer_ns() - t0 > 4000000000ull) {   // 4 s
+#ifdef PB200_MBAR_DEBUG
             printf("paella_b200: mbarrier wait timed out (block %d thread %d bar %u parity %u)\n", blockIdx.x,
                    threadIdx.x, bar, parity);
+#endif
             __trap();
         }
     }
