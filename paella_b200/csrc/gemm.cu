@@ -770,7 +770,8 @@ int gemm_pick_block_n(int64_t M, int64_t N, int64_t K) {
     //   per tile : ~2000 cycles of fill/drain + the epilogue, which does not overlap the main loop
     // and pick the minimum.  tools/gemm_sweep.py measures the per-tile term of 256-wide tiles at 4-22 us (8-40 k cycles)
     // depending on the epilogue; it has not been measured for the narrower widths, so the model keeps its data-sheet constants.
-    static const int force = getenv("PB200_FORCE_BN") ? atoi(getenv("PB200_FORCE_BN")) : 0;   // experiments only
+    // test hook: pins every launch of the process to one width (tests/test_gpu_gemm_matrix.py runs each width in a child)
+    static const int force = getenv("PB200_FORCE_BN") ? atoi(getenv("PB200_FORCE_BN")) : 0;
     if (force == 64 || force == 128 || force == 256) return force;
     const int sms = plan_sm_count();
     const long n_kb = K > 0 ? (long)ceil_div(K, GEMM_BLOCK_K) : 16;

@@ -1,11 +1,21 @@
-"""Shared test helpers: golden fixture loading, config parsing."""
+"""Shared test helpers: golden fixture loading, config parsing, per-case result logs."""
 import ast
+import json
 import os
+import tempfile
 
 import numpy as np
 import torch
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+def log_jsonl(name, payload):
+    """Append one JSON row to <name> in $PB200_TEST_LOG_DIR (default: paella_b200_test_logs under the system temp directory)."""
+    d = os.environ.get("PB200_TEST_LOG_DIR") or os.path.join(tempfile.gettempdir(), "paella_b200_test_logs")
+    os.makedirs(d, exist_ok=True)
+    with open(os.path.join(d, name), "a") as f:
+        f.write(json.dumps(payload) + "\n")
 
 
 def load_golden(name):
