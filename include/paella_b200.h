@@ -276,6 +276,16 @@ int pb200_paella_sample_tokens(pb200_paella* m, const float* features, int batch
                                double temperature, uint64_t seed, uint64_t offset, int64_t* tokens_out,
                                void* workspace, int64_t workspace_bytes, void* stream);
 
+/* pb200_paella_sample_tokens with one random stream per sample, in ONE launch over the batch (a list of per-sample
+ * torch.Generators).  seed_offset: DEVICE uint64 [batch][2] = (seed, philox offset) of sample b's generator before the
+ * draw; offsets are multiples of 4.  Sample b's rows draw exactly what pb200_paella_sample_tokens(batch = 1) draws on
+ * (seed, offset) = seed_offset[b], through the same kernel family and MMA shape, and each generator is to be advanced by
+ * pb200_philox_offset_increment(hw * num_labels).  hw * num_labels <= 2^29 (torch would split a larger draw).
+ * pb200_paella_workspace_bytes(batch, ...) sizes the workspace. */
+int pb200_paella_sample_tokens_per_sample(pb200_paella* m, const float* features, int batch, int hw, int cfg_on, double cfg,
+                                          double temperature, const uint64_t* seed_offset, int64_t* tokens_out,
+                                          void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * VQGAN (ref/src/vqgan.py:45-107).
  * ------------------------------------------------------------------------------------------ */

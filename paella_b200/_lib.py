@@ -98,6 +98,8 @@ SIGNATURES = {
     "pb200_paella_logits": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_sample_tokens": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_uint64,
                                            c_uint64, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_sample_tokens_per_sample": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_void_p,
+                                                      c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_vqgan_create": (c_int, [POINTER(VqganConfig), POINTER(c_void_p)]),
     "pb200_vqgan_destroy": (None, [c_void_p]),
     "pb200_vqgan_weight_bytes": (c_int64, [c_void_p]),

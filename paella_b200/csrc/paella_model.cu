@@ -545,7 +545,8 @@ int64_t pb200_paella_workspace_bytes(const pb200_paella* m, int batch_total, int
     CondWs cw;
     plan_cond(m, batch_total, s_max, s_max, b, cw);
     // logits / sampling scratch: fp16 features for B*H*W rows
-    // fp16 features of the sampler; the shared-Philox kernel reads whole 4*rs-row blocks (rs <= 1184*256/num_labels + 1)
+    // fp16 features of the sampler; the shared-Philox kernel reads whole 4*rs-row blocks (rs <= 1184*256/num_labels + 1) --
+    // with per-sample streams, whole blocks of each sample, which overrun the batch's end by at most the same pad
     const int64_t pad_rows = 4 * ((int64_t)1184 * 256 / m->cfg.num_labels + 2);
     const int64_t samp = (((int64_t)batch_total * h * w + pad_rows) * m->cfg.c_out * 2 + 255) / 256 * 256;
     int64_t need = a.off > b.off ? a.off : b.off;
@@ -869,6 +870,28 @@ int pb200_paella_sample_tokens(pb200_paella* m, const float* features, int batch
         PB_TRY(launch_cast_f16(features, rows * c.c_out, a16, st));
     return launch_fused_sampler(a16, rows, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f / (float)temperature, seed,
                                 offset, tokens_out, st);
+}
+
+int pb200_paella_sample_tokens_per_sample(pb200_paella* m, const float* features, int batch, int hw, int cfg_on, double cfg,
+                                          double temperature, const uint64_t* seed_offset, int64_t* tokens_out, void* workspace,
+                                          int64_t workspace_bytes, void* stream) {
+    PB_CHECK(m->blob != nullptr, "sample_tokens_per_sample: weights not bound");
+    const pb200_paella_config& c = m->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+    PB_CHECK(batch >= 0 && hw >= 0, "sample_tokens_per_sample: bad shape");
+    const int64_t rows = (int64_t)batch * hw;
+    if (rows == 0) return 0;
+    // every sample's last 4*rs-row block may read past its end: at most rows_padded(hw) - hw rows past the last sample
+    PB_CHECK(((int64_t)(batch - 1) * hw + fused_sampler_rows_padded(hw, c.num_labels)) * c.c_out * 2 <= workspace_bytes,
+             "sample_tokens_per_sample: workspace too small (use pb200_paella_workspace_bytes)");
+    PB_CHECK(temperature > 0, "sample_tokens_per_sample: temperature must be positive");
+    __half* a16 = reinterpret_cast<__half*>(workspace);
+    if (cfg_on)
+        PB_TRY(launch_mix_cast_f16(features, features + rows * c.c_out, (float)cfg, (float)(1.0 - cfg), rows * c.c_out, a16, st));
+    else
+        PB_TRY(launch_cast_f16(features, rows * c.c_out, a16, st));
+    return launch_fused_sampler_per_sample(a16, batch, hw, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f / (float)temperature,
+                                           seed_offset, tokens_out, st);
 }
 
 }  // extern "C"

@@ -33,9 +33,19 @@ __device__ __forceinline__ void argmax_merge(float& bv, int& bi, float ov, int o
     if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
 }
 
+// PS (per-sample streams): the R rows are R / hw samples of hw rows; sample b draws on its own generator, (seed, philox
+// offset) = seed_off[2b], seed_off[2b + 1], with rng's stride (the launch policy of ONE sample's draw), and element
+// (row, col) of it is element (row - b hw) * NL + col of that draw -- what a batch-1 launch on that generator would use.
+__device__ __forceinline__ void per_sample_stream(const uint64_t* __restrict__ seed_off, int b, TorchPhilox& s) {
+    s.seed = seed_off[2 * b];
+    s.offset4 = seed_off[2 * b + 1] >> 2;
+}
+
+template <bool PS>
 __global__ void __launch_bounds__(SMP_THREADS, 1)
 fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, int R, int NL,
-                     int Kc, float inv_t, TorchPhilox rng, int64_t* __restrict__ out) {
+                     int Kc, float inv_t, TorchPhilox rng, int hw, const uint64_t* __restrict__ seed_off,
+                     int64_t* __restrict__ out) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t a_base = smem_base;
@@ -84,6 +94,19 @@ fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
         const int row0 = m_idx + cw * 64 + wq * 16 + (lane >> 2);
         float bv[2] = {-INFINITY, -INFINITY};
         int bi[2] = {0x7fffffff, 0x7fffffff};
+        TorchPhilox srng[2] = {rng, rng};
+        uint64_t ebase[2] = {0, 0};
+        if constexpr (PS) {
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const int row = row0 + 8 * rr;
+                if (row < R) {
+                    const int b = row / hw;
+                    per_sample_stream(seed_off, b, srng[rr]);
+                    ebase[rr] = (uint64_t)(row - b * hw) * (uint64_t)NL;
+                }
+            }
+        }
         float acc[SMP_BN / 2];
         ptx::mbar_wait(a_bar, 0);
         int stage = 0;
@@ -114,7 +137,9 @@ fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
                 const int row = row0 + 8 * rr;
                 const int col = ch * SMP_BN + (i >> 2) * 8 + 2 * (lane & 3) + (i & 1);
                 if (row < R && col < NL) {
-                    const float qv = torch_exponential1(u32_to_uniform(torch_philox_u32(rng, (uint64_t)row * (uint64_t)NL + (uint64_t)col)));
+                    const uint32_t bits = PS ? torch_philox_u32(srng[rr], ebase[rr] + (uint64_t)col)
+                                             : torch_philox_u32(rng, (uint64_t)row * (uint64_t)NL + (uint64_t)col);
+                    const float qv = torch_exponential1(u32_to_uniform(bits));
                     const float gum = fmaf(acc[i], inv_t, -__logf(qv));
                     if (gum > bv[rr]) { bv[rr] = gum; bi[rr] = col; }      // columns of a row arrive in increasing order
                 }
@@ -150,9 +175,14 @@ constexpr int SH_W_BYTES = 128 * 128;          // 128 labels x 64 halves
 constexpr int SH_RED_WARPS = 8;                // MMA warps, one reduction row each
 constexpr int SH_SMEM = SMP_MAX_KB * SH_F_BYTES + SH_STAGES * SH_W_BYTES + 1024 + 256 + SH_RED_WARPS * SH_N * 8;
 
+// PS: R / hw samples of hw rows, each with its own 4rs-row blocks (blocks_per_sample of them; the last one of a sample is
+// partial and never straddles into the next sample's draw) and its own stream (see per_sample_stream).  The token tile comes
+// through a 5-D map whose outermost coordinate is the sample; rows past a sample's end are loaded but never written.
+template <bool PS>
 __global__ void __launch_bounds__(SH_THREADS, 1)
 fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __grid_constant__ CUtensorMap tm_w, int R, int NL,
-                            int Kc, int rs, int tasks_per_block, float inv_t, TorchPhilox rng, int64_t* __restrict__ out) {
+                            int Kc, int rs, int tasks_per_block, float inv_t, TorchPhilox rng, int hw, int blocks_per_sample,
+                            const uint64_t* __restrict__ seed_off, int64_t* __restrict__ out) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -170,8 +200,10 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
     const int lane = threadIdx.x & 31;
     const int n_kb = (Kc + 63) / 64;
     const int n_chunks = (NL + 127) / 128;
-    const int blk = blockIdx.x / tasks_per_block;                      // 4rs-row block = Philox call index
-    const int jj0 = (blockIdx.x - blk * tasks_per_block) * SH_JJ;
+    const int sample = PS ? (int)(blockIdx.x / (blocks_per_sample * tasks_per_block)) : 0;
+    const int task = blockIdx.x - sample * blocks_per_sample * tasks_per_block;
+    const int blk = task / tasks_per_block;                            // 4rs-row block = Philox call index
+    const int jj0 = (task - blk * tasks_per_block) * SH_JJ;
 
     if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tm_f);
@@ -186,7 +218,10 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
         ptx::setmaxnreg_dec<40>();
         if (threadIdx.x < 32 && ptx::elect_one()) {
             ptx::mbar_arrive_expect_tx(f_bar, n_kb * SH_F_BYTES);
-            for (int kb = 0; kb < n_kb; ++kb) ptx::tma_load_4d(&tm_f, f_bar, f_base + kb * SH_F_BYTES, kb * 64, 0, jj0, blk);
+            for (int kb = 0; kb < n_kb; ++kb) {
+                if constexpr (PS) ptx::tma_load_5d(&tm_f, f_bar, f_base + kb * SH_F_BYTES, kb * 64, 0, jj0, blk, sample);
+                else ptx::tma_load_4d(&tm_f, f_bar, f_base + kb * SH_F_BYTES, kb * 64, 0, jj0, blk);
+            }
             int stage = 0;
             uint32_t phase = 0;
             for (int ch = 0; ch < n_chunks; ++ch)
@@ -210,6 +245,8 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
         int bi[SH_N / 2];
 #pragma unroll
         for (int i = 0; i < SH_N / 2; ++i) { bv[i] = -INFINITY; bi[i] = 0x7fffffff; }
+        TorchPhilox srng = rng;
+        if constexpr (PS) per_sample_stream(seed_off, sample, srng);
         float acc[SH_N / 2];
         ptx::mbar_wait(f_bar, 0);
         int stage = 0;
@@ -249,7 +286,7 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
                 v[3] = odd ? acc[4 * n + 3] : r1;
                 if (label < NL) {
                     const int jj = jj0 + 2 * n + (q >> 1);
-                    const uint4 r4 = torch_philox_call(rng, (uint64_t)jj * (uint64_t)NL + (uint64_t)label, (uint64_t)blk);
+                    const uint4 r4 = torch_philox_call(srng, (uint64_t)jj * (uint64_t)NL + (uint64_t)label, (uint64_t)blk);
                     const uint32_t bits[4] = {r4.x, r4.y, r4.z, r4.w};
 #pragma unroll
                     for (int g = 0; g < 4; ++g) {
@@ -288,8 +325,12 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
 #pragma unroll
             for (int w = 1; w < SH_RED_WARPS; ++w) argmax_merge(best, besti, red_v[w * SH_N + t], red_i[w * SH_N + t]);
             const int jj = jj0 + t / 4, g = t & 3;
-            const int64_t row = (int64_t)blk * 4 * rs + (int64_t)g * rs + jj;
-            if (jj < rs && row < R) out[row] = besti;
+            const int64_t row = (int64_t)blk * 4 * rs + (int64_t)g * rs + jj;      // within the sample (PS) or the launch
+            if constexpr (PS) {
+                if (jj < rs && row < hw) out[(int64_t)sample * hw + row] = besti;
+            } else {
+                if (jj < rs && row < R) out[row] = besti;
+            }
         }
     }
 }
@@ -301,49 +342,85 @@ int64_t fused_sampler_rows_padded(int64_t R, int NL) {
     return (R + 4 * rs - 1) / (4 * rs) * (4 * rs);
 }
 
-int launch_fused_sampler(const __half* a16, int64_t R, int Kc, const __half* w16, int NL, float inv_t, uint64_t seed,
-                         uint64_t offset, int64_t* out, cudaStream_t st) {
-    PB_CHECK(Kc % 8 == 0 && Kc <= 64 * SMP_MAX_KB, "fused sampler: c_out=%d unsupported (<= %d, multiple of 8)", Kc, 64 * SMP_MAX_KB);
-    PB_CHECK(R * (int64_t)NL < (1ll << 31), "fused sampler: rows*labels >= 2^31 would split the torch kernel (unsupported)");
-    PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
-    if (R == 0) return 0;
+// One launch over n_samp streams of hw rows each: n_samp == 1 with seed_off == nullptr is the single-stream draw (seed,
+// offset) over all rows; otherwise seed_off is the device table of the per-sample streams.  Either way the kernel family
+// and the Philox stride follow torch's launch policy for ONE stream's hw * NL elements.
+static int launch_sampler(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL, float inv_t,
+                          uint64_t seed, uint64_t offset, const uint64_t* seed_off, int64_t* out, cudaStream_t st) {
+    const bool ps = seed_off != nullptr;
+    const int64_t R = n_samp * hw;
+    TorchPhilox rng = make_torch_philox(seed, offset, hw * (int64_t)NL);
     {
         // shared-Philox path: needs stride % NL == 0 (rows of a lane group are whole rows).  The feature buffer must hold
-        // fused_sampler_rows_padded(R, NL) rows (the caller's workspace does); rows >= R are never written to `out`.
-        TorchPhilox rng = make_torch_philox(seed, offset, R * (int64_t)NL);
+        // (n_samp - 1) * hw + fused_sampler_rows_padded(hw, NL) rows (the caller's workspace does); rows past a stream's
+        // end are never written to `out`.
         static const bool no_shared = getenv("PB200_SAMPLER_GENERIC") != nullptr;
         if (!no_shared && rng.stride % (uint32_t)NL == 0 && (int64_t)rng.stride / NL < (1 << 24)) {
             const int rs = (int)(rng.stride / NL);
-            const int n_blocks = (int)((R + 4 * (int64_t)rs - 1) / (4 * (int64_t)rs));
+            const int n_blocks = (int)((hw + 4 * (int64_t)rs - 1) / (4 * (int64_t)rs));
             const int tpb = (rs + SH_JJ - 1) / SH_JJ;
             static DeviceOnce attr2;
             if (attr2.first()) {
-                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
-    }
+                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
+                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
+            }
             ProfScope prof("fused_sampler", 2.0 * (double)R * (double)NL * (double)Kc, st);
             CUtensorMap tf, tw;
-            const int64_t dims[4] = {Kc, 4, rs, n_blocks};
-            const int64_t strides[3] = {(int64_t)rs * Kc * 2, (int64_t)Kc * 2, 4 * (int64_t)rs * Kc * 2};
-            const int box[4] = {64, 4, SH_JJ, 1};
-            PB_TRY(make_tmap_f16_nd(&tf, a16, 4, dims, strides, box));
+            const int64_t dims[5] = {Kc, 4, rs, n_blocks, n_samp};
+            const int64_t strides[4] = {(int64_t)rs * Kc * 2, (int64_t)Kc * 2, 4 * (int64_t)rs * Kc * 2, hw * Kc * 2};
+            const int box[5] = {64, 4, SH_JJ, 1, 1};
+            PB_TRY(make_tmap_f16_nd(&tf, a16, ps ? 5 : 4, dims, strides, box));
             PB_TRY(make_tmap_f16_2d(&tw, w16, NL, Kc, Kc, 128));
-            fused_sampler_shared_kernel<<<n_blocks * tpb, SH_THREADS, SH_SMEM, st>>>(tf, tw, (int)R, NL, Kc, rs, tpb, inv_t, rng, out);
+            const int64_t grid = n_samp * n_blocks * tpb;
+            PB_CHECK(grid < (1ll << 31), "fused sampler: %lld CTAs", (long long)grid);
+            if (ps)
+                fused_sampler_shared_kernel<true><<<(unsigned)grid, SH_THREADS, SH_SMEM, st>>>(tf, tw, (int)R, NL, Kc, rs, tpb, inv_t, rng,
+                                                                                               (int)hw, n_blocks, seed_off, out);
+            else
+                fused_sampler_shared_kernel<false><<<(unsigned)grid, SH_THREADS, SH_SMEM, st>>>(tf, tw, (int)R, NL, Kc, rs, tpb, inv_t, rng,
+                                                                                                (int)hw, n_blocks, nullptr, out);
             PB_LAUNCH_CHECK();
             return 0;
         }
     }
     static DeviceOnce attr_set;
     if (attr_set.first()) {
-        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
+        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
+        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
     }
     ProfScope prof("fused_sampler", 2.0 * (double)R * (double)NL * (double)Kc, st);
     CUtensorMap ta, tw;
     PB_TRY(make_tmap_f16_2d(&ta, a16, R, Kc, Kc, 128));
     PB_TRY(make_tmap_f16_2d(&tw, w16, NL, Kc, Kc, SMP_BN));
-    TorchPhilox rng = make_torch_philox(seed, offset, R * (int64_t)NL);
-    fused_sampler_kernel<<<ceil_div(R, 128), SMP_THREADS, SMP_SMEM, st>>>(ta, tw, (int)R, NL, Kc, inv_t, rng, out);
+    if (ps)
+        fused_sampler_kernel<true><<<ceil_div(R, 128), SMP_THREADS, SMP_SMEM, st>>>(ta, tw, (int)R, NL, Kc, inv_t, rng, (int)hw,
+                                                                                    seed_off, out);
+    else
+        fused_sampler_kernel<false><<<ceil_div(R, 128), SMP_THREADS, SMP_SMEM, st>>>(ta, tw, (int)R, NL, Kc, inv_t, rng, (int)hw,
+                                                                                     nullptr, out);
     PB_LAUNCH_CHECK();
     return 0;
+}
+
+int launch_fused_sampler(const __half* a16, int64_t R, int Kc, const __half* w16, int NL, float inv_t, uint64_t seed,
+                         uint64_t offset, int64_t* out, cudaStream_t st) {
+    PB_CHECK(Kc % 8 == 0 && Kc <= 64 * SMP_MAX_KB, "fused sampler: c_out=%d unsupported (<= %d, multiple of 8)", Kc, 64 * SMP_MAX_KB);
+    PB_CHECK(R * (int64_t)NL < (1ll << 31), "fused sampler: rows*labels >= 2^31 would split the torch kernel (unsupported)");
+    PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
+    if (R == 0) return 0;
+    return launch_sampler(a16, 1, R, Kc, w16, NL, inv_t, seed, offset, nullptr, out, st);
+}
+
+int launch_fused_sampler_per_sample(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL,
+                                    float inv_t, const uint64_t* seed_off, int64_t* out, cudaStream_t st) {
+    PB_CHECK(Kc % 8 == 0 && Kc <= 64 * SMP_MAX_KB, "fused sampler: c_out=%d unsupported (<= %d, multiple of 8)", Kc, 64 * SMP_MAX_KB);
+    PB_CHECK(hw * (int64_t)NL <= (1ll << 29),
+             "fused sampler: a per-sample draw of %lld elements (hw*labels > 2^29) would split the torch kernel (unsupported)",
+             (long long)(hw * (int64_t)NL));
+    PB_CHECK(n_samp * hw < (1ll << 31), "fused sampler: %lld rows", (long long)(n_samp * hw));
+    PB_CHECK(seed_off != nullptr, "fused sampler: per-sample (seed, offset) table is NULL");
+    if (n_samp == 0 || hw == 0) return 0;
+    return launch_sampler(a16, n_samp, hw, Kc, w16, NL, inv_t, 0, 0, seed_off, out, st);
 }
 
 }  // namespace pb

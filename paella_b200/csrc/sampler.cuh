@@ -8,4 +8,8 @@ int64_t fused_sampler_rows_padded(int64_t R, int NL);
 // a16: fp16 [R, Kc] guided features; w16: fp16 [NL, Kc] out_mapper weight; out: int64 [R]
 int launch_fused_sampler(const __half* a16, int64_t R, int Kc, const __half* w16, int NL, float inv_t, uint64_t seed,
                          uint64_t offset, int64_t* out, cudaStream_t st);
+// the same draw with one stream per sample: a16 fp16 [n_samp * hw, Kc] (holding (n_samp - 1) * hw +
+// fused_sampler_rows_padded(hw, NL) rows), seed_off DEVICE uint64 [n_samp][2] = (seed, philox offset); out int64 [n_samp * hw]
+int launch_fused_sampler_per_sample(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL,
+                                    float inv_t, const uint64_t* seed_off, int64_t* out, cudaStream_t st);
 }  // namespace pb

@@ -640,10 +640,24 @@ class Paella(nn.Module):
 
     def sample_tokens(self, feats: torch.Tensor, batch: int, h: int, w: int, cfg: Optional[float], temperature: float,
                       generator=None) -> torch.Tensor:
-        """Fused out_mapper + CFG + temperature + multinomial on torch's random stream (ref/src/utils.py:44-50)."""
+        """Fused out_mapper + CFG + temperature + multinomial on torch's random stream (ref/src/utils.py:44-50).
+        ``generator``: None (the default CUDA generator), one CUDA generator, or a list of ``batch`` of them -- one stream per
+        sample, where sample b draws what this call with batch 1 draws on generator b (ops.check_generators)."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
+        if ops.per_sample(generator):
+            ops.check_generators(generator, batch, dev)
+            ops.check_per_sample_numel(h * w * self.num_labels)
+            with torch.cuda.device(dev):
+                out = torch.empty(batch, h, w, dtype=torch.int64, device=dev)
+                ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, batch, h, w, 1))
+                table = ops.philox_table(generator, h * w * self.num_labels, dev)
+                check(L.pb200_paella_sample_tokens_per_sample(self._handle, ptr(feats), batch, h * w, 1 if cfg is not None else 0,
+                                                              float(cfg) if cfg is not None else 0.0, float(temperature), ptr(table),
+                                                              ptr(out), ptr(ws), ws.numel(), current_stream()),
+                      "pb200_paella_sample_tokens_per_sample")
+            return out
         with torch.cuda.device(dev):
             out = torch.empty(batch, h, w, dtype=torch.int64, device=dev)
             ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, batch, h, w, 1))
@@ -703,12 +717,12 @@ class Paella(nn.Module):
             self._cond_single = memos
         return cond
 
-    def add_noise(self, x, t, mask=None, random_x=None):
-        """ref/src/modules.py:277-283 on torch's random stream."""
+    def add_noise(self, x, t, mask=None, random_x=None, generator=None):
+        """ref/src/modules.py:277-283 on torch's random stream (``generator``: as in ``sample_tokens``)."""
         if mask is None:
-            return ops.add_noise(x, t, random_x, self.num_labels)
+            return ops.add_noise(x, t, random_x, self.num_labels, generator)
         if random_x is None:
-            random_x = ops.randint(self.num_labels, x.shape, x.device)
+            random_x = ops.randint(self.num_labels, x.shape, x.device, generator)
         return torch.where(mask.bool(), random_x, x), mask
 
     def get_loss_weight(self, t, mask, min_val=0.3):    # ref/utils/modules.py:290-291 (training helper)

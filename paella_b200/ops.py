@@ -62,10 +62,66 @@ def skip_philox_for_split(chunks, total_numel: int, device, generator=None) -> N
         take_philox(total_numel, device, generator)
 
 
+# ------------------------------------------------------------------ per-sample generators
+# ``generator`` may be a list of B CUDA generators, one per sample: sample b then draws on its own generator exactly what the
+# op run on that sample alone (batch 1) draws, so its result depends only on its own seed, not on its batch.
+MAX_PER_SAMPLE_NUMEL = 2 ** 29      # torch splits a larger fp32 draw into two kernels (philox_row_chunks)
+
+
+def per_sample(generator) -> bool:
+    return isinstance(generator, (list, tuple))
+
+
+def check_generators(generators, batch: int, device) -> None:
+    """A per-sample generator list: one distinct CUDA generator per sample, all on ``device``."""
+    if len(generators) != batch:
+        raise ValueError(f"generator: got a list of {len(generators)} generators for a batch of {batch} (one per sample)")
+    device = torch.device(device)
+    dev_idx = device.index if device.index is not None else torch.cuda.current_device()
+    seen = set()
+    for i, g in enumerate(generators):
+        if not isinstance(g, torch.Generator) or g.device.type != "cuda":
+            where = g.device if isinstance(g, torch.Generator) else type(g).__name__
+            raise ValueError(f"generator[{i}] must be a CUDA torch.Generator (got {where})")
+        g_idx = g.device.index if g.device.index is not None else torch.cuda.current_device()
+        if g_idx != dev_idx:
+            raise ValueError(f"generator[{i}] is on cuda:{g_idx}, the model on cuda:{dev_idx}")
+        if id(g) in seen:
+            raise ValueError(f"generator[{i}] appears more than once in the list; its state would be ambiguous")
+        seen.add(id(g))
+
+
+def check_per_sample_numel(numel: int) -> None:
+    if numel > MAX_PER_SAMPLE_NUMEL:
+        raise ValueError(f"per-sample generators: one sample's draw of {numel} elements exceeds 2^29, which torch would split "
+                         "into two kernels (unsupported); use a smaller latent grid")
+
+
+def philox_table(generators, numel: int, device) -> torch.Tensor:
+    """Device int64 [B, 2] of (seed, philox offset) for one draw of ``numel`` elements per sample; advances each generator.
+    Built in pinned memory and copied asynchronously: no host synchronisation, no pageable copy."""
+    check_per_sample_numel(numel)
+    vals = []
+    for g in generators:
+        seed, off = take_philox(numel, device, g)
+        if off % 4:
+            raise ValueError(f"generator offset {off} is not a multiple of 4")
+        vals += [seed - 2 ** 64 if seed >= 2 ** 63 else seed, off]       # uint64 seed, bit for bit
+    return torch.tensor(vals, dtype=torch.int64, pin_memory=True).view(-1, 2).to(device, non_blocking=True)
+
+
 # ------------------------------------------------------------------ random ops
 def randint(num_labels: int, size, device, generator=None) -> torch.Tensor:
     """torch.randint(0, num_labels, size, device=device)  [ref/src/utils.py:37]"""
     out = torch.empty(size, dtype=torch.int64, device=device)
+    if per_sample(generator):
+        check_generators(generator, out.shape[0], out.device)
+        per = out[0].numel()
+        check_per_sample_numel(per)
+        for b, g in enumerate(generator):
+            seed, off = take_philox(per, out.device, g)
+            check(lib().pb200_randint(ptr(out[b]), per, num_labels, seed, off, current_stream()), "pb200_randint")
+        return out
     seed, off = take_philox(out.numel(), out.device, generator)
     check(lib().pb200_randint(ptr(out), out.numel(), num_labels, seed, off, current_stream()), "pb200_randint")
     return out
@@ -95,6 +151,11 @@ def multinomial(p: torch.Tensor, generator=None) -> torch.Tensor:
 def resample_logits(logits_c: torch.Tensor, logits_u: Optional[torch.Tensor], cfg: float, temperature: float,
                     mode: str = "multinomial", generator=None) -> torch.Tensor:
     """ref/src/utils.py:45-50 on reference-layout logits [B,K,H,W] -> tokens [B,H,W]."""
+    if per_sample(generator) and mode == "multinomial":
+        check_generators(generator, logits_c.shape[0], logits_c.device)
+        check_per_sample_numel(logits_c[0].numel())
+        return torch.cat([resample_logits(logits_c[b:b + 1], logits_u[b:b + 1] if logits_u is not None else None, cfg, temperature,
+                                          mode, g) for b, g in enumerate(generator)])
     B, K = logits_c.shape[:2]
     hw = logits_c[0, 0].numel()
     lc = logits_c.contiguous().float()
@@ -135,6 +196,19 @@ def add_noise(x: torch.Tensor, t: torch.Tensor, random_x: Optional[torch.Tensor]
     hw = x[0].numel()
     out = torch.empty_like(x)
     mask = torch.empty_like(x) if return_mask else None
+    if per_sample(generator):
+        check_generators(generator, B, x.device)
+        check_per_sample_numel(hw)
+        t = t.contiguous().float()
+        random_x = random_x.contiguous() if random_x is not None else None
+        for b, g in enumerate(generator):
+            seed, off = take_philox(hw, x.device, g)
+            if random_x is None:
+                take_philox(hw, x.device, g)
+            check(lib().pb200_add_noise(ptr(x[b]), ptr(random_x[b]) if random_x is not None else None, ptr(t[b:b + 1]), 1, hw,
+                                        num_labels, seed, off, ptr(out[b]), ptr(mask[b]) if mask is not None else None,
+                                        current_stream()), "pb200_add_noise")
+        return out, mask
     seed, off = take_philox(x.numel(), x.device, generator)
     if random_x is None:
         take_philox(x.numel(), x.device, generator)      # the randint_like draw follows the mask draw

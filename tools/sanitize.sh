@@ -47,6 +47,10 @@ cfg, sd, gg = load_golden("paella_tiny.npz")
 m = Paella(**cfg).to(DEV).eval(); m.load_state_dict(sd)
 feats = torch.randn(2 * 2 * 64, cfg["c_out"], device=DEV, generator=g)
 print("sampler", m.sample_tokens(feats, 2, 8, 8, 4.0, 0.7).shape)
+# per-sample streams: odd B, and 7x7 rows per sample (4 rs = 256 on this small-grid policy) -- every sample's block is partial
+f3 = torch.randn(2 * 3 * 49, cfg["c_out"], device=DEV, generator=g)
+gens = [torch.Generator(device=DEV).manual_seed(s) for s in (1, 2, 3)]
+print("sampler per-sample", m.sample_tokens(f3, 3, 7, 7, 4.0, 0.7, gens).shape)
 p = torch.rand(64, 100, device=DEV, generator=g); print("multinomial", ops.multinomial(p).shape)
 t = torch.from_numpy
 print("forward", m(t(gg["x"]).to(DEV), t(gg["r"]).to(DEV), t(gg["byt5"]).to(DEV), clip=t(gg["clip"]).to(DEV)).shape)
