@@ -70,6 +70,19 @@ int pb200_resample_logits(const float* logits_c, const float* logits_u, int64_t 
 int pb200_resample_quant(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, double cfg,
                          double temperature, const float* codebook, int c_latent, int64_t* out, void* stream);
 
+/* Per-sample sampling parameters.  params: DEVICE float [batch][3] = (cfg_b, 1 - cfg_b, 1 / temperature_b) as the fp32
+ * constants the scalar entry points derive from their double arguments: (float)cfg, (float)(1.0 - cfg) and
+ * 1.0f / (float)temperature.  Sample b is computed with row b exactly as the scalar call on (cfg_b, temperature_b) computes it;
+ * the cfg columns are ignored where there is no guidance (logits_u == NULL, cfg_on == 0). */
+
+/* pb200_resample_logits with per-sample (cfg, 1 - cfg, 1/T) in one launch over the batch; the draw is the scalar call's. */
+int pb200_resample_logits_params(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw,
+                                 const float* params, int mode, uint64_t seed, uint64_t offset, int64_t* out, void* stream);
+
+/* pb200_resample_quant with per-sample (cfg, 1 - cfg, 1/T) in one launch over the batch. */
+int pb200_resample_quant_params(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw,
+                                const float* params, const float* codebook, int c_latent, int64_t* out, void* stream);
+
 /* Paella.add_noise(x, t, random_x=...)            [ref/src/modules.py:277-283]
  *   mask = (rand_like(x.float()) <= t[:,None,None]); x*(1-mask) + random_x*mask
  * x, random_x, out: int64 [B, HW]; t: fp32 [B]; mask_out: int64 [B, HW] or NULL.
@@ -285,6 +298,16 @@ int pb200_paella_sample_tokens(pb200_paella* m, const float* features, int batch
 int pb200_paella_sample_tokens_per_sample(pb200_paella* m, const float* features, int batch, int hw, int cfg_on, double cfg,
                                           double temperature, const uint64_t* seed_offset, int64_t* tokens_out,
                                           void* workspace, int64_t workspace_bytes, void* stream);
+
+/* pb200_paella_sample_tokens with per-sample guidance scale and temperature, in ONE launch over the batch.  params: DEVICE
+ * float [batch][3] of per-sample (cfg, 1 - cfg, 1/T), as for pb200_resample_logits_params: row r of the CFG pre-mix uses
+ * sample r / hw's (cfg, 1 - cfg) and its draw sample r / hw's 1/T.  seed_offset == NULL: one random stream (seed, offset)
+ * over the batch, drawn exactly as pb200_paella_sample_tokens draws it; otherwise the per-sample (seed, offset) table of
+ * pb200_paella_sample_tokens_per_sample (seed and offset are then ignored).  Either way sample b's tokens are those of the
+ * scalar entry point on sample b's parameters. */
+int pb200_paella_sample_tokens_params(pb200_paella* m, const float* features, int batch, int hw, int cfg_on, const float* params,
+                                      uint64_t seed, uint64_t offset, const uint64_t* seed_offset, int64_t* tokens_out,
+                                      void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * VQGAN (ref/src/vqgan.py:45-107).

@@ -62,6 +62,10 @@ SIGNATURES = {
                                       c_uint64, c_uint64, c_void_p, c_void_p]),
     "pb200_resample_quant": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_double, c_double, c_void_p, c_int,
                                      c_void_p, c_void_p]),
+    "pb200_resample_logits_params": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int, c_uint64, c_uint64,
+                                             c_void_p, c_void_p]),
+    "pb200_resample_quant_params": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_int, c_void_p,
+                                            c_void_p]),
     "pb200_add_noise": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_void_p,
                                 c_void_p, c_void_p]),
     "pb200_vq_nearest": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p]),
@@ -100,6 +104,8 @@ SIGNATURES = {
                                            c_uint64, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_sample_tokens_per_sample": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_void_p,
                                                       c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_sample_tokens_params": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_uint64, c_uint64, c_void_p,
+                                                  c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_vqgan_create": (c_int, [POINTER(VqganConfig), POINTER(c_void_p)]),
     "pb200_vqgan_destroy": (None, [c_void_p]),
     "pb200_vqgan_weight_bytes": (c_int64, [c_void_p]),

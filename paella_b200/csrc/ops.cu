@@ -796,17 +796,25 @@ int launch_film_apply(float* x, int64_t M, int N, int P, const float* film, int6
 }
 
 // ------------------------------------------------------------------ casts
+// OP 3: weighted mix with per-row weights: element e takes (wa, wb) = w[3 s], w[3 s + 1] of s = e / per (the sample of its
+// row; per = rows per sample * row length), with OP 2's expression.
 template <int OP>
 __global__ void cast_kernel(const float* __restrict__ a, const float* __restrict__ b, float wa, float wb, int64_t n,
-                            __half* __restrict__ out) {
+                            __half* __restrict__ out, const float* __restrict__ w = nullptr, int64_t per = 0) {
     const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
     if (i >= n) return;
+    int64_t s0 = 0;
+    if (OP == 3) s0 = i / per;
     float v[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         float t = (i + j < n) ? a[i + j] : 0.f;
         if (OP == 1) t = t / (1.0f + expf(-t));                                   // SiLU
         if (OP == 2) t = b ? fmaf(t, wa, b[(i + j < n) ? i + j : 0] * wb) : t * wa;  // weighted mix
+        if (OP == 3) {
+            const int64_t s = (i + j >= (s0 + 1) * per) ? s0 + 1 : s0;
+            if (i + j < n) t = fmaf(t, w[3 * s], b[i + j] * w[3 * s + 1]);
+        }
         v[j] = t;
     }
     if (i + 3 < n && ((reinterpret_cast<uintptr_t>(out + i) & 7) == 0)) {
@@ -837,6 +845,14 @@ int launch_mix_cast_f16(const float* a, const float* b, float wa, float wb, int6
     ProfScope prof("cast", (double)n * (b ? 10.0 : 6.0), st);
     if (n == 0) return 0;
     cast_kernel<2><<<ceil_div(ceil_div(n, 4), 256), 256, 0, st>>>(a, b, wa, wb, n, out);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+int launch_mix_cast_rows_f16(const float* a, const float* b, const float* w, int64_t per, int64_t n, __half* out, cudaStream_t st) {
+    ProfScope prof("cast", (double)n * 10.0, st);
+    if (n == 0) return 0;
+    PB_CHECK(per >= 4, "mix_cast_rows: %lld elements per weight row (< 4)", (long long)per);
+    cast_kernel<3><<<ceil_div(ceil_div(n, 4), 256), 256, 0, st>>>(a, b, 0.f, 0.f, n, out, w, per);
     PB_LAUNCH_CHECK();
     return 0;
 }

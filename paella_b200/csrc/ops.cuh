@@ -51,6 +51,8 @@ int launch_cast_f16(const float* x, int64_t n, __half* out, cudaStream_t st);
 int launch_silu_cast_f16(const float* x, int64_t n, __half* out, cudaStream_t st);
 // out[i] = fp16(a[i]*wa + b[i]*wb)   (b may be null)
 int launch_mix_cast_f16(const float* a, const float* b, float wa, float wb, int64_t n, __half* out, cudaStream_t st);
+// the same mix with per-sample weights: element e uses (wa, wb) = (w[3 s], w[3 s + 1]), s = e / per (w: DEVICE [samples][3])
+int launch_mix_cast_rows_f16(const float* a, const float* b, const float* w, int64_t per, int64_t n, __half* out, cudaStream_t st);
 
 // [B, C, HW] <-> [B, HW, C] fp32
 int launch_nchw_to_nhwc(const float* in, int B, int C, int HW, float* out, cudaStream_t st);

@@ -894,4 +894,27 @@ int pb200_paella_sample_tokens_per_sample(pb200_paella* m, const float* features
                                            seed_offset, tokens_out, st);
 }
 
+int pb200_paella_sample_tokens_params(pb200_paella* m, const float* features, int batch, int hw, int cfg_on, const float* params,
+                                      uint64_t seed, uint64_t offset, const uint64_t* seed_offset, int64_t* tokens_out,
+                                      void* workspace, int64_t workspace_bytes, void* stream) {
+    PB_CHECK(m->blob != nullptr, "sample_tokens_params: weights not bound");
+    PB_CHECK(params != nullptr, "sample_tokens_params: params is NULL");
+    const pb200_paella_config& c = m->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+    PB_CHECK(batch >= 0 && hw >= 0, "sample_tokens_params: bad shape");
+    const int64_t rows = (int64_t)batch * hw;
+    if (rows == 0) return 0;
+    const int64_t need_rows = seed_offset ? (int64_t)(batch - 1) * hw + fused_sampler_rows_padded(hw, c.num_labels)
+                                          : fused_sampler_rows_padded(rows, c.num_labels);
+    PB_CHECK(need_rows * c.c_out * 2 <= workspace_bytes, "sample_tokens_params: workspace too small (use pb200_paella_workspace_bytes)");
+    __half* a16 = reinterpret_cast<__half*>(workspace);
+    // row r mixes with sample r / hw's (cfg, 1 - cfg): the scalar path's expression with per-sample constants
+    if (cfg_on)
+        PB_TRY(launch_mix_cast_rows_f16(features, features + rows * c.c_out, params, (int64_t)hw * c.c_out, rows * c.c_out, a16, st));
+    else
+        PB_TRY(launch_cast_f16(features, rows * c.c_out, a16, st));
+    return launch_fused_sampler_params(a16, batch, hw, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f, params, seed, offset,
+                                       seed_offset, tokens_out, st);
+}
+
 }  // extern "C"

@@ -114,12 +114,17 @@ __global__ void __launch_bounds__(256) multinomial_kernel(const float* __restric
 //   l' = l * (1/T)                    (torch's div-by-CPU-scalar fast path multiplies by the reciprocal)
 //   p  = exp(l' - max) / sum          (softmax dim=1)
 //   tok = argmax_k p_k / q_k
+// params (may be null): DEVICE [B][3] per-sample (cfg, 1 - cfg, 1/T), replacing the three scalars for sample b = blockIdx.y.
 template <int MODE>
-__global__ void __launch_bounds__(256) resample_logits_kernel(const float* __restrict__ lc, const float* __restrict__ lu,
-                                                              int k, int64_t hw, float cfg, float one_minus_cfg,
-                                                              float inv_t, TorchPhilox s, int64_t* __restrict__ out) {
+__global__ void __launch_bounds__(256, 4) resample_logits_kernel(const float* __restrict__ lc, const float* __restrict__ lu,
+                                                                 int k, int64_t hw, float cfg_arg, float one_minus_cfg_arg,
+                                                                 float inv_t_arg, const float* __restrict__ params, TorchPhilox s,
+                                                                 int64_t* __restrict__ out) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t b = blockIdx.y;
+    const float cfg = params ? params[3 * b] : cfg_arg;
+    const float one_minus_cfg = params ? params[3 * b + 1] : one_minus_cfg_arg;
+    const float inv_t = params ? params[3 * b + 2] : inv_t_arg;
     const int64_t pos = (int64_t)blockIdx.x * 32 + lane;
     const bool valid = pos < hw;
     const float* c_ptr = lc + b * (int64_t)k * hw + (valid ? pos : 0);
@@ -188,10 +193,14 @@ __global__ void __launch_bounds__(256) resample_logits_kernel(const float* __res
 // Same CTA shape as resample_logits_kernel: 32 positions x 8 warps striding the labels.
 template <int C>
 __global__ void __launch_bounds__(256) resample_quant_kernel(const float* __restrict__ lc, const float* __restrict__ lu, int k,
-                                                             int64_t hw, float cfg, float one_minus_cfg, float inv_t,
-                                                             const float* __restrict__ codebook, int64_t* __restrict__ out) {
+                                                             int64_t hw, float cfg_arg, float one_minus_cfg_arg, float inv_t_arg,
+                                                             const float* __restrict__ params, const float* __restrict__ codebook,
+                                                             int64_t* __restrict__ out) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t b = blockIdx.y;
+    const float cfg = params ? params[3 * b] : cfg_arg;                   // per-sample parameters as in resample_logits
+    const float one_minus_cfg = params ? params[3 * b + 1] : one_minus_cfg_arg;
+    const float inv_t = params ? params[3 * b + 2] : inv_t_arg;
     const int64_t pos = (int64_t)blockIdx.x * 32 + lane;
     const bool valid = pos < hw;
     const float* c_ptr = lc + b * (int64_t)k * hw + (valid ? pos : 0);
@@ -303,45 +312,74 @@ int pb200_multinomial(const float* p, int64_t rows, int64_t k, uint64_t seed, ui
     return 0;
 }
 
-int pb200_resample_logits(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw,
-                          double cfg, double temperature, int mode, uint64_t seed, uint64_t offset, int64_t* out,
-                          void* stream) {
+}  // extern "C"
+
+namespace pb {
+// python scalars: `logits * cfg` and `(1 - cfg)` are doubles cast to the fp32 op-math type; `temperatures[i]` is an fp32
+// 0-dim CPU tensor and torch multiplies by its fp32 reciprocal.  These are the fp32 constants a per-sample table holds too.
+static int resample_logits(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, double cfg,
+                           double temperature, const float* params, int mode, uint64_t seed, uint64_t offset, int64_t* out,
+                           cudaStream_t st) {
     PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
     PB_CHECK(mode == 0 || mode == 1, "resample: mode must be 0 (multinomial) or 1 (argmax)");
     PB_CHECK(batch * hw * k < (1ll << 31), "resample: B*HW*K >= 2^31 would split the torch kernel (unsupported)");
     if (batch == 0 || hw == 0) return 0;
     TorchPhilox s = make_torch_philox(seed, offset, batch * hw * k);
-    // python scalars: `logits * cfg` and `(1 - cfg)` are doubles cast to the fp32 op-math type;
-    // `temperatures[i]` is an fp32 0-dim CPU tensor and torch multiplies by its fp32 reciprocal.
     const float cfg_f = (float)cfg;
     const float one_minus = (float)(1.0 - cfg);
     const float inv_t = 1.0f / (float)temperature;
     dim3 grid(ceil_div(hw, 32), (unsigned)batch);
     if (mode == 0)
-        resample_logits_kernel<0><<<grid, 256, 0, (cudaStream_t)stream>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus,
-                                                                          inv_t, s, out);
+        resample_logits_kernel<0><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, s, out);
     else
-        resample_logits_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus,
-                                                                          inv_t, s, out);
+        resample_logits_kernel<1><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, s, out);
     PB_LAUNCH_CHECK();
     return 0;
 }
 
-int pb200_resample_quant(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, double cfg,
-                         double temperature, const float* codebook, int c_latent, int64_t* out, void* stream) {
+static int resample_quant(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, double cfg,
+                          double temperature, const float* params, const float* codebook, int c_latent, int64_t* out,
+                          cudaStream_t st) {
     PB_CHECK(c_latent >= 1 && c_latent <= 8, "resample_quant: c_latent %d unsupported (1..8)", c_latent);
     if (batch == 0 || hw == 0) return 0;
     const float cfg_f = (float)cfg, one_minus = (float)(1.0 - cfg), inv_t = 1.0f / (float)temperature;
     dim3 grid(ceil_div(hw, 32), (unsigned)batch);
-    cudaStream_t st = (cudaStream_t)stream;
     switch (c_latent) {
 #define PB_RQ_CASE(C) \
-    case C: resample_quant_kernel<C><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, codebook, out); break;
+    case C: resample_quant_kernel<C><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, codebook, out); break;
         PB_RQ_CASE(1) PB_RQ_CASE(2) PB_RQ_CASE(3) PB_RQ_CASE(4) PB_RQ_CASE(5) PB_RQ_CASE(6) PB_RQ_CASE(7) PB_RQ_CASE(8)
 #undef PB_RQ_CASE
     }
     PB_LAUNCH_CHECK();
     return 0;
+}
+}  // namespace pb
+
+extern "C" {
+
+int pb200_resample_logits(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw,
+                          double cfg, double temperature, int mode, uint64_t seed, uint64_t offset, int64_t* out,
+                          void* stream) {
+    return resample_logits(logits_c, logits_u, batch, k, hw, cfg, temperature, nullptr, mode, seed, offset, out,
+                           (cudaStream_t)stream);
+}
+
+int pb200_resample_logits_params(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw,
+                                 const float* params, int mode, uint64_t seed, uint64_t offset, int64_t* out, void* stream) {
+    PB_CHECK(params != nullptr, "resample_logits_params: params is NULL");
+    return resample_logits(logits_c, logits_u, batch, k, hw, 0.0, 1.0, params, mode, seed, offset, out, (cudaStream_t)stream);
+}
+
+int pb200_resample_quant(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, double cfg,
+                         double temperature, const float* codebook, int c_latent, int64_t* out, void* stream) {
+    return resample_quant(logits_c, logits_u, batch, k, hw, cfg, temperature, nullptr, codebook, c_latent, out,
+                          (cudaStream_t)stream);
+}
+
+int pb200_resample_quant_params(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw,
+                                const float* params, const float* codebook, int c_latent, int64_t* out, void* stream) {
+    PB_CHECK(params != nullptr, "resample_quant_params: params is NULL");
+    return resample_quant(logits_c, logits_u, batch, k, hw, 0.0, 1.0, params, codebook, c_latent, out, (cudaStream_t)stream);
 }
 
 int pb200_add_noise(const int64_t* x, const int64_t* random_x, const float* t, int64_t batch, int64_t hw,

@@ -41,11 +41,17 @@ __device__ __forceinline__ void per_sample_stream(const uint64_t* __restrict__ s
     s.offset4 = seed_off[2 * b + 1] >> 2;
 }
 
-template <bool PS>
+// PP (per-sample parameters): row r of the launch belongs to sample r / phw, whose temperature is params[3 (r / phw) + 2] =
+// 1.0f / (float)T_b (the (cfg, 1 - cfg) columns were applied by the pre-mix); the scalar instances read inv_t instead.
+__device__ __forceinline__ float per_sample_inv_t(const float* __restrict__ params, int64_t row, int phw) {
+    return params[3 * (row / phw) + 2];
+}
+
+template <bool PS, bool PP>
 __global__ void __launch_bounds__(SMP_THREADS, 1)
 fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, int R, int NL,
                      int Kc, float inv_t, TorchPhilox rng, int hw, const uint64_t* __restrict__ seed_off,
-                     int64_t* __restrict__ out) {
+                     const float* __restrict__ params, int phw, int64_t* __restrict__ out) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t a_base = smem_base;
@@ -107,6 +113,12 @@ fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
                 }
             }
         }
+        float it[2] = {inv_t, inv_t};                // the two rows' 1/T
+        if constexpr (PP) {
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr)
+                if (row0 + 8 * rr < R) it[rr] = per_sample_inv_t(params, row0 + 8 * rr, phw);
+        }
         float acc[SMP_BN / 2];
         ptx::mbar_wait(a_bar, 0);
         int stage = 0;
@@ -140,7 +152,7 @@ fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
                     const uint32_t bits = PS ? torch_philox_u32(srng[rr], ebase[rr] + (uint64_t)col)
                                              : torch_philox_u32(rng, (uint64_t)row * (uint64_t)NL + (uint64_t)col);
                     const float qv = torch_exponential1(u32_to_uniform(bits));
-                    const float gum = fmaf(acc[i], inv_t, -__logf(qv));
+                    const float gum = fmaf(acc[i], PP ? it[rr] : inv_t, -__logf(qv));
                     if (gum > bv[rr]) { bv[rr] = gum; bi[rr] = col; }      // columns of a row arrive in increasing order
                 }
             }
@@ -174,15 +186,20 @@ constexpr int SH_F_BYTES = SH_N * 128;         // one k-block of the token tile
 constexpr int SH_W_BYTES = 128 * 128;          // 128 labels x 64 halves
 constexpr int SH_RED_WARPS = 8;                // MMA warps, one reduction row each
 constexpr int SH_SMEM = SMP_MAX_KB * SH_F_BYTES + SH_STAGES * SH_W_BYTES + 1024 + 256 + SH_RED_WARPS * SH_N * 8;
+constexpr int SH_SMEM_PP = SH_SMEM + SH_N * 4;     // + the per-column 1/T of a one-stream task
 
 // PS: R / hw samples of hw rows, each with its own 4rs-row blocks (blocks_per_sample of them; the last one of a sample is
 // partial and never straddles into the next sample's draw) and its own stream (see per_sample_stream).  The token tile comes
 // through a 5-D map whose outermost coordinate is the sample; rows past a sample's end are loaded but never written.
-template <bool PS>
+// PP: per-sample 1/T (per_sample_inv_t).  With PS the CTA's rows are one sample's, so it is one load.  With one stream the
+// four rows r + g rs of a Philox call can belong to different samples: the task's 80 token columns get their 1/T staged in
+// shared memory once, and the epilogue reads them as one float4 per jj (its four g) -- not held in registers.
+template <bool PS, bool PP>
 __global__ void __launch_bounds__(SH_THREADS, 1)
 fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __grid_constant__ CUtensorMap tm_w, int R, int NL,
                             int Kc, int rs, int tasks_per_block, float inv_t, TorchPhilox rng, int hw, int blocks_per_sample,
-                            const uint64_t* __restrict__ seed_off, int64_t* __restrict__ out) {
+                            const uint64_t* __restrict__ seed_off, const float* __restrict__ params, int phw,
+                            int64_t* __restrict__ out) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -195,6 +212,7 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
     uint8_t* tail = smem_gen + (bar_base - smem_base) + 256;
     float* red_v = reinterpret_cast<float*>(tail);                    // [8 warps][SH_N]
     int* red_i = reinterpret_cast<int*>(tail + SH_RED_WARPS * SH_N * 4);
+    float* col_it = reinterpret_cast<float*>(tail + SH_RED_WARPS * SH_N * 8);   // [SH_N] (PP, one stream)
 
     const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
     const int lane = threadIdx.x & 31;
@@ -205,6 +223,13 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
     const int blk = task / tasks_per_block;                            // 4rs-row block = Philox call index
     const int jj0 = (task - blk * tasks_per_block) * SH_JJ;
 
+    if constexpr (PP && !PS) {
+        if (threadIdx.x < SH_N) {                    // token column c = jj_local * 4 + g, as in the reduction below
+            const int jj = jj0 + (int)threadIdx.x / 4, g = threadIdx.x & 3;
+            const int64_t row = (int64_t)blk * 4 * rs + (int64_t)g * rs + jj;
+            col_it[threadIdx.x] = (jj < rs && row < R) ? per_sample_inv_t(params, row, phw) : inv_t;
+        }
+    }
     if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tm_f);
         ptx::prefetch_tensormap(&tm_w);
@@ -247,6 +272,8 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
         for (int i = 0; i < SH_N / 2; ++i) { bv[i] = -INFINITY; bi[i] = 0x7fffffff; }
         TorchPhilox srng = rng;
         if constexpr (PS) per_sample_stream(seed_off, sample, srng);
+        float it_s = inv_t;
+        if constexpr (PP && PS) it_s = params[3 * sample + 2];
         float acc[SH_N / 2];
         ptx::mbar_wait(f_bar, 0);
         int stage = 0;
@@ -288,10 +315,15 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
                     const int jj = jj0 + 2 * n + (q >> 1);
                     const uint4 r4 = torch_philox_call(srng, (uint64_t)jj * (uint64_t)NL + (uint64_t)label, (uint64_t)blk);
                     const uint32_t bits[4] = {r4.x, r4.y, r4.z, r4.w};
+                    float itg[4] = {it_s, it_s, it_s, it_s};
+                    if constexpr (PP && !PS) {
+                        const float4 c4 = reinterpret_cast<const float4*>(col_it)[2 * n + (q >> 1)];
+                        itg[0] = c4.x; itg[1] = c4.y; itg[2] = c4.z; itg[3] = c4.w;
+                    }
 #pragma unroll
                     for (int g = 0; g < 4; ++g) {
                         const float qv = torch_exponential1(u32_to_uniform(bits[g]));
-                        const float gum = fmaf(v[g], inv_t, -__logf(qv));
+                        const float gum = fmaf(v[g], PP ? itg[g] : inv_t, -__logf(qv));
                         if (gum > bv[4 * n + g]) { bv[4 * n + g] = gum; bi[4 * n + g] = label; }
                     }
                 }
@@ -344,10 +376,27 @@ int64_t fused_sampler_rows_padded(int64_t R, int NL) {
 
 // One launch over n_samp streams of hw rows each: n_samp == 1 with seed_off == nullptr is the single-stream draw (seed,
 // offset) over all rows; otherwise seed_off is the device table of the per-sample streams.  Either way the kernel family
-// and the Philox stride follow torch's launch policy for ONE stream's hw * NL elements.
+// and the Philox stride follow torch's launch policy for ONE stream's hw * NL elements.  params == nullptr: one 1/T, inv_t;
+// otherwise the device table [R / phw][3] of per-sample parameters (PP instances).
+template <bool PS, bool PP>
+static void launch_shared(unsigned grid, const CUtensorMap& tf, const CUtensorMap& tw, int R, int NL, int Kc, int rs, int tpb,
+                          float inv_t, TorchPhilox rng, int hw, int n_blocks, const uint64_t* seed_off, const float* params,
+                          int phw, int64_t* out, cudaStream_t st) {
+    fused_sampler_shared_kernel<PS, PP><<<grid, SH_THREADS, PP ? SH_SMEM_PP : SH_SMEM, st>>>(
+        tf, tw, R, NL, Kc, rs, tpb, inv_t, rng, hw, n_blocks, seed_off, params, phw, out);
+}
+
+template <bool PS, bool PP>
+static void launch_generic(unsigned grid, const CUtensorMap& ta, const CUtensorMap& tw, int R, int NL, int Kc, float inv_t,
+                           TorchPhilox rng, int hw, const uint64_t* seed_off, const float* params, int phw, int64_t* out,
+                           cudaStream_t st) {
+    fused_sampler_kernel<PS, PP><<<grid, SMP_THREADS, SMP_SMEM, st>>>(ta, tw, R, NL, Kc, inv_t, rng, hw, seed_off, params, phw, out);
+}
+
 static int launch_sampler(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL, float inv_t,
-                          uint64_t seed, uint64_t offset, const uint64_t* seed_off, int64_t* out, cudaStream_t st) {
-    const bool ps = seed_off != nullptr;
+                          uint64_t seed, uint64_t offset, const uint64_t* seed_off, const float* params, int64_t phw,
+                          int64_t* out, cudaStream_t st) {
+    const bool ps = seed_off != nullptr, pp = params != nullptr;
     const int64_t R = n_samp * hw;
     TorchPhilox rng = make_torch_philox(seed, offset, hw * (int64_t)NL);
     {
@@ -361,8 +410,10 @@ static int launch_sampler(const __half* a16, int64_t n_samp, int64_t hw, int Kc,
             const int tpb = (rs + SH_JJ - 1) / SH_JJ;
             static DeviceOnce attr2;
             if (attr2.first()) {
-                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
-                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
+                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
+                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM));
+                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM_PP));
+                PB_CUDA(cudaFuncSetAttribute(fused_sampler_shared_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_SMEM_PP));
             }
             ProfScope prof("fused_sampler", 2.0 * (double)R * (double)NL * (double)Kc, st);
             CUtensorMap tf, tw;
@@ -373,31 +424,27 @@ static int launch_sampler(const __half* a16, int64_t n_samp, int64_t hw, int Kc,
             PB_TRY(make_tmap_f16_2d(&tw, w16, NL, Kc, Kc, 128));
             const int64_t grid = n_samp * n_blocks * tpb;
             PB_CHECK(grid < (1ll << 31), "fused sampler: %lld CTAs", (long long)grid);
-            if (ps)
-                fused_sampler_shared_kernel<true><<<(unsigned)grid, SH_THREADS, SH_SMEM, st>>>(tf, tw, (int)R, NL, Kc, rs, tpb, inv_t, rng,
-                                                                                               (int)hw, n_blocks, seed_off, out);
-            else
-                fused_sampler_shared_kernel<false><<<(unsigned)grid, SH_THREADS, SH_SMEM, st>>>(tf, tw, (int)R, NL, Kc, rs, tpb, inv_t, rng,
-                                                                                                (int)hw, n_blocks, nullptr, out);
+            auto* fn = ps ? (pp ? launch_shared<true, true> : launch_shared<true, false>)
+                          : (pp ? launch_shared<false, true> : launch_shared<false, false>);
+            fn((unsigned)grid, tf, tw, (int)R, NL, Kc, rs, tpb, inv_t, rng, (int)hw, n_blocks, seed_off, params, (int)phw, out, st);
             PB_LAUNCH_CHECK();
             return 0;
         }
     }
     static DeviceOnce attr_set;
     if (attr_set.first()) {
-        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
-        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
+        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
+        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
+        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
+        PB_CUDA(cudaFuncSetAttribute(fused_sampler_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMP_SMEM));
     }
     ProfScope prof("fused_sampler", 2.0 * (double)R * (double)NL * (double)Kc, st);
     CUtensorMap ta, tw;
     PB_TRY(make_tmap_f16_2d(&ta, a16, R, Kc, Kc, 128));
     PB_TRY(make_tmap_f16_2d(&tw, w16, NL, Kc, Kc, SMP_BN));
-    if (ps)
-        fused_sampler_kernel<true><<<ceil_div(R, 128), SMP_THREADS, SMP_SMEM, st>>>(ta, tw, (int)R, NL, Kc, inv_t, rng, (int)hw,
-                                                                                    seed_off, out);
-    else
-        fused_sampler_kernel<false><<<ceil_div(R, 128), SMP_THREADS, SMP_SMEM, st>>>(ta, tw, (int)R, NL, Kc, inv_t, rng, (int)hw,
-                                                                                     nullptr, out);
+    auto* fn = ps ? (pp ? launch_generic<true, true> : launch_generic<true, false>)
+                  : (pp ? launch_generic<false, true> : launch_generic<false, false>);
+    fn((unsigned)ceil_div(R, 128), ta, tw, (int)R, NL, Kc, inv_t, rng, (int)hw, seed_off, params, (int)phw, out, st);
     PB_LAUNCH_CHECK();
     return 0;
 }
@@ -408,19 +455,33 @@ int launch_fused_sampler(const __half* a16, int64_t R, int Kc, const __half* w16
     PB_CHECK(R * (int64_t)NL < (1ll << 31), "fused sampler: rows*labels >= 2^31 would split the torch kernel (unsupported)");
     PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
     if (R == 0) return 0;
-    return launch_sampler(a16, 1, R, Kc, w16, NL, inv_t, seed, offset, nullptr, out, st);
+    return launch_sampler(a16, 1, R, Kc, w16, NL, inv_t, seed, offset, nullptr, nullptr, 1, out, st);
 }
 
 int launch_fused_sampler_per_sample(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL,
                                     float inv_t, const uint64_t* seed_off, int64_t* out, cudaStream_t st) {
-    PB_CHECK(Kc % 8 == 0 && Kc <= 64 * SMP_MAX_KB, "fused sampler: c_out=%d unsupported (<= %d, multiple of 8)", Kc, 64 * SMP_MAX_KB);
-    PB_CHECK(hw * (int64_t)NL <= (1ll << 29),
-             "fused sampler: a per-sample draw of %lld elements (hw*labels > 2^29) would split the torch kernel (unsupported)",
-             (long long)(hw * (int64_t)NL));
-    PB_CHECK(n_samp * hw < (1ll << 31), "fused sampler: %lld rows", (long long)(n_samp * hw));
     PB_CHECK(seed_off != nullptr, "fused sampler: per-sample (seed, offset) table is NULL");
+    return launch_fused_sampler_params(a16, n_samp, hw, Kc, w16, NL, inv_t, nullptr, 0, 0, seed_off, out, st);
+}
+
+int launch_fused_sampler_params(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL, float inv_t,
+                                const float* params, uint64_t seed, uint64_t offset, const uint64_t* seed_off, int64_t* out,
+                                cudaStream_t st) {
+    PB_CHECK(Kc % 8 == 0 && Kc <= 64 * SMP_MAX_KB, "fused sampler: c_out=%d unsupported (<= %d, multiple of 8)", Kc, 64 * SMP_MAX_KB);
+    PB_CHECK(n_samp * hw < (1ll << 31), "fused sampler: %lld rows", (long long)(n_samp * hw));
+    if (seed_off != nullptr) {
+        PB_CHECK(hw * (int64_t)NL <= (1ll << 29),
+                 "fused sampler: a per-sample draw of %lld elements (hw*labels > 2^29) would split the torch kernel (unsupported)",
+                 (long long)(hw * (int64_t)NL));
+    } else {
+        PB_CHECK(n_samp * hw * (int64_t)NL < (1ll << 31),
+                 "fused sampler: rows*labels >= 2^31 would split the torch kernel (unsupported)");
+        PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
+    }
     if (n_samp == 0 || hw == 0) return 0;
-    return launch_sampler(a16, n_samp, hw, Kc, w16, NL, inv_t, 0, 0, seed_off, out, st);
+    if (seed_off != nullptr)          // one stream per sample: a launch "sample" is a parameter sample
+        return launch_sampler(a16, n_samp, hw, Kc, w16, NL, inv_t, 0, 0, seed_off, params, hw, out, st);
+    return launch_sampler(a16, 1, n_samp * hw, Kc, w16, NL, inv_t, seed, offset, nullptr, params, hw, out, st);
 }
 
 }  // namespace pb

@@ -12,4 +12,10 @@ int launch_fused_sampler(const __half* a16, int64_t R, int Kc, const __half* w16
 // fused_sampler_rows_padded(hw, NL) rows), seed_off DEVICE uint64 [n_samp][2] = (seed, philox offset); out int64 [n_samp * hw]
 int launch_fused_sampler_per_sample(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL,
                                     float inv_t, const uint64_t* seed_off, int64_t* out, cudaStream_t st);
+// per-sample parameters: params DEVICE float [n_samp][3] = (cfg, 1 - cfg, 1/T) of each sample of hw rows (only 1/T is read
+// here).  seed_off == nullptr: one stream (seed, offset) over all n_samp * hw rows, as launch_fused_sampler; otherwise one
+// stream per sample, as launch_fused_sampler_per_sample.  params == nullptr: every row uses inv_t.
+int launch_fused_sampler_params(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL, float inv_t,
+                                const float* params, uint64_t seed, uint64_t offset, const uint64_t* seed_off, int64_t* out,
+                                cudaStream_t st);
 }  // namespace pb

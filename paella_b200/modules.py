@@ -638,11 +638,15 @@ class Paella(nn.Module):
                                         current_stream()), "pb200_paella_logits")
         return out
 
-    def sample_tokens(self, feats: torch.Tensor, batch: int, h: int, w: int, cfg: Optional[float], temperature: float,
-                      generator=None) -> torch.Tensor:
+    def sample_tokens(self, feats: torch.Tensor, batch: int, h: int, w: int, cfg, temperature, generator=None) -> torch.Tensor:
         """Fused out_mapper + CFG + temperature + multinomial on torch's random stream (ref/src/utils.py:44-50).
         ``generator``: None (the default CUDA generator), one CUDA generator, or a list of ``batch`` of them -- one stream per
-        sample, where sample b draws what this call with batch 1 draws on generator b (ops.check_generators)."""
+        sample, where sample b draws what this call with batch 1 draws on generator b (ops.check_generators).
+        ``cfg`` (float or None) and ``temperature`` (float) may also be CPU tensors [batch] of per-sample values; sample b is
+        then computed exactly as this call with its own scalars (ops.sampling_params_table).  ``cfg=None`` is no guidance."""
+        if torch.is_tensor(cfg) or torch.is_tensor(temperature):
+            params = ops.sampling_params_table(cfg, temperature, batch, self._device())
+            return self.sample_tokens_params(feats, batch, h, w, cfg is not None, params, generator)
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -676,6 +680,46 @@ class Paella(nn.Module):
                 check(L.pb200_paella_sample_tokens(self._handle, ptr(f), 1, hi - lo, 1 if cfg is not None else 0,
                                                    float(cfg) if cfg is not None else 0.0, float(temperature), seed, off,
                                                    ptr(flat[lo:hi]), ptr(ws), ws.numel(), current_stream()), "pb200_paella_sample_tokens")
+        return out
+
+    def sample_tokens_params(self, feats: torch.Tensor, batch: int, h: int, w: int, cfg_on: bool, params: torch.Tensor,
+                             generator=None) -> torch.Tensor:
+        """sample_tokens with per-sample guidance scale and temperature in one launch over the batch (per random stream):
+        ``params`` is a device float32 [batch, 3] of (cfg, 1 - cfg, 1/T) (ops.sampling_params_table); its cfg columns are
+        ignored when ``cfg_on`` is False.  Draws on ``generator`` exactly as sample_tokens does."""
+        self._ensure_packed()
+        L = lib()
+        dev = self._device()
+        hw = h * w
+        with torch.cuda.device(dev):
+            out = torch.empty(batch, h, w, dtype=torch.int64, device=dev)
+            ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, batch, h, w, 1))
+            if ops.per_sample(generator):
+                ops.check_generators(generator, batch, dev)
+                ops.check_per_sample_numel(hw * self.num_labels)
+                table = ops.philox_table(generator, hw * self.num_labels, dev)
+                check(L.pb200_paella_sample_tokens_params(self._handle, ptr(feats), batch, hw, int(cfg_on), ptr(params), 0, 0,
+                                                          ptr(table), ptr(out), ptr(ws), ws.numel(), current_stream()),
+                      "pb200_paella_sample_tokens_params")
+                return out
+            n = batch * hw
+            chunks = ops.philox_row_chunks(n, self.num_labels)       # one kernel per 32-bit-indexable piece, like torch
+            flat = out.view(-1)
+            for lo, hi in chunks:
+                if lo % hw or hi % hw:
+                    raise PaellaB200Error("sample_tokens: torch's 32-bit split of this draw falls inside a sample")
+            ops.skip_philox_for_split(chunks, n * self.num_labels, dev, generator)
+            for lo, hi in chunks:
+                seed, off = ops.take_philox((hi - lo) * self.num_labels, dev, generator)
+                if len(chunks) == 1:
+                    f = feats
+                elif cfg_on:
+                    f = torch.cat([feats[lo:hi], feats[n + lo:n + hi]])
+                else:
+                    f = feats[lo:hi]
+                check(L.pb200_paella_sample_tokens_params(self._handle, ptr(f), (hi - lo) // hw, hw, int(cfg_on),
+                                                          ptr(params[lo // hw:hi // hw]), seed, off, None, ptr(flat[lo:hi]), ptr(ws),
+                                                          ws.numel(), current_stream()), "pb200_paella_sample_tokens_params")
         return out
 
     def forward(self, x, r, byt5, clip=None, clip_image=None, x_cat=None, **kwargs):

@@ -110,6 +110,55 @@ def philox_table(generators, numel: int, device) -> torch.Tensor:
     return torch.tensor(vals, dtype=torch.int64, pin_memory=True).view(-1, 2).to(device, non_blocking=True)
 
 
+# ------------------------------------------------------------------ per-sample sampling parameters
+# ``cfg`` and ``temperature`` may be CPU float tensors with one value per sample.  The kernels then read a device table
+# float32 [B, 3] of (cfg, 1 - cfg, 1/T): the fp32 constants the scalar entry points derive from their double arguments,
+# (float)cfg, (float)(1.0 - cfg) and 1.0f / (float)T, so sample b is computed exactly as a scalar call on its own values.
+def per_sample_values(name: str, value, batch: int, pair: bool = False) -> list:
+    """A per-sample argument -- a CPU floating-point tensor [batch] ([batch, 2] for a (start, end) pair) -- as Python floats, each
+    the scalar a call on that sample alone takes.  ValueError for a CUDA tensor (reading it would synchronise the stream), a
+    wrong shape, or a NaN or inf."""
+    if value.device.type != "cpu":
+        raise ValueError(f"{name}: per-sample values must be a CPU tensor (got {value.device}; reading it would synchronise the stream)")
+    if not value.is_floating_point():
+        raise ValueError(f"{name}: per-sample values must be a floating-point tensor (got {value.dtype})")
+    want = (batch, 2) if pair else (batch,)
+    if tuple(value.shape) != want:
+        raise ValueError(f"{name}: per-sample values of shape {list(value.shape)} for a batch of {batch} (expected {list(want)})")
+    if not bool(torch.isfinite(value).all()):
+        raise ValueError(f"{name}: per-sample values must be finite (got {value.tolist()})")
+    return value.tolist()
+
+
+def check_temperatures(name: str, temps) -> None:
+    if not all(t > 0 for t in temps):
+        raise ValueError(f"{name}: every temperature must be > 0 (got {list(temps)})")
+
+
+def sampling_params(cfgs, temperatures) -> torch.Tensor:
+    """CPU float32 [..., 3] of (cfg, 1 - cfg, 1/T) from equally shaped nested lists of Python floats (cfg) and of fp32 values
+    (T): (float)cfg and (float)(1.0 - cfg) from the doubles, 1/T as an fp32 division, like the scalar entry points."""
+    c = torch.tensor(cfgs, dtype=torch.float64)
+    t32 = torch.tensor(temperatures, dtype=torch.float64).float()
+    return torch.stack([c.float(), (1.0 - c).float(), torch.ones_like(t32) / t32], -1)
+
+
+def to_device_async(host: torch.Tensor, device) -> torch.Tensor:
+    """One asynchronous copy from pinned memory: no host synchronisation, no pageable copy."""
+    buf = torch.empty(host.shape, dtype=host.dtype, pin_memory=True)
+    buf.copy_(host)
+    return buf.to(device, non_blocking=True)
+
+
+def sampling_params_table(cfg, temperature, batch: int, device) -> torch.Tensor:
+    """Device float32 [batch, 3] for ``cfg`` (float, None or a CPU tensor [batch]) and ``temperature`` (float or a CPU tensor
+    [batch]); a scalar applies to every sample.  ValueError (nothing enqueued) for a bad per-sample value or a T <= 0."""
+    cfgs = per_sample_values("cfg", cfg, batch) if torch.is_tensor(cfg) else [float(cfg) if cfg is not None else 0.0] * batch
+    temps = per_sample_values("temperature", temperature, batch) if torch.is_tensor(temperature) else [float(temperature)] * batch
+    check_temperatures("temperature", temps)
+    return to_device_async(sampling_params(cfgs, temps), device)
+
+
 # ------------------------------------------------------------------ random ops
 def randint(num_labels: int, size, device, generator=None) -> torch.Tensor:
     """torch.randint(0, num_labels, size, device=device)  [ref/src/utils.py:37]"""
@@ -148,14 +197,30 @@ def multinomial(p: torch.Tensor, generator=None) -> torch.Tensor:
     return out
 
 
-def resample_logits(logits_c: torch.Tensor, logits_u: Optional[torch.Tensor], cfg: float, temperature: float,
-                    mode: str = "multinomial", generator=None) -> torch.Tensor:
-    """ref/src/utils.py:45-50 on reference-layout logits [B,K,H,W] -> tokens [B,H,W]."""
+def resample_logits(logits_c: torch.Tensor, logits_u: Optional[torch.Tensor], cfg, temperature, mode: str = "multinomial",
+                    generator=None) -> torch.Tensor:
+    """ref/src/utils.py:45-50 on reference-layout logits [B,K,H,W] -> tokens [B,H,W].  ``cfg`` and ``temperature`` are floats,
+    or CPU tensors [B] of per-sample values (see sampling_params_table)."""
+    if torch.is_tensor(cfg) or torch.is_tensor(temperature):
+        return resample_logits_params(logits_c, logits_u, sampling_params_table(cfg, temperature, logits_c.shape[0], logits_c.device),
+                                      mode, generator)
+    return _resample_logits(logits_c, logits_u, (float(cfg), float(temperature)), mode, generator)
+
+
+def resample_logits_params(logits_c: torch.Tensor, logits_u: Optional[torch.Tensor], params: torch.Tensor,
+                           mode: str = "multinomial", generator=None) -> torch.Tensor:
+    """resample_logits with per-sample (cfg, 1 - cfg, 1/T): ``params`` device float32 [B, 3] (sampling_params_table), in one
+    launch over the batch per random stream."""
+    return _resample_logits(logits_c, logits_u, params, mode, generator)
+
+
+def _resample_logits(logits_c, logits_u, par, mode, generator):
+    """``par``: (cfg, temperature) floats, or a device params table [B, 3]."""
     if per_sample(generator) and mode == "multinomial":
         check_generators(generator, logits_c.shape[0], logits_c.device)
         check_per_sample_numel(logits_c[0].numel())
-        return torch.cat([resample_logits(logits_c[b:b + 1], logits_u[b:b + 1] if logits_u is not None else None, cfg, temperature,
-                                          mode, g) for b, g in enumerate(generator)])
+        return torch.cat([_resample_logits(logits_c[b:b + 1], logits_u[b:b + 1] if logits_u is not None else None,
+                                           par[b:b + 1] if torch.is_tensor(par) else par, mode, g) for b, g in enumerate(generator)])
     B, K = logits_c.shape[:2]
     hw = logits_c[0, 0].numel()
     lc = logits_c.contiguous().float()
@@ -169,22 +234,45 @@ def resample_logits(logits_c: torch.Tensor, logits_u: Optional[torch.Tensor], cf
             raise _lib.PaellaB200Error("resample_logits: torch's 32-bit split of this draw falls inside a sample")
         b0, b1 = lo // hw, hi // hw
         seed, off = take_philox((hi - lo) * K, lc.device, generator) if m == 0 else (0, 0)
-        check(lib().pb200_resample_logits(ptr(lc[b0:b1]), ptr(lu[b0:b1]) if lu is not None else None, b1 - b0, K, hw, float(cfg),
-                                          float(temperature), m, seed, off, ptr(out[b0:b1]), current_stream()), "pb200_resample_logits")
+        lu_p = ptr(lu[b0:b1]) if lu is not None else None
+        if torch.is_tensor(par):
+            check(lib().pb200_resample_logits_params(ptr(lc[b0:b1]), lu_p, b1 - b0, K, hw, ptr(par[b0:b1]), m, seed, off,
+                                                     ptr(out[b0:b1]), current_stream()), "pb200_resample_logits_params")
+        else:
+            check(lib().pb200_resample_logits(ptr(lc[b0:b1]), lu_p, b1 - b0, K, hw, par[0], par[1], m, seed, off, ptr(out[b0:b1]),
+                                              current_stream()), "pb200_resample_logits")
     return out
 
 
-def resample_quant(logits_c: torch.Tensor, logits_u: Optional[torch.Tensor], cfg: float, temperature: float,
+def resample_quant(logits_c: torch.Tensor, logits_u: Optional[torch.Tensor], cfg, temperature,
                    codebook: torch.Tensor) -> torch.Tensor:
-    """Notebook `mode='quant'`: softmax(l/T) @ codebook, then nearest code -> tokens [B,H,W] (no random draw)."""
+    """Notebook `mode='quant'`: softmax(l/T) @ codebook, then nearest code -> tokens [B,H,W] (no random draw).  ``cfg`` and
+    ``temperature`` as in resample_logits."""
+    if torch.is_tensor(cfg) or torch.is_tensor(temperature):
+        return resample_quant_params(logits_c, logits_u, sampling_params_table(cfg, temperature, logits_c.shape[0], logits_c.device),
+                                     codebook)
+    return _resample_quant(logits_c, logits_u, (float(cfg), float(temperature)), codebook)
+
+
+def resample_quant_params(logits_c: torch.Tensor, logits_u: Optional[torch.Tensor], params: torch.Tensor,
+                          codebook: torch.Tensor) -> torch.Tensor:
+    """resample_quant with per-sample (cfg, 1 - cfg, 1/T) (``params`` as in resample_logits_params), in one launch."""
+    return _resample_quant(logits_c, logits_u, params, codebook)
+
+
+def _resample_quant(logits_c, logits_u, par, codebook):
     B, K = logits_c.shape[:2]
     hw = logits_c[0, 0].numel()
     lc = logits_c.contiguous().float()
     lu = logits_u.contiguous().float() if logits_u is not None else None
     cb = codebook.contiguous().float()
     out = torch.empty((B,) + tuple(logits_c.shape[2:]), dtype=torch.int64, device=lc.device)
-    check(lib().pb200_resample_quant(ptr(lc), ptr(lu), B, K, hw, float(cfg), float(temperature), ptr(cb), cb.shape[1], ptr(out),
-                                     current_stream()), "pb200_resample_quant")
+    if torch.is_tensor(par):
+        check(lib().pb200_resample_quant_params(ptr(lc), ptr(lu), B, K, hw, ptr(par), ptr(cb), cb.shape[1], ptr(out),
+                                                current_stream()), "pb200_resample_quant_params")
+    else:
+        check(lib().pb200_resample_quant(ptr(lc), ptr(lu), B, K, hw, par[0], par[1], ptr(cb), cb.shape[1], ptr(out),
+                                         current_stream()), "pb200_resample_quant")
     return out
 
 

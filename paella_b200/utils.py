@@ -13,6 +13,12 @@ reference does, so ``torch.manual_seed`` means the same thing.  ``generator=[g_0
 stream, consumed in the order a batch-1 loop would: randint over H*W, then per step the multinomial's exponential_ over
 H*W*num_labels (if the step draws) and add_noise's rand over H*W (if it renoises).  A sample's draws then depend only on
 its own seed; its tokens too, bit for bit, where the forward is batch-invariant (DESIGN.md §3 Numerics).
+
+Per-sample settings: ``cfg``, ``temperature``, ``t_start`` and ``t_end`` each also take a CPU float tensor whose first
+dimension is B (``cfg`` [B] in ``sample``, [B, 2] in the other two; ``temperature`` [B, 2]; ``t_start`` / ``t_end`` [B]), in
+any mix with scalar ones.  Sample i is then computed with exactly the scalars a call on its own settings would use: its
+schedules come from the same torch.linspace calls, and the kernels see the same fp32 constants.  The [steps][B] table is
+built on the host once per call and copied to the device once, so the step loop gets no host synchronisation.
 """
 from __future__ import annotations
 
@@ -28,20 +34,64 @@ def _zeros_like_inputs(inputs: Dict[str, torch.Tensor]):
     return {k: (torch.zeros_like(v) if torch.is_tensor(v) else v) for k, v in inputs.items() if v is not None}
 
 
+def _cfg_schedule(cfg, batch: int, steps: int):
+    """``cfg`` of sample_distributed / sample_notebook -> per-step values: None, one list (scalar ``(start, end)``), or one
+    list per sample (a CPU tensor [B, 2]), each from the torch.linspace call the scalar form makes."""
+    if cfg is None:
+        return None
+    if torch.is_tensor(cfg):
+        return [torch.linspace(a, b, steps).tolist() for a, b in ops.per_sample_values("cfg", cfg, batch, pair=True)]
+    return torch.linspace(cfg[0], cfg[1], steps).tolist()
+
+
+def sampling_schedule(batch: int, steps: int, temperature, cfgs, t_start, t_end, per_sample_cfg: bool = False):
+    """The per-call table of per-sample settings, or None when every argument is scalar.
+
+    ``temperature``: (start, end) or a CPU tensor [B, 2]; ``t_start`` / ``t_end``: floats or CPU tensors [B]; ``cfgs``: None, the
+    per-step values, or (``per_sample_cfg``) one such list per sample.  Returns CPU float32 (params [steps, B, 3] of
+    (cfg, 1 - cfg, 1/T), r [steps + 1, B] of the noise levels): sample i's rows are the torch.linspace values a call on its
+    settings alone uses, as the fp32 constants the kernels derive from them (ops.sampling_params).  ValueError for a bad
+    per-sample value or a temperature <= 0."""
+    if not (per_sample_cfg or any(torch.is_tensor(v) for v in (temperature, t_start, t_end))):
+        return None
+    if torch.is_tensor(temperature):
+        tp = ops.per_sample_values("temperature", temperature, batch, pair=True)
+        ops.check_temperatures("temperature", [v for pair in tp for v in pair])
+        temps = torch.stack([torch.linspace(a, b, steps) for a, b in tp])
+    else:
+        ops.check_temperatures("temperature", temperature)
+        temps = torch.linspace(temperature[0], temperature[1], steps).expand(batch, steps)
+    ts = ops.per_sample_values("t_start", t_start, batch) if torch.is_tensor(t_start) else [t_start] * batch
+    te = ops.per_sample_values("t_end", t_end, batch) if torch.is_tensor(t_end) else [t_end] * batch
+    r = torch.stack([torch.linspace(a, b, steps + 1) for a, b in zip(ts, te)])
+    if cfgs is None:
+        c = [[0.0] * steps] * batch
+    else:
+        c = cfgs if per_sample_cfg else [list(cfgs)] * batch
+    params = ops.sampling_params(c, temps.tolist())
+    return params.transpose(0, 1).contiguous(), r.t().contiguous()
+
+
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
-                 codebook=None, generator=None):
+                 codebook=None, generator=None, per_sample_cfg=False):
     B, H, W = latent_shape
     dev = model._device()
     use_cfg_any = cfgs is not None
+    sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg)
     if ops.per_sample(generator):
         ops.check_generators(generator, B, dev)
         ops.check_per_sample_numel(H * W * model.num_labels)
     with torch.inference_mode():
+        if sched is not None:       # one copy for the whole loop: [steps][B][3] params, then [steps + 1][B] noise levels
+            flat = ops.to_device_async(torch.cat([sched[0].view(-1), sched[1].view(-1)]), dev)
+            params_d = flat[:steps * B * 3].view(steps, B, 3)
+            r_d = flat[steps * B * 3:].view(steps + 1, B)
         init_noise = ops.randint(model.num_labels, (B, H, W), dev, generator)
         sampled = init_x.to(dev) if init_x is not None else init_noise.clone()
-        t_list = torch.linspace(t_start, t_end, steps + 1)
-        temperatures = torch.linspace(temperature[0], temperature[1], steps)
+        if sched is None:
+            t_list = torch.linspace(t_start, t_end, steps + 1)
+            temperatures = torch.linspace(temperature[0], temperature[1], steps)
         groups = [model_inputs] + ([unconditional_inputs] if use_cfg_any else [])
         cond_full = model.prepare_conditioning(groups, (H, W))
         cond_only = None
@@ -50,7 +100,6 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             if sampling_quant_steps is not None and i >= sampling_quant_steps:
                 mode = "quant"
             guided = use_cfg_any and i < sampling_conditional_steps
-            t = float(t_list[i])
             if guided:
                 cond, tokens = cond_full, sampled          # one (tokens, r) per CFG pair, see Paella.features
             elif use_cfg_any:
@@ -59,11 +108,17 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 cond, tokens = cond_only, sampled
             else:
                 cond, tokens = cond_full, sampled
-            r = torch.full((tokens.shape[0],), t, dtype=torch.float32, device=dev)
+            if sched is None:
+                r = torch.full((tokens.shape[0],), float(t_list[i]), dtype=torch.float32, device=dev)
+                cfg_i, temp_i = (float(cfgs[i]) if guided else None), float(temperatures[i])
+            else:
+                r, params_i = r_d[i], params_d[i]
             feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided)
-            cfg_i = float(cfgs[i]) if guided else None
             if mode == "multinomial" and not exact:
-                sampled = model.sample_tokens(feats, B, H, W, cfg_i, float(temperatures[i]), generator)
+                if sched is None:
+                    sampled = model.sample_tokens(feats, B, H, W, cfg_i, temp_i, generator)
+                else:
+                    sampled = model.sample_tokens_params(feats, B, H, W, guided, params_i, generator)
             else:
                 n = B * H * W
                 lc = model.logits_from_features(feats[:n], B, H, W)
@@ -71,13 +126,21 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 if mode == "quant":
                     if codebook is None:
                         raise ValueError("mode='quant' needs the VQGAN codebook: pass vqmodel=... (the notebook uses its global `vqmodel`)")
-                    sampled = ops.resample_quant(lc, lu, cfg_i if guided else 0.0, float(temperatures[i]), codebook)
+                    if sched is None:
+                        sampled = ops.resample_quant(lc, lu, cfg_i if guided else 0.0, temp_i, codebook)
+                    else:
+                        sampled = ops.resample_quant_params(lc, lu, params_i, codebook)
+                elif sched is None:
+                    sampled = ops.resample_logits(lc, lu, cfg_i if guided else 0.0, temp_i, mode, generator)
                 else:
-                    sampled = ops.resample_logits(lc, lu, cfg_i if guided else 0.0, float(temperatures[i]), mode, generator)
+                    sampled = ops.resample_logits_params(lc, lu, params_i, mode, generator)
             if collect:
                 intermediates.append(sampled)
             if i < renoise_steps:
-                t_next = torch.full((B,), float(t_list[i + 1]), dtype=torch.float32, device=dev)
+                if sched is None:
+                    t_next = torch.full((B,), float(t_list[i + 1]), dtype=torch.float32, device=dev)
+                else:
+                    t_next = r_d[i + 1]
                 sampled = model.add_noise(sampled, t_next, random_x=init_noise, generator=generator)[0]
                 if collect:
                     intermediates.append(sampled)
@@ -125,12 +188,21 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     ``generator``: None draws on the default CUDA generator; one CUDA ``torch.Generator`` replaces it; a list of B of them gives
     every sample its own stream -- row i draws what this call with batch 1 on sample i's inputs draws after
     ``torch.manual_seed(generator[i].initial_seed())`` (and equals it where the forward is batch-invariant, DESIGN.md §3),
-    and leaves generator i where that call leaves the default generator."""
-    cfgs = [cfg] * steps if cfg else None
+    and leaves generator i where that call leaves the default generator.
+    Per-sample settings (module docstring): ``cfg`` [B], ``temperature`` [B, 2], ``t_start`` / ``t_end`` [B].  A per-sample cfg
+    of 0 is unguided like the scalar ``cfg=0``; so is 1.0, and an all-zero tensor makes the whole call unguided."""
+    per_sample_cfg = torch.is_tensor(cfg)
+    if per_sample_cfg:
+        cfg_vals = [v if v else 1.0 for v in ops.per_sample_values("cfg", cfg, latent_shape[0])]   # f*1 + u*0 = f
+        cfgs = [[v] * steps for v in cfg_vals] if any(cfg.tolist()) else None
+        per_sample_cfg = cfgs is not None
+    else:
+        cfgs = [cfg] * steps if cfg else None
     if cfgs is not None and unconditional_inputs is None:
         raise TypeError("sample(): cfg is set but unconditional_inputs is None")
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, None, steps, renoise_steps,
-                          temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator)
+                          temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
+                          per_sample_cfg=per_sample_cfg)
     return _decode_tail(out, decode, decode_output)
 
 
@@ -138,15 +210,16 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
                        exact=False, generator=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
-    rows [lo, hi) of the single-GPU call draw."""
+    rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
+    ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
         renoise_steps = steps - 1
-    cfgs = torch.linspace(cfg[0], cfg[1], steps).tolist() if cfg is not None else None
+    cfgs = _cfg_schedule(cfg, latent_shape[0], steps)
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
-                          generator=generator)
+                          generator=generator, per_sample_cfg=torch.is_tensor(cfg))
     return out
 
 
@@ -156,15 +229,15 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                     generator=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
-    in ``sample``."""
+    in ``sample``; per-sample settings as in ``sample_distributed``."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
         renoise_steps = steps - 1
     if unconditional_inputs is None:
         unconditional_inputs = _zeros_like_inputs(model_inputs)
-    cfgs = torch.linspace(cfg[0], cfg[1], steps).tolist() if cfg is not None else None
+    cfgs = _cfg_schedule(cfg, latent_shape[0], steps)
     codebook = vqmodel.vquantizer.codebook.weight.data if vqmodel is not None else None
     return _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                         temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, True,
-                        sampling_quant_steps, codebook, generator)
+                        sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg))

@@ -51,6 +51,11 @@ print("sampler", m.sample_tokens(feats, 2, 8, 8, 4.0, 0.7).shape)
 f3 = torch.randn(2 * 3 * 49, cfg["c_out"], device=DEV, generator=g)
 gens = [torch.Generator(device=DEV).manual_seed(s) for s in (1, 2, 3)]
 print("sampler per-sample", m.sample_tokens(f3, 3, 7, 7, 4.0, 0.7, gens).shape)
+# per-sample (cfg, T): the per-row mix and the per-sample 1/T, on per-sample streams and on one stream (staged 1/T columns)
+cfg3, t3 = torch.tensor([4.0, 1.0, 2.5]), torch.tensor([0.7, 1.2, 0.4])
+gens = [torch.Generator(device=DEV).manual_seed(s) for s in (1, 2, 3)]
+print("sampler params per-sample", m.sample_tokens(f3, 3, 7, 7, cfg3, t3, gens).shape)
+print("sampler params one stream", m.sample_tokens(f3, 3, 7, 7, cfg3, t3).shape)
 p = torch.rand(64, 100, device=DEV, generator=g); print("multinomial", ops.multinomial(p).shape)
 t = torch.from_numpy
 print("forward", m(t(gg["x"]).to(DEV), t(gg["r"]).to(DEV), t(gg["byt5"]).to(DEV), clip=t(gg["clip"]).to(DEV)).shape)
