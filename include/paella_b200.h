@@ -91,6 +91,21 @@ int pb200_add_noise(const int64_t* x, const int64_t* random_x, const float* t, i
                     int64_t num_labels, uint64_t seed, uint64_t offset, int64_t* out, int64_t* mask_out,
                     void* stream);
 
+/* One random stream per sample, in ONE launch over the batch (a list of per-sample torch.Generators).  seed_offset: DEVICE
+ * uint64 [batch][2] = (seed, philox offset) of sample b's generator before the draw, offsets multiples of 4.  Sample b draws
+ * exactly what the batch-1 entry point draws on (seed, offset) = seed_offset[b] (torch's launch policy for numel = hw), and
+ * each generator is to be advanced by pb200_philox_offset_increment(hw) per draw.  hw <= 2^29, batch <= 65535.
+ * slot: int32 [batch] or NULL (identity): sample b's row of `out` (and of random_x) is row slot[b] of that buffer. */
+int pb200_randint_per_sample(int64_t* out, const int* slot, int64_t batch, int64_t hw, int64_t num_labels,
+                             const uint64_t* seed_offset, void* stream);
+/* pb200_add_noise per sample: x int64 [batch, hw] and mask_out (or NULL) by sample; t fp32 [batch], and a sample with t < 0
+ * keeps its tokens; random_x (by slot) or NULL -> randint_like drawn after the mask draw, as pb200_add_noise does. */
+int pb200_add_noise_per_sample(const int64_t* x, const int64_t* random_x, const int* slot, const float* t, int64_t batch,
+                               int64_t hw, int64_t num_labels, const uint64_t* seed_offset, int64_t* out, int64_t* mask_out,
+                               void* stream);
+/* out[b] = pool[slot[b]] for rows of hw int64 tokens (b < batch): a step batch gathered from a token pool. */
+int pb200_gather_rows(const int64_t* pool, const int* slot, int64_t batch, int64_t hw, int64_t* out, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Vector quantiser (torchtools.nn.VectorQuantize; call sites ref/src/vqgan.py:94,104).
  * ------------------------------------------------------------------------------------------ */
@@ -276,6 +291,13 @@ int pb200_paella_features(pb200_paella* m, const int64_t* tokens, const float* r
                           int n_attn_weights,
                           int attn_weights_batch, float* features, void* workspace, int64_t workspace_bytes,
                           void* stream);
+/* pb200_paella_features with guidance for only some samples: tokens [Bc,H,W] and r [Bc], Bc = batch_total - n_pairs; sample
+ * Bc + i (i < n_pairs) is sample i under its unconditional rows (kv_slot[Bc + i]).  n_pairs = batch_total / 2 is
+ * cfg_pairs = 1, n_pairs = 0 is cfg_pairs = 0. */
+int pb200_paella_features_pairs(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,
+                                int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
+                                const float* attn_weights, int n_attn_weights, int attn_weights_batch, float* features,
+                                void* workspace, int64_t workspace_bytes, void* stream);
 
 /* out_mapper on features -> logits fp32 NCHW [B, num_labels, H*W]   (ref/src/modules.py:184-187,274) */
 int pb200_paella_logits(pb200_paella* m, const float* features, int batch, int hw, float* logits_nchw,
@@ -308,6 +330,13 @@ int pb200_paella_sample_tokens_per_sample(pb200_paella* m, const float* features
 int pb200_paella_sample_tokens_params(pb200_paella* m, const float* features, int batch, int hw, int cfg_on, const float* params,
                                       uint64_t seed, uint64_t offset, const uint64_t* seed_offset, int64_t* tokens_out,
                                       void* workspace, int64_t workspace_bytes, void* stream);
+/* pb200_paella_sample_tokens_params for the features of pb200_paella_features_pairs, per-sample streams only: features
+ * fp32 [(batch + n_pairs)*HW, c_out]; samples b < n_pairs are guided (CFG mix with their rows at (batch + b)*HW), the others
+ * draw on their conditional rows alone.  n_pairs in {0, batch} computes what pb200_paella_sample_tokens_params with
+ * cfg_on = (n_pairs > 0) computes. */
+int pb200_paella_sample_tokens_pairs(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                                     const uint64_t* seed_offset, int64_t* tokens_out, void* workspace, int64_t workspace_bytes,
+                                     void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * VQGAN (ref/src/vqgan.py:45-107).

@@ -68,7 +68,11 @@ SIGNATURES = {
                                             c_void_p]),
     "pb200_add_noise": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_uint64, c_uint64, c_void_p,
                                 c_void_p, c_void_p]),
-    "pb200_vq_nearest": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "pb200_randint_per_sample": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
+    "pb200_add_noise_per_sample": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                                           c_void_p, c_void_p]),
+    "pb200_gather_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
+    "pb200_vq_nearest":(c_int, [c_void_p, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "pb200_vq_gather": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "pb200_gemm_f16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                POINTER(GemmEpilogue), c_void_p]),
@@ -99,7 +103,11 @@ SIGNATURES = {
     "pb200_paella_c_embeddings": (c_int, [c_void_p, POINTER(Cond), c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_features": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
                                       c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
-    "pb200_paella_logits": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_features_pairs": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
+                                            c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                 c_int64, c_void_p]),
+    "pb200_paella_logits":(c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_sample_tokens": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_uint64,
                                            c_uint64, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_sample_tokens_per_sample": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_void_p,

@@ -646,11 +646,10 @@ int pb200_paella_prepare_cond(pb200_paella* m, const pb200_cond* cond, int batch
     return 0;
 }
 
-int pb200_paella_features(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int cfg_pairs, int h, int w,
-                          const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_weights,
-                          int n_attn_weights,
-                          int attn_weights_batch, float* features, void* workspace, int64_t workspace_bytes,
-                          void* stream) {
+int pb200_paella_features_pairs(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,
+                                int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
+                                const float* attn_weights, int n_attn_weights, int attn_weights_batch, float* features,
+                                void* workspace, int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
     const pb200_paella_config& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -670,18 +669,20 @@ int pb200_paella_features(pb200_paella* m, const int64_t* tokens, const float* r
     int gh[PB200_MAX_LEVELS], gw[PB200_MAX_LEVELS];
     for (int l = 0; l < L; ++l) { gh[l] = (h / ps) >> l; gw[l] = (w / ps) >> l; }
 
-    // Classifier-free-guidance pairs: sample i and sample i + Bt/2 carry the same (tokens, r) and differ only in their
-    // conditioning rows, which enter through the AttnBlocks alone.  Everything before the first AttnBlock (the whole
-    // level-0 down stack of the reference config, 'CT') is therefore computed ONCE for Bt/2 samples and replicated
-    // when the first AttnBlock is reached -- the same arithmetic on the same inputs, not an approximation.
-    PB_CHECK(!cfg_pairs || Bt % 2 == 0, "features: cfg_pairs needs an even batch_total (got %d)", Bt);
-    int Bc = cfg_pairs ? Bt / 2 : Bt;                   // samples currently carried by x
+    // Classifier-free-guidance pairs: the batch is [Bc samples; the unconditional rows of the first n_pairs of them], and
+    // sample i < n_pairs and sample Bc + i carry the same (tokens, r) and differ only in their conditioning rows, which
+    // enter through the AttnBlocks alone.  Everything before the first AttnBlock (the whole level-0 down stack of the
+    // reference config, 'CT') is therefore computed ONCE for the Bc samples, and the first n_pairs samples' rows are
+    // replicated to the tail when the first AttnBlock is reached -- the same arithmetic on the same inputs, not an
+    // approximation.  Guided samples first keeps every replication one contiguous copy.
+    PB_CHECK(n_pairs >= 0 && 2 * n_pairs <= Bt, "features: %d CFG pairs in a batch of %d", n_pairs, Bt);
+    int Bc = Bt - n_pairs;                              // samples currently carried by x
 
     // timestep embedding and every TimestepBlock's (a, b) at once
     PB_TRY(launch_r_embed(r, Bc, c.c_r, ws.r_emb, st));
     PB_TRY(launch_film_table(ws.r_emb, Bc, c.c_r, m->w<float>(m->film_w), m->w<float>(m->film_b), m->film_total, ws.film, st));
     if (Bc < Bt)
-        PB_CUDA(cudaMemcpyAsync(ws.film + (size_t)Bc * m->film_total, ws.film, (size_t)Bc * m->film_total * sizeof(float),
+        PB_CUDA(cudaMemcpyAsync(ws.film + (size_t)Bc * m->film_total, ws.film, (size_t)n_pairs * m->film_total * sizeof(float),
                                 cudaMemcpyDeviceToDevice, st));
     PB_CUDA(cudaMemsetAsync(ws.gsq, 0, (size_t)Bt * 4 * m->max_c * sizeof(uint64_t), st));
     if (Bc < Bt) PB_CUDA(cudaMemsetAsync(ws.gscale, 0, (size_t)Bt * 4 * m->max_c * sizeof(uint64_t), st));
@@ -704,15 +705,15 @@ int pb200_paella_features(pb200_paella* m, const int64_t* tokens, const float* r
     // replicate the shared prefix: x (= xd[l] on the down path) and every saved level output below it
     auto replicate = [&](int level, int attn_index) -> int {
         for (int q = 0; q <= level; ++q) {
-            const size_t n = (size_t)Bc * gh[q] * gw[q] * c.c_hidden[q];
-            PB_CUDA(cudaMemcpyAsync(ws.xd[q] + n, ws.xd[q], n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            const size_t per = (size_t)gh[q] * gw[q] * c.c_hidden[q];
+            PB_CUDA(cudaMemcpyAsync(ws.xd[q] + Bc * per, ws.xd[q], n_pairs * per * sizeof(float), cudaMemcpyDeviceToDevice, st));
         }
         if (attn_index >= 0 && ln_ready == attn_index) {   // the folded-LayerNorm inputs of the AttnBlock that starts here
-            const size_t rows = (size_t)Bc * gh[level] * gw[level];
-            PB_CUDA(cudaMemcpyAsync(ws.a16 + rows * c.c_hidden[level], ws.a16, rows * c.c_hidden[level] * sizeof(__half),
+            const size_t rows = (size_t)Bc * gh[level] * gw[level], pair_rows = (size_t)n_pairs * gh[level] * gw[level];
+            PB_CUDA(cudaMemcpyAsync(ws.a16 + rows * c.c_hidden[level], ws.a16, pair_rows * c.c_hidden[level] * sizeof(__half),
                                     cudaMemcpyDeviceToDevice, st));
             int64_t* stat = ws.lnstat + ws.lnstat_stride * ln_ready;
-            PB_CUDA(cudaMemcpyAsync(stat + 2 * rows, stat, 2 * rows * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+            PB_CUDA(cudaMemcpyAsync(stat + 2 * rows, stat, 2 * pair_rows * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
         }
         Bc = Bt;
         return 0;
@@ -830,12 +831,23 @@ int pb200_paella_features(pb200_paella* m, const int64_t* tokens, const float* r
         e.up_h = gh[0]; e.up_w = gw[0]; e.up_cout = c.c_out;
         PB_TRY(m->gemm(ws.a16, ch, M0, ch, m->clf_w, 4 * (int64_t)c.c_out, e, st));
         PB_TRY(launch_ln_rows(ws.y, (int64_t)Bc * h * w, c.c_out, 1.0f, 0.0f, nullptr, features, st));
-        if (Bc < Bt) {      // a model without any AttnBlock or up path: the two halves are identical to the end
-            const size_t n = (size_t)Bc * h * w * c.c_out;
-            PB_CUDA(cudaMemcpyAsync(features + n, features, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (Bc < Bt) {      // a model without any AttnBlock or up path: the pairs are identical to the end
+            const size_t per = (size_t)h * w * c.c_out;
+            PB_CUDA(cudaMemcpyAsync(features + Bc * per, features, n_pairs * per * sizeof(float), cudaMemcpyDeviceToDevice, st));
         }
     }
     return 0;
+}
+
+int pb200_paella_features(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int cfg_pairs, int h, int w,
+                          const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_weights,
+                          int n_attn_weights,
+                          int attn_weights_batch, float* features, void* workspace, int64_t workspace_bytes,
+                          void* stream) {
+    PB_CHECK(!cfg_pairs || batch_total % 2 == 0, "features: cfg_pairs needs an even batch_total (got %d)", batch_total);
+    return pb200_paella_features_pairs(m, tokens, r, batch_total, cfg_pairs ? batch_total / 2 : 0, h, w, cond_cache, cache_slots,
+                                       kv_slot, s_max, attn_weights, n_attn_weights, attn_weights_batch, features, workspace,
+                                       workspace_bytes, stream);
 }
 
 int pb200_paella_logits(pb200_paella* m, const float* features, int batch, int hw, float* logits_nchw, void* workspace,
@@ -914,6 +926,28 @@ int pb200_paella_sample_tokens_params(pb200_paella* m, const float* features, in
     else
         PB_TRY(launch_cast_f16(features, rows * c.c_out, a16, st));
     return launch_fused_sampler_params(a16, batch, hw, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f, params, seed, offset,
+                                       seed_offset, tokens_out, st);
+}
+
+int pb200_paella_sample_tokens_pairs(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                                     const uint64_t* seed_offset, int64_t* tokens_out, void* workspace, int64_t workspace_bytes,
+                                     void* stream) {
+    PB_CHECK(m->blob != nullptr, "sample_tokens_pairs: weights not bound");
+    PB_CHECK(params != nullptr && seed_offset != nullptr, "sample_tokens_pairs: params and seed_offset are required");
+    const pb200_paella_config& c = m->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+    PB_CHECK(batch >= 0 && hw >= 0 && n_pairs >= 0 && n_pairs <= batch, "sample_tokens_pairs: %d pairs among %d samples", n_pairs,
+             batch);
+    const int64_t rows = (int64_t)batch * hw;
+    if (rows == 0) return 0;
+    PB_CHECK(((int64_t)(batch - 1) * hw + fused_sampler_rows_padded(hw, c.num_labels)) * c.c_out * 2 <= workspace_bytes,
+             "sample_tokens_pairs: workspace too small (use pb200_paella_workspace_bytes)");
+    __half* a16 = reinterpret_cast<__half*>(workspace);
+    // the guided samples' rows get the per-row CFG mix with their unconditional rows at features + rows; the others the cast
+    const int64_t mixed = (int64_t)n_pairs * hw * c.c_out;
+    PB_TRY(launch_mix_cast_rows_f16(features, features + rows * c.c_out, params, (int64_t)hw * c.c_out, mixed, a16, st));
+    PB_TRY(launch_cast_f16(features + mixed, rows * c.c_out - mixed, a16 + mixed, st));
+    return launch_fused_sampler_params(a16, batch, hw, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f, params, 0, 0,
                                        seed_offset, tokens_out, st);
 }
 

@@ -60,6 +60,62 @@ __global__ void add_noise_kernel(const int64_t* __restrict__ x, const int64_t* _
     if (mask_out) mask_out[e] = m ? 1 : 0;
 }
 
+// ------------------------------------------------------------------ one random stream per sample, one launch
+// Sample b = blockIdx.y draws on its own generator: (seed, philox offset) = seed_off[2b], seed_off[2b + 1], with the stride of
+// s (the launch policy of ONE sample's draw of hw elements), so element e of sample b is element e of the batch-1 launch on
+// that generator.  slot (int32 [B] or NULL = identity) places sample b's row of random_x and of out at slot[b] * hw.
+__device__ __forceinline__ TorchPhilox sample_stream(TorchPhilox s, const uint64_t* __restrict__ seed_off, int64_t b) {
+    s.seed = seed_off[2 * b];
+    s.offset4 = seed_off[2 * b + 1] >> 2;
+    return s;
+}
+
+__global__ void randint_per_sample_kernel(int64_t* __restrict__ out, const int* __restrict__ slot, int64_t hw, uint32_t range,
+                                          TorchPhilox s, const uint64_t* __restrict__ seed_off) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= hw) return;
+    const int64_t b = blockIdx.y;
+    const int64_t dst = slot ? slot[b] : b;
+    out[dst * hw + e] = (int64_t)(torch_philox_u32(sample_stream(s, seed_off, b), (uint64_t)e) % range);
+}
+
+// x: int64 [B, hw] (by sample); t: fp32 [B], and a sample with t < 0 keeps x (u >= 0 never passes the mask test: the
+// sampling engine's rows that do not renoise this step).  random_x == NULL: randint_like drawn at the offset after the mask
+// draw, as pb200_add_noise does (rx_inc4 = that offset increment / 4).
+__global__ void add_noise_per_sample_kernel(const int64_t* __restrict__ x, const int64_t* __restrict__ random_x,
+                                            const int* __restrict__ slot, const float* __restrict__ t, int64_t hw,
+                                            uint32_t num_labels, TorchPhilox s, uint64_t rx_inc4,
+                                            const uint64_t* __restrict__ seed_off, int64_t* __restrict__ out,
+                                            int64_t* __restrict__ mask_out) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= hw) return;
+    const int64_t b = blockIdx.y;
+    const int64_t dst = slot ? slot[b] : b;
+    const TorchPhilox sm = sample_stream(s, seed_off, b);
+    float u = u32_to_uniform(torch_philox_u32(sm, (uint64_t)e));
+    u = (u == 1.0f) ? 0.0f : u;
+    const bool m = u <= t[b];
+    int64_t rx;
+    if (random_x) {
+        rx = random_x[dst * hw + e];
+    } else {
+        TorchPhilox sr = sm;
+        sr.offset4 += rx_inc4;
+        rx = (int64_t)(torch_philox_u32(sr, (uint64_t)e) % num_labels);
+    }
+    out[dst * hw + e] = m ? rx : x[b * hw + e];
+    if (mask_out) mask_out[b * hw + e] = m ? 1 : 0;
+}
+
+// out[b] = pool[slot[b]] for rows of hw tokens: the sampling engine's batch of one step, in that step's row order
+__global__ void gather_rows_kernel(const int64_t* __restrict__ pool, const int* __restrict__ slot, int64_t hw,
+                                   int64_t* __restrict__ out) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= hw) return;
+    const int64_t b = blockIdx.y;
+    out[b * hw + e] = pool[(int64_t)slot[b] * hw + e];
+}
+
 // ------------------------------------------------------------------ multinomial(p, 1): argmax p/q, first index on ties
 struct ArgBest {
     float v;
@@ -393,6 +449,48 @@ int pb200_add_noise(const int64_t* x, const int64_t* random_x, const float* t, i
     TorchPhilox s_rx = make_torch_philox(seed, offset + offset_increment(n), n);
     add_noise_kernel<<<ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(x, random_x, t, batch, hw, (uint32_t)num_labels,
                                                                          s_mask, s_rx, out, mask_out);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
+static int check_per_sample(int64_t batch, int64_t hw, const uint64_t* seed_offset, const char* what) {
+    PB_CHECK(seed_offset != nullptr, "%s: per-sample (seed, offset) table is NULL", what);
+    PB_CHECK(batch >= 0 && batch <= 65535, "%s: batch %lld out of range (<= 65535)", what, (long long)batch);
+    PB_CHECK(hw >= 0 && hw <= (1ll << 29), "%s: a per-sample draw of %lld elements (> 2^29) would split the torch kernel", what,
+             (long long)hw);
+    return 0;
+}
+
+int pb200_randint_per_sample(int64_t* out, const int* slot, int64_t batch, int64_t hw, int64_t num_labels,
+                             const uint64_t* seed_offset, void* stream) {
+    PB_TRY(check_per_sample(batch, hw, seed_offset, "randint_per_sample"));
+    PB_CHECK(num_labels > 0 && num_labels < (1ll << 28), "randint_per_sample: range %lld needs the 64-bit path (unsupported)",
+             (long long)num_labels);
+    if (batch == 0 || hw == 0) return 0;
+    const TorchPhilox s = make_torch_philox(0, 0, hw);
+    randint_per_sample_kernel<<<dim3(ceil_div(hw, 256), (unsigned)batch), 256, 0, (cudaStream_t)stream>>>(
+        out, slot, hw, (uint32_t)num_labels, s, seed_offset);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
+int pb200_add_noise_per_sample(const int64_t* x, const int64_t* random_x, const int* slot, const float* t, int64_t batch,
+                               int64_t hw, int64_t num_labels, const uint64_t* seed_offset, int64_t* out, int64_t* mask_out,
+                               void* stream) {
+    PB_TRY(check_per_sample(batch, hw, seed_offset, "add_noise_per_sample"));
+    PB_CHECK(num_labels > 0 && num_labels < (1ll << 28), "add_noise_per_sample: bad num_labels");
+    if (batch == 0 || hw == 0) return 0;
+    const TorchPhilox s = make_torch_philox(0, 0, hw);
+    add_noise_per_sample_kernel<<<dim3(ceil_div(hw, 256), (unsigned)batch), 256, 0, (cudaStream_t)stream>>>(
+        x, random_x, slot, t, hw, (uint32_t)num_labels, s, (uint64_t)offset_increment(hw) / 4, seed_offset, out, mask_out);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
+int pb200_gather_rows(const int64_t* pool, const int* slot, int64_t batch, int64_t hw, int64_t* out, void* stream) {
+    PB_CHECK(batch >= 0 && batch <= 65535 && hw >= 0, "gather_rows: bad shape");
+    if (batch == 0 || hw == 0) return 0;
+    gather_rows_kernel<<<dim3(ceil_div(hw, 256), (unsigned)batch), 256, 0, (cudaStream_t)stream>>>(pool, slot, hw, out);
     PB_LAUNCH_CHECK();
     return 0;
 }

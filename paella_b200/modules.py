@@ -601,18 +601,24 @@ class Paella(nn.Module):
 
     # -------------------------------------------------------------- forward pieces
     def features(self, x: torch.Tensor, r: torch.Tensor, cond: ConditioningCache, attn_weights=None,
-                 attn_weights_batch: int = 0, cfg_pairs: bool = False) -> torch.Tensor:
+                 attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
         evaluated under the conditional rows [0,B) and the unconditional rows [B,2B) of ``cond``; the result has 2B
-        samples, and the conditioning-independent blocks before the first AttnBlock run once per pair."""
+        samples, and the conditioning-independent blocks before the first AttnBlock run once per pair.
+        ``n_pairs``: only the first n_pairs samples of x [B,H,W] are guided; the result has B + n_pairs samples, sample
+        B + i being sample i under its unconditional rows (n_pairs = B is ``cfg_pairs=True``, 0 is unguided)."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
         Bt, H, W = x.shape
-        if cfg_pairs:
-            Bt *= 2
+        if n_pairs is not None:
+            if cfg_pairs or not 0 <= n_pairs <= Bt:
+                raise PaellaB200Error(f"features: n_pairs={n_pairs} for {Bt} samples (and not with cfg_pairs)")
+        else:
+            n_pairs = Bt if cfg_pairs else 0
+        Bt += n_pairs
         if Bt != cond.batch_total:
             raise PaellaB200Error(f"batch {Bt} does not match the conditioning cache ({cond.batch_total})")
         with torch.cuda.device(dev):
@@ -621,10 +627,10 @@ class Paella(nn.Module):
             ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, Bt, H, W, cond.s_max))
             feats = torch.empty(Bt * H * W, self._cfg["c_out"], dtype=torch.float32, device=dev)
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
-            check(L.pb200_paella_features(self._handle, ptr(x), ptr(r), Bt, int(cfg_pairs), H, W, ptr(cond.cache), cond.slots,
-                                          ptr(cond.slot_map), cond.s_max, ptr(aw),
-                                          aw.numel() if aw is not None else 0, attn_weights_batch, ptr(feats), ptr(ws),
-                                          ws.numel(), current_stream()), "pb200_paella_features")
+            check(L.pb200_paella_features_pairs(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                ptr(cond.slot_map), cond.s_max, ptr(aw),
+                                                aw.numel() if aw is not None else 0, attn_weights_batch, ptr(feats), ptr(ws),
+                                                ws.numel(), current_stream()), "pb200_paella_features_pairs")
         return feats
 
     def logits_from_features(self, feats: torch.Tensor, batch: int, h: int, w: int) -> torch.Tensor:
@@ -721,6 +727,55 @@ class Paella(nn.Module):
                                                           ptr(params[lo // hw:hi // hw]), seed, off, None, ptr(flat[lo:hi]), ptr(ws),
                                                           ws.numel(), current_stream()), "pb200_paella_sample_tokens_params")
         return out
+
+    def sample_tokens_pairs(self, feats: torch.Tensor, batch: int, n_pairs: int, h: int, w: int, params: torch.Tensor,
+                            seed_offset: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """sample_tokens_params on the features of ``features(..., n_pairs=n_pairs)``: samples b < n_pairs are guided, the rest
+        draw on their conditional rows alone, all in one launch on per-sample streams (``seed_offset``: ops.philox_table over
+        h * w * num_labels)."""
+        self._ensure_packed()
+        L = lib()
+        dev = self._device()
+        with torch.cuda.device(dev):
+            if out is None:
+                out = torch.empty(batch, h, w, dtype=torch.int64, device=dev)
+            ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, batch, h, w, 1))
+            check(L.pb200_paella_sample_tokens_pairs(self._handle, ptr(feats), batch, n_pairs, h * w, ptr(params), ptr(seed_offset),
+                                                     ptr(out), ptr(ws), ws.numel(), current_stream()),
+                  "pb200_paella_sample_tokens_pairs")
+        return out
+
+    def conditioning_seq_len(self, inputs: Dict[str, torch.Tensor]) -> int:
+        """Length of the conditioning sequence of ``inputs`` (byt5 rows + clip_seq_len per clip / clip_image embedding)."""
+        n = (1 if inputs.get("clip") is not None else 0)
+        ci = inputs.get("clip_image")
+        if ci is not None:
+            n += len(ci) if isinstance(ci, (list, tuple)) else 1
+        return inputs["byt5"].shape[1] + self._cfg["clip_seq_len"] * n
+
+    def write_conditioning(self, cache: ConditioningCache, slot: int, inputs: Dict[str, torch.Tensor], latent_hw) -> None:
+        """Project one sample's conditioning (batch-1 ``inputs``) into slot ``slot`` of an existing cache, as
+        prepare_conditioning projects a group of one; the slot's kv_len becomes this sequence's length, so rows left over
+        from a longer sequence are never attended to.  Host-to-device copies are asynchronous (no stream synchronisation)."""
+        self._ensure_packed()
+        L = lib()
+        dev = self._device()
+
+        def d(v):
+            return v.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
+        with torch.cuda.device(dev):
+            cond = _lib.Cond()
+            byt5 = d(inputs["byt5"])
+            cond.byt5, cond.byt5_len = ptr(byt5).value, byt5.shape[1]
+            clip = d(inputs["clip"]) if inputs.get("clip") is not None else None
+            cond.clip = ptr(clip).value if clip is not None else None
+            ci = inputs.get("clip_image")
+            if ci is not None:
+                ci = torch.stack([d(v) for v in ci]) if isinstance(ci, (list, tuple)) else d(ci)[None]
+                cond.clip_image, cond.n_clip_image = ptr(ci).value, ci.shape[0]
+            ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, 1, latent_hw[0], latent_hw[1], cache.s_max))
+            check(L.pb200_paella_prepare_cond(self._handle, ctypes.byref(cond), 1, slot, cache.slots, cache.s_max, ptr(cache.cache),
+                                              ptr(ws), ws.numel(), current_stream()), "pb200_paella_prepare_cond")
 
     def forward(self, x, r, byt5, clip=None, clip_image=None, x_cat=None, **kwargs):
         """ref/src/modules.py:263-275 / ref/utils/modules.py:268-282: logits [B, num_labels, H, W] fp32."""

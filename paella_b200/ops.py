@@ -97,16 +97,23 @@ def check_per_sample_numel(numel: int) -> None:
                          "into two kernels (unsupported); use a smaller latent grid")
 
 
-def philox_table(generators, numel: int, device) -> torch.Tensor:
-    """Device int64 [B, 2] of (seed, philox offset) for one draw of ``numel`` elements per sample; advances each generator.
-    Built in pinned memory and copied asynchronously: no host synchronisation, no pageable copy."""
+def philox_values(generators, numel: int, device) -> list:
+    """The (seed, philox offset) pairs, flattened, of one draw of ``numel`` elements per sample as int64 values (the uint64
+    seed bit for bit); advances each generator."""
     check_per_sample_numel(numel)
     vals = []
     for g in generators:
         seed, off = take_philox(numel, device, g)
         if off % 4:
             raise ValueError(f"generator offset {off} is not a multiple of 4")
-        vals += [seed - 2 ** 64 if seed >= 2 ** 63 else seed, off]       # uint64 seed, bit for bit
+        vals += [seed - 2 ** 64 if seed >= 2 ** 63 else seed, off]
+    return vals
+
+
+def philox_table(generators, numel: int, device) -> torch.Tensor:
+    """Device int64 [B, 2] of (seed, philox offset) for one draw of ``numel`` elements per sample; advances each generator.
+    Built in pinned memory and copied asynchronously: no host synchronisation, no pageable copy."""
+    vals = philox_values(generators, numel, device)
     return torch.tensor(vals, dtype=torch.int64, pin_memory=True).view(-1, 2).to(device, non_blocking=True)
 
 
@@ -165,14 +172,20 @@ def randint(num_labels: int, size, device, generator=None) -> torch.Tensor:
     out = torch.empty(size, dtype=torch.int64, device=device)
     if per_sample(generator):
         check_generators(generator, out.shape[0], out.device)
-        per = out[0].numel()
-        check_per_sample_numel(per)
-        for b, g in enumerate(generator):
-            seed, off = take_philox(per, out.device, g)
-            check(lib().pb200_randint(ptr(out[b]), per, num_labels, seed, off, current_stream()), "pb200_randint")
-        return out
+        return randint_per_sample(out, num_labels, philox_table(generator, out[0].numel(), out.device))
     seed, off = take_philox(out.numel(), out.device, generator)
     check(lib().pb200_randint(ptr(out), out.numel(), num_labels, seed, off, current_stream()), "pb200_randint")
+    return out
+
+
+def randint_per_sample(out: torch.Tensor, num_labels: int, table: torch.Tensor, slot: Optional[torch.Tensor] = None,
+                       batch: Optional[int] = None) -> torch.Tensor:
+    """One launch of per-sample randint draws: sample b draws on (seed, offset) = ``table[b]`` (philox_table) what a batch-1
+    randint over ``out[0].numel()`` elements draws, into row b of ``out`` (row ``slot[b]`` with an int32 device slot map)."""
+    hw = out[0].numel()
+    n = out.shape[0] if batch is None else batch
+    check(lib().pb200_randint_per_sample(ptr(out), ptr(slot), n, hw, num_labels, ptr(table), current_stream()),
+          "pb200_randint_per_sample")
     return out
 
 
@@ -287,15 +300,11 @@ def add_noise(x: torch.Tensor, t: torch.Tensor, random_x: Optional[torch.Tensor]
     if per_sample(generator):
         check_generators(generator, B, x.device)
         check_per_sample_numel(hw)
-        t = t.contiguous().float()
-        random_x = random_x.contiguous() if random_x is not None else None
-        for b, g in enumerate(generator):
-            seed, off = take_philox(hw, x.device, g)
-            if random_x is None:
-                take_philox(hw, x.device, g)
-            check(lib().pb200_add_noise(ptr(x[b]), ptr(random_x[b]) if random_x is not None else None, ptr(t[b:b + 1]), 1, hw,
-                                        num_labels, seed, off, ptr(out[b]), ptr(mask[b]) if mask is not None else None,
-                                        current_stream()), "pb200_add_noise")
+        table = philox_table(generator, hw, x.device)
+        if random_x is None:
+            philox_values(generator, hw, x.device)          # the randint_like draw follows the mask draw
+        add_noise_per_sample(x, t.contiguous().float(), random_x.contiguous() if random_x is not None else None, num_labels, table,
+                             out, mask)
         return out, mask
     seed, off = take_philox(x.numel(), x.device, generator)
     if random_x is None:
@@ -305,6 +314,22 @@ def add_noise(x: torch.Tensor, t: torch.Tensor, random_x: Optional[torch.Tensor]
     check(lib().pb200_add_noise(ptr(x), ptr(random_x), ptr(t.contiguous().float()), B, hw, num_labels, seed, off, ptr(out),
                                 ptr(mask), current_stream()), "pb200_add_noise")
     return out, mask
+
+
+def add_noise_per_sample(x: torch.Tensor, t: torch.Tensor, random_x: Optional[torch.Tensor], num_labels: int, table: torch.Tensor,
+                         out: torch.Tensor, mask: Optional[torch.Tensor] = None, slot: Optional[torch.Tensor] = None) -> None:
+    """One launch of per-sample add_noise: sample b (x [B, ...], t fp32 [B]) draws its mask on (seed, offset) = ``table[b]`` and
+    takes random_x (or, when None, the randint_like drawn at the next offset) where the mask is set; a sample with t < 0 keeps
+    its tokens.  ``slot`` (int32 [B]) places sample b's rows of random_x and out at row slot[b] of those buffers."""
+    B, hw = x.shape[0], x[0].numel()
+    check(lib().pb200_add_noise_per_sample(ptr(x), ptr(random_x), ptr(slot), ptr(t), B, hw, num_labels, ptr(table), ptr(out),
+                                           ptr(mask), current_stream()), "pb200_add_noise_per_sample")
+
+
+def gather_rows(pool: torch.Tensor, slot: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out[b] = pool[slot[b]] (int64 token rows; ``slot`` int32 [out.shape[0]] on the device), in one launch."""
+    check(lib().pb200_gather_rows(ptr(pool), ptr(slot), out.shape[0], out[0].numel(), ptr(out), current_stream()), "pb200_gather_rows")
+    return out
 
 
 # ------------------------------------------------------------------ vector quantiser

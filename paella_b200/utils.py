@@ -44,15 +44,16 @@ def _cfg_schedule(cfg, batch: int, steps: int):
     return torch.linspace(cfg[0], cfg[1], steps).tolist()
 
 
-def sampling_schedule(batch: int, steps: int, temperature, cfgs, t_start, t_end, per_sample_cfg: bool = False):
-    """The per-call table of per-sample settings, or None when every argument is scalar.
+def sampling_schedule(batch: int, steps: int, temperature, cfgs, t_start, t_end, per_sample_cfg: bool = False,
+                      always: bool = False):
+    """The per-call table of per-sample settings, or None when every argument is scalar (and not ``always``).
 
     ``temperature``: (start, end) or a CPU tensor [B, 2]; ``t_start`` / ``t_end``: floats or CPU tensors [B]; ``cfgs``: None, the
     per-step values, or (``per_sample_cfg``) one such list per sample.  Returns CPU float32 (params [steps, B, 3] of
     (cfg, 1 - cfg, 1/T), r [steps + 1, B] of the noise levels): sample i's rows are the torch.linspace values a call on its
     settings alone uses, as the fp32 constants the kernels derive from them (ops.sampling_params).  ValueError for a bad
     per-sample value or a temperature <= 0."""
-    if not (per_sample_cfg or any(torch.is_tensor(v) for v in (temperature, t_start, t_end))):
+    if not (always or per_sample_cfg or any(torch.is_tensor(v) for v in (temperature, t_start, t_end))):
         return None
     if torch.is_tensor(temperature):
         tp = ops.per_sample_values("temperature", temperature, batch, pair=True)

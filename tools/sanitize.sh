@@ -57,6 +57,22 @@ gens = [torch.Generator(device=DEV).manual_seed(s) for s in (1, 2, 3)]
 print("sampler params per-sample", m.sample_tokens(f3, 3, 7, 7, cfg3, t3, gens).shape)
 print("sampler params one stream", m.sample_tokens(f3, 3, 7, 7, cfg3, t3).shape)
 p = torch.rand(64, 100, device=DEV, generator=g); print("multinomial", ops.multinomial(p).shape)
+# one-launch per-sample RNG on an odd H*W, and the sampling engine: partial CFG pairs, slot maps, a slot reused by a request
+# with a shorter conditioning sequence (slot 0 frees after 1 step and takes the third request)
+x7 = torch.randint(0, 64, (3, 7, 9), device=DEV, generator=g)
+gens = [torch.Generator(device=DEV).manual_seed(s) for s in (1, 2, 3)]
+print("randint per-sample", ops.randint(64, (3, 7, 9), DEV, gens).shape, "add_noise per-sample",
+      ops.add_noise(x7, torch.tensor([0.5, -1.0, 0.9], device=DEV), None, 64, gens)[0].shape)
+from paella_b200.engine import SamplingEngine
+def cond(L, ci):
+    d = {"byt5": torch.randn(1, L, cfg["byt5_embd"], device=DEV, generator=g), "clip": torch.randn(1, cfg["clip_embd"], device=DEV, generator=g)}
+    if ci: d["clip_image"] = torch.randn(1, cfg["clip_embd"], device=DEV, generator=g)
+    return d
+eng = SamplingEngine(m, latent_hw=(8, 8), max_batch=2, max_cond_len=20, unconditional_inputs={k: v * 0 for k, v in cond(4, False).items()})
+eng.submit(cond(12, True), generator=torch.Generator(device=DEV).manual_seed(1), steps=1)
+eng.submit(cond(5, False), generator=torch.Generator(device=DEV).manual_seed(2), steps=3, cfg=None)
+eng.submit(cond(2, False), generator=torch.Generator(device=DEV).manual_seed(3), steps=2, sampling_conditional_steps=1)
+print("engine", [q.result.shape for q in eng.run_until_idle()])
 t = torch.from_numpy
 print("forward", m(t(gg["x"]).to(DEV), t(gg["r"]).to(DEV), t(gg["byt5"]).to(DEV), clip=t(gg["clip"]).to(DEV)).shape)
 torch.cuda.synchronize(); print("sanitizer case 2 done")
