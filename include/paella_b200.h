@@ -298,6 +298,20 @@ int pb200_paella_features_pairs(pb200_paella* m, const int64_t* tokens, const fl
                                 int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
                                 const float* attn_weights, int n_attn_weights, int attn_weights_batch, float* features,
                                 void* workspace, int64_t workspace_bytes, void* stream);
+/* pb200_paella_features_pairs with one attn_weights vector per sample, so that samples whose prompts (and so whose
+ * vectors) differ share one forward.  It replaces the per-call `attn_weights` of CustomMultiheadAttention.forward
+ * (ref/utils/alter_attention.py:23-34), which the notebook's text-to-image cell builds from each prompt's ByT5 length.
+ *   attn_w  fp32 table of rows w_ld floats apart (device memory), or NULL for no weights at all;
+ *   w_len   int32 [rows]: the length of each row (0: the sample is unweighted), or NULL: every row has n_w entries;
+ *   w_row   int32 [w_batch]: the row sample b reads, or NULL: row b;
+ *   w_batch samples [0, w_batch) are weighted (the unconditional tail of a CFG batch is not, as in the reference).
+ * Sample b scales, after the softmax and without renormalising, the last w_len[row] keys of its own [self ; cond] key list
+ * in every AttnBlock.  Each length must not exceed the smallest key count that sample sees in any AttnBlock, where the
+ * reference fails.  w_ld = 0 with w_len = NULL is the single vector of pb200_paella_features_pairs, which is this call. */
+int pb200_paella_features_weighted(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,
+                                   int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
+                                   const float* attn_w, int n_w, int w_ld, const int* w_len, const int* w_row, int w_batch,
+                                   float* features, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* out_mapper on features -> logits fp32 NCHW [B, num_labels, H*W]   (ref/src/modules.py:184-187,274) */
 int pb200_paella_logits(pb200_paella* m, const float* features, int batch, int hw, float* logits_nchw,

@@ -105,6 +105,9 @@ SIGNATURES = {
                                       c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_features_pairs": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
                                             c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_features_weighted": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                               c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64,
+                                               c_void_p]),
     "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_int64, c_void_p]),
     "pb200_paella_logits":(c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),

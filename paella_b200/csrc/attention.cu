@@ -105,8 +105,10 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
     for (int i = 0; i < HD / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
     float m_run[2] = {NEG_BIG, NEG_BIG}, l_run[2] = {0.f, 0.f};
 
-    const bool weighted = p.attn_w != nullptr && b < p.w_batch && p.n_w > 0;
-    const int w_start = Nk - p.n_w;
+    const float* w_row = nullptr;
+    const int n_w = attn_weight_row(p, b, w_row);
+    const bool weighted = n_w > 0;
+    const int w_start = Nk - n_w;
 
     auto load_q_frags = [&]() {
 #pragma unroll
@@ -178,7 +180,7 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int kj = key + (e & 1);
-                    if (kj >= w_start && kj < Nk) s[nt][e] *= p.attn_w[kj - w_start];
+                    if (kj >= w_start && kj < Nk) s[nt][e] *= w_row[kj - w_start];
                 }
             }
         }

@@ -82,8 +82,10 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
     }
     __syncthreads();
 
-    const bool weighted = p.attn_w != nullptr && b < p.w_batch && p.n_w > 0;
-    const int w_start = Nk - p.n_w;
+    const float* w_row = nullptr;
+    const int n_w = attn_weight_row(p, b, w_row);
+    const bool weighted = n_w > 0;
+    const int w_start = Nk - n_w;
     float o[AW_HD / 2];
 #pragma unroll
     for (int i = 0; i < AW_HD / 2; ++i) o[i] = 0.f;
@@ -159,7 +161,7 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
             rs[(i >> 1) & 1] += pv;
             if (weighted) {       // post-softmax, un-renormalised scaling of the last n_w keys
                 const int kj = key0 + col;
-                if (kj >= w_start && col < valid) pv *= p.attn_w[kj - w_start];
+                if (kj >= w_start && col < valid) pv *= w_row[kj - w_start];
             }
             s[i] = pv;
         }

@@ -646,11 +646,12 @@ int pb200_paella_prepare_cond(pb200_paella* m, const pb200_cond* cond, int batch
     return 0;
 }
 
-int pb200_paella_features_pairs(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,
-                                int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
-                                const float* attn_weights, int n_attn_weights, int attn_weights_batch, float* features,
-                                void* workspace, int64_t workspace_bytes, void* stream) {
+int pb200_paella_features_weighted(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,
+                                   int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
+                                   const float* attn_w, int n_w, int w_ld, const int* w_len, const int* w_row, int w_batch,
+                                   float* features, void* workspace, int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
+    PB_CHECK(w_ld >= 0, "features: attention-weight row stride %d < 0", w_ld);
     const pb200_paella_config& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
     const int Bt = batch_total, ps = c.patch_size, L = c.n_levels;
@@ -812,7 +813,8 @@ int pb200_paella_features_pairs(pb200_paella* m, const int64_t* tokens, const fl
                 ap.B = Bt; ap.P = P; ap.S_max = s_max; ap.E = ch; ap.nhead = c.nhead[l];
                 ap.self_attn = c.self_attn;
                 ap.scale_log2 = 1.4426950408889634f / sqrtf((float)(ch / c.nhead[l]));
-                ap.attn_w = attn_weights; ap.n_w = n_attn_weights; ap.w_batch = attn_weights_batch;
+                ap.attn_w = attn_w; ap.n_w = n_w; ap.w_batch = w_batch;
+                ap.w_ld = w_ld; ap.w_len = w_len; ap.w_row = w_row;
                 PB_TRY(launch_attention(ap, st));
                 pb200_gemm_epilogue e2 = epi(PB200_EPI_RESID_F32, m->w<float>(b.outproj_b), x, ch);
                 e2.resid = x; e2.ldr = ch; e2.rows_per_sample = P;
@@ -837,6 +839,15 @@ int pb200_paella_features_pairs(pb200_paella* m, const int64_t* tokens, const fl
         }
     }
     return 0;
+}
+
+int pb200_paella_features_pairs(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,
+                                int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
+                                const float* attn_weights, int n_attn_weights, int attn_weights_batch, float* features,
+                                void* workspace, int64_t workspace_bytes, void* stream) {
+    return pb200_paella_features_weighted(m, tokens, r, batch_total, n_pairs, h, w, cond_cache, cache_slots, kv_slot, s_max,
+                                          attn_weights, n_attn_weights, 0, nullptr, nullptr, attn_weights_batch, features,
+                                          workspace, workspace_bytes, stream);
 }
 
 int pb200_paella_features(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int cfg_pairs, int h, int w,

@@ -14,7 +14,11 @@ A request's tokens are those of ``sample_distributed(model, inputs, uncond, (1, 
 temperature, cfg, t_start, t_end, sampling_conditional_steps, generator=[g])``: the same draws from ``g`` in the same order
 (randint at admission, then per step the sampler's exponential draw and, if the step renoises, the mask draw), the same
 torch.linspace schedules and fp32 kernel constants (utils.sampling_schedule), and ``g`` left at the same offset.  Where the
-forward is batch-invariant (DESIGN.md §3) the tokens are equal bit for bit, whatever else is in flight.
+forward is batch-invariant (DESIGN.md §3) the tokens are equal bit for bit, whatever else is in flight.  With
+``attn_weights=w`` (and ``keep_intermediates=True``) the request's tokens, ``req.intermediates`` and generator offset are those
+of ``sample_notebook(model, inputs, (1, H, W), uncond, init_x, steps, renoise_steps, temperature, cfg, 'multinomial', t_start,
+t_end, sampling_conditional_steps, attn_weights=w, generator=[g])``; each step's batch reads every row's weights from a
+device pool indexed by its token slot.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -38,13 +42,18 @@ from .modules import ConditioningCache, Paella
 
 class Request:
     """One submitted request.  ``result`` is set (a device tensor) in the ``step()`` that retires it: int64 tokens [1, H, W],
-    or with ``decode=True`` the uint8 NHWC image [1, 4H, 4W, 3]."""
+    or with ``decode=True`` the uint8 NHWC image [1, 4H, 4W, 3].  With ``keep_intermediates=True``, ``intermediates`` grows by
+    the sampled tokens of every step, then the renoised tokens if the step renoises."""
 
     def __init__(self, steps: int, renoise_steps: int, cond_steps: int, guided: bool, params: torch.Tensor, r: torch.Tensor,
-                 generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False):
+                 generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False,
+                 attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
+        self.attn_weights = attn_weights         # CPU float32 [n] or None
+        # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
+        self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
         self.slot: Optional[int] = None          # token pool slot and conditional K/V slot
         self.uncond_slot: Optional[int] = None   # unconditional K/V slot
@@ -97,11 +106,16 @@ class SamplingEngine:
         model._ensure_packed()
         self.n_slots = 2 * self.max_batch + 1        # conditional, own unconditional, and the shared unconditional slot
         self.shared_slot = None
+        # per-request attn_weights: a row per token slot, as long as the longest vector max_cond_len admits on this grid (bounded
+        # for a model without AttnBlocks, where the weights have no effect)
+        self.w_max = min(model.max_attn_weights((self.H, self.W), self.s_max), self.H * self.W + self.s_max)
         with torch.cuda.device(self.dev):
             self.tokens = torch.zeros(self.max_batch, self.H, self.W, dtype=torch.int64, device=self.dev)
             self.noise = torch.zeros_like(self.tokens)
             self._x = torch.empty_like(self.tokens)
             self._sampled = torch.empty_like(self.tokens)
+            self.w_pool = torch.zeros(self.max_batch, self.w_max, dtype=torch.float32, device=self.dev)
+            self.w_len = torch.zeros(self.max_batch, dtype=torch.int32, device=self.dev)
             # zero-filled: K/V rows past a slot's kv_len are never attended to, but must be finite (see prepare_conditioning)
             self.cache = ConditioningCache(
                 torch.zeros(L.pb200_paella_cond_cache_bytes(model._handle, self.n_slots, self.s_max), dtype=torch.uint8,
@@ -132,11 +146,14 @@ class SamplingEngine:
 
     def submit(self, model_inputs, unconditional_inputs=None, *, generator=None, steps=12, renoise_steps=None,
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
-               decode=False) -> Request:
+               decode=False, attn_weights=None, keep_intermediates=False) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
-        missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0 or
-        steps < 1.  The request's draws start when it is admitted."""
+        missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
+        steps < 1, or an ``attn_weights`` that is not a finite 1-D CPU float tensor at most as long as the smallest key count
+        the request sees in an AttnBlock.  ``attn_weights`` weights the request's conditional forward as in sample_notebook;
+        ``keep_intermediates`` collects sample_notebook's second value in ``req.intermediates``.  The request's draws start
+        when it is admitted."""
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
         g_idx = generator.device.index if generator.device.index is not None else torch.cuda.current_device()
@@ -157,10 +174,13 @@ class SamplingEngine:
             raise ValueError(f"init_x of shape {list(init_x.shape)}; expected [1, {self.H}, {self.W}]")
         if decode and self.vqmodel is None:
             raise ValueError("decode=True needs the engine's vqmodel")
+        if attn_weights is not None:
+            n_keys = self.model.max_attn_weights((self.H, self.W), self.model.conditioning_seq_len(model_inputs))
+            attn_weights = ops.check_attn_weight_vector("attn_weights", attn_weights, min(n_keys, self.w_max))
         cfgs = U._cfg_schedule(cfg, 1, steps)
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
-                      unconditional_inputs, init_x, bool(decode))
+                      unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates))
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
@@ -177,8 +197,17 @@ class SamplingEngine:
         m = self.model
         hw = self.H * self.W
         table = ops.philox_table([q.generator for q in new], hw, self.dev)
-        slots = ops.to_device_async(torch.tensor([q.slot for q in new], dtype=torch.int32), self.dev)
-        ops.randint_per_sample(self.noise, m.num_labels, table, slot=slots, batch=len(new))
+        # one copy: the slots, then each request's weight row and length, written into the pool (a request without weights
+        # gets length 0, so a reused slot never reads the entries of its previous request)
+        w_rows, w_lens = ops.attn_weights_table([q.attn_weights for q in new], len(new), [self.w_max] * len(new))
+        w_rows = torch.nn.functional.pad(w_rows, (0, self.w_max - w_rows.shape[1]))
+        n = len(new)
+        buf = ops.to_device_async(torch.cat([torch.tensor([q.slot for q in new], dtype=torch.int32), w_lens,
+                                             w_rows.view(torch.int32).view(-1)]), self.dev)
+        slots = buf[:n]
+        self.w_len.index_copy_(0, slots.long(), buf[n:2 * n])
+        self.w_pool.index_copy_(0, slots.long(), buf[2 * n:].view(torch.float32).view(n, self.w_max))
+        ops.randint_per_sample(self.noise, m.num_labels, table, slot=slots, batch=n)
         for q in new:
             src = self.noise[q.slot] if q.init_x is None else q.init_x[0]
             self.tokens[q.slot].copy_(src, non_blocking=True)
@@ -215,9 +244,18 @@ class SamplingEngine:
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_pairs, self.s_max, self.n_slots, kv_slot_d)
-            feats = m.features(x, r_d, cond, n_pairs=n_pairs)
+            if any(q.attn_weights is not None for q in plan.order):       # row b reads the weights of its token slot
+                feats = m.features(x, r_d, cond, self.w_pool, Bc, n_pairs=n_pairs, w_len=self.w_len, w_row=row_slot_d)
+            else:
+                feats = m.features(x, r_d, cond, n_pairs=n_pairs)
             sampled = m.sample_tokens_pairs(feats, Bc, n_pairs, H, W, params_d, draw_d, out=self._sampled[:Bc])
+            for i, q in enumerate(plan.order):
+                if q.intermediates is not None:
+                    q.intermediates.append(sampled[i:i + 1].clone())
             ops.add_noise_per_sample(sampled, t_next_d, self.noise, m.num_labels, renoise_d, self.tokens, slot=row_slot_d)
+            for q, rn in zip(plan.order, plan.renoise):
+                if q.intermediates is not None and rn:
+                    q.intermediates.append(self.tokens[q.slot:q.slot + 1].clone())
 
             for q in plan.order:
                 q.k += 1

@@ -601,14 +601,19 @@ class Paella(nn.Module):
 
     # -------------------------------------------------------------- forward pieces
     def features(self, x: torch.Tensor, r: torch.Tensor, cond: ConditioningCache, attn_weights=None,
-                 attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None) -> torch.Tensor:
+                 attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None,
+                 w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
         evaluated under the conditional rows [0,B) and the unconditional rows [B,2B) of ``cond``; the result has 2B
         samples, and the conditioning-independent blocks before the first AttnBlock run once per pair.
         ``n_pairs``: only the first n_pairs samples of x [B,H,W] are guided; the result has B + n_pairs samples, sample
-        B + i being sample i under its unconditional rows (n_pairs = B is ``cfg_pairs=True``, 0 is unguided)."""
+        B + i being sample i under its unconditional rows (n_pairs = B is ``cfg_pairs=True``, 0 is unguided).
+        ``attn_weights``: one vector for samples [0, attn_weights_batch), or with ``w_len`` a device float32 table [rows, w_ld]
+        of per-sample vectors: sample b < attn_weights_batch reads row ``w_row[b]`` (int32 device [attn_weights_batch]; None:
+        row b) and its first ``w_len[row]`` entries (int32 device [rows]; 0 = unweighted), pb200_paella_features_weighted.
+        Each length must not exceed the sample's max_attn_weights."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -626,6 +631,16 @@ class Paella(nn.Module):
             r = r.to(device=dev, dtype=torch.float32).contiguous()
             ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, Bt, H, W, cond.s_max))
             feats = torch.empty(Bt * H * W, self._cfg["c_out"], dtype=torch.float32, device=dev)
+            if w_len is not None:
+                if attn_weights is None or attn_weights.dim() != 2 or attn_weights.dtype != torch.float32 or w_len.dtype != torch.int32 \
+                        or w_len.numel() != attn_weights.shape[0] or (w_row is not None and w_row.numel() < attn_weights_batch):
+                    raise PaellaB200Error("features: a per-sample weight table is float32 [rows, w_ld] with int32 w_len [rows] "
+                                          "and an optional int32 w_row [attn_weights_batch]")
+                check(L.pb200_paella_features_weighted(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                       ptr(cond.slot_map), cond.s_max, ptr(attn_weights), 0, attn_weights.shape[1],
+                                                       ptr(w_len), ptr(w_row), attn_weights_batch, ptr(feats), ptr(ws), ws.numel(),
+                                                       current_stream()), "pb200_paella_features_weighted")
+                return feats
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
             check(L.pb200_paella_features_pairs(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
                                                 ptr(cond.slot_map), cond.s_max, ptr(aw),
@@ -753,6 +768,24 @@ class Paella(nn.Module):
             n += len(ci) if isinstance(ci, (list, tuple)) else 1
         return inputs["byt5"].shape[1] + self._cfg["clip_seq_len"] * n
 
+    def max_attn_weights(self, latent_hw, cond_len: int) -> int:
+        """The longest ``attn_weights`` vector a sample with ``cond_len`` conditioning rows takes on a ``latent_hw`` token grid:
+        the smallest key count it sees in any AttnBlock (that level's positions with self-attention, plus the conditioning).
+        The reference fails on a longer vector (ref/utils/alter_attention.py:28)."""
+        c = self._cfg
+        ps = c["patch_size"]
+        keys = [((latent_hw[0] // ps) >> i) * ((latent_hw[1] // ps) >> i) * int(c["self_attn"]) + cond_len
+                for i, (kinds, n) in enumerate(zip(c["level_config"], c["blocks"])) if "A" in kinds and n > 0]
+        return min(keys) if keys else 2 ** 31 - 1
+
+    def _attn_weights_table(self, attn_weights, batch: int, latent_hw, cond_len: int):
+        """Per-sample ``attn_weights`` (a list or tuple, ops.attn_weights_table) -> the device table (w [B, w_ld], lengths
+        [B]) in one asynchronous copy; a 1-D tensor or None is returned as is.  ValueError before anything is enqueued."""
+        if not isinstance(attn_weights, (list, tuple)):
+            return attn_weights, None
+        table, lens = ops.attn_weights_table(attn_weights, batch, [self.max_attn_weights(latent_hw, cond_len)] * batch)
+        return ops.attn_weights_to_device(table, lens, self._device())
+
     def write_conditioning(self, cache: ConditioningCache, slot: int, inputs: Dict[str, torch.Tensor], latent_hw) -> None:
         """Project one sample's conditioning (batch-1 ``inputs``) into slot ``slot`` of an existing cache, as
         prepare_conditioning projects a group of one; the slot's kv_len becomes this sequence's length, so rows left over
@@ -778,15 +811,19 @@ class Paella(nn.Module):
                                               ptr(ws), ws.numel(), current_stream()), "pb200_paella_prepare_cond")
 
     def forward(self, x, r, byt5, clip=None, clip_image=None, x_cat=None, **kwargs):
-        """ref/src/modules.py:263-275 / ref/utils/modules.py:268-282: logits [B, num_labels, H, W] fp32."""
+        """ref/src/modules.py:263-275 / ref/utils/modules.py:268-282: logits [B, num_labels, H, W] fp32.
+        ``attn_weights``: one vector for every sample, or a list or tuple of B entries, each None or a 1-D CPU float tensor
+        that weights sample b alone (ValueError for a bad entry, before anything is enqueued)."""
         if x_cat is not None:
             x = torch.cat([x, x_cat], dim=1)
         attn_weights = kwargs.pop("attn_weights", None)
         if kwargs:
             raise TypeError(f"unexpected keyword arguments {sorted(kwargs)}")
         B, H, W = x.shape
+        cond_len = self.conditioning_seq_len({"byt5": byt5, "clip": clip, "clip_image": clip_image})
+        aw, w_len = self._attn_weights_table(attn_weights, B, (H, W), cond_len)
         cond = self._cond_for_forward(byt5, clip, clip_image, (H, W))
-        feats = self.features(x, r, cond, attn_weights, B if attn_weights is not None else 0)
+        feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len)
         return self.logits_from_features(feats, B, H, W)
 
     def _cond_for_forward(self, byt5, clip, clip_image, hw):

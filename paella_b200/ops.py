@@ -150,6 +150,45 @@ def sampling_params(cfgs, temperatures) -> torch.Tensor:
     return torch.stack([c.float(), (1.0 - c).float(), torch.ones_like(t32) / t32], -1)
 
 
+def check_attn_weight_vector(name: str, value, max_len: int) -> torch.Tensor:
+    """One sample's ``attn_weights``: a 1-D CPU floating-point tensor of finite values, at most ``max_len`` long (the smallest
+    key count the sample sees in any AttnBlock; the reference fails on a longer vector).  Returns it as CPU float32.
+    ValueError otherwise, like per_sample_values."""
+    if not torch.is_tensor(value):
+        raise ValueError(f"{name}: expected None or a 1-D CPU float tensor (got {type(value).__name__})")
+    if value.device.type != "cpu":
+        raise ValueError(f"{name}: per-sample weights must be a CPU tensor (got {value.device}; reading it would synchronise the stream)")
+    if not value.is_floating_point() or value.dim() != 1:
+        raise ValueError(f"{name}: expected a 1-D floating-point tensor (got {value.dtype} of shape {list(value.shape)})")
+    if not bool(torch.isfinite(value).all()):
+        raise ValueError(f"{name}: weights must be finite")
+    if value.numel() > max_len:
+        raise ValueError(f"{name}: {value.numel()} weights, but the sample attends to only {max_len} keys in its smallest AttnBlock")
+    return value.float()
+
+
+def attn_weights_table(entries, batch: int, max_lens) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Per-sample ``attn_weights``: a list or tuple of ``batch`` entries, each None (unweighted) or a 1-D CPU float tensor, as
+    the host table the attention kernels read: CPU float32 [batch, w_ld] (row b zero-padded past its length) and int32 [batch]
+    of the row lengths (0 for None).  ``max_lens[b]`` bounds sample b's length (check_attn_weight_vector).  ValueError for the
+    wrong number of entries or a bad entry."""
+    if len(entries) != batch:
+        raise ValueError(f"attn_weights: got {len(entries)} entries for a batch of {batch} (one per sample, None for unweighted)")
+    rows = [None if v is None else check_attn_weight_vector(f"attn_weights[{i}]", v, max_lens[i]) for i, v in enumerate(entries)]
+    lens = torch.tensor([0 if v is None else v.numel() for v in rows], dtype=torch.int32)
+    table = torch.zeros(batch, max(1, int(lens.max()) if batch else 1), dtype=torch.float32)
+    for i, v in enumerate(rows):
+        if v is not None:
+            table[i, :v.numel()] = v
+    return table, lens
+
+
+def attn_weights_to_device(table: torch.Tensor, lens: torch.Tensor, device) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The table of attn_weights_table on the device in one asynchronous copy: (float32 [rows, w_ld], int32 [rows])."""
+    buf = to_device_async(torch.cat([table.view(torch.int32).view(-1), lens]), device)
+    return buf[:table.numel()].view(torch.float32).view(table.shape), buf[table.numel():]
+
+
 def to_device_async(host: torch.Tensor, device) -> torch.Tensor:
     """One asynchronous copy from pinned memory: no host synchronisation, no pageable copy."""
     buf = torch.empty(host.shape, dtype=host.dtype, pin_memory=True)

@@ -2,7 +2,8 @@
 
   sample()               ref/src/utils.py:35-55
   sample_distributed()   ref/src_distributed/utils.py:97-126   (init_x, per-step cfg, sampling_conditional_steps)
-  sample_notebook()      paella_inference.ipynb cell 3          (mode, attn_weights, returns intermediates)
+  sample_notebook()      paella_inference.ipynb cell 3          (mode, attn_weights, returns intermediates; attn_weights
+                                                                 may also be one vector per sample)
 
 Per step the reference runs two forwards, materialises 2 x [B,8192,H,W] fp32 logits and makes ~20 passes
 over them.  Here: conditional and unconditional rows run as ONE batch of 2B through the denoiser (their
@@ -80,6 +81,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     dev = model._device()
     use_cfg_any = cfgs is not None
     sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg)
+    w_table = None
+    if isinstance(attn_weights, (list, tuple)):       # per-sample vectors, for the conditional rows only
+        w_table = ops.attn_weights_table(attn_weights, B, [model.max_attn_weights((H, W), model.conditioning_seq_len(model_inputs))] * B)
     if ops.per_sample(generator):
         ops.check_generators(generator, B, dev)
         ops.check_per_sample_numel(H * W * model.num_labels)
@@ -88,6 +92,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             flat = ops.to_device_async(torch.cat([sched[0].view(-1), sched[1].view(-1)]), dev)
             params_d = flat[:steps * B * 3].view(steps, B, 3)
             r_d = flat[steps * B * 3:].view(steps + 1, B)
+        w_len = None
+        if w_table is not None:      # one copy for the whole loop
+            attn_weights, w_len = ops.attn_weights_to_device(*w_table, dev)
         init_noise = ops.randint(model.num_labels, (B, H, W), dev, generator)
         sampled = init_x.to(dev) if init_x is not None else init_noise.clone()
         if sched is None:
@@ -114,7 +121,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 cfg_i, temp_i = (float(cfgs[i]) if guided else None), float(temperatures[i])
             else:
                 r, params_i = r_d[i], params_d[i]
-            feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided)
+            feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided, w_len=w_len)
             if mode == "multinomial" and not exact:
                 if sched is None:
                     sampled = model.sample_tokens(feats, B, H, W, cfg_i, temp_i, generator)
@@ -230,7 +237,11 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                     generator=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
-    in ``sample``; per-sample settings as in ``sample_distributed``."""
+    in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
+    list or tuple of B entries, each None or a 1-D CPU float tensor that weights sample b's conditional forward alone (the
+    unconditional rows are never weighted, as in the notebook).  Row i then equals row i of the call with vector i for every
+    sample.  ValueError, before anything is enqueued and before any generator advances, for the wrong number of entries, a
+    CUDA, non-1-D or non-finite tensor, or a vector longer than the smallest key count the sample sees in an AttnBlock."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:

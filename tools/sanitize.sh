@@ -73,6 +73,18 @@ eng.submit(cond(12, True), generator=torch.Generator(device=DEV).manual_seed(1),
 eng.submit(cond(5, False), generator=torch.Generator(device=DEV).manual_seed(2), steps=3, cfg=None)
 eng.submit(cond(2, False), generator=torch.Generator(device=DEV).manual_seed(3), steps=2, sampling_conditional_steps=1)
 print("engine", [q.result.shape for q in eng.run_until_idle()])
+# per-sample attn_weights: a vector longer than the conditioning (into the self keys), None and length 1; then an engine
+# whose slot 0 is reused by a request with a shorter vector, and again by one with none
+cw = cond(6, True); cw = {k: v.expand(3, *v.shape[1:]).contiguous() for k, v in cw.items()}
+n_max = m.max_attn_weights((8, 8), m.conditioning_seq_len(cw))
+print("forward per-sample weights", m(torch.randint(0, 64, (3, 8, 8), device=DEV, generator=g), torch.rand(3, device=DEV, generator=g),
+      **cw, attn_weights=[torch.rand(n_max), None, torch.rand(1)]).shape)
+eng = SamplingEngine(m, latent_hw=(8, 8), max_batch=2, max_cond_len=20, unconditional_inputs={k: v * 0 for k, v in cond(4, False).items()})
+eng.submit(cond(12, True), generator=torch.Generator(device=DEV).manual_seed(1), steps=1, attn_weights=torch.rand(21))
+eng.submit(cond(5, False), generator=torch.Generator(device=DEV).manual_seed(2), steps=3, cfg=None, attn_weights=torch.rand(3))
+eng.submit(cond(2, False), generator=torch.Generator(device=DEV).manual_seed(3), steps=1, attn_weights=torch.rand(2))
+eng.submit(cond(3, False), generator=torch.Generator(device=DEV).manual_seed(4), steps=1, keep_intermediates=True)
+print("engine weights", [q.result.shape for q in eng.run_until_idle()])
 t = torch.from_numpy
 print("forward", m(t(gg["x"]).to(DEV), t(gg["r"]).to(DEV), t(gg["byt5"]).to(DEV), clip=t(gg["clip"]).to(DEV)).shape)
 torch.cuda.synchronize(); print("sanitizer case 2 done")
