@@ -90,6 +90,17 @@ int pb200_resample_quant_params(const float* logits_c, const float* logits_u, in
 int pb200_add_noise(const int64_t* x, const int64_t* random_x, const float* t, int64_t batch, int64_t hw,
                     int64_t num_labels, uint64_t seed, uint64_t offset, int64_t* out, int64_t* mask_out,
                     void* stream);
+/* pb200_add_noise restricted to a token region: inpainting / outpainting from source tokens.  With the reference's
+ * explicit-mask add_noise [ref/src/modules.py:277-283, ref/utils/modules.py:282-288] and the init_x of sample_distributed
+ * [ref/src_distributed/utils.py:97-126] it computes, element for element,
+ *   m   = (rand_like(x.float()) <= t[:,None,None]) & region
+ *   out = where(region, x*(1-m) + random_x*m, src)          mask_out = m
+ * src: int64 [B, HW] (the kept tokens), region: uint8 [B, HW] (nonzero = generated), indexed like random_x; both NULL is
+ * pb200_add_noise, which is this call.  The draws are those of pb200_add_noise whatever the region.  A sample with t < 0 is
+ * never renoised, so such a launch only composites: it needs no fresh Philox offset. */
+int pb200_add_noise_region(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region, const float* t,
+                           int64_t batch, int64_t hw, int64_t num_labels, uint64_t seed, uint64_t offset, int64_t* out,
+                           int64_t* mask_out, void* stream);
 
 /* One random stream per sample, in ONE launch over the batch (a list of per-sample torch.Generators).  seed_offset: DEVICE
  * uint64 [batch][2] = (seed, philox offset) of sample b's generator before the draw, offsets multiples of 4.  Sample b draws
@@ -103,6 +114,12 @@ int pb200_randint_per_sample(int64_t* out, const int* slot, int64_t batch, int64
 int pb200_add_noise_per_sample(const int64_t* x, const int64_t* random_x, const int* slot, const float* t, int64_t batch,
                                int64_t hw, int64_t num_labels, const uint64_t* seed_offset, int64_t* out, int64_t* mask_out,
                                void* stream);
+/* pb200_add_noise_per_sample restricted to a token region, as pb200_add_noise_region [ref/src/modules.py:277-283,
+ * ref/utils/modules.py:282-288]: src and region are indexed by slot like random_x and out.  Both NULL is
+ * pb200_add_noise_per_sample, which is this call. */
+int pb200_add_noise_region_per_sample(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region,
+                                      const int* slot, const float* t, int64_t batch, int64_t hw, int64_t num_labels,
+                                      const uint64_t* seed_offset, int64_t* out, int64_t* mask_out, void* stream);
 /* out[b] = pool[slot[b]] for rows of hw int64 tokens (b < batch): a step batch gathered from a token pool. */
 int pb200_gather_rows(const int64_t* pool, const int* slot, int64_t batch, int64_t hw, int64_t* out, void* stream);
 

@@ -71,6 +71,10 @@ SIGNATURES = {
     "pb200_randint_per_sample": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
     "pb200_add_noise_per_sample": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
                                            c_void_p, c_void_p]),
+    "pb200_add_noise_region": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_uint64, c_uint64,
+                                       c_void_p, c_void_p, c_void_p]),
+    "pb200_add_noise_region_per_sample": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64,
+                                                  c_void_p, c_void_p, c_void_p, c_void_p]),
     "pb200_gather_rows": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
     "pb200_vq_nearest":(c_int, [c_void_p, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "pb200_vq_gather": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]),

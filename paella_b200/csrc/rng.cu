@@ -3,7 +3,7 @@
 //   torch.randint        ref/src/utils.py:37
 //   torch.multinomial    ref/src/utils.py:49-50   (q = exponential_(1); argmax(p / q))
 //   CFG/temp/softmax     ref/src/utils.py:45-47
-//   Paella.add_noise     ref/src/modules.py:277-283
+//   Paella.add_noise     ref/src/modules.py:277-283  (and its explicit-mask form, the region sampling of utils._sample_core)
 // PyTorch-side arithmetic: ATen/native/cuda/DistributionTemplates.h, ATen/core/TransformationHelper.h.
 #include "common.cuh"
 #include "paella_b200.h"
@@ -46,7 +46,10 @@ __global__ void rand_kernel(float* __restrict__ out, int64_t numel, TorchPhilox 
 }
 
 // ------------------------------------------------------------------ add_noise
+// src, region (both NULL, or both set; indexed like random_x): region sampling.  Where region[e] == 0 the output is src[e]
+// and the mask is 0: torch.where(region, add_noise(x, t, mask=m & region, random_x), src), the draw unchanged.
 __global__ void add_noise_kernel(const int64_t* __restrict__ x, const int64_t* __restrict__ random_x,
+                                 const int64_t* __restrict__ src, const uint8_t* __restrict__ region,
                                  const float* __restrict__ t, int64_t batch, int64_t hw, uint32_t num_labels,
                                  TorchPhilox s_mask, TorchPhilox s_rx, int64_t* __restrict__ out,
                                  int64_t* __restrict__ mask_out) {
@@ -54,9 +57,10 @@ __global__ void add_noise_kernel(const int64_t* __restrict__ x, const int64_t* _
     if (e >= batch * hw) return;
     float u = u32_to_uniform(torch_philox_u32(s_mask, (uint64_t)e));
     u = (u == 1.0f) ? 0.0f : u;
-    const bool m = u <= t[e / hw];
+    const bool gen = region ? region[e] != 0 : true;
+    const bool m = gen && u <= t[e / hw];
     const int64_t rx = random_x ? random_x[e] : (int64_t)(torch_philox_u32(s_rx, (uint64_t)e) % num_labels);
-    out[e] = m ? rx : x[e];
+    out[e] = gen ? (m ? rx : x[e]) : src[e];
     if (mask_out) mask_out[e] = m ? 1 : 0;
 }
 
@@ -81,8 +85,9 @@ __global__ void randint_per_sample_kernel(int64_t* __restrict__ out, const int* 
 
 // x: int64 [B, hw] (by sample); t: fp32 [B], and a sample with t < 0 keeps x (u >= 0 never passes the mask test: the
 // sampling engine's rows that do not renoise this step).  random_x == NULL: randint_like drawn at the offset after the mask
-// draw, as pb200_add_noise does (rx_inc4 = that offset increment / 4).
+// draw, as pb200_add_noise does (rx_inc4 = that offset increment / 4).  src, region: as in add_noise_kernel, by slot.
 __global__ void add_noise_per_sample_kernel(const int64_t* __restrict__ x, const int64_t* __restrict__ random_x,
+                                            const int64_t* __restrict__ src, const uint8_t* __restrict__ region,
                                             const int* __restrict__ slot, const float* __restrict__ t, int64_t hw,
                                             uint32_t num_labels, TorchPhilox s, uint64_t rx_inc4,
                                             const uint64_t* __restrict__ seed_off, int64_t* __restrict__ out,
@@ -94,7 +99,8 @@ __global__ void add_noise_per_sample_kernel(const int64_t* __restrict__ x, const
     const TorchPhilox sm = sample_stream(s, seed_off, b);
     float u = u32_to_uniform(torch_philox_u32(sm, (uint64_t)e));
     u = (u == 1.0f) ? 0.0f : u;
-    const bool m = u <= t[b];
+    const bool gen = region ? region[dst * hw + e] != 0 : true;
+    const bool m = gen && u <= t[b];
     int64_t rx;
     if (random_x) {
         rx = random_x[dst * hw + e];
@@ -103,7 +109,7 @@ __global__ void add_noise_per_sample_kernel(const int64_t* __restrict__ x, const
         sr.offset4 += rx_inc4;
         rx = (int64_t)(torch_philox_u32(sr, (uint64_t)e) % num_labels);
     }
-    out[dst * hw + e] = m ? rx : x[b * hw + e];
+    out[dst * hw + e] = gen ? (m ? rx : x[b * hw + e]) : src[dst * hw + e];
     if (mask_out) mask_out[b * hw + e] = m ? 1 : 0;
 }
 
@@ -438,19 +444,26 @@ int pb200_resample_quant_params(const float* logits_c, const float* logits_u, in
     return resample_quant(logits_c, logits_u, batch, k, hw, 0.0, 1.0, params, codebook, c_latent, out, (cudaStream_t)stream);
 }
 
-int pb200_add_noise(const int64_t* x, const int64_t* random_x, const float* t, int64_t batch, int64_t hw,
-                    int64_t num_labels, uint64_t seed, uint64_t offset, int64_t* out, int64_t* mask_out,
-                    void* stream) {
+int pb200_add_noise_region(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region, const float* t,
+                           int64_t batch, int64_t hw, int64_t num_labels, uint64_t seed, uint64_t offset, int64_t* out,
+                           int64_t* mask_out, void* stream) {
     PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
     PB_CHECK(num_labels > 0 && num_labels < (1ll << 28), "add_noise: bad num_labels");
+    PB_CHECK((src == nullptr) == (region == nullptr), "add_noise_region: src and region must both be set or both be NULL");
     const int64_t n = batch * hw;
     if (n == 0) return 0;
     TorchPhilox s_mask = make_torch_philox(seed, offset, n);
     TorchPhilox s_rx = make_torch_philox(seed, offset + offset_increment(n), n);
-    add_noise_kernel<<<ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(x, random_x, t, batch, hw, (uint32_t)num_labels,
-                                                                         s_mask, s_rx, out, mask_out);
+    add_noise_kernel<<<ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(x, random_x, src, region, t, batch, hw,
+                                                                         (uint32_t)num_labels, s_mask, s_rx, out, mask_out);
     PB_LAUNCH_CHECK();
     return 0;
+}
+
+int pb200_add_noise(const int64_t* x, const int64_t* random_x, const float* t, int64_t batch, int64_t hw,
+                    int64_t num_labels, uint64_t seed, uint64_t offset, int64_t* out, int64_t* mask_out,
+                    void* stream) {
+    return pb200_add_noise_region(x, random_x, nullptr, nullptr, t, batch, hw, num_labels, seed, offset, out, mask_out, stream);
 }
 
 static int check_per_sample(int64_t batch, int64_t hw, const uint64_t* seed_offset, const char* what) {
@@ -474,17 +487,26 @@ int pb200_randint_per_sample(int64_t* out, const int* slot, int64_t batch, int64
     return 0;
 }
 
-int pb200_add_noise_per_sample(const int64_t* x, const int64_t* random_x, const int* slot, const float* t, int64_t batch,
-                               int64_t hw, int64_t num_labels, const uint64_t* seed_offset, int64_t* out, int64_t* mask_out,
-                               void* stream) {
+int pb200_add_noise_region_per_sample(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region,
+                                      const int* slot, const float* t, int64_t batch, int64_t hw, int64_t num_labels,
+                                      const uint64_t* seed_offset, int64_t* out, int64_t* mask_out, void* stream) {
     PB_TRY(check_per_sample(batch, hw, seed_offset, "add_noise_per_sample"));
     PB_CHECK(num_labels > 0 && num_labels < (1ll << 28), "add_noise_per_sample: bad num_labels");
+    PB_CHECK((src == nullptr) == (region == nullptr), "add_noise_region_per_sample: src and region must both be set or both be NULL");
     if (batch == 0 || hw == 0) return 0;
     const TorchPhilox s = make_torch_philox(0, 0, hw);
     add_noise_per_sample_kernel<<<dim3(ceil_div(hw, 256), (unsigned)batch), 256, 0, (cudaStream_t)stream>>>(
-        x, random_x, slot, t, hw, (uint32_t)num_labels, s, (uint64_t)offset_increment(hw) / 4, seed_offset, out, mask_out);
+        x, random_x, src, region, slot, t, hw, (uint32_t)num_labels, s, (uint64_t)offset_increment(hw) / 4, seed_offset, out,
+        mask_out);
     PB_LAUNCH_CHECK();
     return 0;
+}
+
+int pb200_add_noise_per_sample(const int64_t* x, const int64_t* random_x, const int* slot, const float* t, int64_t batch,
+                               int64_t hw, int64_t num_labels, const uint64_t* seed_offset, int64_t* out, int64_t* mask_out,
+                               void* stream) {
+    return pb200_add_noise_region_per_sample(x, random_x, nullptr, nullptr, slot, t, batch, hw, num_labels, seed_offset, out,
+                                             mask_out, stream);
 }
 
 int pb200_gather_rows(const int64_t* pool, const int* slot, int64_t batch, int64_t hw, int64_t* out, void* stream) {

@@ -18,7 +18,10 @@ forward is batch-invariant (DESIGN.md §3) the tokens are equal bit for bit, wha
 ``attn_weights=w`` (and ``keep_intermediates=True``) the request's tokens, ``req.intermediates`` and generator offset are those
 of ``sample_notebook(model, inputs, (1, H, W), uncond, init_x, steps, renoise_steps, temperature, cfg, 'multinomial', t_start,
 t_end, sampling_conditional_steps, attn_weights=w, generator=[g])``; each step's batch reads every row's weights from a
-device pool indexed by its token slot.
+device pool indexed by its token slot.  With ``region=`` (bool [1, H, W], True where tokens are generated) and ``init_x`` (the
+source tokens kept elsewhere) a request inpaints or outpaints as ``sample_distributed(..., init_x, region=region)`` does: its
+source tokens and region sit in device pools by token slot, and the step's one add-noise launch puts every row's source
+tokens back outside its region (a request without a region has an all-True row).
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -47,11 +50,14 @@ class Request:
 
     def __init__(self, steps: int, renoise_steps: int, cond_steps: int, guided: bool, params: torch.Tensor, r: torch.Tensor,
                  generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False,
-                 attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False):
+                 attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
+                 region: Optional[torch.Tensor] = None):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
         self.attn_weights = attn_weights         # CPU float32 [n] or None
+        self.region = region                     # bool [1, H, W] or None, until admission
+        self.has_region = region is not None
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -116,6 +122,10 @@ class SamplingEngine:
             self._sampled = torch.empty_like(self.tokens)
             self.w_pool = torch.zeros(self.max_batch, self.w_max, dtype=torch.float32, device=self.dev)
             self.w_len = torch.zeros(self.max_batch, dtype=torch.int32, device=self.dev)
+            # per-request regions: source tokens and region (True = generated) by token slot
+            self.src = torch.zeros_like(self.tokens)
+            self.region = torch.ones(self.max_batch, self.H, self.W, dtype=torch.bool, device=self.dev)
+            self._neg_t = torch.full((self.max_batch,), -1.0, dtype=torch.float32, device=self.dev)   # composite-only t
             # zero-filled: K/V rows past a slot's kv_len are never attended to, but must be finite (see prepare_conditioning)
             self.cache = ConditioningCache(
                 torch.zeros(L.pb200_paella_cond_cache_bytes(model._handle, self.n_slots, self.s_max), dtype=torch.uint8,
@@ -146,14 +156,15 @@ class SamplingEngine:
 
     def submit(self, model_inputs, unconditional_inputs=None, *, generator=None, steps=12, renoise_steps=None,
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
-               decode=False, attn_weights=None, keep_intermediates=False) -> Request:
+               decode=False, attn_weights=None, keep_intermediates=False, region=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
         steps < 1, or an ``attn_weights`` that is not a finite 1-D CPU float tensor at most as long as the smallest key count
-        the request sees in an AttnBlock.  ``attn_weights`` weights the request's conditional forward as in sample_notebook;
-        ``keep_intermediates`` collects sample_notebook's second value in ``req.intermediates``.  The request's draws start
-        when it is admitted."""
+        the request sees in an AttnBlock, or a ``region`` that is not a bool [1, H, W] tensor on the CPU or the model's device
+        or comes without init_x.  ``attn_weights`` weights the request's conditional forward as in sample_notebook;
+        ``keep_intermediates`` collects sample_notebook's second value in ``req.intermediates``; ``region`` inpaints or
+        outpaints init_x as in sample_distributed.  The request's draws start when it is admitted."""
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
         g_idx = generator.device.index if generator.device.index is not None else torch.cuda.current_device()
@@ -172,6 +183,7 @@ class SamplingEngine:
             raise ValueError("cfg is set but there are no unconditional inputs (per request or engine-wide)")
         if init_x is not None and tuple(init_x.shape) != (1, self.H, self.W):
             raise ValueError(f"init_x of shape {list(init_x.shape)}; expected [1, {self.H}, {self.W}]")
+        U.check_region(region, init_x, (1, self.H, self.W), self.dev)
         if decode and self.vqmodel is None:
             raise ValueError("decode=True needs the engine's vqmodel")
         if attn_weights is not None:
@@ -180,7 +192,7 @@ class SamplingEngine:
         cfgs = U._cfg_schedule(cfg, 1, steps)
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
-                      unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates))
+                      unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region)
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
@@ -198,23 +210,38 @@ class SamplingEngine:
         hw = self.H * self.W
         table = ops.philox_table([q.generator for q in new], hw, self.dev)
         # one copy: the slots, then each request's weight row and length, written into the pool (a request without weights
-        # gets length 0, so a reused slot never reads the entries of its previous request)
+        # gets length 0, so a reused slot never reads the entries of its previous request), then each request's region row
+        # (all True without a region, for the same reason) and the source tokens that come from the CPU
         w_rows, w_lens = ops.attn_weights_table([q.attn_weights for q in new], len(new), [self.w_max] * len(new))
         w_rows = torch.nn.functional.pad(w_rows, (0, self.w_max - w_rows.shape[1]))
         n = len(new)
-        buf = ops.to_device_async(torch.cat([torch.tensor([q.slot for q in new], dtype=torch.int32), w_lens,
-                                             w_rows.view(torch.int32).view(-1)]), self.dev)
-        slots = buf[:n]
-        self.w_len.index_copy_(0, slots.long(), buf[n:2 * n])
-        self.w_pool.index_copy_(0, slots.long(), buf[2 * n:].view(torch.float32).view(n, self.w_max))
+        regions = torch.ones(n, self.H, self.W, dtype=torch.bool)
+        for j, q in enumerate(new):
+            if q.has_region and q.region.device.type == "cpu":
+                regions[j] = q.region[0]
+        host_src = [q for q in new if q.has_region and q.init_x.device.type == "cpu"]
+        src_row = {id(q): j for j, q in enumerate(host_src)}
+        srcs = torch.cat([q.init_x.to(torch.int64) for q in host_src]) if host_src else torch.zeros(0, dtype=torch.int64)
+        slots, w_lens_d, w_rows_d, regions_d, srcs_d = ops.to_device_packed(
+            [torch.tensor([q.slot for q in new], dtype=torch.int32), w_lens, w_rows, regions, srcs], self.dev)
+        self.w_len.index_copy_(0, slots.long(), w_lens_d)
+        self.w_pool.index_copy_(0, slots.long(), w_rows_d)
+        self.region.index_copy_(0, slots.long(), regions_d)
         ops.randint_per_sample(self.noise, m.num_labels, table, slot=slots, batch=n)
         for q in new:
-            src = self.noise[q.slot] if q.init_x is None else q.init_x[0]
-            self.tokens[q.slot].copy_(src, non_blocking=True)
+            s = q.slot
+            if q.has_region:             # tokens = where(region, noise, init_x)
+                if q.region.device.type != "cpu":
+                    self.region[s].copy_(q.region[0], non_blocking=True)
+                self.src[s].copy_(srcs_d[src_row[id(q)]] if id(q) in src_row else q.init_x[0], non_blocking=True)
+                ops.composite(self.noise[s:s + 1], self.src[s:s + 1], self.region[s:s + 1], self._neg_t[:1], out=self.tokens[s:s + 1])
+            else:
+                src = self.noise[s] if q.init_x is None else q.init_x[0]
+                self.tokens[s].copy_(src, non_blocking=True)
             m.write_conditioning(self.cache, q.slot, q.inputs, (self.H, self.W))
             if q.uncond is not None:
                 m.write_conditioning(self.cache, q.uncond_slot, q.uncond, (self.H, self.W))
-            q.inputs = q.uncond = q.init_x = None
+            q.inputs = q.uncond = q.init_x = q.region = None
         self._active += new
 
     def step(self) -> List[Request]:
@@ -251,8 +278,13 @@ class SamplingEngine:
             sampled = m.sample_tokens_pairs(feats, Bc, n_pairs, H, W, params_d, draw_d, out=self._sampled[:Bc])
             for i, q in enumerate(plan.order):
                 if q.intermediates is not None:
-                    q.intermediates.append(sampled[i:i + 1].clone())
-            ops.add_noise_per_sample(sampled, t_next_d, self.noise, m.num_labels, renoise_d, self.tokens, slot=row_slot_d)
+                    s = q.slot
+                    q.intermediates.append(ops.composite(sampled[i:i + 1], self.src[s:s + 1], self.region[s:s + 1], self._neg_t[:1])
+                                           if q.has_region else sampled[i:i + 1].clone())
+            # every row back into its slot, renoised or not; with a region in the batch, each row's source tokens outside it
+            regions = any(q.has_region for q in plan.order)
+            ops.add_noise_per_sample(sampled, t_next_d, self.noise, m.num_labels, renoise_d, self.tokens, slot=row_slot_d,
+                                     src=self.src if regions else None, region=self.region if regions else None)
             for q, rn in zip(plan.order, plan.renoise):
                 if q.intermediates is not None and rn:
                     q.intermediates.append(self.tokens[q.slot:q.slot + 1].clone())

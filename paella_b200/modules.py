@@ -853,10 +853,14 @@ class Paella(nn.Module):
             self._cond_single = memos
         return cond
 
-    def add_noise(self, x, t, mask=None, random_x=None, generator=None):
-        """ref/src/modules.py:277-283 on torch's random stream (``generator``: as in ``sample_tokens``)."""
+    def add_noise(self, x, t, mask=None, random_x=None, generator=None, src=None, region=None):
+        """ref/src/modules.py:277-283 on torch's random stream (``generator``: as in ``sample_tokens``).  ``src`` and ``region``
+        (device tensors shaped like x, with mask=None): the tokens outside the region are src's and are never renoised
+        (ops.add_noise)."""
         if mask is None:
-            return ops.add_noise(x, t, random_x, self.num_labels, generator)
+            return ops.add_noise(x, t, random_x, self.num_labels, generator, src=src, region=region)
+        if region is not None:
+            raise ValueError("add_noise: region applies to the drawn mask (mask=None); with an explicit mask, pass mask & region")
         if random_x is None:
             random_x = ops.randint(self.num_labels, x.shape, x.device, generator)
         return torch.where(mask.bool(), random_x, x), mask

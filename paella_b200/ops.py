@@ -196,6 +196,22 @@ def to_device_async(host: torch.Tensor, device) -> torch.Tensor:
     return buf.to(device, non_blocking=True)
 
 
+def to_device_packed(parts, device) -> list:
+    """Several CPU tensors in one asynchronous copy from pinned memory: returns their device copies, each with its own dtype
+    and shape, each starting at an 8-byte boundary of one buffer."""
+    chunks, offs, n = [], [], 0
+    for p in parts:
+        pad = -n % 8
+        if pad:
+            chunks.append(torch.zeros(pad, dtype=torch.uint8))
+            n += pad
+        offs.append(n)
+        chunks.append(p.contiguous().reshape(-1).view(torch.uint8))
+        n += p.numel() * p.element_size()
+    buf = to_device_async(torch.cat(chunks), device)
+    return [buf[o:o + p.numel() * p.element_size()].view(p.dtype).view(p.shape) for o, p in zip(offs, parts)]
+
+
 def sampling_params_table(cfg, temperature, batch: int, device) -> torch.Tensor:
     """Device float32 [batch, 3] for ``cfg`` (float, None or a CPU tensor [batch]) and ``temperature`` (float or a CPU tensor
     [batch]); a scalar applies to every sample.  ValueError (nothing enqueued) for a bad per-sample value or a T <= 0."""
@@ -328,14 +344,26 @@ def _resample_quant(logits_c, logits_u, par, codebook):
     return out
 
 
+def _region_u8(region: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """A bool or uint8 device region as the kernels' uint8 bytes (a view, no copy)."""
+    if region is None:
+        return None
+    region = region.contiguous()
+    return region.view(torch.uint8) if region.dtype == torch.bool else region
+
+
 def add_noise(x: torch.Tensor, t: torch.Tensor, random_x: Optional[torch.Tensor], num_labels: int, generator=None,
-              return_mask: bool = True):
-    """Paella.add_noise with mask=None  [ref/src/modules.py:277-283]"""
+              return_mask: bool = True, src: Optional[torch.Tensor] = None, region: Optional[torch.Tensor] = None):
+    """Paella.add_noise with mask=None  [ref/src/modules.py:277-283].  With ``src`` (int64, like x) and ``region`` (bool or
+    uint8, like x): where(region, add_noise(x, t, mask=m & region, random_x), src) for the mask m this call draws -- the
+    same draws as without a region; the returned mask is m & region."""
     x = x.contiguous()
     B = x.shape[0]
     hw = x[0].numel()
     out = torch.empty_like(x)
     mask = torch.empty_like(x) if return_mask else None
+    src = src.contiguous() if src is not None else None
+    region = _region_u8(region)
     if per_sample(generator):
         check_generators(generator, B, x.device)
         check_per_sample_numel(hw)
@@ -343,26 +371,40 @@ def add_noise(x: torch.Tensor, t: torch.Tensor, random_x: Optional[torch.Tensor]
         if random_x is None:
             philox_values(generator, hw, x.device)          # the randint_like draw follows the mask draw
         add_noise_per_sample(x, t.contiguous().float(), random_x.contiguous() if random_x is not None else None, num_labels, table,
-                             out, mask)
+                             out, mask, src=src, region=region)
         return out, mask
     seed, off = take_philox(x.numel(), x.device, generator)
     if random_x is None:
         take_philox(x.numel(), x.device, generator)      # the randint_like draw follows the mask draw
     else:
         random_x = random_x.contiguous()
-    check(lib().pb200_add_noise(ptr(x), ptr(random_x), ptr(t.contiguous().float()), B, hw, num_labels, seed, off, ptr(out),
-                                ptr(mask), current_stream()), "pb200_add_noise")
+    check(lib().pb200_add_noise_region(ptr(x), ptr(random_x), ptr(src), ptr(region), ptr(t.contiguous().float()), B, hw, num_labels,
+                                       seed, off, ptr(out), ptr(mask), current_stream()), "pb200_add_noise_region")
     return out, mask
 
 
+def composite(x: torch.Tensor, src: torch.Tensor, region: torch.Tensor, neg_t: torch.Tensor,
+              out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """where(region, x, src) for int64 x, src and a bool / uint8 region of one shape [B, ...]: the add-noise launch with every
+    t < 0 (``neg_t``, fp32 [B] on the device), which renoises nothing and so takes no Philox offset from any generator."""
+    x = x.contiguous()
+    out = torch.empty_like(x) if out is None else out
+    check(lib().pb200_add_noise_region(ptr(x), None, ptr(src.contiguous()), ptr(_region_u8(region)), ptr(neg_t), x.shape[0],
+                                       x[0].numel(), 1, 0, 0, ptr(out), None, current_stream()), "pb200_add_noise_region")
+    return out
+
+
 def add_noise_per_sample(x: torch.Tensor, t: torch.Tensor, random_x: Optional[torch.Tensor], num_labels: int, table: torch.Tensor,
-                         out: torch.Tensor, mask: Optional[torch.Tensor] = None, slot: Optional[torch.Tensor] = None) -> None:
+                         out: torch.Tensor, mask: Optional[torch.Tensor] = None, slot: Optional[torch.Tensor] = None,
+                         src: Optional[torch.Tensor] = None, region: Optional[torch.Tensor] = None) -> None:
     """One launch of per-sample add_noise: sample b (x [B, ...], t fp32 [B]) draws its mask on (seed, offset) = ``table[b]`` and
     takes random_x (or, when None, the randint_like drawn at the next offset) where the mask is set; a sample with t < 0 keeps
-    its tokens.  ``slot`` (int32 [B]) places sample b's rows of random_x and out at row slot[b] of those buffers."""
+    its tokens.  ``slot`` (int32 [B]) places sample b's rows of random_x and out at row slot[b] of those buffers.  ``src`` and
+    ``region`` (read at the same rows): outside the region the output is src and the mask 0, as in add_noise."""
     B, hw = x.shape[0], x[0].numel()
-    check(lib().pb200_add_noise_per_sample(ptr(x), ptr(random_x), ptr(slot), ptr(t), B, hw, num_labels, ptr(table), ptr(out),
-                                           ptr(mask), current_stream()), "pb200_add_noise_per_sample")
+    check(lib().pb200_add_noise_region_per_sample(ptr(x), ptr(random_x), ptr(src), ptr(_region_u8(region)), ptr(slot), ptr(t), B, hw,
+                                                  num_labels, ptr(table), ptr(out), ptr(mask), current_stream()),
+          "pb200_add_noise_region_per_sample")
 
 
 def gather_rows(pool: torch.Tensor, slot: torch.Tensor, out: torch.Tensor) -> torch.Tensor:

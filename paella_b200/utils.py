@@ -20,6 +20,13 @@ dimension is B (``cfg`` [B] in ``sample``, [B, 2] in the other two; ``temperatur
 any mix with scalar ones.  Sample i is then computed with exactly the scalars a call on its own settings would use: its
 schedules come from the same torch.linspace calls, and the kernels see the same fp32 constants.  The [steps][B] table is
 built on the host once per call and copied to the device once, so the step loop gets no host synchronisation.
+
+Inpainting and outpainting: ``region`` (sample_distributed, sample_notebook), a bool tensor [B, H, W], True where tokens are
+generated, with ``init_x`` holding the source tokens kept everywhere else.  The loop starts from where(region, randint, init_x),
+puts init_x back outside the region after every step's sampling, and renoises only inside it (mask & region); its random draws
+are those of the call without a region, so a generator ends at the same offset.  An all-True region is the call without
+init_x, bit for bit; an all-False one returns init_x.  ``token_region`` and ``outpaint_canvas`` build the arguments from a
+pixel mask or from a smaller token grid placed on a larger canvas.
 """
 from __future__ import annotations
 
@@ -74,11 +81,62 @@ def sampling_schedule(batch: int, steps: int, temperature, cfgs, t_start, t_end,
     return params.transpose(0, 1).contiguous(), r.t().contiguous()
 
 
+def check_region(region, init_x, latent_shape, device) -> None:
+    """ValueError unless ``region`` is None or a bool tensor of ``latent_shape`` [B, H, W] on the CPU or on ``device``, with an
+    ``init_x`` of the same shape and placement (the source tokens)."""
+    if region is None:
+        return
+    if init_x is None:
+        raise ValueError("region needs init_x: the source tokens kept outside the region")
+    device = torch.device(device)
+    for name, v in (("region", region), ("init_x", init_x)):
+        if not torch.is_tensor(v):
+            raise ValueError(f"{name}: expected a tensor (got {type(v).__name__})")
+        if tuple(v.shape) != tuple(latent_shape):
+            raise ValueError(f"{name} of shape {list(v.shape)}; expected {list(latent_shape)}")
+        if v.device.type != "cpu" and v.device != device:
+            raise ValueError(f"{name} is on {v.device}, the model on {device}")
+    if region.dtype != torch.bool:
+        raise ValueError(f"region: expected a bool tensor, True where tokens are generated (got {region.dtype})")
+    if init_x.dtype.is_floating_point or init_x.dtype == torch.bool:
+        raise ValueError(f"init_x: expected integer token indices (got {init_x.dtype})")
+
+
+def token_region(pixel_mask: torch.Tensor, patch: int = 4) -> torch.Tensor:
+    """The token region of a pixel mask for the f4 codec: bool [..., h, w] (True = regenerate) -> bool [..., h/4, w/4], True
+    where any pixel of the token's 4x4 patch is True.  CPU tensors, no device work."""
+    if not torch.is_tensor(pixel_mask) or pixel_mask.device.type != "cpu":
+        raise ValueError("token_region: expected a CPU tensor")
+    if pixel_mask.dim() < 2 or pixel_mask.shape[-2] % patch or pixel_mask.shape[-1] % patch:
+        raise ValueError(f"token_region: a pixel mask of shape {list(pixel_mask.shape)}; its last two sizes must be multiples of {patch}")
+    h, w = pixel_mask.shape[-2:]
+    m = pixel_mask.bool().reshape(*pixel_mask.shape[:-2], h // patch, patch, w // patch, patch)
+    return m.any(-1).any(-2)
+
+
+def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Outpainting arguments: ``tokens`` int [B, h, w] placed with its top-left corner at (top, left) of a canvas
+    ``canvas_hw`` = (H, W).  Returns (init_x int64 [B, H, W], region bool [B, H, W]): the source tokens on the canvas (0
+    elsewhere) and a region that is True everywhere except under them.  CPU tensors, no device work."""
+    if not torch.is_tensor(tokens) or tokens.device.type != "cpu" or tokens.dim() != 3:
+        raise ValueError("outpaint_canvas: expected CPU tokens [B, h, w]")
+    B, h, w = tokens.shape
+    H, W = int(canvas_hw[0]), int(canvas_hw[1])
+    if not (0 <= top and top + h <= H and 0 <= left and left + w <= W):
+        raise ValueError(f"outpaint_canvas: a {h}x{w} grid at ({top}, {left}) does not fit a {H}x{W} canvas")
+    init_x = torch.zeros(B, H, W, dtype=torch.int64)
+    init_x[:, top:top + h, left:left + w] = tokens
+    region = torch.ones(B, H, W, dtype=torch.bool)
+    region[:, top:top + h, left:left + w] = False
+    return init_x, region
+
+
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
-                 codebook=None, generator=None, per_sample_cfg=False):
+                 codebook=None, generator=None, per_sample_cfg=False, region=None):
     B, H, W = latent_shape
     dev = model._device()
+    check_region(region, init_x, latent_shape, dev)
     use_cfg_any = cfgs is not None
     sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg)
     w_table = None
@@ -88,15 +146,25 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         ops.check_generators(generator, B, dev)
         ops.check_per_sample_numel(H * W * model.num_labels)
     with torch.inference_mode():
-        if sched is not None:       # one copy for the whole loop: [steps][B][3] params, then [steps + 1][B] noise levels
-            flat = ops.to_device_async(torch.cat([sched[0].view(-1), sched[1].view(-1)]), dev)
-            params_d = flat[:steps * B * 3].view(steps, B, 3)
-            r_d = flat[steps * B * 3:].view(steps + 1, B)
+        # one copy for the whole loop: [steps][B][3] params and [steps + 1][B] noise levels, and a CPU region
+        region_host = region is not None and region.device.type == "cpu"
+        parts = (list(sched) if sched is not None else []) + ([region] if region_host else [])
+        parts_d = ops.to_device_packed(parts, dev) if parts else []
+        if sched is not None:
+            params_d, r_d = parts_d[0], parts_d[1]
+        region_d = None
+        if region is not None:       # bool [B, H, W], True where tokens are generated
+            region_d = parts_d[-1] if region_host else region.contiguous()
         w_len = None
         if w_table is not None:      # one copy for the whole loop
             attn_weights, w_len = ops.attn_weights_to_device(*w_table, dev)
         init_noise = ops.randint(model.num_labels, (B, H, W), dev, generator)
-        sampled = init_x.to(dev) if init_x is not None else init_noise.clone()
+        if region_d is not None:     # where(region, init_noise, init_x)
+            src_d = init_x.to(device=dev, dtype=torch.int64).contiguous()
+            neg_t = torch.full((B,), -1.0, dtype=torch.float32, device=dev)
+            sampled = ops.composite(init_noise, src_d, region_d, neg_t)
+        else:
+            sampled = init_x.to(dev) if init_x is not None else init_noise.clone()
         if sched is None:
             t_list = torch.linspace(t_start, t_end, steps + 1)
             temperatures = torch.linspace(temperature[0], temperature[1], steps)
@@ -142,6 +210,10 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                     sampled = ops.resample_logits(lc, lu, cfg_i if guided else 0.0, temp_i, mode, generator)
                 else:
                     sampled = ops.resample_logits_params(lc, lu, params_i, mode, generator)
+            # outside the region the tokens are init_x's again; a renoising step composites in its own launch, so the
+            # composite is a launch of its own only where an intermediate shows it or nothing renoises
+            if region_d is not None and (collect or i >= renoise_steps):
+                sampled = ops.composite(sampled, src_d, region_d, neg_t)
             if collect:
                 intermediates.append(sampled)
             if i < renoise_steps:
@@ -149,7 +221,10 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                     t_next = torch.full((B,), float(t_list[i + 1]), dtype=torch.float32, device=dev)
                 else:
                     t_next = r_d[i + 1]
-                sampled = model.add_noise(sampled, t_next, random_x=init_noise, generator=generator)[0]
+                if region_d is None:
+                    sampled = model.add_noise(sampled, t_next, random_x=init_noise, generator=generator)[0]
+                else:
+                    sampled = model.add_noise(sampled, t_next, random_x=init_noise, generator=generator, src=src_d, region=region_d)[0]
                 if collect:
                     intermediates.append(sampled)
     return sampled, intermediates
@@ -216,10 +291,13 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
 
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
-                       exact=False, generator=None):
+                       exact=False, generator=None, region=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
-    ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute."""
+    ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
+    docstring): bool [B, H, W] on the CPU or the model's device, True where tokens are generated; ``init_x`` then holds the
+    tokens kept elsewhere.  ValueError, before anything is enqueued and before any generator advances, for a region without
+    init_x, of another shape or dtype, or on another device."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -227,21 +305,22 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     cfgs = _cfg_schedule(cfg, latent_shape[0], steps)
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
-                          generator=generator, per_sample_cfg=torch.is_tensor(cfg))
+                          generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region)
     return out
 
 
 def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None, init_x=None, steps=12, renoise_steps=None,
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
-                    generator=None):
+                    generator=None, region=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
     list or tuple of B entries, each None or a 1-D CPU float tensor that weights sample b's conditional forward alone (the
     unconditional rows are never weighted, as in the notebook).  Row i then equals row i of the call with vector i for every
     sample.  ValueError, before anything is enqueued and before any generator advances, for the wrong number of entries, a
-    CUDA, non-1-D or non-finite tensor, or a vector longer than the smallest key count the sample sees in an AttnBlock."""
+    CUDA, non-1-D or non-finite tensor, or a vector longer than the smallest key count the sample sees in an AttnBlock.
+    ``region`` as in ``sample_distributed``; every intermediate holds init_x's tokens outside it."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -252,4 +331,4 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     codebook = vqmodel.vquantizer.codebook.weight.data if vqmodel is not None else None
     return _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                         temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, True,
-                        sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg))
+                        sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region)

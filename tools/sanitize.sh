@@ -85,6 +85,23 @@ eng.submit(cond(5, False), generator=torch.Generator(device=DEV).manual_seed(2),
 eng.submit(cond(2, False), generator=torch.Generator(device=DEV).manual_seed(3), steps=1, attn_weights=torch.rand(2))
 eng.submit(cond(3, False), generator=torch.Generator(device=DEV).manual_seed(4), steps=1, keep_intermediates=True)
 print("engine weights", [q.result.shape for q in eng.run_until_idle()])
+# region sampling: the masked add-noise on an odd H*W with a slot map, region rows and a plain (all-True) row, a t < 0 row;
+# then an engine whose slot 0 is reused by a request without a region
+reg = torch.rand(3, 7, 9, device=DEV, generator=g) < 0.5; reg[1] = True
+src7 = torch.randint(0, 64, (3, 7, 9), device=DEV, generator=g)
+t7 = torch.tensor([0.5, -1.0, 0.9], device=DEV)
+pool = torch.zeros_like(x7)
+ops.add_noise_per_sample(x7, t7, x7, 64, ops.philox_table([torch.Generator(device=DEV).manual_seed(s) for s in (4, 5, 6)], 63, DEV),
+                         pool, slot=torch.tensor([2, 0, 1], dtype=torch.int32, device=DEV), src=src7, region=reg)
+print("add_noise region", ops.add_noise(x7, t7, None, 64, [torch.Generator(device=DEV).manual_seed(s) for s in (7, 8, 9)],
+                                        src=src7, region=reg)[0].shape, ops.add_noise(x7, t7, x7, 64, src=src7, region=reg)[0].shape)
+eng = SamplingEngine(m, latent_hw=(8, 8), max_batch=2, max_cond_len=20, unconditional_inputs={k: v * 0 for k, v in cond(4, False).items()})
+eng.submit(cond(5, False), generator=torch.Generator(device=DEV).manual_seed(1), steps=1,
+           init_x=torch.randint(0, 64, (1, 8, 8)), region=torch.rand(1, 8, 8) < 0.5)
+eng.submit(cond(3, False), generator=torch.Generator(device=DEV).manual_seed(2), steps=2, cfg=None,
+           init_x=torch.randint(0, 64, (1, 8, 8), device=DEV), region=torch.rand(1, 8, 8) < 0.3, keep_intermediates=True)
+eng.submit(cond(2, False), generator=torch.Generator(device=DEV).manual_seed(3), steps=1)
+print("engine regions", [q.result.shape for q in eng.run_until_idle()])
 t = torch.from_numpy
 print("forward", m(t(gg["x"]).to(DEV), t(gg["r"]).to(DEV), t(gg["byt5"]).to(DEV), clip=t(gg["clip"]).to(DEV)).shape)
 torch.cuda.synchronize(); print("sanitizer case 2 done")
