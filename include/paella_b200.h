@@ -368,6 +368,31 @@ int pb200_paella_sample_tokens_params(pb200_paella* m, const float* features, in
 int pb200_paella_sample_tokens_pairs(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
                                      const uint64_t* seed_offset, int64_t* tokens_out, void* workspace, int64_t workspace_bytes,
                                      void* stream);
+/* pb200_paella_sample_tokens_pairs for a batch in which some samples do not draw this step (they are sampled in another
+ * mode, pb200_paella_resample_samples).  skip: int32 [batch]; a sample with skip[b] != 0 takes no part in the launch: its
+ * rows of tokens_out are left as they are and its seed_offset entry is not read (its generator is not to be advanced).
+ * Every other sample's tokens are those of pb200_paella_sample_tokens_pairs, which is this call with skip = NULL. */
+int pb200_paella_sample_tokens_pairs_skip(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                                          const uint64_t* seed_offset, const int* skip, int64_t* tokens_out, void* workspace,
+                                          int64_t workspace_bytes, void* stream);
+
+/* The notebook's non-multinomial sampling modes (paella_inference.ipynb cell 3) for a list of samples of the features of
+ * pb200_paella_features_pairs, so that samples in different modes share one forward.  For each listed sample s the call
+ * computes what pb200_paella_logits followed by pb200_resample_logits_params (mode = 1, argmax) or
+ * pb200_resample_quant_params (mode = 2, quant: softmax @ codebook, then the nearest code) computes for that sample on its
+ * own, and writes its tokens to rows [s*hw, (s+1)*hw) of tokens_out.  Neither mode draws a random number.
+ *   features  fp32 [(batch + n_pairs)*hw, c_out]: sample s's rows at s*hw, a guided sample's unconditional rows at
+ *             (batch + s)*hw;
+ *   samples   int32 [n]: distinct sample indices; samples[0, n_guided) are guided (each < n_pairs) and are mixed with
+ *             their unconditional logits, the others are not;
+ *   params    fp32 [batch][3] of per-sample (cfg, 1 - cfg, 1/T), as for pb200_resample_logits_params;
+ *   codebook  fp32 [num_labels][c_latent] for mode 2 (c_latent 1..8), ignored for mode 1.
+ * The samples go through the out_mapper GEMM at most `chunk` guided (or 2*chunk unguided) at a time, so the logits scratch
+ * is bounded by pb200_paella_resample_workspace_bytes(chunk, hw) = 2*chunk*hw*(2*c_out + 4*num_labels) bytes (rounded). */
+int64_t pb200_paella_resample_workspace_bytes(const pb200_paella* m, int chunk, int hw);
+int pb200_paella_resample_samples(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const int* samples, int n,
+                                  int n_guided, const float* params, int mode, const float* codebook, int c_latent, int chunk,
+                                  int64_t* tokens_out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * VQGAN (ref/src/vqgan.py:45-107).

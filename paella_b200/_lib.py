@@ -114,6 +114,11 @@ SIGNATURES = {
                                                c_void_p]),
     "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_int64, c_void_p]),
+    "pb200_paella_sample_tokens_pairs_skip": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                      c_void_p, c_int64, c_void_p]),
+    "pb200_paella_resample_workspace_bytes": (c_int64, [c_void_p, c_int, c_int]),
+    "pb200_paella_resample_samples": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,
+                                              c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_logits":(c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_sample_tokens": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_uint64,
                                            c_uint64, c_void_p, c_void_p, c_int64, c_void_p]),

@@ -857,6 +857,34 @@ int launch_mix_cast_rows_f16(const float* a, const float* b, const float* w, int
     return 0;
 }
 
+// Gather + cast of whole samples: packed block j (per elements) is the fp32 block src[j] of `a`, src[j] = samples[j] for
+// j < n_list, batch + samples[j - n_list] for the others (a sample's unconditional rows after the batch).  Each element is
+// converted as cast_kernel<0> converts it (round to nearest).  per % 4 == 0, so a thread's four elements share one block.
+__global__ void gather_cast_kernel(const float* __restrict__ a, const int* __restrict__ samples, int n_list, int batch, int64_t per,
+                                   __half* __restrict__ out) {
+    const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    if (i >= per) return;
+    const int j = blockIdx.y;
+    const int64_t src = j < n_list ? samples[j] : (int64_t)batch + samples[j - n_list];
+    const float4 v = *reinterpret_cast<const float4*>(a + src * per + i);
+    uint2 pk;
+    pk.x = pack_half2(v.x, v.y);
+    pk.y = pack_half2(v.z, v.w);
+    *reinterpret_cast<uint2*>(out + (int64_t)j * per + i) = pk;
+}
+
+int launch_gather_cast_f16(const float* a, const int* samples, int n_list, int n_blocks, int batch, int64_t per, __half* out,
+                           cudaStream_t st) {
+    ProfScope prof("cast", (double)n_blocks * per * 6.0, st);
+    if (n_blocks == 0 || per == 0) return 0;
+    PB_CHECK(per % 4 == 0 && n_blocks <= 65535 && n_blocks <= 2 * n_list, "gather_cast: %d blocks of %lld elements", n_blocks,
+             (long long)per);
+    dim3 grid((unsigned)ceil_div(ceil_div(per, 4), 256), (unsigned)n_blocks);
+    gather_cast_kernel<<<grid, 256, 0, st>>>(a, samples, n_list, batch, per, out);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
 // ------------------------------------------------------------------ layout
 // [B, R, Cc] -> [B, Cc, R] through a 32x33 shared tile
 __global__ void transpose_kernel(const float* __restrict__ in, int R, int Cc, float* __restrict__ out) {

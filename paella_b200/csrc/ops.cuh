@@ -53,6 +53,14 @@ int launch_silu_cast_f16(const float* x, int64_t n, __half* out, cudaStream_t st
 int launch_mix_cast_f16(const float* a, const float* b, float wa, float wb, int64_t n, __half* out, cudaStream_t st);
 // the same mix with per-sample weights: element e uses (wa, wb) = (w[3 s], w[3 s + 1]), s = e / per (w: DEVICE [samples][3])
 int launch_mix_cast_rows_f16(const float* a, const float* b, const float* w, int64_t per, int64_t n, __half* out, cudaStream_t st);
+// the fp16 cast of whole samples of `per` elements into n_blocks packed blocks: block j < n_list is sample samples[j] of a,
+// block j >= n_list is sample batch + samples[j - n_list] (samples: DEVICE int32 [n_list]); per % 4 == 0
+int launch_gather_cast_f16(const float* a, const int* samples, int n_list, int n_blocks, int batch, int64_t per, __half* out,
+                           cudaStream_t st);
+// resample_logits_kernel<1> (mode 1, argmax) or resample_quant_kernel (mode 2) over `batch` packed samples of logits whose
+// output sample is map[b] (DEVICE int32 [batch]): params row and token row map[b] (rng.cu)
+int launch_resample_mapped(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, const float* params,
+                           const int* map, int mode, const float* codebook, int c_latent, int64_t* out, cudaStream_t st);
 
 // [B, C, HW] <-> [B, HW, C] fp32
 int launch_nchw_to_nhwc(const float* in, int B, int C, int HW, float* out, cudaStream_t st);

@@ -4,6 +4,7 @@
 //   forward                  ref/src/modules.py:263-275 (_down_encode :234-247, _up_decode :249-261)
 // The x- and t-independent half of every AttnBlock (kv_mapper + K/V projection of the conditioning rows,
 // ref/src/modules.py:77 + nn.MultiheadAttention in_proj rows [E:3E]) is hoisted into pb200_paella_prepare_cond.
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <string>
@@ -943,6 +944,13 @@ int pb200_paella_sample_tokens_params(pb200_paella* m, const float* features, in
 int pb200_paella_sample_tokens_pairs(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
                                      const uint64_t* seed_offset, int64_t* tokens_out, void* workspace, int64_t workspace_bytes,
                                      void* stream) {
+    return pb200_paella_sample_tokens_pairs_skip(m, features, batch, n_pairs, hw, params, seed_offset, nullptr, tokens_out, workspace,
+                                                 workspace_bytes, stream);
+}
+
+int pb200_paella_sample_tokens_pairs_skip(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                                          const uint64_t* seed_offset, const int* skip, int64_t* tokens_out, void* workspace,
+                                          int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "sample_tokens_pairs: weights not bound");
     PB_CHECK(params != nullptr && seed_offset != nullptr, "sample_tokens_pairs: params and seed_offset are required");
     const pb200_paella_config& c = m->cfg;
@@ -959,7 +967,55 @@ int pb200_paella_sample_tokens_pairs(pb200_paella* m, const float* features, int
     PB_TRY(launch_mix_cast_rows_f16(features, features + rows * c.c_out, params, (int64_t)hw * c.c_out, mixed, a16, st));
     PB_TRY(launch_cast_f16(features + mixed, rows * c.c_out - mixed, a16 + mixed, st));
     return launch_fused_sampler_params(a16, batch, hw, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f, params, 0, 0,
-                                       seed_offset, tokens_out, st);
+                                       seed_offset, tokens_out, st, skip);
+}
+
+// scratch of pb200_paella_resample_samples: fp16 features and fp32 logits of 2 * chunk sample blocks
+static int64_t resample_scratch(const pb200_paella_config& c, int chunk, int hw, int64_t* logits_off) {
+    const int64_t blocks = 2 * (int64_t)chunk;
+    const int64_t a_bytes = (blocks * hw * c.c_out * 2 + 255) / 256 * 256;
+    if (logits_off) *logits_off = a_bytes;
+    return a_bytes + blocks * hw * (int64_t)c.num_labels * 4;
+}
+
+int64_t pb200_paella_resample_workspace_bytes(const pb200_paella* m, int chunk, int hw) {
+    if (m == nullptr) { set_error("resample_workspace_bytes: null model handle"); return -1; }
+    if (chunk < 1 || hw < 1) { set_error("resample_workspace_bytes: chunk and hw must be >= 1"); return -1; }
+    return resample_scratch(m->cfg, chunk, hw, nullptr);
+}
+
+int pb200_paella_resample_samples(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const int* samples, int n,
+                                  int n_guided, const float* params, int mode, const float* codebook, int c_latent, int chunk,
+                                  int64_t* tokens_out, void* workspace, int64_t workspace_bytes, void* stream) {
+    PB_CHECK(m->blob != nullptr, "resample_samples: weights not bound");
+    PB_CHECK(samples != nullptr && params != nullptr, "resample_samples: samples and params are required");
+    PB_CHECK(mode == 1 || (mode == 2 && codebook != nullptr), "resample_samples: mode %d (1 = argmax, 2 = quant with a codebook)", mode);
+    PB_CHECK(batch >= 0 && hw > 0 && n_pairs >= 0 && n_pairs <= batch && n >= 0 && n <= batch && n_guided >= 0 && n_guided <= n &&
+             n_guided <= n_pairs, "resample_samples: %d samples (%d guided) of a batch of %d with %d pairs", n, n_guided, batch, n_pairs);
+    PB_CHECK(chunk >= 1 && chunk <= 32767, "resample_samples: chunk %d", chunk);
+    const pb200_paella_config& c = m->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+    int64_t logits_off = 0;
+    PB_CHECK(resample_scratch(c, chunk, hw, &logits_off) <= workspace_bytes,
+             "resample_samples: workspace too small (use pb200_paella_resample_workspace_bytes)");
+    __half* a16 = reinterpret_cast<__half*>(workspace);
+    float* logits = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(workspace) + logits_off);
+    const int64_t per = (int64_t)hw * c.c_out;
+    // guided samples first, `chunk` at a time (conditional then unconditional blocks), then the others 2 * chunk at a time: every
+    // launch fills at most 2 * chunk blocks of the scratch
+    for (int i = 0; i < n;) {
+        const bool guided = i < n_guided;
+        const int cnt = guided ? std::min(chunk, n_guided - i) : std::min(2 * chunk, n - i);
+        const int blocks = guided ? 2 * cnt : cnt;
+        PB_TRY(launch_gather_cast_f16(features, samples + i, cnt, blocks, batch, per, a16, st));
+        pb200_gemm_epilogue e = epi(PB200_EPI_NCHW_F32, nullptr, logits, 0);
+        e.rows_per_sample = hw;
+        PB_TRY(m->gemm(a16, c.c_out, (int64_t)blocks * hw, c.c_out, m->out_w, c.num_labels, e, st));
+        const float* lu = guided ? logits + (int64_t)cnt * c.num_labels * hw : nullptr;
+        PB_TRY(launch_resample_mapped(logits, lu, cnt, c.num_labels, hw, params, samples + i, mode, codebook, c_latent, tokens_out, st));
+        i += cnt;
+    }
+    return 0;
 }
 
 }  // extern "C"

@@ -6,6 +6,7 @@
 //   Paella.add_noise     ref/src/modules.py:277-283  (and its explicit-mask form, the region sampling of utils._sample_core)
 // PyTorch-side arithmetic: ATen/native/cuda/DistributionTemplates.h, ATen/core/TransformationHelper.h.
 #include "common.cuh"
+#include "ops.cuh"
 #include "paella_b200.h"
 
 #include <float.h>
@@ -177,16 +178,19 @@ __global__ void __launch_bounds__(256) multinomial_kernel(const float* __restric
 //   p  = exp(l' - max) / sum          (softmax dim=1)
 //   tok = argmax_k p_k / q_k
 // params (may be null): DEVICE [B][3] per-sample (cfg, 1 - cfg, 1/T), replacing the three scalars for sample b = blockIdx.y.
+// map (may be null): DEVICE int32 [gridDim.y]; the logits of launch sample b = blockIdx.y are those of output sample map[b],
+// whose params row and token row it uses -- a packed launch over some samples writes straight into the batch's rows.
 template <int MODE>
 __global__ void __launch_bounds__(256, 4) resample_logits_kernel(const float* __restrict__ lc, const float* __restrict__ lu,
                                                                  int k, int64_t hw, float cfg_arg, float one_minus_cfg_arg,
                                                                  float inv_t_arg, const float* __restrict__ params, TorchPhilox s,
-                                                                 int64_t* __restrict__ out) {
+                                                                 const int* __restrict__ map, int64_t* __restrict__ out) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t b = blockIdx.y;
-    const float cfg = params ? params[3 * b] : cfg_arg;
-    const float one_minus_cfg = params ? params[3 * b + 1] : one_minus_cfg_arg;
-    const float inv_t = params ? params[3 * b + 2] : inv_t_arg;
+    const int64_t ob = map ? (int64_t)map[b] : b;       // output sample
+    const float cfg = params ? params[3 * ob] : cfg_arg;
+    const float one_minus_cfg = params ? params[3 * ob + 1] : one_minus_cfg_arg;
+    const float inv_t = params ? params[3 * ob + 2] : inv_t_arg;
     const int64_t pos = (int64_t)blockIdx.x * 32 + lane;
     const bool valid = pos < hw;
     const float* c_ptr = lc + b * (int64_t)k * hw + (valid ? pos : 0);
@@ -209,7 +213,7 @@ __global__ void __launch_bounds__(256, 4) resample_logits_kernel(const float* __
         if (warp == 0) {
             ArgBest bb{red[0][lane], redi[0][lane]};
             for (int w = 1; w < 8; ++w) bb = better(bb, ArgBest{red[w][lane], redi[w][lane]});
-            if (valid) out[b * hw + pos] = bb.idx;
+            if (valid) out[ob * hw + pos] = bb.idx;
         }
         return;
     }
@@ -257,12 +261,13 @@ template <int C>
 __global__ void __launch_bounds__(256) resample_quant_kernel(const float* __restrict__ lc, const float* __restrict__ lu, int k,
                                                              int64_t hw, float cfg_arg, float one_minus_cfg_arg, float inv_t_arg,
                                                              const float* __restrict__ params, const float* __restrict__ codebook,
-                                                             int64_t* __restrict__ out) {
+                                                             const int* __restrict__ map, int64_t* __restrict__ out) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t b = blockIdx.y;
-    const float cfg = params ? params[3 * b] : cfg_arg;                   // per-sample parameters as in resample_logits
-    const float one_minus_cfg = params ? params[3 * b + 1] : one_minus_cfg_arg;
-    const float inv_t = params ? params[3 * b + 2] : inv_t_arg;
+    const int64_t ob = map ? (int64_t)map[b] : b;       // output sample, as in resample_logits_kernel
+    const float cfg = params ? params[3 * ob] : cfg_arg;                  // per-sample parameters as in resample_logits
+    const float one_minus_cfg = params ? params[3 * ob + 1] : one_minus_cfg_arg;
+    const float inv_t = params ? params[3 * ob + 2] : inv_t_arg;
     const int64_t pos = (int64_t)blockIdx.x * 32 + lane;
     const bool valid = pos < hw;
     const float* c_ptr = lc + b * (int64_t)k * hw + (valid ? pos : 0);
@@ -330,7 +335,7 @@ __global__ void __launch_bounds__(256) resample_quant_kernel(const float* __rest
         int bj = redi[0][lane];
         for (int w = 1; w < 8; ++w)
             if (red[w][lane] < bd || (red[w][lane] == bd && redi[w][lane] < bj)) { bd = red[w][lane]; bj = redi[w][lane]; }
-        out[b * hw + pos] = bj;
+        out[ob * hw + pos] = bj;
     }
 }
 
@@ -381,8 +386,9 @@ namespace pb {
 // 0-dim CPU tensor and torch multiplies by its fp32 reciprocal.  These are the fp32 constants a per-sample table holds too.
 static int resample_logits(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, double cfg,
                            double temperature, const float* params, int mode, uint64_t seed, uint64_t offset, int64_t* out,
-                           cudaStream_t st) {
+                           cudaStream_t st, const int* map = nullptr) {
     PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
+    PB_CHECK(map == nullptr || mode == 1, "resample: an output map is for argmax only");
     PB_CHECK(mode == 0 || mode == 1, "resample: mode must be 0 (multinomial) or 1 (argmax)");
     PB_CHECK(batch * hw * k < (1ll << 31), "resample: B*HW*K >= 2^31 would split the torch kernel (unsupported)");
     if (batch == 0 || hw == 0) return 0;
@@ -392,28 +398,37 @@ static int resample_logits(const float* logits_c, const float* logits_u, int64_t
     const float inv_t = 1.0f / (float)temperature;
     dim3 grid(ceil_div(hw, 32), (unsigned)batch);
     if (mode == 0)
-        resample_logits_kernel<0><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, s, out);
+        resample_logits_kernel<0><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, s, nullptr, out);
     else
-        resample_logits_kernel<1><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, s, out);
+        resample_logits_kernel<1><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, s, map, out);
     PB_LAUNCH_CHECK();
     return 0;
 }
 
 static int resample_quant(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, double cfg,
                           double temperature, const float* params, const float* codebook, int c_latent, int64_t* out,
-                          cudaStream_t st) {
+                          cudaStream_t st, const int* map = nullptr) {
     PB_CHECK(c_latent >= 1 && c_latent <= 8, "resample_quant: c_latent %d unsupported (1..8)", c_latent);
     if (batch == 0 || hw == 0) return 0;
     const float cfg_f = (float)cfg, one_minus = (float)(1.0 - cfg), inv_t = 1.0f / (float)temperature;
     dim3 grid(ceil_div(hw, 32), (unsigned)batch);
     switch (c_latent) {
 #define PB_RQ_CASE(C) \
-    case C: resample_quant_kernel<C><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, codebook, out); break;
+    case C: resample_quant_kernel<C><<<grid, 256, 0, st>>>(logits_c, logits_u, (int)k, hw, cfg_f, one_minus, inv_t, params, codebook, map, out); break;
         PB_RQ_CASE(1) PB_RQ_CASE(2) PB_RQ_CASE(3) PB_RQ_CASE(4) PB_RQ_CASE(5) PB_RQ_CASE(6) PB_RQ_CASE(7) PB_RQ_CASE(8)
 #undef PB_RQ_CASE
     }
     PB_LAUNCH_CHECK();
     return 0;
+}
+
+int launch_resample_mapped(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, const float* params,
+                           const int* map, int mode, const float* codebook, int c_latent, int64_t* out, cudaStream_t st) {
+    PB_CHECK(params != nullptr && map != nullptr, "resample_mapped: params and map are required");
+    PB_CHECK(batch <= 65535, "resample_mapped: %lld samples in one launch (grid.y)", (long long)batch);
+    if (mode == 1) return resample_logits(logits_c, logits_u, batch, k, hw, 0.0, 1.0, params, 1, 0, 0, out, st, map);
+    PB_CHECK(mode == 2, "resample_mapped: mode %d (1 = argmax, 2 = quant)", mode);
+    return resample_quant(logits_c, logits_u, batch, k, hw, 0.0, 1.0, params, codebook, c_latent, out, st, map);
 }
 }  // namespace pb
 

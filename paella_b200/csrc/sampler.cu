@@ -36,6 +36,8 @@ __device__ __forceinline__ void argmax_merge(float& bv, int& bi, float ov, int o
 // PS (per-sample streams): the R rows are R / hw samples of hw rows; sample b draws on its own generator, (seed, philox
 // offset) = seed_off[2b], seed_off[2b + 1], with rng's stride (the launch policy of ONE sample's draw), and element
 // (row, col) of it is element (row - b hw) * NL + col of that draw -- what a batch-1 launch on that generator would use.
+// skip (PS only, may be null): int32 [R / hw]; a sample with skip[b] != 0 does not draw this step and its rows of `out` are
+// left as they are (a CTA whose rows all belong to such samples returns at once).
 __device__ __forceinline__ void per_sample_stream(const uint64_t* __restrict__ seed_off, int b, TorchPhilox& s) {
     s.seed = seed_off[2 * b];
     s.offset4 = seed_off[2 * b + 1] >> 2;
@@ -51,7 +53,7 @@ template <bool PS, bool PP>
 __global__ void __launch_bounds__(SMP_THREADS, 1)
 fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_w, int R, int NL,
                      int Kc, float inv_t, TorchPhilox rng, int hw, const uint64_t* __restrict__ seed_off,
-                     const float* __restrict__ params, int phw, int64_t* __restrict__ out) {
+                     const float* __restrict__ params, int phw, const int* __restrict__ skip, int64_t* __restrict__ out) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t a_base = smem_base;
@@ -66,6 +68,15 @@ fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
     const int n_kb = (Kc + 63) / 64;
     const int n_chunks = (NL + SMP_BN - 1) / SMP_BN;
     const int m_idx = blockIdx.x * 128;
+    if constexpr (PS) {
+        // a tile whose rows all belong to samples that do not draw this step has nothing to write
+        if (skip != nullptr) {
+            const int b_last = (min(m_idx + 128, R) - 1) / hw;
+            int b = m_idx / hw;
+            while (b <= b_last && skip[b] != 0) ++b;
+            if (b > b_last) return;
+        }
+    }
 
     if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tm_a);
@@ -164,7 +175,7 @@ fused_sampler_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
             for (int o = 1; o <= 2; o <<= 1)
                 argmax_merge(bv[rr], bi[rr], __shfl_xor_sync(0xffffffffu, bv[rr], o), __shfl_xor_sync(0xffffffffu, bi[rr], o));
             const int row = row0 + 8 * rr;
-            if ((lane & 3) == 0 && row < R) out[row] = bi[rr];
+            if ((lane & 3) == 0 && row < R && !(PS && skip != nullptr && skip[row / hw] != 0)) out[row] = bi[rr];
         }
     }
 }
@@ -199,7 +210,7 @@ __global__ void __launch_bounds__(SH_THREADS, 1)
 fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __grid_constant__ CUtensorMap tm_w, int R, int NL,
                             int Kc, int rs, int tasks_per_block, float inv_t, TorchPhilox rng, int hw, int blocks_per_sample,
                             const uint64_t* __restrict__ seed_off, const float* __restrict__ params, int phw,
-                            int64_t* __restrict__ out) {
+                            const int* __restrict__ skip, int64_t* __restrict__ out) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -222,6 +233,9 @@ fused_sampler_shared_kernel(const __grid_constant__ CUtensorMap tm_f, const __gr
     const int task = blockIdx.x - sample * blocks_per_sample * tasks_per_block;
     const int blk = task / tasks_per_block;                            // 4rs-row block = Philox call index
     const int jj0 = (task - blk * tasks_per_block) * SH_JJ;
+    if constexpr (PS) {
+        if (skip != nullptr && skip[sample] != 0) return;      // the CTA's sample does not draw this step: no TMA, no write
+    }
 
     if constexpr (PP && !PS) {
         if (threadIdx.x < SH_N) {                    // token column c = jj_local * 4 + g, as in the reduction below
@@ -381,21 +395,22 @@ int64_t fused_sampler_rows_padded(int64_t R, int NL) {
 template <bool PS, bool PP>
 static void launch_shared(unsigned grid, const CUtensorMap& tf, const CUtensorMap& tw, int R, int NL, int Kc, int rs, int tpb,
                           float inv_t, TorchPhilox rng, int hw, int n_blocks, const uint64_t* seed_off, const float* params,
-                          int phw, int64_t* out, cudaStream_t st) {
+                          int phw, const int* skip, int64_t* out, cudaStream_t st) {
     fused_sampler_shared_kernel<PS, PP><<<grid, SH_THREADS, PP ? SH_SMEM_PP : SH_SMEM, st>>>(
-        tf, tw, R, NL, Kc, rs, tpb, inv_t, rng, hw, n_blocks, seed_off, params, phw, out);
+        tf, tw, R, NL, Kc, rs, tpb, inv_t, rng, hw, n_blocks, seed_off, params, phw, skip, out);
 }
 
 template <bool PS, bool PP>
 static void launch_generic(unsigned grid, const CUtensorMap& ta, const CUtensorMap& tw, int R, int NL, int Kc, float inv_t,
-                           TorchPhilox rng, int hw, const uint64_t* seed_off, const float* params, int phw, int64_t* out,
-                           cudaStream_t st) {
-    fused_sampler_kernel<PS, PP><<<grid, SMP_THREADS, SMP_SMEM, st>>>(ta, tw, R, NL, Kc, inv_t, rng, hw, seed_off, params, phw, out);
+                           TorchPhilox rng, int hw, const uint64_t* seed_off, const float* params, int phw, const int* skip,
+                           int64_t* out, cudaStream_t st) {
+    fused_sampler_kernel<PS, PP><<<grid, SMP_THREADS, SMP_SMEM, st>>>(ta, tw, R, NL, Kc, inv_t, rng, hw, seed_off, params, phw, skip,
+                                                                      out);
 }
 
 static int launch_sampler(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL, float inv_t,
                           uint64_t seed, uint64_t offset, const uint64_t* seed_off, const float* params, int64_t phw,
-                          int64_t* out, cudaStream_t st) {
+                          const int* skip, int64_t* out, cudaStream_t st) {
     const bool ps = seed_off != nullptr, pp = params != nullptr;
     const int64_t R = n_samp * hw;
     TorchPhilox rng = make_torch_philox(seed, offset, hw * (int64_t)NL);
@@ -426,7 +441,7 @@ static int launch_sampler(const __half* a16, int64_t n_samp, int64_t hw, int Kc,
             PB_CHECK(grid < (1ll << 31), "fused sampler: %lld CTAs", (long long)grid);
             auto* fn = ps ? (pp ? launch_shared<true, true> : launch_shared<true, false>)
                           : (pp ? launch_shared<false, true> : launch_shared<false, false>);
-            fn((unsigned)grid, tf, tw, (int)R, NL, Kc, rs, tpb, inv_t, rng, (int)hw, n_blocks, seed_off, params, (int)phw, out, st);
+            fn((unsigned)grid, tf, tw, (int)R, NL, Kc, rs, tpb, inv_t, rng, (int)hw, n_blocks, seed_off, params, (int)phw, skip, out, st);
             PB_LAUNCH_CHECK();
             return 0;
         }
@@ -444,7 +459,7 @@ static int launch_sampler(const __half* a16, int64_t n_samp, int64_t hw, int Kc,
     PB_TRY(make_tmap_f16_2d(&tw, w16, NL, Kc, Kc, SMP_BN));
     auto* fn = ps ? (pp ? launch_generic<true, true> : launch_generic<true, false>)
                   : (pp ? launch_generic<false, true> : launch_generic<false, false>);
-    fn((unsigned)ceil_div(R, 128), ta, tw, (int)R, NL, Kc, inv_t, rng, (int)hw, seed_off, params, (int)phw, out, st);
+    fn((unsigned)ceil_div(R, 128), ta, tw, (int)R, NL, Kc, inv_t, rng, (int)hw, seed_off, params, (int)phw, skip, out, st);
     PB_LAUNCH_CHECK();
     return 0;
 }
@@ -455,7 +470,7 @@ int launch_fused_sampler(const __half* a16, int64_t R, int Kc, const __half* w16
     PB_CHECK(R * (int64_t)NL < (1ll << 31), "fused sampler: rows*labels >= 2^31 would split the torch kernel (unsupported)");
     PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
     if (R == 0) return 0;
-    return launch_sampler(a16, 1, R, Kc, w16, NL, inv_t, seed, offset, nullptr, nullptr, 1, out, st);
+    return launch_sampler(a16, 1, R, Kc, w16, NL, inv_t, seed, offset, nullptr, nullptr, 1, nullptr, out, st);
 }
 
 int launch_fused_sampler_per_sample(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL,
@@ -466,7 +481,8 @@ int launch_fused_sampler_per_sample(const __half* a16, int64_t n_samp, int64_t h
 
 int launch_fused_sampler_params(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL, float inv_t,
                                 const float* params, uint64_t seed, uint64_t offset, const uint64_t* seed_off, int64_t* out,
-                                cudaStream_t st) {
+                                cudaStream_t st, const int* skip) {
+    PB_CHECK(skip == nullptr || seed_off != nullptr, "fused sampler: a skip table needs per-sample streams");
     PB_CHECK(Kc % 8 == 0 && Kc <= 64 * SMP_MAX_KB, "fused sampler: c_out=%d unsupported (<= %d, multiple of 8)", Kc, 64 * SMP_MAX_KB);
     PB_CHECK(n_samp * hw < (1ll << 31), "fused sampler: %lld rows", (long long)(n_samp * hw));
     if (seed_off != nullptr) {
@@ -480,8 +496,8 @@ int launch_fused_sampler_params(const __half* a16, int64_t n_samp, int64_t hw, i
     }
     if (n_samp == 0 || hw == 0) return 0;
     if (seed_off != nullptr)          // one stream per sample: a launch "sample" is a parameter sample
-        return launch_sampler(a16, n_samp, hw, Kc, w16, NL, inv_t, 0, 0, seed_off, params, hw, out, st);
-    return launch_sampler(a16, 1, n_samp * hw, Kc, w16, NL, inv_t, seed, offset, nullptr, params, hw, out, st);
+        return launch_sampler(a16, n_samp, hw, Kc, w16, NL, inv_t, 0, 0, seed_off, params, hw, skip, out, st);
+    return launch_sampler(a16, 1, n_samp * hw, Kc, w16, NL, inv_t, seed, offset, nullptr, params, hw, nullptr, out, st);
 }
 
 }  // namespace pb

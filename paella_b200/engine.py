@@ -21,13 +21,20 @@ t_end, sampling_conditional_steps, attn_weights=w, generator=[g])``; each step's
 device pool indexed by its token slot.  With ``region=`` (bool [1, H, W], True where tokens are generated) and ``init_x`` (the
 source tokens kept elsewhere) a request inpaints or outpaints as ``sample_distributed(..., init_x, region=region)`` does: its
 source tokens and region sit in device pools by token slot, and the step's one add-noise launch puts every row's source
-tokens back outside its region (a request without a region has an all-True row).
+tokens back outside its region (a request without a region has an all-True row).  With ``mode='argmax'`` or ``'quant'`` and
+``sampling_quant_steps=k`` (steps i >= k use 'quant'; 'quant' needs the engine's ``vqmodel``) the request's tokens, intermediates
+and generator offset are those of ``sample_notebook(model, inputs, (1, H, W), uncond, init_x, steps, renoise_steps, temperature,
+cfg, mode, t_start, t_end, sampling_conditional_steps, sampling_quant_steps, attn_weights, vqmodel=vq, generator=[g],
+region=region)``: a step in argmax or quant mode draws nothing from ``g`` (only its mask draw, if it renoises).
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
 builds one table (noise levels, (cfg, 1 - cfg, 1/T), renoise targets, Philox (seed, offset) pairs, row -> slot maps) and
 sends it to the device with one asynchronous copy; the step itself is a gather of the rows from the token pool, the forward,
-one fused-sampler launch and one per-sample add-noise launch that writes every row back into its slot.  The host knows which
+one fused-sampler launch and one per-sample add-noise launch that writes every row back into its slot.  A step whose rows are
+in several sampling modes adds each row's mode to the table: the fused sampler skips the argmax and quant rows, which then go
+through the out_mapper GEMM to logits (a bounded number of samples at a time) and the argmax or quant kernel, one call per mode
+(Paella.sample_tokens_modes).  The host knows which
 requests finish at which step, so ``step()`` never synchronises.
 """
 from __future__ import annotations
@@ -51,13 +58,14 @@ class Request:
     def __init__(self, steps: int, renoise_steps: int, cond_steps: int, guided: bool, params: torch.Tensor, r: torch.Tensor,
                  generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False,
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
-                 region: Optional[torch.Tensor] = None):
+                 region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
         self.attn_weights = attn_weights         # CPU float32 [n] or None
         self.region = region                     # bool [1, H, W] or None, until admission
         self.has_region = region is not None
+        self.mode, self.quant_steps = mode, quant_steps      # sampling mode, and the step from which 'quant' is used (or None)
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -69,6 +77,10 @@ class Request:
     def done(self) -> bool:
         return self.result is not None
 
+    def mode_at(self, k: int) -> str:
+        """The sampling mode of step k: 'quant' from step ``sampling_quant_steps`` on, the request's own mode before."""
+        return ops.mode_at(self.mode, self.quant_steps, k)
+
 
 class StepPlan:
     """The host tables of one step (CPU tensors), rows in batch order: guided requests first."""
@@ -79,6 +91,8 @@ class StepPlan:
         self.r = torch.stack([q.r[q.k] for q in order])
         self.params = torch.stack([q.params[q.k] for q in order])
         self.renoise = [q.k < q.renoise_steps for q in order]
+        self.modes = [q.mode_at(q.k) for q in order]
+        self.draws = [md == "multinomial" for md in self.modes]     # only multinomial rows draw the sampler's exponentials
         # a row that does not renoise keeps its tokens (t < 0 never passes the mask test)
         self.t_next = torch.stack([q.r[q.k + 1] if rn else torch.tensor(-1.0) for q, rn in zip(order, self.renoise)])
         self.row_slot = torch.tensor([q.slot for q in order], dtype=torch.int32)
@@ -156,15 +170,20 @@ class SamplingEngine:
 
     def submit(self, model_inputs, unconditional_inputs=None, *, generator=None, steps=12, renoise_steps=None,
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
-               decode=False, attn_weights=None, keep_intermediates=False, region=None) -> Request:
+               decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
+               sampling_quant_steps=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
         steps < 1, or an ``attn_weights`` that is not a finite 1-D CPU float tensor at most as long as the smallest key count
         the request sees in an AttnBlock, or a ``region`` that is not a bool [1, H, W] tensor on the CPU or the model's device
-        or comes without init_x.  ``attn_weights`` weights the request's conditional forward as in sample_notebook;
-        ``keep_intermediates`` collects sample_notebook's second value in ``req.intermediates``; ``region`` inpaints or
-        outpaints init_x as in sample_distributed.  The request's draws start when it is admitted."""
+        or comes without init_x, a ``mode`` other than 'multinomial', 'argmax' or 'quant', a ``sampling_quant_steps`` that is not
+        None or an int >= 0, or a request that would use 'quant' on an engine without vqmodel.  ``attn_weights`` weights the
+        request's conditional forward as in sample_notebook; ``keep_intermediates`` collects sample_notebook's second value in
+        ``req.intermediates``; ``region`` inpaints or outpaints init_x as in sample_distributed; ``mode`` and
+        ``sampling_quant_steps`` choose each step's sampling mode as in sample_notebook (step k uses 'quant' if
+        k >= sampling_quant_steps, ``mode`` otherwise; 'quant' reads the codebook of the engine's vqmodel).  The request's draws
+        start when it is admitted."""
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
         g_idx = generator.device.index if generator.device.index is not None else torch.cuda.current_device()
@@ -186,13 +205,18 @@ class SamplingEngine:
         U.check_region(region, init_x, (1, self.H, self.W), self.dev)
         if decode and self.vqmodel is None:
             raise ValueError("decode=True needs the engine's vqmodel")
+        mode = ops.check_mode("mode", mode)
+        sampling_quant_steps = ops.check_quant_steps("sampling_quant_steps", sampling_quant_steps)
+        if self.vqmodel is None and any(ops.mode_at(mode, sampling_quant_steps, k) == "quant" for k in range(steps)):
+            raise ValueError("mode 'quant' (or sampling_quant_steps) needs the VQGAN codebook: build the engine with vqmodel=...")
         if attn_weights is not None:
             n_keys = self.model.max_attn_weights((self.H, self.W), self.model.conditioning_seq_len(model_inputs))
             attn_weights = ops.check_attn_weight_vector("attn_weights", attn_weights, min(n_keys, self.w_max))
         cfgs = U._cfg_schedule(cfg, 1, steps)
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
-                      unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region)
+                      unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
+                      sampling_quant_steps)
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
@@ -256,11 +280,13 @@ class SamplingEngine:
             Bc, n_pairs = len(plan.order), plan.n_pairs
             hw = H * W
             draw, renoise = [], []
-            for q, rn in zip(plan.order, plan.renoise):          # per request: the sampler's draw, then the mask draw
-                draw += ops.philox_values([q.generator], hw * m.num_labels, dev)
+            for q, dr, rn in zip(plan.order, plan.draws, plan.renoise):     # per request: the sampler's draw, then the mask draw
+                draw += ops.philox_values([q.generator], hw * m.num_labels, dev) if dr else [0, 0]
                 renoise += ops.philox_values([q.generator], hw, dev) if rn else [0, 0]
+            mixed = not all(plan.draws)
+            modes = ops.mode_table(plan.modes) if mixed else torch.zeros(0, dtype=torch.int32)
             f32 = torch.cat([plan.r, plan.params.view(-1), plan.t_next] + ([torch.zeros(1)] if Bc % 2 else []))
-            i32 = torch.cat([plan.row_slot, plan.kv_slot] + ([torch.zeros(1, dtype=torch.int32)] if n_pairs % 2 else []))
+            i32 = torch.cat([plan.row_slot, plan.kv_slot, modes] + ([torch.zeros(1, dtype=torch.int32)] if (n_pairs + modes.numel()) % 2 else []))
             host = torch.cat([torch.tensor(draw + renoise, dtype=torch.int64), f32.view(torch.int64), i32.view(torch.int64)])
             buf = ops.to_device_async(host, dev)                 # the step's one host-to-device copy
             draw_d, renoise_d = buf[:2 * Bc].view(Bc, 2), buf[2 * Bc:4 * Bc].view(Bc, 2)
@@ -268,6 +294,7 @@ class SamplingEngine:
             i32_d = buf[4 * Bc + f32.numel() // 2:].view(torch.int32)
             r_d, params_d, t_next_d = f32_d[:Bc], f32_d[Bc:4 * Bc].view(Bc, 3), f32_d[4 * Bc:5 * Bc]
             row_slot_d, kv_slot_d = i32_d[:Bc], i32_d[Bc:2 * Bc + n_pairs]
+            modes_d = i32_d[2 * Bc + n_pairs:2 * Bc + n_pairs + modes.numel()]
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_pairs, self.s_max, self.n_slots, kv_slot_d)
@@ -275,7 +302,11 @@ class SamplingEngine:
                 feats = m.features(x, r_d, cond, self.w_pool, Bc, n_pairs=n_pairs, w_len=self.w_len, w_row=row_slot_d)
             else:
                 feats = m.features(x, r_d, cond, n_pairs=n_pairs)
-            sampled = m.sample_tokens_pairs(feats, Bc, n_pairs, H, W, params_d, draw_d, out=self._sampled[:Bc])
+            if mixed:       # argmax and quant rows through the logits path, the multinomial rows in one fused-sampler launch
+                sampled = m.sample_tokens_modes(feats, Bc, n_pairs, H, W, params_d, draw_d, plan.modes, modes_d, self._codebook(),
+                                                out=self._sampled[:Bc])
+            else:
+                sampled = m.sample_tokens_pairs(feats, Bc, n_pairs, H, W, params_d, draw_d, out=self._sampled[:Bc])
             for i, q in enumerate(plan.order):
                 if q.intermediates is not None:
                     s = q.slot
@@ -307,6 +338,9 @@ class SamplingEngine:
             self._free.sort()
             self._active = [q for q in self._active if q.k < q.steps]
             return done
+
+    def _codebook(self) -> Optional[torch.Tensor]:
+        return self.vqmodel.vquantizer.codebook.weight.data if self.vqmodel is not None else None
 
     def run_until_idle(self) -> List[Request]:
         """Step until nothing is active or queued; returns every request finished on the way, in finishing order."""

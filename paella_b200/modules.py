@@ -760,6 +760,54 @@ class Paella(nn.Module):
                   "pb200_paella_sample_tokens_pairs")
         return out
 
+    def resample_workspace_bytes(self, hw: int, chunk: int = ops.RESAMPLE_CHUNK) -> int:
+        """Scratch of sample_tokens_modes' argmax and quant samples: fp16 features and fp32 logits of 2 * chunk samples."""
+        self._ensure_packed()
+        return int(lib().pb200_paella_resample_workspace_bytes(self._handle, chunk, hw))
+
+    def sample_tokens_modes(self, feats: torch.Tensor, batch: int, n_pairs: int, h: int, w: int, params: torch.Tensor,
+                            seed_offset: torch.Tensor, modes: Sequence[str], table: torch.Tensor, codebook: Optional[torch.Tensor] = None,
+                            out: Optional[torch.Tensor] = None, chunk: int = ops.RESAMPLE_CHUNK) -> torch.Tensor:
+        """sample_tokens_pairs with a sampling mode per sample (``modes``: batch names of ops.SAMPLING_MODES; ``table``: their
+        ops.mode_table on the device).  The multinomial samples draw in one fused-sampler launch, the others skipped through the
+        table's codes (their ``seed_offset`` rows are not read); then each other mode present runs pb200_paella_resample_samples
+        over its samples: the out_mapper GEMM to logits, ``chunk`` guided samples at a time, and the argmax or quant kernel,
+        which draw nothing.  Sample b's tokens are those of sample_notebook's step in mode b.  ``codebook``: the VQGAN codebook
+        fp32 [num_labels, c_latent], for 'quant'."""
+        self._ensure_packed()
+        L = lib()
+        dev = self._device()
+        hw = h * w
+        count = {md: sum(1 for x in modes if x == md) for md in ops.SAMPLING_MODES}
+        if len(modes) != batch or sum(count.values()) != batch:
+            raise PaellaB200Error(f"sample_tokens_modes: {len(modes)} modes for {batch} samples (each one of {ops.SAMPLING_MODES})")
+        if count["quant"] and (codebook is None or codebook.shape[0] != self.num_labels):
+            raise PaellaB200Error("sample_tokens_modes: 'quant' needs the VQGAN codebook [num_labels, c_latent]")
+        with torch.cuda.device(dev):
+            if out is None:
+                out = torch.empty(batch, h, w, dtype=torch.int64, device=dev)
+            ws = self._ws(max(L.pb200_paella_workspace_bytes(self._handle, batch, h, w, 1),
+                              L.pb200_paella_resample_workspace_bytes(self._handle, chunk, hw) if count["multinomial"] < batch else 0))
+            if count["multinomial"]:
+                skip = table[:batch] if count["multinomial"] < batch else None
+                check(L.pb200_paella_sample_tokens_pairs_skip(self._handle, ptr(feats), batch, n_pairs, hw, ptr(params), ptr(seed_offset),
+                                                              ptr(skip), ptr(out), ptr(ws), ws.numel(), current_stream()),
+                      "pb200_paella_sample_tokens_pairs_skip")
+            off, lists = batch, []
+            for code, md in ((1, "argmax"), (2, "quant")):
+                lists.append((code, [b for b, x in enumerate(modes) if x == md], off))
+                off += count[md]
+            cb = codebook.contiguous().float() if count["quant"] else None
+            for code, samples, o in lists:
+                if not samples:
+                    continue
+                n_guided = sum(1 for b in samples if b < n_pairs)       # ascending: the guided samples come first
+                check(L.pb200_paella_resample_samples(self._handle, ptr(feats), batch, n_pairs, hw, ptr(table[o:o + len(samples)]),
+                                                      len(samples), n_guided, ptr(params), code, ptr(cb) if code == 2 else None,
+                                                      cb.shape[1] if code == 2 else 0, chunk, ptr(out), ptr(ws), ws.numel(),
+                                                      current_stream()), "pb200_paella_resample_samples")
+        return out
+
     def conditioning_seq_len(self, inputs: Dict[str, torch.Tensor]) -> int:
         """Length of the conditioning sequence of ``inputs`` (byt5 rows + clip_seq_len per clip / clip_image embedding)."""
         n = (1 if inputs.get("clip") is not None else 0)

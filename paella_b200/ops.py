@@ -221,6 +221,42 @@ def sampling_params_table(cfg, temperature, batch: int, device) -> torch.Tensor:
     return to_device_async(sampling_params(cfgs, temps), device)
 
 
+# ------------------------------------------------------------------ per-sample sampling modes
+# The notebook's sampling modes (paella_inference.ipynb cell 3).  'multinomial' draws H*W*num_labels exponentials per step; 'argmax'
+# and 'quant' draw nothing.  A step with several modes sends one int32 table to the device: the mode code of every sample, then
+# the samples in argmax mode, then the samples in quant mode, each list ascending.
+SAMPLING_MODES = ("multinomial", "argmax", "quant")
+RESAMPLE_CHUNK = 8      # guided samples per out_mapper GEMM of pb200_paella_resample_samples (bounds its logits scratch)
+
+
+def check_mode(name: str, mode) -> str:
+    if not isinstance(mode, str) or mode not in SAMPLING_MODES:
+        raise ValueError(f"{name}={mode!r}: expected one of {', '.join(SAMPLING_MODES)}")
+    return mode
+
+
+def check_quant_steps(name: str, value) -> Optional[int]:
+    """``sampling_quant_steps``: None, or a non-negative int (steps i >= value use 'quant')."""
+    if value is None:
+        return None
+    if isinstance(value, bool) or not isinstance(value, int) or value < 0:
+        raise ValueError(f"{name}={value!r}: expected None or an int >= 0")
+    return value
+
+
+def mode_at(mode: str, quant_steps: Optional[int], step: int) -> str:
+    """The mode of step ``step`` (0-based) of a sample: 'quant' from step ``quant_steps`` on, its own mode before."""
+    return "quant" if quant_steps is not None and step >= quant_steps else mode
+
+
+def mode_table(modes) -> torch.Tensor:
+    """CPU int32 table of one step's per-sample modes (see above): [B] codes (SAMPLING_MODES index), then the argmax samples,
+    then the quant samples."""
+    codes = [SAMPLING_MODES.index(md) for md in modes]
+    lists = [b for c in (1, 2) for b, cb in enumerate(codes) if cb == c]
+    return torch.tensor(codes + lists, dtype=torch.int32)
+
+
 # ------------------------------------------------------------------ random ops
 def randint(num_labels: int, size, device, generator=None) -> torch.Tensor:
     """torch.randint(0, num_labels, size, device=device)  [ref/src/utils.py:37]"""

@@ -3,7 +3,8 @@
   sample()               ref/src/utils.py:35-55
   sample_distributed()   ref/src_distributed/utils.py:97-126   (init_x, per-step cfg, sampling_conditional_steps)
   sample_notebook()      paella_inference.ipynb cell 3          (mode, attn_weights, returns intermediates; attn_weights
-                                                                 may also be one vector per sample)
+                                                                 may also be one vector per sample, mode and
+                                                                 sampling_quant_steps one entry per sample)
 
 Per step the reference runs two forwards, materialises 2 x [B,8192,H,W] fp32 logits and makes ~20 passes
 over them.  Here: conditional and unconditional rows run as ONE batch of 2B through the denoiser (their
@@ -133,12 +134,15 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
-                 codebook=None, generator=None, per_sample_cfg=False, region=None):
+                 codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None):
+    """``modes``: None, or per step the list of B mode names (sampling_modes) -- a step whose modes differ samples each row in
+    its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the scalar path in that mode."""
     B, H, W = latent_shape
     dev = model._device()
     check_region(region, init_x, latent_shape, dev)
     use_cfg_any = cfgs is not None
-    sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg)
+    mixed_steps = modes is not None and any(len(set(ms)) > 1 for ms in modes)
+    sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg, always=mixed_steps)
     w_table = None
     if isinstance(attn_weights, (list, tuple)):       # per-sample vectors, for the conditional rows only
         w_table = ops.attn_weights_table(attn_weights, B, [model.max_attn_weights((H, W), model.conditioning_seq_len(model_inputs))] * B)
@@ -173,7 +177,11 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         cond_only = None
         intermediates = []
         for i in range(steps):
-            if sampling_quant_steps is not None and i >= sampling_quant_steps:
+            step_modes = None
+            if modes is not None:
+                step_modes = modes[i] if len(set(modes[i])) > 1 else None
+                mode = modes[i][0]
+            elif sampling_quant_steps is not None and i >= sampling_quant_steps:
                 mode = "quant"
             guided = use_cfg_any and i < sampling_conditional_steps
             if guided:
@@ -190,7 +198,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             else:
                 r, params_i = r_d[i], params_d[i]
             feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided, w_len=w_len)
-            if mode == "multinomial" and not exact:
+            if step_modes is not None:
+                sampled = _sample_modes_step(model, feats, B, H, W, guided, params_i, step_modes, generator, codebook, dev)
+            elif mode == "multinomial" and not exact:
                 if sched is None:
                     sampled = model.sample_tokens(feats, B, H, W, cfg_i, temp_i, generator)
                 else:
@@ -228,6 +238,47 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 if collect:
                     intermediates.append(sampled)
     return sampled, intermediates
+
+
+def _sample_modes_step(model, feats, B, H, W, guided, params, step_modes, generators, codebook, dev):
+    """One step of a batch whose samples are in different modes, on per-sample generators: the multinomial samples draw what
+    a batch-1 step draws on their own generators, the others draw nothing.  The draws and the mode table go to the device in
+    one asynchronous copy."""
+    vals = []
+    for g, md in zip(generators, step_modes):
+        vals += ops.philox_values([g], H * W * model.num_labels, dev) if md == "multinomial" else [0, 0]
+    seed_d, table_d = ops.to_device_packed([torch.tensor(vals, dtype=torch.int64).view(-1, 2), ops.mode_table(step_modes)], dev)
+    return model.sample_tokens_modes(feats, B, B if guided else 0, H, W, params, seed_d, step_modes, table_d, codebook)
+
+
+def sampling_modes(mode, sampling_quant_steps, batch: int, steps: int, generator=None, exact: bool = False, codebook=None):
+    """sample_notebook's ``mode`` and ``sampling_quant_steps`` -> None when both are scalar or a list's entries are all equal
+    (the scalar path), otherwise per step the list of ``batch`` mode names (ops.mode_at).  ValueError, before anything is
+    enqueued, for a list of the wrong length, an unknown mode, a quant step that is not None or an int >= 0, 'quant' at some
+    step without a codebook, and -- for a step whose modes differ -- a call without per-sample generators or with exact=True."""
+    if not isinstance(mode, (list, tuple)) and not isinstance(sampling_quant_steps, (list, tuple)):
+        return None
+    per = []
+    for name, v in (("mode", mode), ("sampling_quant_steps", sampling_quant_steps)):
+        if isinstance(v, (list, tuple)):
+            if len(v) != batch:
+                raise ValueError(f"{name}: got {len(v)} entries for a batch of {batch} (one per sample)")
+            per.append(list(v))
+        else:
+            per.append([v] * batch)
+    ms = [ops.check_mode(f"mode[{b}]", v) for b, v in enumerate(per[0])]
+    qs = [ops.check_quant_steps(f"sampling_quant_steps[{b}]", v) for b, v in enumerate(per[1])]
+    table = [[ops.mode_at(md, q, i) for md, q in zip(ms, qs)] for i in range(steps)]
+    if codebook is None and any("quant" in row for row in table):
+        raise ValueError("mode='quant' needs the VQGAN codebook: pass vqmodel=... (the notebook uses its global `vqmodel`)")
+    if len(set(ms)) == 1 and len(set(qs)) == 1:
+        return None
+    if any(len(set(row)) > 1 for row in table):
+        if not ops.per_sample(generator):
+            raise ValueError("samples in different sampling modes draw per sample: pass generator=[g_0, ..., g_{B-1}]")
+        if exact:
+            raise ValueError("exact=True is the multinomial parity path; it does not take per-sample modes")
+    return table
 
 
 def load_conditional_models(byt5_model_name, vqgan_path, device):
@@ -320,7 +371,11 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     unconditional rows are never weighted, as in the notebook).  Row i then equals row i of the call with vector i for every
     sample.  ValueError, before anything is enqueued and before any generator advances, for the wrong number of entries, a
     CUDA, non-1-D or non-finite tensor, or a vector longer than the smallest key count the sample sees in an AttnBlock.
-    ``region`` as in ``sample_distributed``; every intermediate holds init_x's tokens outside it."""
+    ``region`` as in ``sample_distributed``; every intermediate holds init_x's tokens outside it.
+    Per-sample modes: ``mode`` may be a list or tuple of B mode names and ``sampling_quant_steps`` one of B entries, each None
+    or an int >= 0; row i then equals row i of the call with mode i and quant step i for every sample, on per-sample
+    generators.  A call whose modes differ within a step needs ``generator=[g_0, ..., g_{B-1}]`` (the argmax and quant rows draw
+    nothing, the multinomial ones draw per sample); one whose entries are all equal is the scalar call (sampling_modes)."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -329,6 +384,11 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
         unconditional_inputs = _zeros_like_inputs(model_inputs)
     cfgs = _cfg_schedule(cfg, latent_shape[0], steps)
     codebook = vqmodel.vquantizer.codebook.weight.data if vqmodel is not None else None
+    modes = sampling_modes(mode, sampling_quant_steps, latent_shape[0], steps, generator, exact, codebook)
+    if modes is None and isinstance(mode, (list, tuple)):
+        mode = mode[0]
+    if modes is None and isinstance(sampling_quant_steps, (list, tuple)):
+        sampling_quant_steps = sampling_quant_steps[0]
     return _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                         temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, True,
-                        sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region)
+                        sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes)
