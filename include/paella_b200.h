@@ -235,6 +235,18 @@ int pb200_film_apply(float* x, int64_t rows, int n, int rows_per_sample, const f
 int pb200_attention(const void* qkv16, const void* ckv16, const int* kv_len, void* out16, int batch, int positions, int s_max,
                     int embed, int nhead, int self_attn, const float* attn_weights, int n_weights, int weighted_batch,
                     void* stream);
+/* pb200_attention with shared conditioning slots and a per-sample weight table (pb200_attention is this call with
+ * kv_slot = NULL, n_slots = 0, weights_ld = 0, weights_len = weights_row = NULL):
+ *   kv_slot      int32 [batch]: the block of s_max rows of ckv16 (and the entry of kv_len) sample b reads, or NULL: block b;
+ *   n_slots      blocks in ckv16 and entries in kv_len (0: batch);
+ *   attn_weights fp32 table of rows weights_ld floats apart; sample b < weighted_batch reads row weights_row[b] (NULL: row b),
+ *                whose first weights_len[row] entries (NULL: n_weights) scale the last weights_len[row] keys of its own
+ *                [self ; cond] list; a length of 0 leaves the sample unweighted.  weights_ld = 0 with weights_len = NULL is
+ *                one vector of n_weights entries shared by every sample. */
+int pb200_attention_slots(const void* qkv16, const void* ckv16, const int* kv_len, const int* kv_slot, int n_slots, void* out16,
+                          int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
+                          int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
+                          void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Denoiser (ref/src/modules.py:109-283, ref/utils/modules.py) as an opaque handle.

@@ -91,6 +91,8 @@ SIGNATURES = {
     "pb200_film_apply": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_int64, c_int64, c_void_p]),
     "pb200_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                 c_int, c_int, c_void_p]),
+    "pb200_attention_slots": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                      c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "pb200_paella_create": (c_int, [POINTER(PaellaConfig), POINTER(c_void_p)]),
     "pb200_paella_destroy": (None, [c_void_p]),
     "pb200_paella_weight_bytes": (c_int64, [c_void_p]),

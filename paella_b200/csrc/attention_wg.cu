@@ -103,7 +103,9 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
         const uint32_t sb = base + AW_OFF_STAGE + st * AW_STAGE;
         ptx::mbar_wait(full_bar(st), (c >> 1) & 1);
         // V [key][dim] -> Vt [dim][key] with the 128-byte swizzle: the 80 8x8 blocks (8 key blocks x 10 dim blocks) through
-        // ldmatrix.trans, 20 per warp; thread t receives dim 8 db + t/4, keys 8 kb + 2 (t%4) + {0, 1} = one 4-byte store
+        // ldmatrix.trans, 20 per warp; thread t receives dim 8 db + t/4, keys 8 kb + 2 (t%4) + {0, 1} = one 4-byte store.
+        // Keys at or past `valid` are written as zeros: the 64-row box runs into the next sample's rows, or the slot's rows
+        // past kv_len and the next slot, and their P of 0 would still turn an Inf or NaN there into NaN in O += P V.
         {
             const uint32_t vraw = sb + AW_K64 + AW_K16;
             uint8_t* vt = gbase + AW_OFF_VT;
@@ -117,8 +119,9 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
                     const int m = wq * 20 + j * 4 + q, kb = m & 7, d = (m >> 3) * 8 + (lane >> 2);
-                    const int byte = 2 * (kb * 8 + 2 * (lane & 3));
-                    *reinterpret_cast<uint32_t*>(vt + d * 128 + (((byte >> 4) ^ (d & 7)) << 4) + (byte & 15)) = r[q];
+                    const int key = kb * 8 + 2 * (lane & 3), byte = 2 * key;
+                    const uint32_t v2 = key + 1 < valid ? r[q] : key < valid ? r[q] & 0xffffu : 0u;
+                    *reinterpret_cast<uint32_t*>(vt + d * 128 + (((byte >> 4) ^ (d & 7)) << 4) + (byte & 15)) = v2;
                 }
             }
         }

@@ -142,18 +142,29 @@ int pb200_film_apply(float* x, int64_t rows, int n, int rows_per_sample, const f
 int pb200_attention(const void* qkv16, const void* ckv16, const int* kv_len, void* out16, int batch, int positions, int s_max,
                     int embed, int nhead, int self_attn, const float* attn_weights, int n_weights, int weighted_batch,
                     void* stream) {
+    return pb200_attention_slots(qkv16, ckv16, kv_len, nullptr, 0, out16, batch, positions, s_max, embed, nhead, self_attn,
+                                 attn_weights, n_weights, 0, nullptr, nullptr, weighted_batch, stream);
+}
+
+int pb200_attention_slots(const void* qkv16, const void* ckv16, const int* kv_len, const int* kv_slot, int n_slots, void* out16,
+                          int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
+                          int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
+                          void* stream) {
     PB_CHECK(qkv16 && out16 && (ckv16 || s_max == 0), "attention: null pointer");
     PB_CHECK(self_attn || s_max > 0, "attention: no keys");
+    PB_CHECK(n_slots >= 0 && weights_ld >= 0, "attention: negative slot count or weight stride");
     AttnParams p{};
     p.qkv = reinterpret_cast<const __half*>(qkv16);
     p.ckv = reinterpret_cast<const __half*>(ckv16 ? ckv16 : qkv16);
     p.kv_len = kv_len;
-    p.kv_slot = nullptr;
+    p.kv_slot = kv_slot;
+    p.n_slots = n_slots;
     p.out = reinterpret_cast<__half*>(out16);
     p.B = batch; p.P = positions; p.S_max = s_max; p.E = embed; p.nhead = nhead;
     p.self_attn = self_attn;
     p.scale_log2 = 1.4426950408889634f / sqrtf((float)(embed / (nhead > 0 ? nhead : 1)));
     p.attn_w = attn_weights; p.n_w = attn_weights ? n_weights : 0; p.w_batch = weighted_batch;
+    p.w_ld = weights_ld; p.w_len = weights_len; p.w_row = weights_row;
     return launch_attention(p, (cudaStream_t)stream);
 }
 

@@ -23,11 +23,10 @@ M, N, K, P = 2048, 1280, 640, 16          # the a_scale path
 a = torch.randn(M, K, device=DEV, generator=g).half(); w = (torch.randn(N, K, device=DEV, generator=g) / math.sqrt(K)).half()
 x = torch.randn(M, N, device=DEV, generator=g); s = (1 + 0.3 * torch.randn(M // P, K, device=DEV, generator=g)).half()
 ops.gemm_f16(a, w, _lib.EPI_RESID_F32, x, bias=None, resid=x, rows_per_sample=P, a_scale=s)
-# attention: wgmma kernel (head_dim 80) and mma.sync kernel
-import test_gpu_attention as ta
-print("attn wgmma", ta._run(2, 64, 20, 2, 80, True, True, False)[:2])
-print("attn wgmma P=16", ta._run(2, 16, 12, 2, 80, True, False, True)[:2])
-print("attn mma", ta._run(2, 16, 12, 2, 32, True, True, False)[:2])
+# attention: wgmma kernel (head_dim 80: shared slots, the last slot read; a weight table) and mma.sync kernel
+import test_gpu_attention_matrix as ta
+for kernel, cid in (("wgmma", "slots-above-B-hd80"), ("wgmma", "table-w_row-shared-hd80"), ("mma", "hd32-P16-S20-varlen-vec5-hd32")):
+    print("attn", kernel, cid, ta._run(ta._make(next(c for c in ta._cases(kernel) if c["id"] == cid))).shape)
 # codec ResBlock front (row statistics + patch kernel), partial patches
 from paella_b200.vqgan import ResBlock
 blk = ResBlock(192, 768).to(DEV).eval()
