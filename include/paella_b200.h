@@ -151,8 +151,11 @@ enum pb200_epilogue {
                                  * s = ln_shift[row] (0 if NULL).  LayerNorm is invariant under a per-row shift, so any s
                                  * is exact; an s near the row mean keeps the fp16 rounding of the copy relative to the row's
                                  * SPREAD instead of its offset (the executor passes the mean the previous AttnBlock saw). */
-    PB200_EPI_F16_LN = 7       /* out fp16 = rstd[row]*(acc - mean'[row]*ln_wsum[n]) + bias, (mean', rstd) of the shifted
+    PB200_EPI_F16_LN = 7,      /* out fp16 = rstd[row]*(acc - mean'[row]*ln_wsum[n]) + bias, (mean', rstd) of the shifted
                                  * rows from ln_stat; if ln_mean_out: ln_mean_out[row] = ln_shift[row] + mean' (true mean) */
+    PB200_EPI_RESID_LN_INV_F32 = 8 /* RESID_LN_F32 with batch-invariant statistics: each 32-column chunk's row sums are
+                                 * rounded to the ln_stat fixed point on their own and added as integers, so ln_stat does
+                                 * not depend on the tile width (which the planner picks from M) or the CTA order */
 };
 
 typedef struct pb200_gemm_epilogue {
@@ -278,6 +281,11 @@ const char* pb200_paella_param_name(const pb200_paella* m, int i);
 int64_t pb200_paella_param_numel(const pb200_paella* m, int i);
 /* convert one reference-layout fp32 parameter (device pointer) into the packed blob. */
 int pb200_paella_load_param(pb200_paella* m, const char* name, const float* src, int64_t numel, void* stream);
+/* Handle option (default 0).  on = 1: batch-invariant forward -- every sample's features are bit-identical whatever batch,
+ * batch position, CFG pairing or GPU count it runs in (the folded LayerNorm's row statistics use
+ * PB200_EPI_RESID_LN_INV_F32).  on = 0: the default arithmetic.  Set it before forwards are enqueued, not concurrently
+ * with them: forwards already enqueued keep the mode they were enqueued with. */
+int pb200_paella_set_batch_invariant(pb200_paella* m, int on);
 
 /* conditioning for `batch` samples: byt5 fp32 [B, L, byt5_embd]; clip / clip_image fp32
  * [B, clip_embd] or NULL; n_clip_image images (list-valued clip_image, ref/utils/modules.py:228-235,

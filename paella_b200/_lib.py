@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libpaella_b200.so")
 
 PB200_MAX_LEVELS = 4
 
-EPI_F16, EPI_F32, EPI_GELU_F16, EPI_RESID_F32, EPI_UNPATCH_F32, EPI_NCHW_F32, EPI_RESID_LN_F32, EPI_F16_LN = range(8)
+EPI_F16, EPI_F32, EPI_GELU_F16, EPI_RESID_F32, EPI_UNPATCH_F32, EPI_NCHW_F32, EPI_RESID_LN_F32, EPI_F16_LN, EPI_RESID_LN_INV_F32 = range(9)
 
 
 class GemmEpilogue(ctypes.Structure):
@@ -101,6 +101,7 @@ SIGNATURES = {
     "pb200_paella_param_name": (c_char_p, [c_void_p, c_int]),
     "pb200_paella_param_numel": (c_int64, [c_void_p, c_int]),
     "pb200_paella_load_param": (c_int, [c_void_p, c_char_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_set_batch_invariant": (c_int, [c_void_p, c_int]),
     "pb200_paella_workspace_bytes": (c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
     "pb200_paella_cond_cache_bytes": (c_int64, [c_void_p, c_int, c_int]),
     "pb200_paella_prepare_cond": (c_int, [c_void_p, POINTER(Cond), c_int, c_int, c_int, c_int, c_void_p, c_void_p,

@@ -149,6 +149,17 @@ struct EpiPre<PB200_EPI_RESID_LN_F32> {
     float ln_s = 0.f, ln_q = 0.f;      // this lane's row: sum / sum of squares over the chunks of the tile done so far
     float shift = 0.f;                 // this lane's row: the shift subtracted before the fp16 copy and the statistics
 };
+// batch-invariant variant: each 32-column chunk's sums are rounded to the ln_stat fixed point on their own and added as
+// integers, so a row's statistic does not depend on how many chunks share a tile (BLOCK_N, which the planner picks from M)
+template <>
+struct EpiPre<PB200_EPI_RESID_LN_INV_F32> {
+    float4 r[8];
+    float shift = 0.f;
+};
+template <int MODE>
+constexpr bool is_resid_ln = MODE == PB200_EPI_RESID_LN_F32 || MODE == PB200_EPI_RESID_LN_INV_F32;
+template <int MODE>
+constexpr bool is_resid = MODE == PB200_EPI_RESID_F32 || is_resid_ln<MODE>;
 
 // Coalescing.  The epilogue hands every lane one ROW of the chunk (32 consecutive columns), so a direct 16-byte store
 // per lane touches 32 different 128-byte lines per instruction and the LSU serialises them.  The chunk is therefore transposed inside the
@@ -206,10 +217,10 @@ __device__ __forceinline__ void epilogue_preload(const pb200_gemm_epilogue& ep, 
             if (ep.ln_mean_out) ep.ln_mean_out[row] = (ep.ln_shift ? ep.ln_shift[row] : 0.f) + mean;
         }
     }
-    if constexpr (MODE == PB200_EPI_RESID_LN_F32) {
+    if constexpr (is_resid_ln<MODE>) {
         if (first_chunk) pre.shift = (ep.ln_shift && row < M) ? ep.ln_shift[row] : 0.f;
     }
-    if constexpr (MODE == PB200_EPI_RESID_F32 || MODE == PB200_EPI_RESID_LN_F32) {
+    if constexpr (is_resid<MODE>) {
         const int col = col0 + (lane & 7) * 4;       // transposed layout: item i = row of lane (lane & 24) + i
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -351,13 +362,13 @@ __device__ __forceinline__ void epilogue_chunk(const pb200_gemm_epilogue& ep, in
                     if (col0 + j < N) atomicAdd(sq + (int64_t)(row / P) * N + col0 + j, fx(v[j]));
             }
         }
-    } else if (MODE == PB200_EPI_RESID_F32 || MODE == PB200_EPI_RESID_LN_F32) {
+    } else if (is_resid<MODE>) {
         // (bias was added above in the row-per-lane layout); the rest runs in the transposed, coalesced layout
         transpose8x8_f4(v, lane);
         const int col = col0 + (lane & 7) * 4;
         float* obase = reinterpret_cast<float*>(ep.out);
         float ls[8], lq[8], sh[8];
-        if constexpr (MODE == PB200_EPI_RESID_LN_F32) {
+        if constexpr (is_resid_ln<MODE>) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 ls[i] = lq[i] = 0.f;
@@ -369,7 +380,7 @@ __device__ __forceinline__ void epilogue_chunk(const pb200_gemm_epilogue& ep, in
             const int r = __shfl_sync(0xffffffffu, row, (lane & 24) + i);
             if (r < M && col < N) {
                 float4 rr = make_float4(0.f, 0.f, 0.f, 0.f);
-                if constexpr (MODE == PB200_EPI_RESID_F32 || MODE == PB200_EPI_RESID_LN_F32) rr = pre.r[i];
+                if constexpr (is_resid<MODE>) rr = pre.r[i];
                 float4 y;
                 y.x = fmaf(v[i * 4 + 0], ep.alpha, rr.x); y.y = fmaf(v[i * 4 + 1], ep.alpha, rr.y);
                 y.z = fmaf(v[i * 4 + 2], ep.alpha, rr.z); y.w = fmaf(v[i * 4 + 3], ep.alpha, rr.w);
@@ -381,7 +392,7 @@ __device__ __forceinline__ void epilogue_chunk(const pb200_gemm_epilogue& ep, in
                     y.z = fmaf(y.z, 1.0f + a.z, b.z); y.w = fmaf(y.w, 1.0f + a.w, b.w);
                 }
                 *reinterpret_cast<float4*>(obase + (int64_t)r * ep.ldo + col) = y;
-                if constexpr (MODE == PB200_EPI_RESID_LN_F32) {
+                if constexpr (is_resid_ln<MODE>) {
                     y.x -= sh[i]; y.y -= sh[i]; y.z -= sh[i]; y.w -= sh[i];      // (after the fp32 store of the true value)
                     uint2 pk;
                     pk.x = pack_half2(y.x, y.y);
@@ -392,7 +403,7 @@ __device__ __forceinline__ void epilogue_chunk(const pb200_gemm_epilogue& ep, in
                 }
             }
         }
-        if constexpr (MODE == PB200_EPI_RESID_LN_F32) {
+        if constexpr (is_resid_ln<MODE>) {
             // row statistics of the finished rows: item i of lane (a,b) is row 8a+i, columns 4b..4b+3 -> transpose-reduce
             // over the 8 lanes of the group; lane 8a+b ends with the sums of row 8a+b, i.e. of its own `row`
 #pragma unroll
@@ -406,8 +417,18 @@ __device__ __forceinline__ void epilogue_chunk(const pb200_gemm_epilogue& ep, in
                     lq[i] = q_keep + __shfl_xor_sync(0xffffffffu, q_send, o);
                 }
             }
-            pre.ln_s += ls[0];          // flushed once per tile by epilogue_finish (one atomic pair per row and warp)
-            pre.ln_q += lq[0];
+            if constexpr (MODE == PB200_EPI_RESID_LN_INV_F32) {
+                // one atomic pair per row and chunk: two int64 accumulators held across a 256-wide tile's chunks made
+                // ptxas spill them
+                if (row < M) {
+                    unsigned long long* st = reinterpret_cast<unsigned long long*>(ep.ln_stat) + 2 * (int64_t)row;
+                    atomicAdd(st, (unsigned long long)__float2ll_rn(ls[0] * 1048576.0f));
+                    atomicAdd(st + 1, (unsigned long long)__float2ll_rn(lq[0] * 65536.0f));
+                }
+            } else {        // flushed once per tile by epilogue_finish (one atomic pair per row and warp)
+                pre.ln_s += ls[0];
+                pre.ln_q += lq[0];
+            }
         }
     } else if (MODE == PB200_EPI_UNPATCH_F32) {
         if (!row_ok) return;
@@ -732,6 +753,8 @@ static int launch_mode(const CUtensorMap& ta, const CUtensorMap& tb, const pb200
     if (ep.a_scale) {       // GlobalResponseNorm folded into the A operand: the two residual epilogues only
         if (ep.mode == PB200_EPI_RESID_F32) return launch_cfg<BLOCK_N, PB200_EPI_RESID_F32, 0, true>(ta, tb, ep, M, N, K, st);
         if (ep.mode == PB200_EPI_RESID_LN_F32) return launch_cfg<BLOCK_N, PB200_EPI_RESID_LN_F32, 0, true>(ta, tb, ep, M, N, K, st);
+        if (ep.mode == PB200_EPI_RESID_LN_INV_F32)
+            return launch_cfg<BLOCK_N, PB200_EPI_RESID_LN_INV_F32, 0, true>(ta, tb, ep, M, N, K, st);
         PB_CHECK(false, "gemm: a_scale is only built for the RESID epilogues (mode %d)", ep.mode);
     }
     switch (ep.mode) {
@@ -743,6 +766,7 @@ static int launch_mode(const CUtensorMap& ta, const CUtensorMap& tb, const pb200
         case PB200_EPI_NCHW_F32: return launch_cfg<BLOCK_N, PB200_EPI_NCHW_F32>(ta, tb, ep, M, N, K, st);
         case PB200_EPI_RESID_LN_F32: return launch_cfg<BLOCK_N, PB200_EPI_RESID_LN_F32>(ta, tb, ep, M, N, K, st);
         case PB200_EPI_F16_LN: return launch_cfg<BLOCK_N, PB200_EPI_F16_LN>(ta, tb, ep, M, N, K, st);
+        case PB200_EPI_RESID_LN_INV_F32: return launch_cfg<BLOCK_N, PB200_EPI_RESID_LN_INV_F32>(ta, tb, ep, M, N, K, st);
     }
     PB_CHECK(false, "gemm: unknown epilogue mode %d", ep.mode);
     return 1;
@@ -795,23 +819,23 @@ int gemm_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, const
     PB_CHECK(M > 0 && N > 0 && K > 0, "gemm: empty problem");
     PB_CHECK(N % 8 == 0, "gemm: N=%lld must be a multiple of 8", (long long)N);
     PB_CHECK(ep.out != nullptr, "gemm: null output");
-    if (ep.mode == PB200_EPI_RESID_F32 || ep.mode == PB200_EPI_RESID_LN_F32)
-        PB_CHECK(ep.resid != nullptr, "gemm: RESID epilogue without resid");
-    if (ep.mode == PB200_EPI_RESID_LN_F32) PB_CHECK(ep.out16 && ep.ln_stat, "gemm: RESID_LN needs out16 and ln_stat");
+    const bool resid_ln = ep.mode == PB200_EPI_RESID_LN_F32 || ep.mode == PB200_EPI_RESID_LN_INV_F32;
+    if (ep.mode == PB200_EPI_RESID_F32 || resid_ln) PB_CHECK(ep.resid != nullptr, "gemm: RESID epilogue without resid");
+    if (resid_ln) PB_CHECK(ep.out16 && ep.ln_stat, "gemm: RESID_LN needs out16 and ln_stat");
     if (ep.mode == PB200_EPI_F16_LN)
         PB_CHECK(ep.ln_stat && ep.ln_wsum && ep.ln_c > 0, "gemm: F16_LN needs ln_stat, ln_wsum and ln_c");
     if (ep.mode == PB200_EPI_UNPATCH_F32)
         PB_CHECK(ep.up_cout % 8 == 0 && ep.up_cout * 4 == N && (int64_t)ep.up_h * ep.up_w > 0,
                  "gemm: bad un-patchify geometry");
-    if ((ep.mode == PB200_EPI_GELU_F16 && ep.sqsum) || ((ep.mode == PB200_EPI_RESID_F32 || ep.mode == PB200_EPI_RESID_LN_F32) && ep.film) ||
+    if ((ep.mode == PB200_EPI_GELU_F16 && ep.sqsum) || ((ep.mode == PB200_EPI_RESID_F32 || resid_ln) && ep.film) ||
         ep.mode == PB200_EPI_NCHW_F32)
         PB_CHECK(ep.rows_per_sample > 0, "gemm: rows_per_sample required");
     if (ep.a_scale)
         PB_CHECK(gemm_can_scale_a(M, N, K, ep.rows_per_sample) && ep.a_scale_ld % 8 == 0 && ((uintptr_t)ep.a_scale & 15) == 0,
                  "gemm: a_scale needs rows_per_sample dividing or divided by 128, K %% 64 == 0");
-    static const char* kTags[8] = {"gemm_f16", "gemm_f32", "gemm_gelu_sqsum", "gemm_resid", "gemm_unpatch", "gemm_nchw",
-                                   "gemm_resid", "gemm_f16"};
-    ProfScope prof(ep.mode >= 0 && ep.mode < 8 ? kTags[ep.mode] : "gemm", 2.0 * (double)M * (double)N * (double)K, st);
+    static const char* kTags[9] = {"gemm_f16", "gemm_f32", "gemm_gelu_sqsum", "gemm_resid", "gemm_unpatch", "gemm_nchw",
+                                   "gemm_resid", "gemm_f16", "gemm_resid"};
+    ProfScope prof(ep.mode >= 0 && ep.mode < 9 ? kTags[ep.mode] : "gemm", 2.0 * (double)M * (double)N * (double)K, st);
     switch (block_n) {
         case 64: return launch_mode<64>(ta, tb, ep, (int)M, (int)N, (int)K, st);
         case 128: return launch_mode<128>(ta, tb, ep, (int)M, (int)N, (int)K, st);

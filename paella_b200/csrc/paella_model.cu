@@ -145,6 +145,7 @@ struct pb200_paella {
     int64_t emb_table = -1, emb_w = -1, emb_b = -1, byt5_w = -1, byt5_b = -1, clip_w = -1, clip_b = -1, clipimg_w = -1,
             clipimg_b = -1, clf_w = -1, clf_b = -1, out_w = -1, film_w = -1, film_b = -1;
     int film_total = 0, n_attn = 0, max_c = 0;
+    bool batch_invariant = false;      // pb200_paella_set_batch_invariant
     std::map<std::tuple<const void*, int64_t, int64_t, int64_t, int>, CUtensorMap> tmaps;
 
     int64_t add_param(const std::string& name, int64_t numel, int kind, int64_t dst_numel, int elem_bytes, int d0 = 0,
@@ -503,6 +504,13 @@ int pb200_paella_bind_weights(pb200_paella* m, void* blob) {
     return 0;
 }
 
+int pb200_paella_set_batch_invariant(pb200_paella* m, int on) {
+    PB_CHECK(m != nullptr, "set_batch_invariant: null model handle");
+    PB_CHECK(on == 0 || on == 1, "set_batch_invariant: on=%d (0 or 1)", on);
+    m->batch_invariant = on != 0;
+    return 0;
+}
+
 int pb200_paella_num_params(const pb200_paella* m) { return (int)m->params.size(); }
 const char* pb200_paella_param_name(const pb200_paella* m, int i) {
     return (i >= 0 && i < (int)m->params.size()) ? m->params[i].name.c_str() : "";
@@ -774,7 +782,8 @@ int pb200_paella_features_weighted(pb200_paella* m, const int64_t* tokens, const
                     PB_TRY(launch_grn_fused(ws.h16, Bc, P, 4 * ch, stat, stat_next, 4 * m->max_c, m->w<float>(b.gamma), m->w<float>(b.beta), ws.grn_mult, st));
                 // the next AttnBlock's LayerNorm is folded into its QKV GEMM when this block feeds it directly
                 const bool fold = b.ln_fold_attn >= 0;
-                pb200_gemm_epilogue e2 = epi(fold ? PB200_EPI_RESID_LN_F32 : PB200_EPI_RESID_F32, m->w<float>(fold_grn ? b.b2_fold : b.b2), x, ch);
+                const int ln_mode = m->batch_invariant ? PB200_EPI_RESID_LN_INV_F32 : PB200_EPI_RESID_LN_F32;
+                pb200_gemm_epilogue e2 = epi(fold ? ln_mode : PB200_EPI_RESID_F32, m->w<float>(fold_grn ? b.b2_fold : b.b2), x, ch);
                 if (fold_grn) { e2.a_scale = grn_s16; e2.a_scale_ld = 4 * (int64_t)ch; }
                 e2.resid = x; e2.ldr = ch; e2.rows_per_sample = P;
                 if (b.film_off >= 0) { e2.film = ws.film; e2.film_ld = m->film_total; e2.film_off = b.film_off; }

@@ -14,7 +14,8 @@ A request's tokens are those of ``sample_distributed(model, inputs, uncond, (1, 
 temperature, cfg, t_start, t_end, sampling_conditional_steps, generator=[g])``: the same draws from ``g`` in the same order
 (randint at admission, then per step the sampler's exponential draw and, if the step renoises, the mask draw), the same
 torch.linspace schedules and fp32 kernel constants (utils.sampling_schedule), and ``g`` left at the same offset.  Where the
-forward is batch-invariant (DESIGN.md §3) the tokens are equal bit for bit, whatever else is in flight.  With
+forward is batch-invariant (DESIGN.md §3: on the default model with ``model.batch_invariant = True``) the tokens are equal
+bit for bit, whatever else is in flight.  With
 ``attn_weights=w`` (and ``keep_intermediates=True``) the request's tokens, ``req.intermediates`` and generator offset are those
 of ``sample_notebook(model, inputs, (1, H, W), uncond, init_x, steps, renoise_steps, temperature, cfg, 'multinomial', t_start,
 t_end, sampling_conditional_steps, attn_weights=w, generator=[g])``; each step's batch reads every row's weights from a
@@ -35,12 +36,14 @@ one fused-sampler launch and one per-sample add-noise launch that writes every r
 in several sampling modes adds each row's mode to the table: the fused sampler skips the argmax and quant rows, which then go
 through the out_mapper GEMM to logits (a bounded number of samples at a time) and the argmax or quant kernel, one call per mode
 (Paella.sample_tokens_modes).  The host knows which
-requests finish at which step, so ``step()`` never synchronises.
+requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
+in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
+and own unconditional slots alike; the cache rows equal per-request projections bit for bit in either mode.
 """
 from __future__ import annotations
 
 import collections
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -97,6 +100,43 @@ class StepPlan:
         self.t_next = torch.stack([q.r[q.k + 1] if rn else torch.tensor(-1.0) for q, rn in zip(order, self.renoise)])
         self.row_slot = torch.tensor([q.slot for q in order], dtype=torch.int32)
         self.kv_slot = torch.tensor([q.slot for q in order] + [q.uncond_slot for q in order[:self.n_pairs]], dtype=torch.int32)
+
+
+def cond_layout(inputs: Dict[str, torch.Tensor]) -> Tuple[int, bool, int]:
+    """The sequence layout of one request's conditioning: (byt5 length, clip present, number of clip images).  Requests with
+    one layout have the same sequence length and the same mapper launches, so they can be projected as one batch."""
+    ci = inputs.get("clip_image")
+    n_img = 0 if ci is None else (len(ci) if isinstance(ci, (list, tuple)) else 1)
+    return int(inputs["byt5"].shape[1]), inputs.get("clip") is not None, n_img
+
+
+def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List[int]]:
+    """Group the conditioning writes of one admission -- (cache slot, layout) pairs with distinct slots -- into runs of
+    contiguous slots that share one layout, in ascending slot order.  Each run is a list of indices into ``writes`` and is
+    projected by one prepare_cond call at its first slot."""
+    runs: List[List[int]] = []
+    for i in sorted(range(len(writes)), key=lambda i: writes[i][0]):
+        if runs and writes[i][0] == writes[runs[-1][-1]][0] + 1 and writes[i][1] == writes[runs[-1][-1]][1]:
+            runs[-1].append(i)
+        else:
+            runs.append([i])
+    return runs
+
+
+def _cat_inputs(inputs: List[Dict[str, torch.Tensor]], dev) -> Dict[str, torch.Tensor]:
+    """Batch-1 conditioning dicts of one layout -> one batch, on ``dev``."""
+    if len(inputs) == 1:
+        return inputs[0]
+
+    def cat(ts):
+        return torch.cat([t.to(device=dev, dtype=torch.float32, non_blocking=True) for t in ts])
+    out = {"byt5": cat([x["byt5"] for x in inputs])}
+    if inputs[0].get("clip") is not None:
+        out["clip"] = cat([x["clip"] for x in inputs])
+    if inputs[0].get("clip_image") is not None:
+        per = [list(ci) if isinstance(ci, (list, tuple)) else [ci] for ci in (x["clip_image"] for x in inputs)]
+        out["clip_image"] = [cat([p[j] for p in per]) for j in range(len(per[0]))]
+    return out
 
 
 def build_step_plan(active: List[Request]) -> StepPlan:
@@ -262,9 +302,13 @@ class SamplingEngine:
             else:
                 src = self.noise[s] if q.init_x is None else q.init_x[0]
                 self.tokens[s].copy_(src, non_blocking=True)
-            m.write_conditioning(self.cache, q.slot, q.inputs, (self.H, self.W))
-            if q.uncond is not None:
-                m.write_conditioning(self.cache, q.uncond_slot, q.uncond, (self.H, self.W))
+        # the conditional and own unconditional K/V of the admitted requests: one projection per run of contiguous slots with
+        # one sequence layout (the rows equal per-request projections bit for bit: the conditioning path has no statistic
+        # that spans rows)
+        writes = [(q.slot, q.inputs) for q in new] + [(q.uncond_slot, q.uncond) for q in new if q.uncond is not None]
+        for run in admission_runs([(slot, cond_layout(x)) for slot, x in writes]):
+            m.write_conditioning(self.cache, writes[run[0]][0], _cat_inputs([writes[i][1] for i in run], self.dev), (self.H, self.W))
+        for q in new:
             q.inputs = q.uncond = q.init_x = q.region = None
         self._active += new
 

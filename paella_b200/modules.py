@@ -341,6 +341,25 @@ class Paella(nn.Module):
         self._packed_key = None
         self._workspace = None
         self._cond_single = None
+        self._batch_invariant = False
+
+    @property
+    def batch_invariant(self) -> bool:
+        """Batch-invariant forward (default False).  True: every sample's features, logits and tokens are bit-identical
+        whatever batch, batch position, CFG pairing or GPU count it runs in -- on any model and latent grid, so every
+        "bit for bit" statement of utils.sample*, SamplingEngine and sample_distributed's shards holds on the default model
+        too.  It changes how the folded LayerNorm's row statistics are summed (DESIGN.md §3 Numerics), so the results
+        differ in the last bits from the default mode.  Set it between calls, not while forwards of this model are being
+        enqueued from another thread; TypeError for a non-bool."""
+        return self._batch_invariant
+
+    @batch_invariant.setter
+    def batch_invariant(self, on: bool) -> None:
+        if not isinstance(on, bool):
+            raise TypeError(f"batch_invariant must be a bool (got {type(on).__name__})")
+        if self._handle is not None:
+            check(lib().pb200_paella_set_batch_invariant(self._handle, int(on)), "pb200_paella_set_batch_invariant")
+        self._batch_invariant = on
 
     # -------------------------------------------------------------- initialisation (ref/src/modules.py:189-210)
     def _reference_init(self, blocks, num_labels):
@@ -403,6 +422,7 @@ class Paella(nn.Module):
             h = ctypes.c_void_p()
             check(L.pb200_paella_create(ctypes.byref(cfg), ctypes.byref(h)), "pb200_paella_create")
             self._handle = h
+            check(L.pb200_paella_set_batch_invariant(h, int(self._batch_invariant)), "pb200_paella_set_batch_invariant")
         with torch.cuda.device(dev):
             nbytes = L.pb200_paella_weight_bytes(self._handle)
             if self._blob is None or self._blob.numel() != nbytes or self._blob.device != dev:
@@ -835,9 +855,10 @@ class Paella(nn.Module):
         return ops.attn_weights_to_device(table, lens, self._device())
 
     def write_conditioning(self, cache: ConditioningCache, slot: int, inputs: Dict[str, torch.Tensor], latent_hw) -> None:
-        """Project one sample's conditioning (batch-1 ``inputs``) into slot ``slot`` of an existing cache, as
-        prepare_conditioning projects a group of one; the slot's kv_len becomes this sequence's length, so rows left over
-        from a longer sequence are never attended to.  Host-to-device copies are asynchronous (no stream synchronisation)."""
+        """Project the conditioning of B samples (``inputs`` with batch B, one sequence layout) into slots [slot, slot + B)
+        of an existing cache, as prepare_conditioning projects a group; each slot's kv_len becomes this sequence's length, so
+        rows left over from a longer sequence are never attended to.  Host-to-device copies are asynchronous (no stream
+        synchronisation)."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -854,8 +875,9 @@ class Paella(nn.Module):
             if ci is not None:
                 ci = torch.stack([d(v) for v in ci]) if isinstance(ci, (list, tuple)) else d(ci)[None]
                 cond.clip_image, cond.n_clip_image = ptr(ci).value, ci.shape[0]
-            ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, 1, latent_hw[0], latent_hw[1], cache.s_max))
-            check(L.pb200_paella_prepare_cond(self._handle, ctypes.byref(cond), 1, slot, cache.slots, cache.s_max, ptr(cache.cache),
+            B = byt5.shape[0]
+            ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, B, latent_hw[0], latent_hw[1], cache.s_max))
+            check(L.pb200_paella_prepare_cond(self._handle, ctypes.byref(cond), B, slot, cache.slots, cache.s_max, ptr(cache.cache),
                                               ptr(ws), ws.numel(), current_stream()), "pb200_paella_prepare_cond")
 
     def forward(self, x, r, byt5, clip=None, clip_image=None, x_cat=None, **kwargs):

@@ -480,7 +480,7 @@ def gemm_f16(a: torch.Tensor, w: torch.Tensor, mode: int, out: torch.Tensor, bia
     ep.bias = ptr(bias).value if bias is not None else None
     ep.out = ptr(out).value
     ep.ldo = out.shape[-1] if mode in (_lib.EPI_F16, _lib.EPI_F32, _lib.EPI_GELU_F16, _lib.EPI_RESID_F32, _lib.EPI_RESID_LN_F32,
-                                       _lib.EPI_F16_LN) else 0
+                                       _lib.EPI_F16_LN, _lib.EPI_RESID_LN_INV_F32) else 0
     ep.out16 = ptr(out16).value if out16 is not None else None
     ep.ln_stat = ptr(ln_stat).value if ln_stat is not None else None
     ep.ln_wsum = ptr(ln_wsum).value if ln_wsum is not None else None

@@ -24,7 +24,8 @@ def rank_seed(base_seed: int, rank: int) -> int:
     """Per-shard generator seed.  Multi-GPU parity is defined per shard against a single-GPU run of that
     shard with this seed (SURVEY.md §8e).  With per-sample generators instead (``sample(..., generator=generators)``), a
     shard given ``generators[lo:hi]`` draws exactly what rows [lo, hi) of the single-GPU run draw, whatever the shard
-    layout, and reproduces their tokens exactly where the forward is batch-invariant (DESIGN.md §3)."""
+    layout, and reproduces their tokens exactly where the forward is batch-invariant (DESIGN.md §3: on the default model with
+    ``model.batch_invariant = True`` on every rank)."""
     return base_seed + rank
 
 

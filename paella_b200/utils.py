@@ -14,7 +14,8 @@ add_noise's rand_like) come from the torch CUDA generator's own Philox stream, c
 reference does, so ``torch.manual_seed`` means the same thing.  ``generator=[g_0, ..., g_{B-1}]`` gives each sample its own
 stream, consumed in the order a batch-1 loop would: randint over H*W, then per step the multinomial's exponential_ over
 H*W*num_labels (if the step draws) and add_noise's rand over H*W (if it renoises).  A sample's draws then depend only on
-its own seed; its tokens too, bit for bit, where the forward is batch-invariant (DESIGN.md §3 Numerics).
+its own seed; its tokens too, bit for bit, where the forward is batch-invariant (DESIGN.md §3 Numerics): on the default
+model with ``model.batch_invariant = True``, on the tiny test model in either mode.
 
 Per-sample settings: ``cfg``, ``temperature``, ``t_start`` and ``t_end`` each also take a CPU float tensor whose first
 dimension is B (``cfg`` [B] in ``sample``, [B, 2] in the other two; ``temperature`` [B, 2]; ``t_start`` / ``t_end`` [B]), in
