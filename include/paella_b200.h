@@ -20,7 +20,7 @@
 extern "C" {
 #endif
 
-#define PB200_ABI_VERSION 3      /* 3: pb200_vq_mlp_fused removed */
+#define PB200_ABI_VERSION 4      /* 4: GEMM A-operand scaling and the two always-0 pb200_gemm_plan outputs removed */
 
 const char* pb200_last_error(void);
 int pb200_abi_version(void);
@@ -181,19 +181,14 @@ typedef struct pb200_gemm_epilogue {
     int ln_c;                  /* F16_LN: number of columns the statistics cover (= K of this GEMM) */
     const float* ln_shift;     /* RESID_LN / F16_LN: fp32 [M] per-row shift the producer subtracted, or NULL (= 0) */
     float* ln_mean_out;        /* F16_LN: fp32 [M] true row mean (shift + mean of the shifted row), or NULL */
-    const void* a_scale;       /* RESID / RESID_LN: fp16 [M / rows_per_sample, a_scale_ld] per-(sample, k) factors multiplied into
-                                  the A operand on its way to the tensor core (GlobalResponseNorm folded into the GEMM that
-                                  consumes it: A'[m,k] = A[m,k] * a_scale[m / rows_per_sample, k]), or NULL.  Needs
-                                  K % 64 == 0 and rows_per_sample dividing 128 (>= 16) or a multiple of 128 */
-    int64_t a_scale_ld;
 } pb200_gemm_epilogue;
 
 int pb200_gemm_f16(const void* a, int64_t lda, const void* w, int64_t ldw, int64_t m, int64_t n, int64_t k,
                    const pb200_gemm_epilogue* epi, void* stream);
 /* Host-side tile plan pb200_gemm_f16 would use for an [m,k] x [n,k]^T problem on `sm_count` multiprocessors (0 = the
- * current device, or 132 without one): BLOCK_N; two_sm and tail_block_n are always 0 on sm_90a (one CTA per tile, every
- * tile BLOCK_N wide).  Pure arithmetic, no device work. */
-int pb200_gemm_plan(int64_t m, int64_t n, int64_t k, int sm_count, int* block_n, int* two_sm, int* tail_block_n);
+ * current device, or 132 without one): BLOCK_N (one CTA per tile, every tile BLOCK_N wide).  Pure arithmetic, no device
+ * work. */
+int pb200_gemm_plan(int64_t m, int64_t n, int64_t k, int sm_count, int* block_n);
 
 /* ------------------------------------------------------------------------------------------
  * Block-level kernels: what the reference's building-block modules (ref/src/modules.py:7-106)

@@ -22,7 +22,7 @@ class GemmEpilogue(ctypes.Structure):
         ("ldr", c_int64), ("alpha", c_float), ("sqsum", c_void_p), ("rows_per_sample", c_int), ("film", c_void_p),
         ("film_ld", c_int64), ("film_off", c_int64), ("remap_in", c_int), ("remap_out", c_int), ("up_h", c_int),
         ("up_w", c_int), ("up_cout", c_int), ("out16", c_void_p), ("ln_stat", c_void_p), ("ln_wsum", c_void_p),
-        ("ln_c", c_int), ("ln_shift", c_void_p), ("ln_mean_out", c_void_p), ("a_scale", c_void_p), ("a_scale_ld", c_int64),
+        ("ln_c", c_int), ("ln_shift", c_void_p), ("ln_mean_out", c_void_p),
     ]
 
 
@@ -80,7 +80,7 @@ SIGNATURES = {
     "pb200_vq_gather": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "pb200_gemm_f16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                POINTER(GemmEpilogue), c_void_p]),
-    "pb200_gemm_plan": (c_int, [c_int64, c_int64, c_int64, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
+    "pb200_gemm_plan": (c_int, [c_int64, c_int64, c_int64, c_int, POINTER(c_int)]),
     "pb200_layernorm": (c_int, [c_void_p, c_int64, c_int, ctypes.c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pb200_nchw_to_nhwc": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pb200_nhwc_to_nchw": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -172,7 +172,7 @@ def lib() -> ctypes.CDLL:
             fn = getattr(l, name)        # AttributeError here = header/library mismatch
             fn.restype = res
             fn.argtypes = args
-        if l.pb200_abi_version() != 3:
+        if l.pb200_abi_version() != 4:
             raise PaellaB200Error("libpaella_b200.so ABI version mismatch")
         _lib = l
     return _lib

@@ -68,27 +68,6 @@ struct ProfScope {
     ~ProfScope();
 };
 
-// ---------------------------------------------------------------- in-kernel timeline tracing (development aid)
-// PB200_TRACE=<kernel>:<file> makes the named warp-specialised kernel record, for CTA 0 of ONE launch, what each role was doing
-// when: one 64-bit word per event = clock64() << 16 | event << 8 | (item & 255), appended to the role's own log (one thread per
-// role writes, so no atomics).  The host dumps the log as text after the launch (a device synchronisation: tracing mode only).
-constexpr int TRACE_ROLES = 16;
-constexpr int TRACE_PER_ROLE = 4096;
-struct TraceBuf {
-    unsigned long long* buf;      // [TRACE_ROLES] cursors, then TRACE_ROLES x TRACE_PER_ROLE events; nullptr = tracing off
-};
-__device__ __forceinline__ void trace_ev(const TraceBuf& t, int role, int ev, int item) {
-    if (t.buf == nullptr || blockIdx.x != 0) return;
-    const unsigned long long n = t.buf[role];
-    t.buf[role] = n + 1;
-    if (n < (unsigned long long)TRACE_PER_ROLE)
-        t.buf[TRACE_ROLES + role * TRACE_PER_ROLE + n] = ((unsigned long long)clock64() << 16) | ((unsigned long long)(ev & 255) << 8) | (unsigned long long)(item & 255);
-}
-// host side (core.cu): returns a zeroed device buffer if PB200_TRACE names `kernel` and this is the launch to trace, else {nullptr}
-TraceBuf trace_begin(const char* kernel);
-// synchronises, writes the text dump (role, event, item, cycle) and frees the buffer
-int trace_end(const char* kernel, TraceBuf t, const char* const* role_names, const char* const* event_names);
-
 // ---------------------------------------------------------------- small device helpers
 // Lets a dependent kernel launched with programmatic stream serialization (the wgmma GEMMs, see ptx.cuh) start its
 // prologue while this kernel's last CTAs are still running.  No effect otherwise.

@@ -92,50 +92,6 @@ ProfScope::~ProfScope() {
     cudaEventRecord(g_recs[slot].e1, st);
 }
 
-// ------------------------------------------------------------------ timeline tracing (PB200_TRACE=<kernel>:<file>[:<launch#>])
-static int g_trace_seen = 0;
-TraceBuf trace_begin(const char* kernel) {
-    TraceBuf t{nullptr};
-    static const char* env = getenv("PB200_TRACE");
-    if (!env) return t;
-    const std::string e(env);
-    const size_t c = e.find(':');
-    if (c == std::string::npos || e.substr(0, c) != kernel) return t;
-    const size_t c2 = e.find(':', c + 1);
-    const int want = c2 == std::string::npos ? 40 : atoi(e.c_str() + c2 + 1);      // default: the 40th launch (past warm-up)
-    if (g_trace_seen++ != want) return t;
-    const size_t bytes = sizeof(unsigned long long) * (TRACE_ROLES + (size_t)TRACE_ROLES * TRACE_PER_ROLE);
-    if (cudaMalloc(&t.buf, bytes) != cudaSuccess) { t.buf = nullptr; return t; }
-    cudaMemset(t.buf, 0, bytes);
-    return t;
-}
-int trace_end(const char* kernel, TraceBuf t, const char* const* role_names, const char* const* event_names) {
-    if (!t.buf) return 0;
-    const std::string e(getenv("PB200_TRACE"));
-    const size_t c = e.find(':'), c2 = e.find(':', c + 1);
-    const std::string path = e.substr(c + 1, c2 == std::string::npos ? std::string::npos : c2 - c - 1);
-    PB_CUDA(cudaDeviceSynchronize());
-    std::vector<unsigned long long> h(TRACE_ROLES + (size_t)TRACE_ROLES * TRACE_PER_ROLE);
-    PB_CUDA(cudaMemcpy(h.data(), t.buf, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    cudaFree(t.buf);
-    FILE* f = fopen(path.c_str(), "w");
-    PB_CHECK(f != nullptr, "trace: cannot open %s", path.c_str());
-    unsigned long long t0 = ~0ull;
-    for (int r = 0; r < TRACE_ROLES; ++r)
-        for (unsigned long long i = 0; i < h[r] && i < (unsigned long long)TRACE_PER_ROLE; ++i) {
-            const unsigned long long v = h[TRACE_ROLES + r * TRACE_PER_ROLE + i] >> 16;
-            t0 = v < t0 ? v : t0;
-        }
-    fprintf(f, "# %s: CTA 0, cycles since the first event\n# role event item cycle\n", kernel);
-    for (int r = 0; r < TRACE_ROLES; ++r)
-        for (unsigned long long i = 0; i < h[r] && i < (unsigned long long)TRACE_PER_ROLE; ++i) {
-            const unsigned long long w = h[TRACE_ROLES + r * TRACE_PER_ROLE + i];
-            fprintf(f, "%s %s %d %llu\n", role_names[r], event_names[(w >> 8) & 255], (int)(w & 255), (w >> 16) - t0);
-        }
-    fclose(f);
-    return 0;
-}
-
 }  // namespace pb
 
 extern "C" {

@@ -473,17 +473,11 @@ __device__ __forceinline__ void epilogue_finish(const pb200_gemm_epilogue& ep, i
 // AMODE 0: A is a [M,K] matrix.  AMODE 1/2: A rows are gathered by TMA straight from an NHWC fp16 activation
 // (im2col-free convolution): a 128-row tile is a th x tw patch of the output grid and k-block kb selects a filter
 // tap and a 64-channel slice; out-of-image taps are zero-filled by the TMA unit (the conv's zero padding).
-// ASCALE (GlobalResponseNorm folded into the A operand, ref/src/modules.py:37-40 + :53): the A tile is multiplied in shared
-// memory, between TMA and MMA, by a per-(sample, k) fp16 factor  s[b, k] = 1 + gamma[k] * Nx[b, k]  -- GEMM2 of a ResBlock then
-// computes (h * s) W2^T + (W2 beta + b2) = GRN(h) W2^T + b2 without the separate read-modify-write pass over the 4c-wide hidden.
-// The [samples x 64] slice of s lands in the stage beside A and W; each MMA warpgroup rescales its own 64 rows in place (one
-// HMUL2 rounding, the fp16 product), fences the generic->async proxy and only then issues its wgmma.
-template <int BLOCK_N, int MODE, int AMODE, bool ASCALE>
+template <int BLOCK_N, int MODE, int AMODE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                const __grid_constant__ CUtensorMap tm_s, const pb200_gemm_epilogue ep, const ConvGeom geom, int M, int N,
-                int K) {
-    using L = GemmSmem<BLOCK_N, ASCALE>;
+                const pb200_gemm_epilogue ep, const ConvGeom geom, int M, int N, int K) {
+    using L = GemmSmem<BLOCK_N>;
     constexpr int NSUB = BLOCK_N > 128 ? 2 : 1;          // a 256-wide tile is issued as two n128 wgmma per k-step
     constexpr int SUBN = BLOCK_N / NSUB;
     extern __shared__ uint8_t smem_raw[];
@@ -500,8 +494,6 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
     const int n_tiles_m = AMODE == 0 ? (M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M : geom.batch * geom.tiles_y * geom.tiles_x;
     const int n_kb = (K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
     const int n_units = n_tiles_m * n_tiles_n;
-    const int P = ep.rows_per_sample;
-    const int ns = ASCALE ? (P >= GEMM_BLOCK_M ? 1 : GEMM_BLOCK_M / P) : 0;      // samples in a 128-row tile
 
     if (threadIdx.x == 0) {
         ptx::prefetch_tensormap(&tm_a);
@@ -537,7 +529,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
                 }
                 for (int kb = 0; kb < n_kb; ++kb) {
                     ptx::mbar_wait(empty_bar(stage), phase ^ 1);
-                    ptx::mbar_arrive_expect_tx(full_bar(stage), (uint32_t)(L::A_BYTES + L::B_BYTES + ns * GEMM_BLOCK_K * 2));
+                    ptx::mbar_arrive_expect_tx(full_bar(stage), (uint32_t)(L::A_BYTES + L::B_BYTES));
                     const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
                     if (AMODE == 0) {
                         ptx::tma_load_2d(&tm_a, full_bar(stage), sa, kb * GEMM_BLOCK_K, m_idx);
@@ -561,8 +553,6 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
                     ptx::tma_load_2d(&tm_b, full_bar(stage), sa + L::A_BYTES, kb * GEMM_BLOCK_K, n_idx);
                     ptx::tma_load_2d(&tm_b, full_bar(stage), sa + L::A_BYTES + L::B_BYTES / 2, kb * GEMM_BLOCK_K,
                                      n_idx + BLOCK_N / 2);
-                    if (ASCALE)
-                        ptx::tma_load_2d(&tm_s, full_bar(stage), sa + L::A_BYTES + L::B_BYTES, kb * GEMM_BLOCK_K, m_idx / P);
                     if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
                 }
             }
@@ -585,28 +575,6 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
             for (int kb = 0; kb < n_kb; ++kb) {
                 ptx::mbar_wait(full_bar(stage), phase);
                 const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
-                if (ASCALE) {
-                    // thread = half a row: chunks [4 (tid & 1), +4) of row 64 cw + tid / 2; logical 16-byte chunk j of row r
-                    // sits at j ^ (r & 7) (128-byte swizzle)
-                    const int r = cw * 64 + (tid >> 1);
-                    const int sl = P >= GEMM_BLOCK_M ? 0 : min(r / P, ns - 1);
-                    uint8_t* sg = smem_gen + stage * L::STAGE_BYTES;
-                    uint4* arow = reinterpret_cast<uint4*>(sg + r * 128);
-                    const uint4* srow = reinterpret_cast<const uint4*>(sg + L::A_BYTES + L::B_BYTES + sl * 128);
-#pragma unroll
-                    for (int jj = 0; jj < 4; ++jj) {
-                        const int j = (tid & 1) * 4 + jj;
-                        uint4 av = arow[j ^ (r & 7)];
-                        const uint4 sv = srow[j];
-                        __half2* a2 = reinterpret_cast<__half2*>(&av);
-                        const __half2* s2 = reinterpret_cast<const __half2*>(&sv);
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) a2[e] = __hmul2(a2[e], s2[e]);
-                        arow[j ^ (r & 7)] = av;
-                    }
-                    ptx::fence_proxy_async_smem();       // the rescaled rows must be visible to the tensor core's async proxy
-                    ptx::bar_sync(1 + cw, 128);
-                }
                 const uint64_t da = ptx::wgmma_desc_kmajor_sw128(sa + (uint32_t)cw * (64 * 128));
                 const uint64_t db = ptx::wgmma_desc_kmajor_sw128(sa + L::A_BYTES);
                 ptx::wgmma_fence();
@@ -685,25 +653,18 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
 }
 
 // ------------------------------------------------------------------ dispatch
-template <int BLOCK_N, int MODE, int AMODE = 0, bool ASCALE = false>
+template <int BLOCK_N, int MODE, int AMODE = 0>
 static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const pb200_gemm_epilogue& ep, int M, int N, int K,
                       cudaStream_t st, const ConvGeom* geom = nullptr) {
-    using L = GemmSmem<BLOCK_N, ASCALE>;
+    using L = GemmSmem<BLOCK_N>;
     static DeviceOnce attr_set;
     if (attr_set.first()) {
-        PB_CUDA(cudaFuncSetAttribute(gemm_f16_kernel<BLOCK_N, MODE, AMODE, ASCALE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        PB_CUDA(cudaFuncSetAttribute(gemm_f16_kernel<BLOCK_N, MODE, AMODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      L::SMEM_BYTES));
     }
     ConvGeom g;
     memset(&g, 0, sizeof(g));
     if (geom) g = *geom;
-    CUtensorMap ts = ta;            // placeholder when unused
-    if (ASCALE) {
-        const int P = ep.rows_per_sample;
-        const int ns = P >= GEMM_BLOCK_M ? 1 : GEMM_BLOCK_M / P;
-        const int64_t samples = ((int64_t)M + P - 1) / P;
-        PB_TRY(make_tmap_f16_2d_box(&ts, ep.a_scale, samples, K, ep.a_scale_ld, GEMM_BLOCK_K, ns, 0));
-    }
     const int tiles_m = AMODE == 0 ? ceil_div(M, GEMM_BLOCK_M) : g.batch * g.tiles_y * g.tiles_x;
     const int n_units = tiles_m * ceil_div(N, BLOCK_N);
     const int grid = n_units < sm_count() ? n_units : sm_count();
@@ -719,7 +680,7 @@ static int launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const pb200_
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 1 : 0;
-    PB_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_kernel<BLOCK_N, MODE, AMODE, ASCALE>, ta, tb, ts, ep, g, M, N, K));
+    PB_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_kernel<BLOCK_N, MODE, AMODE>, ta, tb, ep, g, M, N, K));
     PB_LAUNCH_CHECK();
     return 0;
 }
@@ -750,13 +711,6 @@ int gemm_conv_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, 
 template <int BLOCK_N>
 static int launch_mode(const CUtensorMap& ta, const CUtensorMap& tb, const pb200_gemm_epilogue& ep, int M, int N, int K,
                        cudaStream_t st) {
-    if (ep.a_scale) {       // GlobalResponseNorm folded into the A operand: the two residual epilogues only
-        if (ep.mode == PB200_EPI_RESID_F32) return launch_cfg<BLOCK_N, PB200_EPI_RESID_F32, 0, true>(ta, tb, ep, M, N, K, st);
-        if (ep.mode == PB200_EPI_RESID_LN_F32) return launch_cfg<BLOCK_N, PB200_EPI_RESID_LN_F32, 0, true>(ta, tb, ep, M, N, K, st);
-        if (ep.mode == PB200_EPI_RESID_LN_INV_F32)
-            return launch_cfg<BLOCK_N, PB200_EPI_RESID_LN_INV_F32, 0, true>(ta, tb, ep, M, N, K, st);
-        PB_CHECK(false, "gemm: a_scale is only built for the RESID epilogues (mode %d)", ep.mode);
-    }
     switch (ep.mode) {
         case PB200_EPI_F16: return launch_cfg<BLOCK_N, PB200_EPI_F16>(ta, tb, ep, M, N, K, st);
         case PB200_EPI_F32: return launch_cfg<BLOCK_N, PB200_EPI_F32>(ta, tb, ep, M, N, K, st);
@@ -778,13 +732,6 @@ static int plan_sm_count() {
     if (g_plan_sms > 0) return g_plan_sms;
     const int s = sm_count();
     return s > 0 ? s : 132;
-}
-
-bool gemm_can_scale_a(int64_t M, int64_t N, int64_t K, int rows_per_sample) {
-    (void)M; (void)N;
-    const int P = rows_per_sample;
-    if (P <= 0 || K % GEMM_BLOCK_K != 0) return false;
-    return P >= GEMM_BLOCK_M ? P % GEMM_BLOCK_M == 0 : (GEMM_BLOCK_M % P == 0 && GEMM_BLOCK_M / P <= 8);
 }
 
 int gemm_pick_block_n(int64_t M, int64_t N, int64_t K) {
@@ -830,9 +777,6 @@ int gemm_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, const
     if ((ep.mode == PB200_EPI_GELU_F16 && ep.sqsum) || ((ep.mode == PB200_EPI_RESID_F32 || resid_ln) && ep.film) ||
         ep.mode == PB200_EPI_NCHW_F32)
         PB_CHECK(ep.rows_per_sample > 0, "gemm: rows_per_sample required");
-    if (ep.a_scale)
-        PB_CHECK(gemm_can_scale_a(M, N, K, ep.rows_per_sample) && ep.a_scale_ld % 8 == 0 && ((uintptr_t)ep.a_scale & 15) == 0,
-                 "gemm: a_scale needs rows_per_sample dividing or divided by 128, K %% 64 == 0");
     static const char* kTags[9] = {"gemm_f16", "gemm_f32", "gemm_gelu_sqsum", "gemm_resid", "gemm_unpatch", "gemm_nchw",
                                    "gemm_resid", "gemm_f16", "gemm_resid"};
     ProfScope prof(ep.mode >= 0 && ep.mode < 9 ? kTags[ep.mode] : "gemm", 2.0 * (double)M * (double)N * (double)K, st);
@@ -857,13 +801,10 @@ int gemm_f16(const void* a, int64_t lda, const void* w, int64_t ldw, int64_t M, 
 
 }  // namespace pb
 
-extern "C" int pb200_gemm_plan(int64_t m, int64_t n, int64_t k, int sm_count, int* block_n, int* two_sm, int* tail_block_n) {
-    PB_CHECK(m > 0 && n > 0 && k > 0 && block_n && two_sm && tail_block_n, "gemm_plan: bad arguments");
+extern "C" int pb200_gemm_plan(int64_t m, int64_t n, int64_t k, int sm_count, int* block_n) {
+    PB_CHECK(m > 0 && n > 0 && k > 0 && block_n, "gemm_plan: bad arguments");
     pb::g_plan_sms = sm_count > 0 ? sm_count : 0;
-    const int bn = pb::gemm_pick_block_n(m, n, k);
-    *block_n = bn;
-    *two_sm = 0;            // Hopper has no 2-SM MMA: every tile is one CTA's
-    *tail_block_n = 0;      // ... and every tile is BLOCK_N wide
+    *block_n = pb::gemm_pick_block_n(m, n, k);
     pb::g_plan_sms = 0;
     return 0;
 }

@@ -12,14 +12,13 @@ constexpr int GEMM_CONSUMERS = 2;    // MMA warpgroups, 64 rows of the tile each
 constexpr int GEMM_THREADS = 128 * (1 + GEMM_CONSUMERS);      // + the producer warpgroup
 constexpr int GEMM_EPI_STRIDE = 65;  // fp32 row stride of the epilogue slab (odd: the row-per-lane reads are conflict-free)
 constexpr int GEMM_EPI_BYTES = GEMM_CONSUMERS * 64 * GEMM_EPI_STRIDE * 4;
-constexpr int GEMM_ASCALE_BYTES = 1024;        // up to 8 samples x 64 factors per 128-row tile and k-block
 constexpr int SMEM_PER_BLOCK_MAX = 232448;     // 227 KB: the opt-in limit of one block on sm_90
 
-template <int BLOCK_N, bool ASCALE = false>
+template <int BLOCK_N>
 struct GemmSmem {
     static constexpr int A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
     static constexpr int B_BYTES = BLOCK_N * GEMM_BLOCK_K * 2;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES + (ASCALE ? GEMM_ASCALE_BYTES : 0);
+    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int FIXED = GEMM_EPI_BYTES + 1024 /*alignment slack*/ + 256 /*barriers*/;
     static constexpr int FIT = (SMEM_PER_BLOCK_MAX - FIXED) / STAGE_BYTES;
     static constexpr int STAGES = FIT > 8 ? 8 : FIT;
@@ -59,8 +58,6 @@ int gemm_conv_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, 
 
 // BLOCK_N that minimises a tensor / L2 cycle model of the launch (see gemm.cu)
 int gemm_pick_block_n(int64_t M, int64_t N, int64_t K = 0);
-// whether gemm_launch can take ep.a_scale for this problem (sample rows aligned with the 128-row tiles, K % 64 == 0)
-bool gemm_can_scale_a(int64_t M, int64_t N, int64_t K, int rows_per_sample);
 
 // tb: tensor map of W with box rows block_n / 2
 int gemm_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, const pb200_gemm_epilogue& ep, int64_t M,

@@ -594,10 +594,9 @@ int launch_dwconv_ln(const float* x, const float* skip, const float* w_packed, c
 // occupancy in ncu; the stream itself is now the only thing a CTA does).
 __device__ __forceinline__ float grn_fx(unsigned long long q) { return __ull2float_rn(q) * (1.0f / 16777216.0f); }
 
-template <typename OutT>
 __global__ void __launch_bounds__(512) grn_scale_kernel(int N, const unsigned long long* __restrict__ sq,
                                                         unsigned long long* __restrict__ sq_next, const float* __restrict__ gamma,
-                                                        OutT* __restrict__ scale, int zero_per_sample) {
+                                                        float* __restrict__ scale, int zero_per_sample) {
     pdl_launch_dependents();
     const int b = blockIdx.x;
     const unsigned long long* sqb = sq + (int64_t)b * N;
@@ -613,11 +612,8 @@ __global__ void __launch_bounds__(512) grn_scale_kernel(int N, const unsigned lo
     float tot = 0.f;
     for (int i = 0; i < (int)(blockDim.x >> 5); ++i) tot += red[i];
     const float inv_denom = 1.0f / (tot / N + 1e-6f);
-    for (int i = threadIdx.x; i < N; i += blockDim.x) {
-        const float v = fmaf(__ldg(gamma + i), sqrtf(grn_fx(sqb[i])) * inv_denom, 1.0f);
-        if constexpr (sizeof(OutT) == 2) scale[(int64_t)b * N + i] = __float2half_rn(v);
-        else scale[(int64_t)b * N + i] = v;
-    }
+    for (int i = threadIdx.x; i < N; i += blockDim.x)
+        scale[(int64_t)b * N + i] = fmaf(__ldg(gamma + i), sqrtf(grn_fx(sqb[i])) * inv_denom, 1.0f);
     for (int i = threadIdx.x; i < zero_per_sample; i += blockDim.x) sq_next[(int64_t)b * zero_per_sample + i] = 0ull;
 }
 
@@ -664,17 +660,6 @@ __global__ void __launch_bounds__(256) grn_apply_kernel(__half* __restrict__ h, 
     }
 }
 
-// Only the multipliers (fp16 [B, N]): the GEMM that consumes the hidden applies them to its A operand (pb200_gemm_epilogue::a_scale)
-int launch_grn_scale_f16(int B, int N, const uint64_t* sq, uint64_t* sq_next, int zero_per_sample, const float* gamma, __half* scale,
-                         cudaStream_t st) {
-    ProfScope prof("grn", (double)B * N * 10.0, st);
-    if (B == 0) return 0;
-    grn_scale_kernel<__half><<<B, 512, 0, st>>>(N, reinterpret_cast<const unsigned long long*>(sq), reinterpret_cast<unsigned long long*>(sq_next),
-                                               gamma, scale, zero_per_sample);
-    PB_LAUNCH_CHECK();
-    return 0;
-}
-
 int launch_grn_fused(__half* h, int B, int P, int N, const uint64_t* sq, uint64_t* sq_next, int zero_per_sample, const float* gamma,
                      const float* beta, float* scale_scratch, cudaStream_t st) {
     ProfScope prof("grn", (double)B * P * N * 4.0, st);
@@ -682,8 +667,8 @@ int launch_grn_fused(__half* h, int B, int P, int N, const uint64_t* sq, uint64_
     PB_CHECK(scale_scratch != nullptr, "grn: scale scratch [B, N] fp32 required");
     if (B == 0 || P == 0) return 0;
     PB_CHECK(B <= 65535, "grn: batch too large");
-    grn_scale_kernel<float><<<B, 512, 0, st>>>(N, reinterpret_cast<const unsigned long long*>(sq), reinterpret_cast<unsigned long long*>(sq_next),
-                                              gamma, scale_scratch, zero_per_sample);
+    grn_scale_kernel<<<B, 512, 0, st>>>(N, reinterpret_cast<const unsigned long long*>(sq), reinterpret_cast<unsigned long long*>(sq_next),
+                                        gamma, scale_scratch, zero_per_sample);
     PB_LAUNCH_CHECK();
     // rows per CTA: 16 (two 8-row groups, the second in flight while the first is converted), 8 when that leaves SMs idle
     const int nch = N >> 3;

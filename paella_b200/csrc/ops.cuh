@@ -34,10 +34,6 @@ int launch_vq_front_fused(const float* x, int B, int h, int w, int c, const floa
 int launch_grn_fused(__half* h, int B, int P, int N, const uint64_t* sq, uint64_t* sq_next, int zero_per_sample, const float* gamma,
                      const float* beta, float* scale_scratch, cudaStream_t st);
 
-// the GRN multipliers alone, fp16 [B, N] (+ zeroing of sq_next): for a consumer GEMM that scales its A operand (a_scale)
-int launch_grn_scale_f16(int B, int N, const uint64_t* sq, uint64_t* sq_next, int zero_per_sample, const float* gamma, __half* scale,
-                         cudaStream_t st);
-
 // gen_r_embedding: r [B] -> [B, c_r]
 int launch_r_embed(const float* r, int B, int c_r, float* out, cudaStream_t st);
 // all TimestepBlock mappers at once: out[b, j] = bias[j] + sum_i r_embed[b,i] * W[j,i]; W [total, c_r]

@@ -82,18 +82,6 @@ __global__ void __launch_bounds__(256) rowsum_f16_kernel(const __half* __restric
     if (lane == 0) out[r] = s;
 }
 
-// out[n] = b2[n] + sum_k fp32(w2[n, k]) * beta[k]: the GlobalResponseNorm shift pushed through the Linear that follows it
-// (GRN(h) W2^T + b2 = (h * s) W2^T + (W2 beta + b2)); warp per output row
-__global__ void __launch_bounds__(256) fold_bias_kernel(const __half* __restrict__ w2, const float* __restrict__ beta,
-                                                        const float* __restrict__ b2, int rows, int cols, float* __restrict__ out) {
-    const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (r >= rows) return;
-    float s = 0.f;
-    for (int k = lane; k < cols; k += 32) s = fmaf(__half2float(w2[(int64_t)r * cols + k]), beta[k], s);
-    s = warp_sum(s);
-    if (lane == 0) out[r] = s + b2[r];
-}
-
 struct ParamSpec {
     std::string name;
     int64_t numel;      // reference tensor numel
@@ -103,14 +91,6 @@ struct ParamSpec {
     int d0, d1, d2;
     int64_t rowsum_off = -1;     // fp32 [rowsum_rows]: row sums of the packed fp16 matrix [rowsum_rows, rowsum_cols]
     int rowsum_rows = 0, rowsum_cols = 0;
-    int fold_group = -1;         // index into pb200_paella::folds (channelwise.2.beta / .4.weight / .4.bias of one MLP)
-};
-
-// derived parameter of one ResBlock / FeedForwardBlock MLP: b2_fold = channelwise.4.bias + channelwise.4.weight . channelwise.2.beta
-struct FoldGroup {
-    int64_t w2, beta, b2, out;
-    int c;
-    int loaded = 0;              // parameters of the group seen by load_param since the blob was bound
 };
 
 enum BlockKind { BK_RES, BK_TIME, BK_ATTN, BK_FF, BK_DOWN, BK_UP, BK_SAVE };
@@ -118,7 +98,6 @@ enum BlockKind { BK_RES, BK_TIME, BK_ATTN, BK_FF, BK_DOWN, BK_UP, BK_SAVE };
 struct BlockPlan {
     int kind, level, c, c_skip;
     int64_t dw_w = -1, dw_b = -1, w1 = -1, b1 = -1, gamma = -1, beta = -1, w2 = -1, b2 = -1;
-    int64_t b2_fold = -1;           // fp32 [c]: b2 + W2 beta (GRN shift folded through the second Linear)
     int64_t film_off = -1;          // RES/FF: fused FiLM of the following TimestepBlock; TIME: own offset
     bool film_fused = false;        // TIME: already applied by the previous block's epilogue
     int64_t kvm_w = -1, kvm_b = -1, inproj_w = -1, inproj_b = -1, outproj_w = -1, outproj_b = -1;
@@ -139,7 +118,6 @@ struct pb200_paella {
     std::vector<ParamSpec> params;
     std::unordered_map<std::string, int> by_name;
     std::vector<BlockPlan> blocks;
-    std::vector<FoldGroup> folds;
     int64_t weight_bytes = 0;
     uint8_t* blob = nullptr;
     int64_t emb_table = -1, emb_w = -1, emb_b = -1, byt5_w = -1, byt5_b = -1, clip_w = -1, clip_b = -1, clipimg_w = -1,
@@ -251,13 +229,6 @@ static int build_plan(pb200_paella* m) {
             b.beta = m->f32(pre + "channelwise.2.beta", 4 * ch);
             b.w2 = m->f16(pre + "channelwise.4.weight", (int64_t)4 * ch * ch);
             b.b2 = m->f32(pre + "channelwise.4.bias", ch);
-            b.b2_fold = m->weight_bytes;
-            m->weight_bytes += ((int64_t)ch * 4 + 255) / 256 * 256;
-            FoldGroup fg;
-            fg.w2 = b.w2; fg.beta = b.beta; fg.b2 = b.b2; fg.out = b.b2_fold; fg.c = ch;
-            for (const char* suffix : {"channelwise.2.beta", "channelwise.4.weight", "channelwise.4.bias"})
-                m->params[m->by_name[pre + suffix]].fold_group = (int)m->folds.size();
-            m->folds.push_back(fg);
         };
         if (bt == 'C') {
             b.kind = BK_RES;
@@ -500,7 +471,6 @@ int pb200_paella_bind_weights(pb200_paella* m, void* blob) {
     PB_CHECK(((uintptr_t)blob & 255) == 0, "weight blob must be 256-byte aligned");
     m->blob = reinterpret_cast<uint8_t*>(blob);
     m->tmaps.clear();
-    for (FoldGroup& g : m->folds) g.loaded = 0;
     return 0;
 }
 
@@ -533,14 +503,6 @@ int pb200_paella_load_param(pb200_paella* m, const char* name, const float* src,
             reinterpret_cast<const __half*>(m->blob + p.dst_off), p.rowsum_rows, p.rowsum_cols,
             reinterpret_cast<float*>(m->blob + p.rowsum_off));
         PB_LAUNCH_CHECK();
-    }
-    if (p.fold_group >= 0) {     // the derived bias is (re)computed whenever its three inputs are all present in the blob
-        FoldGroup& g = m->folds[p.fold_group];
-        if (++g.loaded >= 3) {
-            fold_bias_kernel<<<ceil_div(g.c, 8), 256, 0, (cudaStream_t)stream>>>(m->w<__half>(g.w2), m->w<float>(g.beta), m->w<float>(g.b2),
-                                                                              g.c, 4 * g.c, m->w<float>(g.out));
-            PB_LAUNCH_CHECK();
-        }
     }
     return 0;
 }
@@ -769,22 +731,12 @@ int pb200_paella_features_weighted(pb200_paella* m, const int64_t* tokens, const
                 grn_flip ^= 1;
                 e1.sqsum = stat; e1.rows_per_sample = P;
                 PB_TRY(m->gemm(ws.a16, ch, M, ch, b.w1, 4 * (int64_t)ch, e1, st));
-                // GlobalResponseNorm: folded into GEMM2's A operand where its tiles line up with the samples (multipliers only,
-                // shift pushed into the bias), else applied to the hidden in place
-                // The fold removes the stand-alone GRN pass over the 4c-wide hidden but makes each MMA warpgroup rescale its A
-                // rows in shared memory before every k-block's wgmma; DESIGN.md section 5.1 has the A/B on the bench step.
-                static const bool fold_on = getenv("PB200_GRN_FOLD") != nullptr;
-                const bool fold_grn = fold_on && gemm_can_scale_a(M, ch, 4 * (int64_t)ch, P);
-                __half* grn_s16 = reinterpret_cast<__half*>(ws.grn_mult);
-                if (fold_grn)
-                    PB_TRY(launch_grn_scale_f16(Bc, 4 * ch, stat, stat_next, 4 * m->max_c, m->w<float>(b.gamma), grn_s16, st));
-                else
-                    PB_TRY(launch_grn_fused(ws.h16, Bc, P, 4 * ch, stat, stat_next, 4 * m->max_c, m->w<float>(b.gamma), m->w<float>(b.beta), ws.grn_mult, st));
+                // GlobalResponseNorm, applied to the hidden in place
+                PB_TRY(launch_grn_fused(ws.h16, Bc, P, 4 * ch, stat, stat_next, 4 * m->max_c, m->w<float>(b.gamma), m->w<float>(b.beta), ws.grn_mult, st));
                 // the next AttnBlock's LayerNorm is folded into its QKV GEMM when this block feeds it directly
                 const bool fold = b.ln_fold_attn >= 0;
                 const int ln_mode = m->batch_invariant ? PB200_EPI_RESID_LN_INV_F32 : PB200_EPI_RESID_LN_F32;
-                pb200_gemm_epilogue e2 = epi(fold ? ln_mode : PB200_EPI_RESID_F32, m->w<float>(fold_grn ? b.b2_fold : b.b2), x, ch);
-                if (fold_grn) { e2.a_scale = grn_s16; e2.a_scale_ld = 4 * (int64_t)ch; }
+                pb200_gemm_epilogue e2 = epi(fold ? ln_mode : PB200_EPI_RESID_F32, m->w<float>(b.b2), x, ch);
                 e2.resid = x; e2.ldr = ch; e2.rows_per_sample = P;
                 if (b.film_off >= 0) { e2.film = ws.film; e2.film_ld = m->film_total; e2.film_off = b.film_off; }
                 if (fold) {

@@ -470,7 +470,7 @@ def vq_gather(idx: torch.Tensor, codebook: torch.Tensor) -> torch.Tensor:
 # ------------------------------------------------------------------ GEMM (unit-test surface)
 def gemm_f16(a: torch.Tensor, w: torch.Tensor, mode: int, out: torch.Tensor, bias=None, resid=None, alpha: float = 1.0,
              sqsum=None, rows_per_sample: int = 0, film=None, film_off: int = 0, remap=(0, 0), up=(0, 0, 0), out16=None,
-             ln_stat=None, ln_wsum=None, ln_shift=None, ln_mean_out=None, a_scale=None) -> torch.Tensor:
+             ln_stat=None, ln_wsum=None, ln_shift=None, ln_mean_out=None) -> torch.Tensor:
     """out = epilogue(a[M,K] @ w[N,K]^T); a, w fp16 contiguous."""
     assert a.dtype == torch.float16 and w.dtype == torch.float16 and a.shape[1] == w.shape[1]
     M, K = a.shape
@@ -487,8 +487,6 @@ def gemm_f16(a: torch.Tensor, w: torch.Tensor, mode: int, out: torch.Tensor, bia
     ep.ln_c = K if mode == _lib.EPI_F16_LN else 0
     ep.ln_shift = ptr(ln_shift).value if ln_shift is not None else None
     ep.ln_mean_out = ptr(ln_mean_out).value if ln_mean_out is not None else None
-    ep.a_scale = ptr(a_scale).value if a_scale is not None else None
-    ep.a_scale_ld = a_scale.stride(0) if a_scale is not None else 0
     ep.resid = ptr(resid).value if resid is not None else None
     ep.ldr = resid.shape[-1] if resid is not None else 0
     ep.alpha = alpha

@@ -31,7 +31,7 @@ def test_ctypes_table_mirrors_header():
     from paella_b200 import _lib
     assert sorted(_lib.SIGNATURES) == _header_functions()
     l = _lib.lib()
-    assert l.pb200_abi_version() == 3
+    assert l.pb200_abi_version() == 4
     assert l.pb200_last_error() is not None
 
 
@@ -113,15 +113,15 @@ def test_gemm_tile_plan_on_a_148_sm_part():
     L = _lib.lib()
 
     def plan(m, n, k, sms=148):
-        bn, two, tail = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        _lib.check(L.pb200_gemm_plan(m, n, k, sms, ctypes.byref(bn), ctypes.byref(two), ctypes.byref(tail)), "gemm_plan")
-        return bn.value, two.value, tail.value
-    assert plan(8192, 1280, 5120) == (256, 0, 0)
-    assert plan(8192, 1280, 1280) == (256, 0, 0)
-    assert plan(8192, 5120, 1280) == (256, 0, 0)
-    assert plan(8192, 3840, 1280) == (256, 0, 0)
-    assert plan(64, 1280, 1280) == (64, 0, 0)
-    assert plan(300, 640, 64) == (64, 0, 0)
+        bn = ctypes.c_int()
+        _lib.check(L.pb200_gemm_plan(m, n, k, sms, ctypes.byref(bn)), "gemm_plan")
+        return bn.value
+    assert plan(8192, 1280, 5120) == 256
+    assert plan(8192, 1280, 1280) == 256
+    assert plan(8192, 5120, 1280) == 256
+    assert plan(8192, 3840, 1280) == 256
+    assert plan(64, 1280, 1280) == 64
+    assert plan(300, 640, 64) == 64
 
 
 def test_gemm_tile_plan_on_a_132_sm_part():
@@ -132,21 +132,20 @@ def test_gemm_tile_plan_on_a_132_sm_part():
     L = _lib.lib()
 
     def plan(m, n, k, sms=132):
-        bn, two, tail = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        _lib.check(L.pb200_gemm_plan(m, n, k, sms, ctypes.byref(bn), ctypes.byref(two), ctypes.byref(tail)), "gemm_plan")
-        return bn.value, two.value, tail.value
+        bn = ctypes.c_int()
+        _lib.check(L.pb200_gemm_plan(m, n, k, sms, ctypes.byref(bn)), "gemm_plan")
+        return bn.value
     # level-1 MLP GEMMs, out-projection and QKV projection: 256-wide tiles
-    assert plan(8192, 1280, 5120) == (256, 0, 0)
-    assert plan(8192, 1280, 1280) == (256, 0, 0)
-    assert plan(8192, 5120, 1280) == (256, 0, 0)
-    assert plan(8192, 3840, 1280) == (256, 0, 0)
+    assert plan(8192, 1280, 5120) == 256
+    assert plan(8192, 1280, 1280) == 256
+    assert plan(8192, 5120, 1280) == 256
+    assert plan(8192, 3840, 1280) == 256
     # a single 128-row tile with a short N: narrow tiles spread it over more SMs
-    assert plan(64, 1280, 1280) == (64, 0, 0)
+    assert plan(64, 1280, 1280) == 64
     # every answer is a legal configuration, on any SM count
     for sms in (148, 132, 66):
         for m, n, k in [(8192, 1280, 5120), (300, 640, 64), (32768, 2560, 640), (2048, 1280, 1280), (12032, 512, 256)]:
-            bn, two, tail = plan(m, n, k, sms)
-            assert bn in (64, 128, 256) and two == 0 and tail == 0
+            assert plan(m, n, k, sms) in (64, 128, 256)
 
 
 def test_product_never_imports_oracle():

@@ -2,8 +2,8 @@
 do not depend on the batch it runs in, on the default model, with the GEMM planner free to pick its tile widths.
 
   * GEMM: PB200_EPI_RESID_LN_INV_F32 at BLOCK_N 64, 128 and 256 (one child process per width: PB200_FORCE_BN is read once
-    per process) gives bit-identical out, out16 and ln_stat across the widths and at any row offset of a larger M, with and
-    without a_scale; out and out16 equal RESID_LN's; every element within an fp64 bound
+    per process) gives bit-identical out, out16 and ln_stat across the widths and at any row offset of a larger M; out and
+    out16 equal RESID_LN's; every element within an fp64 bound
   * forward: the default model's features of a sample alone vs inside batches of 2, 5 and 64 (32x32, 64x64, 48x48; CFG pairs
     or not; mixed conditioning lengths), torch.equal with the mode on, while the planner picks several widths; the same run
     with the mode off differs
@@ -55,8 +55,8 @@ def default_model():
 
 
 # ------------------------------------------------------------------ 1. GEMM epilogue, every width
-M_SMALL, M_BIG, N, K, P = 64, 1000, 1000, 640, 64       # N % 32 == 8: a partial last chunk; K % 64 == 0 for a_scale
-OFF_PLAIN, OFF_SCALE = 200, 3 * P                        # row offset of the embedded problem (a_scale: a whole sample)
+M_SMALL, M_BIG, N, K, P = 64, 1000, 1000, 640, 64       # N % 32 == 8: a partial last chunk
+OFF = 200                                                # row offset of the embedded problem
 
 
 def _gemm_inputs():
@@ -66,45 +66,35 @@ def _gemm_inputs():
     bias = torch.randn(N, generator=g) * 0.1
     resid = torch.randn(M_SMALL, N, generator=g) + 3.0                 # an offset the shift removes
     shift = resid.mean(1) + 0.01 * torch.randn(M_SMALL, generator=g)
-    s = (1.0 + 0.2 * torch.randn(M_BIG // P + 1, K, generator=g)).half()
     filler = (torch.randn(M_BIG, K, generator=g) * 0.5).half()
     filler_r = torch.randn(M_BIG, N, generator=g)
-    return a, w, bias, resid, shift, s, filler, filler_r
+    return a, w, bias, resid, shift, filler, filler_r
 
 
-def _gemm_run(mode, ascale, big):
+def _gemm_run(mode, big):
     from paella_b200 import ops
-    a, w, bias, resid, shift, s, filler, filler_r = [t.to(DEV) for t in _gemm_inputs()]
-    off = (OFF_SCALE if ascale else OFF_PLAIN) if big else 0
+    a, w, bias, resid, shift, filler, filler_r = [t.to(DEV) for t in _gemm_inputs()]
+    off = OFF if big else 0
     M = M_BIG if big else M_SMALL
     A, R, SH = filler.clone()[:M], filler_r.clone()[:M], torch.zeros(M, device=DEV)
     A[off:off + M_SMALL], R[off:off + M_SMALL], SH[off:off + M_SMALL] = a, resid, shift
-    scale = None
-    if ascale:
-        scale = s.clone()
-        if not big:
-            scale = s[OFF_SCALE // P:OFF_SCALE // P + 1].contiguous()     # the embedded sample's own factors
     out16 = torch.empty(M, N, dtype=torch.float16, device=DEV)
     stat = torch.zeros(M, 2, dtype=torch.int64, device=DEV)
     x = R.clone()
-    ops.gemm_f16(A.contiguous(), w, mode, x, bias=bias, resid=x, out16=out16, ln_stat=stat, ln_shift=SH, a_scale=scale,
-                 rows_per_sample=P)
+    ops.gemm_f16(A.contiguous(), w, mode, x, bias=bias, resid=x, out16=out16, ln_stat=stat, ln_shift=SH, rows_per_sample=P)
     sl = slice(off, off + M_SMALL)
     return x[sl].cpu(), out16[sl].cpu(), stat[sl].cpu()
 
 
 def _gemm_child(path):
-    """Every case at this process's width (PB200_FORCE_BN): {(mode, ascale, big): (out, out16, ln_stat)}."""
-    res = {(mode, ascale, big): _gemm_run(mode, ascale, big)
-           for mode in (EPI_RESID_LN, EPI_RESID_LN_INV) for ascale in (False, True) for big in (False, True)}
+    """Every case at this process's width (PB200_FORCE_BN): {(mode, big): (out, out16, ln_stat)}."""
+    res = {(mode, big): _gemm_run(mode, big) for mode in (EPI_RESID_LN, EPI_RESID_LN_INV) for big in (False, True)}
     torch.cuda.synchronize()
     torch.save(res, path)
 
 
-def _check_fp64_bound(out, out16, stat, ascale):
-    a, w, bias, resid, shift, s, _, _ = _gemm_inputs()
-    if ascale:
-        a = (a.to(DEV) * s[OFF_SCALE // P].to(DEV)).cpu()         # the fp16 product the kernel forms in shared memory
+def _check_fp64_bound(out, out16, stat):
+    a, w, bias, resid, shift, _, _ = _gemm_inputs()
     a64, w64 = a.double(), w.double()
     acc = a64 @ w64.T
     absacc = a64.abs() @ w64.abs().T
@@ -137,21 +127,19 @@ def test_inv_epilogue_is_width_and_offset_invariant_at_every_width():
                                text=True, timeout=900, cwd=os.path.dirname(HERE))
             assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-3000:]
             res[bn] = torch.load(path)
-    for ascale in (False, True):
-        ref = res[64][(EPI_RESID_LN_INV, ascale, False)]
-        for bn in (64, 128, 256):
-            for big in (False, True):
-                got = res[bn][(EPI_RESID_LN_INV, ascale, big)]
-                for name, x, y in zip(("out", "out16", "ln_stat"), got, ref):
-                    assert torch.equal(x, y), f"BLOCK_N {bn}, a_scale {ascale}, embedded {big}: {name} differs from BLOCK_N 64 alone"
-            # the fp32 output and its fp16 copy are RESID_LN's; only the statistic's summation differs
-            plain = res[bn][(EPI_RESID_LN, ascale, False)]
-            assert torch.equal(plain[0], ref[0]) and torch.equal(plain[1], ref[1])
-        worst = _check_fp64_bound(*ref, ascale)
-        # the default epilogue's statistic does depend on the width (the reason for the INV mode)
-        differs = any(not torch.equal(res[bn][(EPI_RESID_LN, ascale, False)][2], res[64][(EPI_RESID_LN, ascale, False)][2])
-                      for bn in (128, 256))
-        _log({"test": "inv_epilogue", "a_scale": ascale, "worst_err_over_bound": worst, "resid_ln_stat_differs_across_widths": differs})
+    ref = res[64][(EPI_RESID_LN_INV, False)]
+    for bn in (64, 128, 256):
+        for big in (False, True):
+            got = res[bn][(EPI_RESID_LN_INV, big)]
+            for name, x, y in zip(("out", "out16", "ln_stat"), got, ref):
+                assert torch.equal(x, y), f"BLOCK_N {bn}, embedded {big}: {name} differs from BLOCK_N 64 alone"
+        # the fp32 output and its fp16 copy are RESID_LN's; only the statistic's summation differs
+        plain = res[bn][(EPI_RESID_LN, False)]
+        assert torch.equal(plain[0], ref[0]) and torch.equal(plain[1], ref[1])
+    worst = _check_fp64_bound(*ref)
+    # the default epilogue's statistic does depend on the width (the reason for the INV mode)
+    differs = any(not torch.equal(res[bn][(EPI_RESID_LN, False)][2], res[64][(EPI_RESID_LN, False)][2]) for bn in (128, 256))
+    _log({"test": "inv_epilogue", "worst_err_over_bound": worst, "resid_ln_stat_differs_across_widths": differs})
 
 
 # ------------------------------------------------------------------ 2. forward, default model, planner free
@@ -175,8 +163,8 @@ def _planned_widths(m, hw, batches):
             if "A" not in kinds:
                 continue
             Mr = B * ((hw // 2) >> lvl) ** 2
-            bn, two, tail = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-            assert lib().pb200_gemm_plan(Mr, ch, 4 * ch, 0, ctypes.byref(bn), ctypes.byref(two), ctypes.byref(tail)) == 0
+            bn = ctypes.c_int()
+            assert lib().pb200_gemm_plan(Mr, ch, 4 * ch, 0, ctypes.byref(bn)) == 0
             widths.add(bn.value)
     return widths
 

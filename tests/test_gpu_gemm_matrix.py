@@ -1,6 +1,6 @@
 """Every instantiation of the wgmma GEMM (csrc/gemm.cu) against an fp64 reference, not only the tile widths the planner picks.
 
-The kernel is instantiated per (BLOCK_N in {64, 128, 256}, epilogue, A mode, a_scale).  PB200_FORCE_BN (read once per process)
+The kernel is instantiated per (BLOCK_N in {64, 128, 256}, epilogue, A mode).  PB200_FORCE_BN (read once per process)
 pins the width, so each width runs in a child process; the planner's own choice runs in-process.  Every case calls
 pb200_gemm_f16 through the C ABI with leading dimensions and base offsets that differ from the dense values, puts every output
 inside a larger buffer prefilled with a sentinel bit pattern, and checks:
@@ -11,8 +11,7 @@ inside a larger buffer prefilled with a sentinel bit pattern, and checks:
     least SENS_MIN times its bound (computed from the fp64 data, so loosening TAU until the test means nothing fails here);
   * bit for bit, that nothing outside the logical outputs changed and that no sentinel is left inside them;
   * the GRN statistic (sqsum), the LayerNorm statistics (ln_stat, ln_mean_out) and the fp16 copy (out16) likewise;
-  * a_scale: bit-equality with the same kernel on the pre-scaled A;  GELU + sqsum and RESID_LN: a second launch gives
-    bit-identical statistics (integer atomics);
+  * GELU + sqsum and RESID_LN: a second launch gives bit-identical statistics (integer atomics);
   * the im2col-free conv A modes 1 and 2 through the f4 codec against the CPU oracle (latents 2e-3, decode 1e-3).
 One row per case (width, mode, error/bound, sensitivity) is appended to gemm_matrix.jsonl in $PB200_TEST_LOG_DIR (see
 helpers.log_jsonl).
@@ -46,7 +45,7 @@ U32, U16 = 2.0 ** -24, 2.0 ** -11
 
 MULTI_WAVE_M = 132 * 128 + 37            # 133 row tiles: every CTA walks several units and the stage ring wraps across tiles
 WIDTHS = ("plan", 64, 128, 256)
-STAGES = {64: 8, 128: 6, 256: 4}         # GemmSmem<BLOCK_N>::STAGES without a_scale (K = 1000 has 16 k-blocks)
+STAGES = {64: 8, 128: 6, 256: 4}         # GemmSmem<BLOCK_N>::STAGES (K = 1000 has 16 k-blocks)
 MODES = {"F16": 0, "F32": 1, "GELU": 2, "RESID": 3, "UNPATCH": 4, "NCHW": 5, "RESID_LN": 6, "F16_LN": 7}
 SENTINEL = {torch.float32: (torch.int32, 0x7FC0DEAD), torch.float16: (torch.int16, 0x7E5A),
             torch.int64: (torch.int64, 0x5EE55EE55EE55EE5)}
@@ -89,11 +88,6 @@ def _cases(width):
     for hw, B in ((45, 3), (100, 170), (7, 1), (33, 4)):
         for N, K in ((Ns[1], 72), (Ns[4], 1000), (Ns[5], 40), (Ns[0], 64)):
             add("NCHW", B * hw, N, K, P=hw, nobias=N == Ns[4])
-    # GlobalResponseNorm folded into A: K % 64 == 0, samples of 16..256 rows, a_scale_ld > K
-    for mode in ("RESID", "RESID_LN"):
-        for P, M, K in ((16, 1000, 576), (64, 129, 64), (128, 300, 1024), (256, 700, 128), (64, MULTI_WAVE_M, 640)):
-            add(mode, M, bn + 8 if P != 128 else 3 * bn + 8, K, ascale=P, alias=P == 64, film=P if P == 16 else None,
-                shift=mode == "RESID_LN" and P >= 128)
     if width != "plan":
         cases += [dict(id="CONV-24x36", mode="CONV", geom=(3, 24, 36)), dict(id="CONV-256x200", mode="CONV", geom=(1, 256, 200))]
     ids = [c["id"] for c in cases]
@@ -191,7 +185,7 @@ def _epilogue64(s, acc):
 
 
 def _reference(s):
-    a64, w64 = s["a_eff"].double(), s["w"].double()
+    a64, w64 = s["a"].double(), s["w"].double()
     K = a64.shape[1]
     acc = a64 @ w64.t()
     sabs = a64.abs() @ w64.abs().t()
@@ -231,14 +225,13 @@ def _make(c):
         row_offset = torch.randn(M, 1, device=DEV, generator=gen) * 0.5 + 0.3
     s["a_buf"], s["a"] = _operand(M, K, s["lda"], 8 * (1 + seed % 4), gen, row_offset=row_offset)
     s["w_buf"], s["w"] = _operand(N, K, s["ldw"], 8 * (1 + (seed >> 5) % 3), gen, scale=1.0 / math.sqrt(K))
-    s["a_eff"] = s["a"]
     s["alpha"] = c.get("alpha", 1.0)
     ep = dict(mode=MODES[mode], alpha=s["alpha"])
     bias = None if c.get("nobias") else torch.randn(N, device=DEV, generator=gen) * 0.5
     s["bias"], s["bias64"] = bias, (bias.double() if bias is not None else None)
     ep["bias"] = bias.data_ptr() if bias is not None else None
     s["out_dtype"] = torch.float16 if mode in ("F16", "GELU", "F16_LN") else torch.float32
-    P = c.get("P") or c.get("film") or c.get("ascale") or 0
+    P = c.get("P") or c.get("film") or 0
     ep["rows_per_sample"] = P
     s["film64"], s["resid64"] = None, None
     guards = {}
@@ -299,17 +292,6 @@ def _make(c):
             rs = torch.arange(M, device=DEV) // Pf
             s["film64"] = (film[rs, off:off + N].double(), film[rs, off + N:off + 2 * N].double())
             ep.update(film=film.data_ptr(), film_ld=fld, film_off=off)
-        if c.get("ascale"):
-            Pa = c["ascale"]
-            ns = (M + Pa - 1) // Pa
-            sld = K + 8 * (1 + seed % 3)
-            sb = torch.full((ns * sld + 8,), float("nan"), dtype=torch.float16, device=DEV)
-            sv = sb[:ns * sld].view(ns, sld)[:, :K]
-            sv.copy_((1.0 + 0.5 * torch.randn(ns, K, device=DEV, generator=gen)).half())
-            s["ascale_buf"], s["ascale"] = sb, sv
-            rs = torch.arange(M, device=DEV) // Pa
-            s["a_eff"] = (s["a"].float() * sv.float()[rs]).half()       # HMUL2: one rounding of the exact product
-            ep.update(a_scale=sb.data_ptr(), a_scale_ld=sld)
     if mode == "RESID_LN":
         # out16 is indexed with the fp32 output's ldo
         o16 = _Guarded(torch.float16, M * ep["ldo"], 2 * ep["ldo"] + 16, 2 * ep["ldo"] + 3)
@@ -361,7 +343,7 @@ def _check(s, width):
     got = out.at(idx).double()
     assert bool(torch.isfinite(got).all()), "non-finite output"
     ratio = float(((got - s["ref"]).abs() / s["bound"]).max())
-    row = dict(width=width, mode=mode, a_scale=bool(s["ep"].get("a_scale")), amode=0, M=M, N=N, K=s["K"],
+    row = dict(width=width, mode=mode, amode=0, M=M, N=N, K=s["K"],
                err_over_bound=ratio, sensitivity=s["sens"], case=s["id"])
     if width == "plan":
         row["block_n"] = _plan(M, N, s["K"], 0)
@@ -417,13 +399,6 @@ def _run_case(c, width):
     _launch(s)
     first = {name: g.bits.clone() for name, (g, _, _) in s["guards"].items()}
     row = _check(s, width)
-    if c.get("ascale"):
-        # the same kernel width on the pre-scaled A: identical MMAs and accumulation order -> identical bits
-        a_pre = s["a_eff"].contiguous()
-        again = _relaunch(s, initial, a=a_pre, lda=s["K"], ep=dict(s["ep"], a_scale=None, a_scale_ld=0))
-        for name in first:
-            assert torch.equal(again[name], first[name]), f"a_scale: {name} differs from the kernel on the pre-scaled A"
-        row["prescaled_bit_equal"] = True
     if c.get("det"):
         again = _relaunch(s, initial)
         for name in ("sqsum", "ln_stat"):
@@ -435,8 +410,8 @@ def _run_case(c, width):
 
 def _plan(M, N, K, sms=132):
     from paella_b200 import _lib
-    bn, two, tail = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    _lib.check(_lib.lib().pb200_gemm_plan(M, N, K, sms, ctypes.byref(bn), ctypes.byref(two), ctypes.byref(tail)), "gemm_plan")
+    bn = ctypes.c_int()
+    _lib.check(_lib.lib().pb200_gemm_plan(M, N, K, sms, ctypes.byref(bn)), "gemm_plan")
     return bn.value
 
 
@@ -491,9 +466,9 @@ def _run_conv(c, width):
     dec = m.decode_indices(d["idx"].to(DEV)).cpu()
     lat_r = float((lat - d["lat"]).abs().max()) / CONV_LAT_BOUND
     dec_r = float((dec - d["dec"]).abs().max()) / CONV_DEC_BOUND
-    rows = [dict(width=width, mode="F32", a_scale=False, amode=1, M=B * (H // 4) * (W // 4), case=c["id"],
+    rows = [dict(width=width, mode="F32", amode=1, M=B * (H // 4) * (W // 4), case=c["id"],
                  err_over_bound=lat_r, sensitivity=d["lat_sens"]),
-            dict(width=width, mode="F32", a_scale=False, amode=2, M=B * H * W // 4, case=c["id"],
+            dict(width=width, mode="F32", amode=2, M=B * H * W // 4, case=c["id"],
                  err_over_bound=dec_r, sensitivity=d["dec_sens"])]
     rows[0]["lat_max_abs"], rows[1]["dec_max_abs"] = lat_r * CONV_LAT_BOUND, dec_r * CONV_DEC_BOUND
     for r in rows:

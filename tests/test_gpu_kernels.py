@@ -257,67 +257,6 @@ def test_gemm_resid_film_inplace(M, N, K, P):
     assert err < 1e-4
 
 
-@pytest.mark.parametrize("M,N,K,P", [(8192, 1280, 5120, 64), (2048, 1280, 5120, 16), (8256, 1280, 640, 64), (16384, 1280, 5120, 256),
-                                     (8192, 1280, 5120, 128), (8192, 1280, 5120, 32)])
-def test_gemm_a_scale_equals_gemm_on_prescaled_a(M, N, K, P):
-    """GlobalResponseNorm folded into GEMM2's A operand (pb200_gemm_epilogue::a_scale): multiplying the A tile by the
-    per-(sample, k) fp16 factors in shared memory (one HMUL2 rounding, = the fp16 product) must give EXACTLY what the same
-    kernel gives on an A matrix pre-multiplied the same way -- same MMAs, same accumulation order.  Shapes: the level-1 / level-2
-    MLP GEMM2 of the bench, a ragged last tile, samples spanning two tiles, one and four samples per 128-row tile."""
-    from paella_b200 import _lib
-    ops = _ops()
-    g = torch.Generator(device=DEV).manual_seed(21)
-    a = torch.randn(M, K, device=DEV, generator=g).half()
-    w = (torch.randn(N, K, device=DEV, generator=g) / math.sqrt(K)).half()
-    bias = torch.randn(N, device=DEV, generator=g)
-    x = torch.randn(M, N, device=DEV, generator=g)
-    B = (M + P - 1) // P
-    s = (1.0 + 0.5 * torch.randn(B, K, device=DEV, generator=g)).half()
-    rows = torch.arange(M, device=DEV) // P
-    a_pre = (a.float() * s.float()[rows]).half()              # fp32 product of two fp16 values is exact; one rounding to fp16
-    want = x.clone()
-    ops.gemm_f16(a_pre, w, _lib.EPI_RESID_F32, want, bias=bias, resid=want, rows_per_sample=P)
-    got = x.clone()
-    ops.gemm_f16(a, w, _lib.EPI_RESID_F32, got, bias=bias, resid=got, rows_per_sample=P, a_scale=s)
-    torch.cuda.synchronize()
-    ref = a_pre.float() @ w.float().t() + bias + x
-    _log("gemm_a_scale", {"M": M, "N": N, "K": K, "P": P, "equal": bool(torch.equal(got, want)),
-                          "max_abs_vs_torch": float((got - ref).abs().max())})
-    assert torch.equal(got, want)
-    assert float((got - ref).abs().max()) < 2e-4
-
-
-def test_grn_fold_matches_separate_grn_pass():
-    """Model level: GRN folded into GEMM2 (opt-in PB200_GRN_FOLD=1, child process) vs the separate in-place GRN pass (default):
-    features of the reference-default denoiser agree to fp16-rounding noise (the fold rounds h*s once, the pass rounds
-    h*s + beta once and adds beta through the fp32 bias instead)."""
-    import subprocess, sys
-    code = r"""
-import os, sys, torch
-sys.path.insert(0, %r)
-import bench
-from paella_b200.synth import synthetic_conditioning
-m = bench.build_model(torch.device('cuda'))
-cond, uncond = synthetic_conditioning(4, 16, device='cuda')
-c = m.prepare_conditioning([cond, uncond], (32, 32))
-x = torch.randint(0, 8192, (4, 32, 32), device='cuda', generator=torch.Generator(device='cuda').manual_seed(1))
-r = torch.tensor([0.9, 0.6, 0.3, 0.1], device='cuda')
-f = m.features(x, r, c, cfg_pairs=True)
-torch.save(f.cpu(), sys.argv[1])
-""" % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    import tempfile
-    outs = []
-    with tempfile.TemporaryDirectory() as d:
-        for i, env in enumerate(({"PB200_GRN_FOLD": "1"}, {})):
-            path = os.path.join(d, f"f{i}.pt")
-            r = subprocess.run([sys.executable, "-c", code, path], capture_output=True, text=True, env=dict(os.environ, **env))
-            assert r.returncode == 0, r.stderr[-3000:]
-            outs.append(torch.load(path))
-    d = outs[0] - outs[1]
-    _log("grn_fold_vs_pass", {"max_abs": float(d.abs().max()), "rms": float(d.pow(2).mean().sqrt()), "feat_rms": float(outs[1].pow(2).mean().sqrt())})
-    assert float(d.abs().max()) < 2e-2 and float(d.pow(2).mean().sqrt()) < 2e-3          # LayerNorm'd features are O(1)
-
-
 @pytest.mark.parametrize("M,C,N,P", [(8192, 1280, 3840, 64), (1024, 128, 384, 16), (300, 64, 96, 100)])
 def test_gemm_layernorm_folded_across_two_gemms(M, C, N, P):
     """RESID_LN producer (fp32 x, fp16 copy, fixed-point row statistics) + F16_LN consumer:

@@ -75,8 +75,8 @@ def _time_one(M, N, K, mode, P):
 def _plan(M, N, K, sms):
     from paella_b200 import _lib
     L = _lib.lib()
-    bn, two, tail = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-    _lib.check(L.pb200_gemm_plan(M, N, K, sms, ctypes.byref(bn), ctypes.byref(two), ctypes.byref(tail)), "gemm_plan")
+    bn = ctypes.c_int()
+    _lib.check(L.pb200_gemm_plan(M, N, K, sms, ctypes.byref(bn)), "gemm_plan")
     return bn.value
 
 

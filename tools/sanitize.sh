@@ -11,7 +11,7 @@ sys.path.insert(0, os.getcwd()); sys.path.insert(0, os.path.join(os.getcwd(), "t
 from paella_b200 import _lib, ops
 DEV = "cuda"
 g = torch.Generator(device=DEV).manual_seed(0)
-# wgmma GEMMs: every tile width, GELU+sqsum, RESID (+a_scale), LN fold
+# wgmma GEMMs: every tile width, GELU+sqsum, RESID, LN fold
 for (M, N, K) in [(128, 128, 64), (300, 136, 128), (512, 256, 128)]:
     a = torch.randn(M, K, device=DEV, generator=g).half(); w = (torch.randn(N, K, device=DEV, generator=g) / math.sqrt(K)).half()
     bias = torch.randn(N, device=DEV, generator=g)
@@ -19,10 +19,6 @@ for (M, N, K) in [(128, 128, 64), (300, 136, 128), (512, 256, 128)]:
     o16 = torch.zeros(M, N, device=DEV, dtype=torch.float16); sq = torch.zeros(max(1, M // 4), N, device=DEV, dtype=torch.int64)
     ops.gemm_f16(a, w, _lib.EPI_GELU_F16, o16, bias=bias, sqsum=sq, rows_per_sample=4)
     x = torch.randn(M, N, device=DEV, generator=g); ops.gemm_f16(a, w, _lib.EPI_RESID_F32, x, bias=bias, resid=x)
-M, N, K, P = 2048, 1280, 640, 16          # the a_scale path
-a = torch.randn(M, K, device=DEV, generator=g).half(); w = (torch.randn(N, K, device=DEV, generator=g) / math.sqrt(K)).half()
-x = torch.randn(M, N, device=DEV, generator=g); s = (1 + 0.3 * torch.randn(M // P, K, device=DEV, generator=g)).half()
-ops.gemm_f16(a, w, _lib.EPI_RESID_F32, x, bias=None, resid=x, rows_per_sample=P, a_scale=s)
 # attention: wgmma kernel (head_dim 80: shared slots, the last slot read; a weight table) and mma.sync kernel
 import test_gpu_attention_matrix as ta
 for kernel, cid in (("wgmma", "slots-above-B-hd80"), ("wgmma", "table-w_row-shared-hd80"), ("mma", "hd32-P16-S20-varlen-vec5-hd32")):

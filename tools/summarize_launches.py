@@ -25,8 +25,6 @@ def main(src, dst, title):
         m = re.search(r"(gemm_f16(?:_cg2)?_kernel)<(\d+), ?(\d+)(?:, ?(\d+))?", name)
         if m:
             key = f"{m.group(1)}<BN={m.group(2)}, {EPI.get(int(m.group(3)), m.group(3))}" + (f", AMODE={m.group(4)}>" if m.group(4) else ">")
-            if re.search(r"<\d+, ?\d+, ?true>", name):
-                key = key[:-1] + ", A-scale (GRN fold)>"
         else:
             key = re.sub(r"\(.*", "", re.sub(r"<.*", "", name)).replace("void ", "")
         agg[key][0] += 1
