@@ -20,7 +20,8 @@
 extern "C" {
 #endif
 
-#define PB200_ABI_VERSION 4      /* 4: GEMM A-operand scaling and the two always-0 pb200_gemm_plan outputs removed */
+#define PB200_ABI_VERSION 4      /* 4: GEMM A-operand scaling and the two always-0 pb200_gemm_plan outputs removed.
+                                    * Bumped when an entry point changes or goes away; new entry points keep it. */
 
 const char* pb200_last_error(void);
 int pb200_abi_version(void);
@@ -390,6 +391,27 @@ int pb200_paella_sample_tokens_pairs(pb200_paella* m, const float* features, int
 int pb200_paella_sample_tokens_pairs_skip(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
                                           const uint64_t* seed_offset, const int* skip, int64_t* tokens_out, void* workspace,
                                           int64_t workspace_bytes, void* stream);
+
+/* Top-k / top-p truncated draws: pb200_paella_sample_tokens_params and pb200_paella_sample_tokens_pairs_skip with a per-sample
+ * truncation table, top_k DEVICE int32 [batch] and top_p DEVICE float [batch] (both or neither; NULL is exactly the call
+ * without the table, which is what the two functions above are).  For a token of sample b, with s_j = l_j * (1/T) the fp32
+ * product of its guided logit and 1/T:
+ *   top_k[b] = k >= 1: the kept set is {j : s_j >= tau_k}, tau_k the k-th largest s_j counting equal values separately (all
+ *     ties at the boundary are kept); k >= num_labels keeps every label, still through the truncation kernels;
+ *   top_p[b] = p in (0, 1): with w_j = exp(s_j - m) over the top-k kept set (m the row maximum), the kept set is
+ *     {j : s_j >= tau_p}, tau_p the largest kept s_j with sum_{s_i >= tau_p} w_i >= p * sum w_i (boundary ties kept);
+ *   the draw is unchanged: token = argmax over the kept j of (s_j - log q_j), the same Exp(1) variates at the same Philox
+ *     elements as the untruncated call, so excluded labels still consume theirs and a generator advances as without truncation.
+ * 0 and 1.0 are off; the tables are read on the device, so k < 0 and p outside (0, 1] are not diagnosed here (they are off).
+ * Numerics: w_j is fp32 expf (<= 2 ulp) of the fp32 difference, summed as fixed-point floor(2^32 w_j) in 64-bit integers
+ * (order-independent), and the mass test is evaluated in fp64 on those sums.  Truncation applies to the multinomial draw only. */
+int pb200_paella_sample_tokens_params_trunc(pb200_paella* m, const float* features, int batch, int hw, int cfg_on,
+                                            const float* params, uint64_t seed, uint64_t offset, const uint64_t* seed_offset,
+                                            const int* top_k, const float* top_p, int64_t* tokens_out, void* workspace,
+                                            int64_t workspace_bytes, void* stream);
+int pb200_paella_sample_tokens_pairs_trunc(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                                           const uint64_t* seed_offset, const int* skip, const int* top_k, const float* top_p,
+                                           int64_t* tokens_out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* The notebook's non-multinomial sampling modes (paella_inference.ipynb cell 3) for a list of samples of the features of
  * pb200_paella_features_pairs, so that samples in different modes share one forward.  For each listed sample s the call

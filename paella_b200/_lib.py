@@ -119,6 +119,10 @@ SIGNATURES = {
                                                  c_int64, c_void_p]),
     "pb200_paella_sample_tokens_pairs_skip": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                       c_void_p, c_int64, c_void_p]),
+    "pb200_paella_sample_tokens_pairs_trunc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                       c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_sample_tokens_params_trunc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_uint64, c_uint64,
+                                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_resample_workspace_bytes": (c_int64, [c_void_p, c_int, c_int]),
     "pb200_paella_resample_samples": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,
                                               c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),

@@ -882,7 +882,16 @@ int pb200_paella_sample_tokens_per_sample(pb200_paella* m, const float* features
 int pb200_paella_sample_tokens_params(pb200_paella* m, const float* features, int batch, int hw, int cfg_on, const float* params,
                                       uint64_t seed, uint64_t offset, const uint64_t* seed_offset, int64_t* tokens_out,
                                       void* workspace, int64_t workspace_bytes, void* stream) {
+    return pb200_paella_sample_tokens_params_trunc(m, features, batch, hw, cfg_on, params, seed, offset, seed_offset, nullptr, nullptr,
+                                                   tokens_out, workspace, workspace_bytes, stream);
+}
+
+int pb200_paella_sample_tokens_params_trunc(pb200_paella* m, const float* features, int batch, int hw, int cfg_on,
+                                            const float* params, uint64_t seed, uint64_t offset, const uint64_t* seed_offset,
+                                            const int* top_k, const float* top_p, int64_t* tokens_out, void* workspace,
+                                            int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "sample_tokens_params: weights not bound");
+    PB_CHECK((top_k == nullptr) == (top_p == nullptr), "sample_tokens_params: the truncation table needs both top_k and top_p");
     PB_CHECK(params != nullptr, "sample_tokens_params: params is NULL");
     const pb200_paella_config& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -899,7 +908,7 @@ int pb200_paella_sample_tokens_params(pb200_paella* m, const float* features, in
     else
         PB_TRY(launch_cast_f16(features, rows * c.c_out, a16, st));
     return launch_fused_sampler_params(a16, batch, hw, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f, params, seed, offset,
-                                       seed_offset, tokens_out, st);
+                                       seed_offset, tokens_out, st, nullptr, top_k, top_p);
 }
 
 int pb200_paella_sample_tokens_pairs(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
@@ -912,7 +921,15 @@ int pb200_paella_sample_tokens_pairs(pb200_paella* m, const float* features, int
 int pb200_paella_sample_tokens_pairs_skip(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
                                           const uint64_t* seed_offset, const int* skip, int64_t* tokens_out, void* workspace,
                                           int64_t workspace_bytes, void* stream) {
+    return pb200_paella_sample_tokens_pairs_trunc(m, features, batch, n_pairs, hw, params, seed_offset, skip, nullptr, nullptr,
+                                                  tokens_out, workspace, workspace_bytes, stream);
+}
+
+int pb200_paella_sample_tokens_pairs_trunc(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                                           const uint64_t* seed_offset, const int* skip, const int* top_k, const float* top_p,
+                                           int64_t* tokens_out, void* workspace, int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "sample_tokens_pairs: weights not bound");
+    PB_CHECK((top_k == nullptr) == (top_p == nullptr), "sample_tokens_pairs: the truncation table needs both top_k and top_p");
     PB_CHECK(params != nullptr && seed_offset != nullptr, "sample_tokens_pairs: params and seed_offset are required");
     const pb200_paella_config& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -928,7 +945,7 @@ int pb200_paella_sample_tokens_pairs_skip(pb200_paella* m, const float* features
     PB_TRY(launch_mix_cast_rows_f16(features, features + rows * c.c_out, params, (int64_t)hw * c.c_out, mixed, a16, st));
     PB_TRY(launch_cast_f16(features + mixed, rows * c.c_out - mixed, a16 + mixed, st));
     return launch_fused_sampler_params(a16, batch, hw, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f, params, 0, 0,
-                                       seed_offset, tokens_out, st, skip);
+                                       seed_offset, tokens_out, st, skip, top_k, top_p);
 }
 
 // scratch of pb200_paella_resample_samples: fp16 features and fp32 logits of 2 * chunk sample blocks

@@ -17,7 +17,10 @@ int launch_fused_sampler_per_sample(const __half* a16, int64_t n_samp, int64_t h
 // stream per sample, as launch_fused_sampler_per_sample.  params == nullptr: every row uses inv_t.
 // skip (per-sample streams only): DEVICE int32 [n_samp]; a sample with skip[b] != 0 does not draw, its rows of out are not
 // written (and its seed_off entry is not read).  nullptr: every sample draws.
+// top_k / top_p (with params, both or neither): DEVICE int32 [n_samp] and float [n_samp], sample b's top-k and top-p (0 and
+// 1.0 are off; see TruncSmem in sampler.cu); nullptr: the untruncated instances.
 int launch_fused_sampler_params(const __half* a16, int64_t n_samp, int64_t hw, int Kc, const __half* w16, int NL, float inv_t,
                                 const float* params, uint64_t seed, uint64_t offset, const uint64_t* seed_off, int64_t* out,
-                                cudaStream_t st, const int* skip = nullptr);
+                                cudaStream_t st, const int* skip = nullptr, const int* top_k = nullptr,
+                                const float* top_p = nullptr);
 }  // namespace pb

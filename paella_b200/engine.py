@@ -26,7 +26,9 @@ tokens back outside its region (a request without a region has an all-True row).
 ``sampling_quant_steps=k`` (steps i >= k use 'quant'; 'quant' needs the engine's ``vqmodel``) the request's tokens, intermediates
 and generator offset are those of ``sample_notebook(model, inputs, (1, H, W), uncond, init_x, steps, renoise_steps, temperature,
 cfg, mode, t_start, t_end, sampling_conditional_steps, sampling_quant_steps, attn_weights, vqmodel=vq, generator=[g],
-region=region)``: a step in argmax or quant mode draws nothing from ``g`` (only its mask draw, if it renoises).
+region=region)``: a step in argmax or quant mode draws nothing from ``g`` (only its mask draw, if it renoises).  With
+``top_k`` / ``top_p`` a request's multinomial steps are truncated as in ``sample_notebook(..., top_k=k, top_p=p)``; the draws,
+and so the generator offsets, are those of the untruncated request.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -35,7 +37,9 @@ sends it to the device with one asynchronous copy; the step itself is a gather o
 one fused-sampler launch and one per-sample add-noise launch that writes every row back into its slot.  A step whose rows are
 in several sampling modes adds each row's mode to the table: the fused sampler skips the argmax and quant rows, which then go
 through the out_mapper GEMM to logits (a bounded number of samples at a time) and the argmax or quant kernel, one call per mode
-(Paella.sample_tokens_modes).  The host knows which
+(Paella.sample_tokens_modes).  A step in which some request truncates adds each row's (k, p) to the table, and the fused sampler
+reads them there (0 and 1.0 for the rows that do not); a step in which none does launches exactly as without truncation.
+The host knows which
 requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
 in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
 and own unconditional slots alike; the cache rows equal per-request projections bit for bit in either mode.
@@ -61,7 +65,8 @@ class Request:
     def __init__(self, steps: int, renoise_steps: int, cond_steps: int, guided: bool, params: torch.Tensor, r: torch.Tensor,
                  generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False,
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
-                 region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None):
+                 region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
+                 top_k: int = 0, top_p: float = 1.0):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -69,6 +74,7 @@ class Request:
         self.region = region                     # bool [1, H, W] or None, until admission
         self.has_region = region is not None
         self.mode, self.quant_steps = mode, quant_steps      # sampling mode, and the step from which 'quant' is used (or None)
+        self.top_k, self.top_p = top_k, top_p    # the truncation table's row: 0 and 1.0 are off
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -96,6 +102,10 @@ class StepPlan:
         self.renoise = [q.k < q.renoise_steps for q in order]
         self.modes = [q.mode_at(q.k) for q in order]
         self.draws = [md == "multinomial" for md in self.modes]     # only multinomial rows draw the sampler's exponentials
+        # the truncation table, when a row that draws truncates (otherwise the step launches without one)
+        self.truncates = any(dr and (q.top_k > 0 or q.top_p < 1.0) for q, dr in zip(order, self.draws))
+        self.top_k = torch.tensor([q.top_k for q in order], dtype=torch.int32)
+        self.top_p = torch.tensor([q.top_p for q in order], dtype=torch.float32)
         # a row that does not renoise keeps its tokens (t < 0 never passes the mask test)
         self.t_next = torch.stack([q.r[q.k + 1] if rn else torch.tensor(-1.0) for q, rn in zip(order, self.renoise)])
         self.row_slot = torch.tensor([q.slot for q in order], dtype=torch.int32)
@@ -121,6 +131,35 @@ def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List
         else:
             runs.append([i])
     return runs
+
+
+def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tuple[torch.Tensor, Dict[str, Tuple[str, int, int]]]:
+    """The step's one host-to-device buffer: int64 [(seed, offset) pairs of the sampler's draw, then of the mask draw], then the
+    float32 part [r, params (3 per row), t_next, (top_p)], then the int32 part [row_slot, kv_slot, (mode table), (top_k)], each
+    part padded to whole int64 words.  top_p / top_k are present only when ``plan.truncates``, the mode table only when the step
+    mixes modes.  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
+    Bc, n_pairs = len(plan.order), plan.n_pairs
+    mixed = not all(plan.draws)
+    modes = ops.mode_table(plan.modes) if mixed else torch.zeros(0, dtype=torch.int32)
+    f32_parts = [("r", plan.r), ("params", plan.params.view(-1)), ("t_next", plan.t_next)]
+    i32_parts = [("row_slot", plan.row_slot), ("kv_slot", plan.kv_slot), ("modes", modes)]
+    if plan.truncates:
+        f32_parts.append(("top_p", plan.top_p))
+        i32_parts.append(("top_k", plan.top_k))
+    layout: Dict[str, Tuple[str, int, int]] = {}
+    for dt, parts in (("f32", f32_parts), ("i32", i32_parts)):
+        o = 0
+        for name, v in parts:
+            layout[name] = (dt, o, v.numel())
+            o += v.numel()
+    f32 = torch.cat([v for _, v in f32_parts])
+    i32 = torch.cat([v for _, v in i32_parts])
+    f32 = torch.cat([f32, torch.zeros(f32.numel() % 2)])
+    i32 = torch.cat([i32, torch.zeros(i32.numel() % 2, dtype=torch.int32)])
+    host = torch.cat([torch.tensor(draw + renoise, dtype=torch.int64), f32.view(torch.int64), i32.view(torch.int64)])
+    layout["f32"] = ("i64", 4 * Bc, f32.numel() // 2)
+    layout["i32"] = ("i64", 4 * Bc + f32.numel() // 2, i32.numel() // 2)
+    return host, layout
 
 
 def _cat_inputs(inputs: List[Dict[str, torch.Tensor]], dev) -> Dict[str, torch.Tensor]:
@@ -211,7 +250,7 @@ class SamplingEngine:
     def submit(self, model_inputs, unconditional_inputs=None, *, generator=None, steps=12, renoise_steps=None,
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
-               sampling_quant_steps=None) -> Request:
+               sampling_quant_steps=None, top_k=None, top_p=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -222,8 +261,9 @@ class SamplingEngine:
         request's conditional forward as in sample_notebook; ``keep_intermediates`` collects sample_notebook's second value in
         ``req.intermediates``; ``region`` inpaints or outpaints init_x as in sample_distributed; ``mode`` and
         ``sampling_quant_steps`` choose each step's sampling mode as in sample_notebook (step k uses 'quant' if
-        k >= sampling_quant_steps, ``mode`` otherwise; 'quant' reads the codebook of the engine's vqmodel).  The request's draws
-        start when it is admitted."""
+        k >= sampling_quant_steps, ``mode`` otherwise; 'quant' reads the codebook of the engine's vqmodel).  ``top_k`` (None or
+        an int >= 0) and ``top_p`` (None or a float in (0, 1]) truncate the request's multinomial steps as in sample_notebook;
+        ValueError for any other value.  The request's draws start when it is admitted."""
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
         g_idx = generator.device.index if generator.device.index is not None else torch.cuda.current_device()
@@ -233,6 +273,10 @@ class SamplingEngine:
             raise ValueError("generator is already used by a request in flight")
         if not isinstance(steps, int) or steps < 1:
             raise ValueError(f"steps={steps!r}: expected an int >= 1")
+        for name, v in (("top_k", top_k), ("top_p", top_p)):
+            if torch.is_tensor(v):
+                raise ValueError(f"{name}: a request takes one value (got a tensor)")
+        trunc = ops.truncation_table(top_k, top_p, 1, self.model.num_labels)
         renoise_steps = steps - 1 if renoise_steps is None else int(renoise_steps)
         cond_steps = steps if sampling_conditional_steps is None else int(sampling_conditional_steps)
         self._check_cond("model_inputs", model_inputs)
@@ -256,7 +300,7 @@ class SamplingEngine:
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
-                      sampling_quant_steps)
+                      sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)))
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
@@ -328,17 +372,18 @@ class SamplingEngine:
                 draw += ops.philox_values([q.generator], hw * m.num_labels, dev) if dr else [0, 0]
                 renoise += ops.philox_values([q.generator], hw, dev) if rn else [0, 0]
             mixed = not all(plan.draws)
-            modes = ops.mode_table(plan.modes) if mixed else torch.zeros(0, dtype=torch.int32)
-            f32 = torch.cat([plan.r, plan.params.view(-1), plan.t_next] + ([torch.zeros(1)] if Bc % 2 else []))
-            i32 = torch.cat([plan.row_slot, plan.kv_slot, modes] + ([torch.zeros(1, dtype=torch.int32)] if (n_pairs + modes.numel()) % 2 else []))
-            host = torch.cat([torch.tensor(draw + renoise, dtype=torch.int64), f32.view(torch.int64), i32.view(torch.int64)])
+            host, lay = step_host_table(plan, draw, renoise)
             buf = ops.to_device_async(host, dev)                 # the step's one host-to-device copy
             draw_d, renoise_d = buf[:2 * Bc].view(Bc, 2), buf[2 * Bc:4 * Bc].view(Bc, 2)
-            f32_d = buf[4 * Bc:4 * Bc + f32.numel() // 2].view(torch.float32)
-            i32_d = buf[4 * Bc + f32.numel() // 2:].view(torch.int32)
-            r_d, params_d, t_next_d = f32_d[:Bc], f32_d[Bc:4 * Bc].view(Bc, 3), f32_d[4 * Bc:5 * Bc]
-            row_slot_d, kv_slot_d = i32_d[:Bc], i32_d[Bc:2 * Bc + n_pairs]
-            modes_d = i32_d[2 * Bc + n_pairs:2 * Bc + n_pairs + modes.numel()]
+            parts = {"f32": buf[lay["f32"][1]:lay["f32"][1] + lay["f32"][2]].view(torch.float32),
+                     "i32": buf[lay["i32"][1]:lay["i32"][1] + lay["i32"][2]].view(torch.int32)}
+
+            def part(name):
+                dt, o, n = lay[name]
+                return parts[dt][o:o + n]
+            r_d, params_d, t_next_d = part("r"), part("params").view(Bc, 3), part("t_next")
+            row_slot_d, kv_slot_d, modes_d = part("row_slot"), part("kv_slot"), part("modes")
+            trunc_d = (part("top_k"), part("top_p")) if plan.truncates else None
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_pairs, self.s_max, self.n_slots, kv_slot_d)
@@ -348,9 +393,9 @@ class SamplingEngine:
                 feats = m.features(x, r_d, cond, n_pairs=n_pairs)
             if mixed:       # argmax and quant rows through the logits path, the multinomial rows in one fused-sampler launch
                 sampled = m.sample_tokens_modes(feats, Bc, n_pairs, H, W, params_d, draw_d, plan.modes, modes_d, self._codebook(),
-                                                out=self._sampled[:Bc])
+                                                out=self._sampled[:Bc], trunc=trunc_d)
             else:
-                sampled = m.sample_tokens_pairs(feats, Bc, n_pairs, H, W, params_d, draw_d, out=self._sampled[:Bc])
+                sampled = m.sample_tokens_pairs(feats, Bc, n_pairs, H, W, params_d, draw_d, out=self._sampled[:Bc], trunc=trunc_d)
             for i, q in enumerate(plan.order):
                 if q.intermediates is not None:
                     s = q.slot

@@ -724,10 +724,13 @@ class Paella(nn.Module):
         return out
 
     def sample_tokens_params(self, feats: torch.Tensor, batch: int, h: int, w: int, cfg_on: bool, params: torch.Tensor,
-                             generator=None) -> torch.Tensor:
+                             generator=None, trunc=None) -> torch.Tensor:
         """sample_tokens with per-sample guidance scale and temperature in one launch over the batch (per random stream):
         ``params`` is a device float32 [batch, 3] of (cfg, 1 - cfg, 1/T) (ops.sampling_params_table); its cfg columns are
-        ignored when ``cfg_on`` is False.  Draws on ``generator`` exactly as sample_tokens does."""
+        ignored when ``cfg_on`` is False.  Draws on ``generator`` exactly as sample_tokens does.  ``trunc``: None, or the
+        device truncation table (int32 k [batch], float32 p [batch]) of ops.truncation_table: sample b's draw keeps its top-k /
+        top-p codes (pb200_paella_sample_tokens_params_trunc), on the same random draws."""
+        tk, tp = trunc if trunc is not None else (None, None)
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -739,9 +742,9 @@ class Paella(nn.Module):
                 ops.check_generators(generator, batch, dev)
                 ops.check_per_sample_numel(hw * self.num_labels)
                 table = ops.philox_table(generator, hw * self.num_labels, dev)
-                check(L.pb200_paella_sample_tokens_params(self._handle, ptr(feats), batch, hw, int(cfg_on), ptr(params), 0, 0,
-                                                          ptr(table), ptr(out), ptr(ws), ws.numel(), current_stream()),
-                      "pb200_paella_sample_tokens_params")
+                check(L.pb200_paella_sample_tokens_params_trunc(self._handle, ptr(feats), batch, hw, int(cfg_on), ptr(params), 0, 0,
+                                                                ptr(table), ptr(tk), ptr(tp), ptr(out), ptr(ws), ws.numel(),
+                                                                current_stream()), "pb200_paella_sample_tokens_params_trunc")
                 return out
             n = batch * hw
             chunks = ops.philox_row_chunks(n, self.num_labels)       # one kernel per 32-bit-indexable piece, like torch
@@ -758,16 +761,19 @@ class Paella(nn.Module):
                     f = torch.cat([feats[lo:hi], feats[n + lo:n + hi]])
                 else:
                     f = feats[lo:hi]
-                check(L.pb200_paella_sample_tokens_params(self._handle, ptr(f), (hi - lo) // hw, hw, int(cfg_on),
-                                                          ptr(params[lo // hw:hi // hw]), seed, off, None, ptr(flat[lo:hi]), ptr(ws),
-                                                          ws.numel(), current_stream()), "pb200_paella_sample_tokens_params")
+                sl = slice(lo // hw, hi // hw)
+                check(L.pb200_paella_sample_tokens_params_trunc(self._handle, ptr(f), (hi - lo) // hw, hw, int(cfg_on), ptr(params[sl]),
+                                                                seed, off, None, ptr(tk[sl] if tk is not None else None),
+                                                                ptr(tp[sl] if tp is not None else None), ptr(flat[lo:hi]), ptr(ws),
+                                                                ws.numel(), current_stream()), "pb200_paella_sample_tokens_params_trunc")
         return out
 
     def sample_tokens_pairs(self, feats: torch.Tensor, batch: int, n_pairs: int, h: int, w: int, params: torch.Tensor,
-                            seed_offset: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                            seed_offset: torch.Tensor, out: Optional[torch.Tensor] = None, trunc=None) -> torch.Tensor:
         """sample_tokens_params on the features of ``features(..., n_pairs=n_pairs)``: samples b < n_pairs are guided, the rest
         draw on their conditional rows alone, all in one launch on per-sample streams (``seed_offset``: ops.philox_table over
-        h * w * num_labels)."""
+        h * w * num_labels).  ``trunc`` as in sample_tokens_params."""
+        tk, tp = trunc if trunc is not None else (None, None)
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -775,9 +781,9 @@ class Paella(nn.Module):
             if out is None:
                 out = torch.empty(batch, h, w, dtype=torch.int64, device=dev)
             ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, batch, h, w, 1))
-            check(L.pb200_paella_sample_tokens_pairs(self._handle, ptr(feats), batch, n_pairs, h * w, ptr(params), ptr(seed_offset),
-                                                     ptr(out), ptr(ws), ws.numel(), current_stream()),
-                  "pb200_paella_sample_tokens_pairs")
+            check(L.pb200_paella_sample_tokens_pairs_trunc(self._handle, ptr(feats), batch, n_pairs, h * w, ptr(params), ptr(seed_offset),
+                                                           None, ptr(tk), ptr(tp), ptr(out), ptr(ws), ws.numel(), current_stream()),
+                  "pb200_paella_sample_tokens_pairs_trunc")
         return out
 
     def resample_workspace_bytes(self, hw: int, chunk: int = ops.RESAMPLE_CHUNK) -> int:
@@ -787,13 +793,15 @@ class Paella(nn.Module):
 
     def sample_tokens_modes(self, feats: torch.Tensor, batch: int, n_pairs: int, h: int, w: int, params: torch.Tensor,
                             seed_offset: torch.Tensor, modes: Sequence[str], table: torch.Tensor, codebook: Optional[torch.Tensor] = None,
-                            out: Optional[torch.Tensor] = None, chunk: int = ops.RESAMPLE_CHUNK) -> torch.Tensor:
+                            out: Optional[torch.Tensor] = None, chunk: int = ops.RESAMPLE_CHUNK, trunc=None) -> torch.Tensor:
         """sample_tokens_pairs with a sampling mode per sample (``modes``: batch names of ops.SAMPLING_MODES; ``table``: their
         ops.mode_table on the device).  The multinomial samples draw in one fused-sampler launch, the others skipped through the
         table's codes (their ``seed_offset`` rows are not read); then each other mode present runs pb200_paella_resample_samples
         over its samples: the out_mapper GEMM to logits, ``chunk`` guided samples at a time, and the argmax or quant kernel,
         which draw nothing.  Sample b's tokens are those of sample_notebook's step in mode b.  ``codebook``: the VQGAN codebook
-        fp32 [num_labels, c_latent], for 'quant'."""
+        fp32 [num_labels, c_latent], for 'quant'.  ``trunc`` (sample_tokens_params) truncates the multinomial samples' draws;
+        the argmax and quant samples ignore it."""
+        tk, tp = trunc if trunc is not None else (None, None)
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -810,9 +818,9 @@ class Paella(nn.Module):
                               L.pb200_paella_resample_workspace_bytes(self._handle, chunk, hw) if count["multinomial"] < batch else 0))
             if count["multinomial"]:
                 skip = table[:batch] if count["multinomial"] < batch else None
-                check(L.pb200_paella_sample_tokens_pairs_skip(self._handle, ptr(feats), batch, n_pairs, hw, ptr(params), ptr(seed_offset),
-                                                              ptr(skip), ptr(out), ptr(ws), ws.numel(), current_stream()),
-                      "pb200_paella_sample_tokens_pairs_skip")
+                check(L.pb200_paella_sample_tokens_pairs_trunc(self._handle, ptr(feats), batch, n_pairs, hw, ptr(params), ptr(seed_offset),
+                                                               ptr(skip), ptr(tk), ptr(tp), ptr(out), ptr(ws), ws.numel(),
+                                                               current_stream()), "pb200_paella_sample_tokens_pairs_trunc")
             off, lists = batch, []
             for code, md in ((1, "argmax"), (2, "quant")):
                 lists.append((code, [b for b, x in enumerate(modes) if x == md], off))

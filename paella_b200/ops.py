@@ -221,6 +221,51 @@ def sampling_params_table(cfg, temperature, batch: int, device) -> torch.Tensor:
     return to_device_async(sampling_params(cfgs, temps), device)
 
 
+# ------------------------------------------------------------------ top-k / top-p truncation
+# The fused sampler keeps, per token, the top-k codes and then the smallest top set holding a fraction top-p of the probability
+# (include/paella_b200.h, pb200_paella_sample_tokens_params_trunc); the draw is otherwise unchanged.  The kernels read a device
+# table of int32 k [B] and float32 p [B], 0 and 1.0 meaning off.
+def _truncation_values(name: str, value, batch: int, is_k: bool) -> list:
+    if value is None:
+        return [None] * batch
+    if torch.is_tensor(value):
+        if value.device.type != "cpu":
+            raise ValueError(f"{name}: per-sample values must be a CPU tensor (got {value.device}; reading it would synchronise the stream)")
+        if tuple(value.shape) != (batch,):
+            raise ValueError(f"{name}: per-sample values of shape {list(value.shape)} for a batch of {batch} (expected [{batch}])")
+        if is_k and (value.is_floating_point() or value.is_complex() or value.dtype == torch.bool):
+            raise ValueError(f"{name}: per-sample values must be an integer tensor (got {value.dtype})")
+        if not is_k and not value.is_floating_point():
+            raise ValueError(f"{name}: per-sample values must be a floating-point tensor (got {value.dtype})")
+        vals = value.tolist()
+    else:
+        if is_k and (isinstance(value, bool) or not isinstance(value, int)):
+            raise ValueError(f"{name}={value!r}: expected None, an int >= 0 or a CPU integer tensor [{batch}]")
+        if not is_k and (isinstance(value, bool) or not isinstance(value, (int, float))):
+            raise ValueError(f"{name}={value!r}: expected None, a float in (0, 1] or a CPU float tensor [{batch}]")
+        vals = [value] * batch
+    for v in vals:
+        if is_k and v < 0:
+            raise ValueError(f"{name}: every k must be >= 0 (0 is off; got {vals})")
+        if not is_k and not 0.0 < v <= 1.0:        # NaN fails this too
+            raise ValueError(f"{name}: every p must be in (0, 1] (1.0 is off; got {vals})")
+    return vals
+
+
+def truncation_table(top_k, top_p, batch: int, num_labels: int) -> Optional[Tuple[torch.Tensor, torch.Tensor]]:
+    """``top_k`` (None, an int >= 0, or a CPU integer tensor [batch]) and ``top_p`` (None, a float in (0, 1], or a CPU float
+    tensor [batch]) as the host truncation table: (int32 k [batch], float32 p [batch]), with k = 0 where the row keeps every
+    code (None, 0 or k >= num_labels) and p = 1.0 where it does (None or 1.0).  None when no row truncates.  ValueError, before
+    anything is enqueued, for a non-integer or negative k, a p <= 0, > 1 or NaN, a CUDA tensor, or a wrong shape."""
+    ks = _truncation_values("top_k", top_k, batch, True)
+    ps = _truncation_values("top_p", top_p, batch, False)
+    k = torch.tensor([0 if v is None or v >= num_labels else int(v) for v in ks], dtype=torch.int32)
+    p = torch.tensor([1.0 if v is None else float(v) for v in ps], dtype=torch.float32)
+    if not bool((k > 0).any()) and not bool((p < 1.0).any()):
+        return None
+    return k, p
+
+
 # ------------------------------------------------------------------ per-sample sampling modes
 # The notebook's sampling modes (paella_inference.ipynb cell 3).  'multinomial' draws H*W*num_labels exponentials per step; 'argmax'
 # and 'quant' draw nothing.  A step with several modes sends one int32 table to the device: the mode code of every sample, then

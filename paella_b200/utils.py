@@ -29,6 +29,12 @@ puts init_x back outside the region after every step's sampling, and renoises on
 are those of the call without a region, so a generator ends at the same offset.  An all-True region is the call without
 init_x, bit for bit; an all-False one returns init_x.  ``token_region`` and ``outpaint_canvas`` build the arguments from a
 pixel mask or from a smaller token grid placed on a larger canvas.
+
+Truncated sampling: ``top_k`` and ``top_p`` (all three functions; None, a scalar, or a CPU tensor [B]) restrict each token's
+multinomial draw to its k most likely codes, then to the smallest top set of them holding a fraction p of the probability
+(ops.truncation_table; pb200_paella_sample_tokens_params_trunc).  The draw uses the same random numbers as without
+truncation, so every generator ends at the same offset and the per-sample guarantees above hold for truncated rows too.
+Argmax and quant steps are not truncated; ``exact=True`` does not take truncation.
 """
 from __future__ import annotations
 
@@ -135,15 +141,19 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
-                 codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None):
+                 codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None):
     """``modes``: None, or per step the list of B mode names (sampling_modes) -- a step whose modes differ samples each row in
-    its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the scalar path in that mode."""
+    its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the scalar path in that mode.  ``top_k`` /
+    ``top_p``: the truncation of the multinomial draws (module docstring); a truncating call takes the per-sample table path."""
     B, H, W = latent_shape
     dev = model._device()
     check_region(region, init_x, latent_shape, dev)
+    trunc = ops.truncation_table(top_k, top_p, B, model.num_labels)
+    if exact and trunc is not None:
+        raise ValueError("exact=True restates the reference op for op, which has no top_k / top_p truncation")
     use_cfg_any = cfgs is not None
     mixed_steps = modes is not None and any(len(set(ms)) > 1 for ms in modes)
-    sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg, always=mixed_steps)
+    sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg, always=mixed_steps or trunc is not None)
     w_table = None
     if isinstance(attn_weights, (list, tuple)):       # per-sample vectors, for the conditional rows only
         w_table = ops.attn_weights_table(attn_weights, B, [model.max_attn_weights((H, W), model.conditioning_seq_len(model_inputs))] * B)
@@ -153,10 +163,11 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     with torch.inference_mode():
         # one copy for the whole loop: [steps][B][3] params and [steps + 1][B] noise levels, and a CPU region
         region_host = region is not None and region.device.type == "cpu"
-        parts = (list(sched) if sched is not None else []) + ([region] if region_host else [])
+        parts = (list(sched) if sched is not None else []) + (list(trunc) if trunc is not None else []) + ([region] if region_host else [])
         parts_d = ops.to_device_packed(parts, dev) if parts else []
         if sched is not None:
             params_d, r_d = parts_d[0], parts_d[1]
+        trunc_d = (parts_d[2], parts_d[3]) if trunc is not None else None
         region_d = None
         if region is not None:       # bool [B, H, W], True where tokens are generated
             region_d = parts_d[-1] if region_host else region.contiguous()
@@ -200,12 +211,12 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 r, params_i = r_d[i], params_d[i]
             feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided, w_len=w_len)
             if step_modes is not None:
-                sampled = _sample_modes_step(model, feats, B, H, W, guided, params_i, step_modes, generator, codebook, dev)
+                sampled = _sample_modes_step(model, feats, B, H, W, guided, params_i, step_modes, generator, codebook, dev, trunc_d)
             elif mode == "multinomial" and not exact:
                 if sched is None:
                     sampled = model.sample_tokens(feats, B, H, W, cfg_i, temp_i, generator)
                 else:
-                    sampled = model.sample_tokens_params(feats, B, H, W, guided, params_i, generator)
+                    sampled = model.sample_tokens_params(feats, B, H, W, guided, params_i, generator, trunc_d)
             else:
                 n = B * H * W
                 lc = model.logits_from_features(feats[:n], B, H, W)
@@ -241,7 +252,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     return sampled, intermediates
 
 
-def _sample_modes_step(model, feats, B, H, W, guided, params, step_modes, generators, codebook, dev):
+def _sample_modes_step(model, feats, B, H, W, guided, params, step_modes, generators, codebook, dev, trunc=None):
     """One step of a batch whose samples are in different modes, on per-sample generators: the multinomial samples draw what
     a batch-1 step draws on their own generators, the others draw nothing.  The draws and the mode table go to the device in
     one asynchronous copy."""
@@ -249,7 +260,7 @@ def _sample_modes_step(model, feats, B, H, W, guided, params, step_modes, genera
     for g, md in zip(generators, step_modes):
         vals += ops.philox_values([g], H * W * model.num_labels, dev) if md == "multinomial" else [0, 0]
     seed_d, table_d = ops.to_device_packed([torch.tensor(vals, dtype=torch.int64).view(-1, 2), ops.mode_table(step_modes)], dev)
-    return model.sample_tokens_modes(feats, B, B if guided else 0, H, W, params, seed_d, step_modes, table_d, codebook)
+    return model.sample_tokens_modes(feats, B, B if guided else 0, H, W, params, seed_d, step_modes, table_d, codebook, trunc=trunc)
 
 
 def sampling_modes(mode, sampling_quant_steps, batch: int, steps: int, generator=None, exact: bool = False, codebook=None):
@@ -315,7 +326,8 @@ def _decode_tail(tokens, decode, decode_output):
 
 
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
-           cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None):
+           cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
+           top_k=None, top_p=None):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -325,7 +337,9 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     ``torch.manual_seed(generator[i].initial_seed())`` (and equals it where the forward is batch-invariant, DESIGN.md §3),
     and leaves generator i where that call leaves the default generator.
     Per-sample settings (module docstring): ``cfg`` [B], ``temperature`` [B, 2], ``t_start`` / ``t_end`` [B].  A per-sample cfg
-    of 0 is unguided like the scalar ``cfg=0``; so is 1.0, and an all-zero tensor makes the whole call unguided."""
+    of 0 is unguided like the scalar ``cfg=0``; so is 1.0, and an all-zero tensor makes the whole call unguided.
+    ``top_k`` / ``top_p`` (module docstring): None, a scalar, or a CPU tensor [B]; ValueError, before anything is enqueued and
+    before any generator advances, for a bad value and for truncation with exact=True."""
     per_sample_cfg = torch.is_tensor(cfg)
     if per_sample_cfg:
         cfg_vals = [v if v else 1.0 for v in ops.per_sample_values("cfg", cfg, latent_shape[0])]   # f*1 + u*0 = f
@@ -337,19 +351,20 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
         raise TypeError("sample(): cfg is set but unconditional_inputs is None")
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, None, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
-                          per_sample_cfg=per_sample_cfg)
+                          per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p)
     return _decode_tail(out, decode, decode_output)
 
 
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
-                       exact=False, generator=None, region=None):
+                       exact=False, generator=None, region=None, top_k=None, top_p=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
     docstring): bool [B, H, W] on the CPU or the model's device, True where tokens are generated; ``init_x`` then holds the
     tokens kept elsewhere.  ValueError, before anything is enqueued and before any generator advances, for a region without
-    init_x, of another shape or dtype, or on another device."""
+    init_x, of another shape or dtype, or on another device.  ``top_k`` / ``top_p`` as in ``sample``; a shard given
+    ``top_k[lo:hi]`` computes what rows [lo, hi) compute."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -357,14 +372,14 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     cfgs = _cfg_schedule(cfg, latent_shape[0], steps)
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
-                          generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region)
+                          generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p)
     return out
 
 
 def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None, init_x=None, steps=12, renoise_steps=None,
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
-                    generator=None, region=None):
+                    generator=None, region=None, top_k=None, top_p=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -376,7 +391,8 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     Per-sample modes: ``mode`` may be a list or tuple of B mode names and ``sampling_quant_steps`` one of B entries, each None
     or an int >= 0; row i then equals row i of the call with mode i and quant step i for every sample, on per-sample
     generators.  A call whose modes differ within a step needs ``generator=[g_0, ..., g_{B-1}]`` (the argmax and quant rows draw
-    nothing, the multinomial ones draw per sample); one whose entries are all equal is the scalar call (sampling_modes)."""
+    nothing, the multinomial ones draw per sample); one whose entries are all equal is the scalar call (sampling_modes).
+    ``top_k`` / ``top_p`` as in ``sample``: they truncate the multinomial steps only."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -392,4 +408,5 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
         sampling_quant_steps = sampling_quant_steps[0]
     return _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                         temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, True,
-                        sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes)
+                        sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes,
+                        top_k=top_k, top_p=top_p)
