@@ -212,6 +212,10 @@ int pb200_cast_f16(const float* x, int64_t n, int silu, void* out16, void* strea
  * [ref/src/modules.py:46-47,57-58] */
 int pb200_dwconv_ln(const float* x, const float* skip, const float* w_packed, const float* bias, int batch, int h, int w,
                     int c, int k, void* out16, void* stream);
+/* pb200_dwconv_ln with per-sample circular padding: sample b wraps on the axes of wrap[b] (DEVICE uint8 [batch]; bit 0 x,
+ * bit 1 y), zero padding elsewhere.  wrap = NULL is pb200_dwconv_ln. */
+int pb200_dwconv_ln_tiled(const float* x, const float* skip, const float* w_packed, const float* bias, int batch, int h, int w,
+                          int c, int k, const uint8_t* wrap, void* out16, void* stream);
 /* GlobalResponseNorm in place on the fp16 hidden [batch, rows_per_sample, n] of a PB200_EPI_GELU_F16 GEMM whose
  * epilogue accumulated sqsum (2^-24 fixed point); zeroes zero_per_sample entries per sample of sqsum_next;
  * scale_scratch = caller-owned fp32 [batch, n] (the per-sample multipliers 1 + gamma * Nx, written then read)
@@ -345,6 +349,14 @@ int pb200_paella_features_weighted(pb200_paella* m, const int64_t* tokens, const
                                    int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
                                    const float* attn_w, int n_w, int w_ld, const int* w_len, const int* w_row, int w_batch,
                                    float* features, void* workspace, int64_t workspace_bytes, void* stream);
+/* pb200_paella_features_weighted with seamless tiling: wrap = DEVICE uint8 [batch_total - n_pairs], one byte per sample, bit 0
+ * wraps x (left and right edges), bit 1 wraps y.  On a wrapped axis the ResBlocks' depthwise convolutions pad circularly
+ * (Conv2d padding_mode='circular'); the unconditional row batch_total - n_pairs + i reads byte i.  Nothing else depends on
+ * it.  wrap = NULL is pb200_paella_features_weighted, the same launches; a byte-0 sample gives the same bits either way. */
+int pb200_paella_features_tiled(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h, int w,
+                                const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                                int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, float* features,
+                                void* workspace, int64_t workspace_bytes, void* stream);
 
 /* out_mapper on features -> logits fp32 NCHW [B, num_labels, H*W]   (ref/src/modules.py:184-187,274) */
 int pb200_paella_logits(pb200_paella* m, const float* features, int batch, int hw, float* logits_nchw,
@@ -478,6 +490,13 @@ int pb200_vqgan_resblock(float* x_nhwc, int batch, int h, int w, int c, const fl
 enum { PB200_IMG_F32_NCHW = 0, PB200_IMG_F32_NCHW_CLAMP01 = 1, PB200_IMG_U8_NHWC = 2 };
 int pb200_vqgan_decode_ex(pb200_vqgan* m, const int64_t* indices, const float* latents_nchw, int batch, int h, int w,
                           void* img, int img_mode, void* workspace, int64_t workspace_bytes, void* stream);
+/* pb200_vqgan_decode_ex with seamless tiling: wrap = DEVICE uint8 [batch] (bit 0 wraps x, bit 1 wraps y).  On a wrapped axis
+ * the ResBlocks' ReplicationPad2d becomes circular padding and ConvTranspose2d(k4, s2, p1) reads its input indices modulo the
+ * grid, so decode(roll(tokens, (a, b))) == roll(decode(tokens), (4a, 4b)).  wrap = NULL is pb200_vqgan_decode_ex; a byte-0
+ * sample gives its bits. */
+int pb200_vqgan_decode_tiled(pb200_vqgan* m, const int64_t* indices, const float* latents_nchw, int batch, int h, int w,
+                             void* img, int img_mode, const uint8_t* wrap, void* workspace, int64_t workspace_bytes,
+                             void* stream);
 
 /* Re-read the host-mirrored scalars (the six ResBlock gammas, kernel arguments) from the bound weight blob.  Needed when
  * the blob was filled by anything other than pb200_vqgan_load_param on this handle (NCCL broadcast, a packed file,

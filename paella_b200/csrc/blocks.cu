@@ -109,6 +109,14 @@ int pb200_dwconv_ln(const float* x, const float* skip, const float* w_packed, co
     return launch_dwconv_ln(x, skip, w_packed, bias, batch, h, w, c, k, reinterpret_cast<__half*>(out16), (cudaStream_t)stream);
 }
 
+int pb200_dwconv_ln_tiled(const float* x, const float* skip, const float* w_packed, const float* bias, int batch, int h, int w,
+                          int c, int k, const uint8_t* wrap, void* out16, void* stream) {
+    PB_CHECK(x && w_packed && bias && out16, "dwconv_ln: null pointer");
+    if (batch == 0) return 0;
+    return launch_dwconv_ln(x, skip, w_packed, bias, batch, h, w, c, k, reinterpret_cast<__half*>(out16), (cudaStream_t)stream,
+                            wrap, batch);
+}
+
 int pb200_grn_f16(void* h16, int batch, int rows_per_sample, int n, const uint64_t* sqsum, uint64_t* sqsum_next,
                   int zero_per_sample, const float* gamma, const float* beta, float* scale_scratch, void* stream) {
     PB_CHECK(h16 && sqsum && sqsum_next && gamma && beta && scale_scratch, "grn_f16: null pointer");

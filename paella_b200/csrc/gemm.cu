@@ -547,7 +547,7 @@ gemm_f16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant_
                         const int ty = tap >> 1, tx = tap & 1;
                         const int oy = geom.py == 0 ? (ty == 0 ? 0 : -1) : (ty == 0 ? 1 : 0);
                         const int ox = geom.px == 0 ? (tx == 0 ? 0 : -1) : (tx == 0 ? 1 : 0);
-                        ptx::tma_load_4d(&tm_a, full_bar(stage), sa, cc * 64, cx0 + ox, cy0 + oy, cb);
+                        ptx::tma_load_4d(&tm_a, full_bar(stage), sa, cc * 64, cx0 + ox + geom.org, cy0 + oy + geom.org, cb);
                     }
                     // the W map's box is half a tile (BLOCK_N/2 rows): two loads
                     ptx::tma_load_2d(&tm_b, full_bar(stage), sa + L::A_BYTES, kb * GEMM_BLOCK_K, n_idx);

@@ -51,6 +51,7 @@ struct ConvGeom {
     int gh, gw;               // GEMM-row grid (mode 1: conv output grid; mode 2: convT input grid)
     int cin, n_cchunk;        // input channels, ceil(cin / 64)
     int oh, ow, sy, sx, py, px;   // output pixel of grid position (y,x): ((b*oh + y*sy + py)*ow + x*sx + px)
+    int org;                  // mode 2: map coordinate of grid position 0 (1 when the map covers a [B,H+2,W+2,C] bordered copy)
 };
 
 int gemm_conv_launch(const CUtensorMap& ta, const CUtensorMap& tb, int block_n, const pb200_gemm_epilogue& ep,

@@ -133,10 +133,21 @@ int launch_ln_patchify2(const float* x, int B, int h, int w, int c, __half* out,
 
 // ------------------------------------------------------------------ depthwise conv + LayerNorm (warp per position)
 // NV = float4 chunks per lane: supports c <= NV*128.
-template <int NV, bool SKIP>
+// WRAP: per-sample seamless tiling.  Sample b reads the byte wrap[b < n_base ? b : b - n_base] (the unconditional rows of a
+// CFG batch, b >= n_base, read the byte of their pair); bit 0 wraps x, bit 1 wraps y.  On a wrapped axis every tap reads its
+// coordinate modulo the grid size (Conv2d padding_mode='circular', also on grids smaller than the kernel); on an unwrapped
+// axis the arithmetic is the zero-padding instance's, so a byte-0 sample gives its bits.
+__device__ __forceinline__ int wrap_mod(int i, int n) { const int r = i % n; return r < 0 ? r + n : r; }
+
+__device__ __forceinline__ int wrap_code(const uint8_t* __restrict__ wrap, int b, int n_base) {
+    return wrap[b < n_base ? b : b - n_base];
+}
+
+template <int NV, bool SKIP, bool WRAP>
 __global__ void __launch_bounds__(128) dwconv_ln_kernel(const float* __restrict__ x, const float* __restrict__ skip,
                                                         const float* __restrict__ wp, const float* __restrict__ bias,
-                                                        int B, int h, int w, int c, int k, __half* __restrict__ out) {
+                                                        int B, int h, int w, int c, int k, __half* __restrict__ out,
+                                                        const uint8_t* __restrict__ wrap, int n_base) {
     // one CTA = a 2x2 patch of positions of one sample (4 warps, small CTAs for occupancy); the four 3x3 halos overlap so
     // half of the tap rows come from L1
     pdl_launch_dependents();
@@ -149,6 +160,7 @@ __global__ void __launch_bounds__(128) dwconv_ln_kernel(const float* __restrict_
     const int64_t pos = ((int64_t)b * h + y) * w + xx;
     const int nvq = c >> 2;          // float4 chunks in a row
     const int pad = k >> 1;
+    const int wc = WRAP ? wrap_code(wrap, b, n_base) : 0;
     float4 acc[NV];
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
@@ -156,11 +168,13 @@ __global__ void __launch_bounds__(128) dwconv_ln_kernel(const float* __restrict_
         acc[i] = q < nvq ? __ldg(reinterpret_cast<const float4*>(bias) + q) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
     for (int ky = 0; ky < k; ++ky) {
-        const int iy = y + ky - pad;
-        if (iy < 0 || iy >= h) continue;
+        int iy = y + ky - pad;
+        if (WRAP && (wc & 2)) iy = wrap_mod(iy, h);
+        else if (iy < 0 || iy >= h) continue;
         for (int kx = 0; kx < k; ++kx) {
-            const int ix = xx + kx - pad;
-            if (ix < 0 || ix >= w) continue;
+            int ix = xx + kx - pad;
+            if (WRAP && (wc & 1)) ix = wrap_mod(ix, w);
+            else if (ix < 0 || ix >= w) continue;
             const int64_t ipos = ((int64_t)b * h + iy) * w + ix;
             const int tap = ky * k + kx;
             if (!SKIP) {
@@ -261,10 +275,12 @@ __device__ __forceinline__ void block_sum16(float (&s)[DW_NPOS], float* red, flo
     __syncthreads();
 }
 
-template <bool SKIP, int MAXT>
+// WRAP: as in dwconv_ln_kernel.  An unwrapped y keeps the CTA-uniform row test; a wrapped axis reads its halo modulo the grid.
+template <bool SKIP, int MAXT, bool WRAP>
 __global__ void __launch_bounds__(MAXT, (MAXT == 320 ? 2 : 1)) dwconv3_ln_patch_kernel(const float* __restrict__ x, const float* __restrict__ skip,
                                                                 const float* __restrict__ wp, const float* __restrict__ bias,
-                                                                int B, int h, int w, int c, __half* __restrict__ out) {
+                                                                int B, int h, int w, int c, __half* __restrict__ out,
+                                                                const uint8_t* __restrict__ wrap, int n_base) {
     __shared__ float red[32 * DW_NPOS];
     __shared__ float tot[2][DW_NPOS];
     pdl_launch_dependents();
@@ -275,6 +291,7 @@ __global__ void __launch_bounds__(MAXT, (MAXT == 320 ? 2 : 1)) dwconv3_ln_patch_
     const int b = blockIdx.x / (tiles_x * tiles_y);
     const int tr = blockIdx.x - b * (tiles_x * tiles_y);
     const int y0 = (tr / tiles_x) * DW_PH, x0 = (tr % tiles_x) * DW_PW;
+    const int wc = WRAP ? wrap_code(wrap, b, n_base) : 0;
 
     float4 acc[DW_PH][DW_PW];
     {
@@ -286,8 +303,9 @@ __global__ void __launch_bounds__(MAXT, (MAXT == 320 ? 2 : 1)) dwconv3_ln_patch_
     }
 #pragma unroll
     for (int r = 0; r < DW_PH + 2; ++r) {
-        const int iy = y0 - 1 + r;
-        if (iy < 0 || iy >= h) continue;                 // CTA-uniform: a zero-padding row contributes nothing
+        int iy = y0 - 1 + r;
+        if (WRAP && (wc & 2)) iy = wrap_mod(iy, h);
+        else if (iy < 0 || iy >= h) continue;            // CTA-uniform: a zero-padding row contributes nothing
         // input row r feeds output row oy with ky = r - oy
         float4 wt[DW_PH][3][SKIP ? 2 : 1];
 #pragma unroll
@@ -308,7 +326,8 @@ __global__ void __launch_bounds__(MAXT, (MAXT == 320 ? 2 : 1)) dwconv3_ln_patch_
         const int64_t rowbase = ((int64_t)b * h + iy) * w;
 #pragma unroll
         for (int j = 0; j < DW_PW + 2; ++j) {
-            const int ix = x0 - 1 + j;
+            int ix = x0 - 1 + j;
+            if (WRAP && (wc & 1)) ix = wrap_mod(ix, w);
             const bool ok = ix >= 0 && ix < w;
             const int64_t ipos = rowbase + (ok ? ix : x0);
             float4 v0, v1;
@@ -379,22 +398,30 @@ __global__ void __launch_bounds__(MAXT, (MAXT == 320 ? 2 : 1)) dwconv3_ln_patch_
 }
 
 static int dwconv3_patch_launch(const float* x, const float* skip, const float* wp, const float* bias, int B, int h, int w,
-                                int c, __half* out, cudaStream_t st) {
+                                int c, __half* out, const uint8_t* wrap, int n_base, cudaStream_t st) {
     const int64_t grid = (int64_t)B * ceil_div(h, DW_PH) * ceil_div(w, DW_PW);
     PB_CHECK(grid < (1ll << 31), "dwconv: grid too large");
     const int threads = ceil_div(c / 4, 32) * 32;
-#define PB_DW_LAUNCH(MAXT)                                                                                              \
+#define PB_DW_LAUNCH_W(MAXT, WRAP)                                                                                      \
     do {                                                                                                                \
         if (skip)                                                                                                       \
-            dwconv3_ln_patch_kernel<true, MAXT><<<(unsigned)grid, threads, 0, st>>>(x, skip, wp, bias, B, h, w, c, out); \
+            dwconv3_ln_patch_kernel<true, MAXT, WRAP><<<(unsigned)grid, threads, 0, st>>>(x, skip, wp, bias, B, h, w, c, out, \
+                                                                                          wrap, n_base);                \
         else                                                                                                            \
-            dwconv3_ln_patch_kernel<false, MAXT><<<(unsigned)grid, threads, 0, st>>>(x, skip, wp, bias, B, h, w, c, out); \
+            dwconv3_ln_patch_kernel<false, MAXT, WRAP><<<(unsigned)grid, threads, 0, st>>>(x, skip, wp, bias, B, h, w, c, out, \
+                                                                                           wrap, n_base);               \
+    } while (0)
+#define PB_DW_LAUNCH(MAXT)                   \
+    do {                                     \
+        if (wrap) PB_DW_LAUNCH_W(MAXT, true); \
+        else PB_DW_LAUNCH_W(MAXT, false);     \
     } while (0)
     if (threads <= 64) PB_DW_LAUNCH(64);
     else if (threads <= 160) PB_DW_LAUNCH(160);
     else if (threads <= 320) PB_DW_LAUNCH(320);
     else PB_DW_LAUNCH(640);
 #undef PB_DW_LAUNCH
+#undef PB_DW_LAUNCH_W
     PB_LAUNCH_CHECK();
     return 0;
 }
@@ -426,11 +453,14 @@ __global__ void __launch_bounds__(256) row_stats_kernel(const float* __restrict_
     if (lane == 0) stats[row] = make_float2(mean, rstd);
 }
 
-template <int MAXT, int MINB>
+// WRAP: per-sample seamless tiling (wrap[b], bit 0 = x, bit 1 = y): a wrapped axis replaces ReplicationPad2d's clamped coordinate
+// by the coordinate modulo the grid size (circular padding); an unwrapped one keeps the clamp.
+template <int MAXT, int MINB, bool WRAP>
 __global__ void __launch_bounds__(MAXT, MINB) vq_front_patch_kernel(const float* __restrict__ x, const float2* __restrict__ stats,
                                                               const float* __restrict__ wp, const float* __restrict__ bias,
                                                               float a0, float g1, float g2, float a3, float g4, int B, int h, int w,
-                                                              int c, float* __restrict__ x_out, __half* __restrict__ a16) {
+                                                              int c, float* __restrict__ x_out, __half* __restrict__ a16,
+                                                              const uint8_t* __restrict__ wrap) {
     __shared__ float red[32 * DW_NPOS];
     __shared__ float tot[2][DW_NPOS];
     __shared__ float2 st_s[DW_PH + 2][DW_PW + 2];
@@ -441,8 +471,10 @@ __global__ void __launch_bounds__(MAXT, MINB) vq_front_patch_kernel(const float*
     const int b = blockIdx.x / (tiles_x * tiles_y);
     const int tr = blockIdx.x - b * (tiles_x * tiles_y);
     const int y0 = (tr / tiles_x) * DW_PH, x0 = (tr % tiles_x) * DW_PW;
-    auto cy = [&](int y) { return min(max(y, 0), h - 1); };           // ReplicationPad2d(1) = clamped coordinates
-    auto cx = [&](int xx) { return min(max(xx, 0), w - 1); };
+    const int wc = WRAP ? wrap[b] : 0;
+    // ReplicationPad2d(1) = clamped coordinates; circular on a wrapped axis
+    auto cy = [&](int y) { return (WRAP && (wc & 2)) ? wrap_mod(y, h) : min(max(y, 0), h - 1); };
+    auto cx = [&](int xx) { return (WRAP && (wc & 1)) ? wrap_mod(xx, w) : min(max(xx, 0), w - 1); };
     if (threadIdx.x < (DW_PH + 2) * (DW_PW + 2)) {
         const int r = threadIdx.x / (DW_PW + 2), j = threadIdx.x - r * (DW_PW + 2);
         st_s[r][j] = stats[((int64_t)b * h + cy(y0 - 1 + r)) * w + cx(x0 - 1 + j)];
@@ -532,7 +564,7 @@ __global__ void __launch_bounds__(MAXT, MINB) vq_front_patch_kernel(const float*
 bool vq_front_fused_ok(int c, int h, int w) { return c % 4 == 0 && c >= 4 * (DW_PH + 2) * (DW_PW + 2) && c <= 512 && h >= 1 && w >= 1; }
 
 int launch_vq_front_fused(const float* x, int B, int h, int w, int c, const float* w9, const float* bias, const float* gam,
-                          float2* stats_scratch, float* x_out, __half* a16, cudaStream_t st) {
+                          float2* stats_scratch, float* x_out, __half* a16, cudaStream_t st, const uint8_t* wrap) {
     PB_CHECK(vq_front_fused_ok(c, h, w), "vq_front: width %d not handled by the patch kernel", c);
     const int64_t M = (int64_t)B * h * w;
     if (M == 0) return 0;
@@ -546,29 +578,41 @@ int launch_vq_front_fused(const float* x, int B, int h, int w, int c, const floa
     PB_CHECK(grid < (1ll << 31), "vq_front: grid too large");
     const int threads = ceil_div(c / 4, 32) * 32;
     // 3 CTAs of 96 threads per SM at 168 registers (capping at 128 registers for a fourth CTA spills)
-    if (threads <= 64)
-        vq_front_patch_kernel<64, 6><<<(unsigned)grid, threads, 0, st>>>(x, stats_scratch, w9, bias, 1.0f + gam[0], gam[1], gam[2], 1.0f + gam[3], gam[4], B, h, w, c, x_out, a16);
-    else
-        vq_front_patch_kernel<128, 3><<<(unsigned)grid, threads, 0, st>>>(x, stats_scratch, w9, bias, 1.0f + gam[0], gam[1], gam[2], 1.0f + gam[3], gam[4], B, h, w, c, x_out, a16);
+#define PB_VQF_LAUNCH(MAXT, MINB, WRAP)                                                                                 \
+    vq_front_patch_kernel<MAXT, MINB, WRAP><<<(unsigned)grid, threads, 0, st>>>(x, stats_scratch, w9, bias, 1.0f + gam[0], gam[1], \
+                                                                                gam[2], 1.0f + gam[3], gam[4], B, h, w, c, x_out,  \
+                                                                                a16, wrap)
+    if (threads <= 64) {
+        if (wrap) PB_VQF_LAUNCH(64, 6, true);
+        else PB_VQF_LAUNCH(64, 6, false);
+    } else {
+        if (wrap) PB_VQF_LAUNCH(128, 3, true);
+        else PB_VQF_LAUNCH(128, 3, false);
+    }
+#undef PB_VQF_LAUNCH
     PB_LAUNCH_CHECK();
     return 0;
 }
 
 template <int NV>
 static int dwconv_dispatch(const float* x, const float* skip, const float* wp, const float* bias, int B, int h, int w,
-                           int c, int k, __half* out, cudaStream_t st) {
+                           int c, int k, __half* out, const uint8_t* wrap, int n_base, cudaStream_t st) {
     const int64_t grid = (int64_t)B * ((h + 1) / 2) * ((w + 1) / 2);
     PB_CHECK(grid < (1ll << 31), "dwconv: grid too large");
-    if (skip)
-        dwconv_ln_kernel<NV, true><<<(unsigned)grid, 128, 0, st>>>(x, skip, wp, bias, B, h, w, c, k, out);
+    if (skip && wrap)
+        dwconv_ln_kernel<NV, true, true><<<(unsigned)grid, 128, 0, st>>>(x, skip, wp, bias, B, h, w, c, k, out, wrap, n_base);
+    else if (wrap)
+        dwconv_ln_kernel<NV, false, true><<<(unsigned)grid, 128, 0, st>>>(x, skip, wp, bias, B, h, w, c, k, out, wrap, n_base);
+    else if (skip)
+        dwconv_ln_kernel<NV, true, false><<<(unsigned)grid, 128, 0, st>>>(x, skip, wp, bias, B, h, w, c, k, out, wrap, n_base);
     else
-        dwconv_ln_kernel<NV, false><<<(unsigned)grid, 128, 0, st>>>(x, skip, wp, bias, B, h, w, c, k, out);
+        dwconv_ln_kernel<NV, false, false><<<(unsigned)grid, 128, 0, st>>>(x, skip, wp, bias, B, h, w, c, k, out, wrap, n_base);
     PB_LAUNCH_CHECK();
     return 0;
 }
 
 int launch_dwconv_ln(const float* x, const float* skip, const float* w_packed, const float* bias, int B, int h, int w,
-                     int c, int k, __half* out, cudaStream_t st) {
+                     int c, int k, __half* out, cudaStream_t st, const uint8_t* wrap, int n_base) {
     ProfScope prof("dwconv_ln", (double)B * h * w * c * (skip ? 10.0 : 6.0), st);
     PB_CHECK(c % 8 == 0, "dwconv: c=%d must be a multiple of 8", c);
     PB_CHECK(k % 2 == 1, "dwconv: kernel_size %d must be odd", k);
@@ -576,11 +620,11 @@ int launch_dwconv_ln(const float* x, const float* skip, const float* w_packed, c
     // the patch kernel takes the wide levels only: at 640 channels its 152 registers x 160 threads leave 15% occupancy
     static const bool patch_all = getenv("PB200_DWCONV_PATCH") != nullptr;
     if (k == 3 && c <= 2560 && !old_kernel && (patch_all || (c > 640 && w >= DW_PW)))
-        return dwconv3_patch_launch(x, skip, w_packed, bias, B, h, w, c, out, st);
-    if (c <= 128) return dwconv_dispatch<1>(x, skip, w_packed, bias, B, h, w, c, k, out, st);
-    if (c <= 640) return dwconv_dispatch<5>(x, skip, w_packed, bias, B, h, w, c, k, out, st);
-    if (c <= 1280) return dwconv_dispatch<10>(x, skip, w_packed, bias, B, h, w, c, k, out, st);
-    if (c <= 2560) return dwconv_dispatch<20>(x, skip, w_packed, bias, B, h, w, c, k, out, st);
+        return dwconv3_patch_launch(x, skip, w_packed, bias, B, h, w, c, out, wrap, n_base, st);
+    if (c <= 128) return dwconv_dispatch<1>(x, skip, w_packed, bias, B, h, w, c, k, out, wrap, n_base, st);
+    if (c <= 640) return dwconv_dispatch<5>(x, skip, w_packed, bias, B, h, w, c, k, out, wrap, n_base, st);
+    if (c <= 1280) return dwconv_dispatch<10>(x, skip, w_packed, bias, B, h, w, c, k, out, wrap, n_base, st);
+    if (c <= 2560) return dwconv_dispatch<20>(x, skip, w_packed, bias, B, h, w, c, k, out, wrap, n_base, st);
     PB_CHECK(false, "dwconv: c=%d > 2560 unsupported", c);
     return 1;
 }
@@ -819,6 +863,43 @@ int launch_cast_f16(const float* x, int64_t n, __half* out, cudaStream_t st) {
     PB_LAUNCH_CHECK();
     return 0;
 }
+// fp32 NHWC [B,h,w,c] -> fp16 NHWC [B,h+2,w+2,c] with a border one position wide: sample b's border holds circular copies on
+// the axes wrap[b] wraps (bit 0 = x, bit 1 = y) and zeros on the others.  Interior values are rounded as cast_kernel<0> rounds
+// them.  Thread = 4 channels of one padded position; c % 4 == 0.
+__global__ void pad_cast_kernel(const float* __restrict__ x, int B, int h, int w, int c, const uint8_t* __restrict__ wrap,
+                                __half* __restrict__ out) {
+    const int nq = c >> 2;
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (int64_t)B * (h + 2) * (w + 2) * nq) return;
+    const int q = (int)(i % nq);
+    const int64_t pos = i / nq;
+    const int pw = w + 2, ph = h + 2;
+    const int b = (int)(pos / ((int64_t)ph * pw));
+    const int rem = (int)(pos - (int64_t)b * ph * pw);
+    int y = rem / pw - 1, xx = rem % pw - 1;
+    const int wc = wrap[b];
+    bool ok = true;
+    if (y < 0 || y >= h) { if (wc & 2) y = wrap_mod(y, h); else ok = false; }
+    if (xx < 0 || xx >= w) { if (wc & 1) xx = wrap_mod(xx, w); else ok = false; }
+    uint2 pk = make_uint2(0u, 0u);
+    if (ok) {
+        const float4 v = *(reinterpret_cast<const float4*>(x + (((int64_t)b * h + y) * w + xx) * c) + q);
+        pk.x = pack_half2(v.x, v.y);
+        pk.y = pack_half2(v.z, v.w);
+    }
+    *reinterpret_cast<uint2*>(out + pos * c + q * 4) = pk;
+}
+
+int launch_pad_cast_f16(const float* x, int B, int h, int w, int c, const uint8_t* wrap, __half* out, cudaStream_t st) {
+    ProfScope prof("cast", (double)B * (h + 2) * (w + 2) * c * 6.0, st);
+    PB_CHECK(c % 4 == 0 && wrap != nullptr, "pad_cast: c=%d must be a multiple of 4, with a wrap table", c);
+    const int64_t n = (int64_t)B * (h + 2) * (w + 2) * (c / 4);
+    if (n == 0) return 0;
+    pad_cast_kernel<<<ceil_div(n, 256), 256, 0, st>>>(x, B, h, w, c, wrap, out);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
 int launch_silu_cast_f16(const float* x, int64_t n, __half* out, cudaStream_t st) {
     ProfScope prof("cast", (double)n * 6.0, st);
     if (n == 0) return 0;

@@ -19,14 +19,17 @@ int launch_ln_patchify2(const float* x, int B, int h, int w, int c, __half* out,
 
 // ResBlock front: depthwise kxk conv (zero pad k/2; optional [x,skip] 2-channel groups) + bias + LN -> fp16 [M,c]
 // w_packed: fp32 [k*k][per][c] (per = 1, or 2 with skip), bias fp32 [c]
+// wrap (optional, DEVICE uint8): sample b wraps around on the axes of wrap[b < n_base ? b : b - n_base] (bit 0 x, bit 1 y);
+// NULL launches the zero-padding kernels
 int launch_dwconv_ln(const float* x, const float* skip, const float* w_packed, const float* bias, int B, int h, int w,
-                     int c, int k, __half* out, cudaStream_t st);
+                     int c, int k, __half* out, cudaStream_t st, const uint8_t* wrap = nullptr, int n_base = 0);
 
 // codec ResBlock front in one pass (ref/src/vqgan.py:36-40; see ops.cu): x' = x + g2*(dw3x3(reppad(LN(x)(1+g0)+g1)) + bias) -> x_out
 // (a buffer other than x), a16 = fp16(LN(x')(1+g3)+g4).  gam = the block's gammas on the HOST; stats_scratch: B*h*w float2.
+// wrap (optional, DEVICE uint8 [B]): circular instead of replication padding on the axes of wrap[b] (bit 0 x, bit 1 y)
 bool vq_front_fused_ok(int c, int h, int w);
 int launch_vq_front_fused(const float* x, int B, int h, int w, int c, const float* w9, const float* bias, const float* gam,
-                          float2* stats_scratch, float* x_out, __half* a16, cudaStream_t st);
+                          float2* stats_scratch, float* x_out, __half* a16, cudaStream_t st, const uint8_t* wrap = nullptr);
 
 // GlobalResponseNorm: h[b,p,n] = h*(1 + gamma[n]*Gx[b,n]/(mean_n Gx + 1e-6)) + beta[n], Gx = sqrt(sq[b,n]) (2^-24 fixed point);
 // zeroes all B*zero_per_sample entries of sq_next (the other buffer of a ping-pong pair) for the next block.
@@ -45,6 +48,9 @@ int launch_film_apply(float* x, int64_t M, int N, int P, const float* film, int6
 
 int launch_cast_f16(const float* x, int64_t n, __half* out, cudaStream_t st);
 int launch_silu_cast_f16(const float* x, int64_t n, __half* out, cudaStream_t st);
+// fp32 NHWC [B,h,w,c] -> fp16 [B,h+2,w+2,c] with a one-position border: circular copies on the axes wrap[b] (DEVICE uint8 [B];
+// bit 0 x, bit 1 y) wraps, zeros elsewhere (the ConvTranspose2d input of a tiled decode)
+int launch_pad_cast_f16(const float* x, int B, int h, int w, int c, const uint8_t* wrap, __half* out, cudaStream_t st);
 // out[i] = fp16(a[i]*wa + b[i]*wb)   (b may be null)
 int launch_mix_cast_f16(const float* a, const float* b, float wa, float wb, int64_t n, __half* out, cudaStream_t st);
 // the same mix with per-sample weights: element e uses (wa, wb) = (w[3 s], w[3 s + 1]), s = e / per (w: DEVICE [samples][3])

@@ -621,6 +621,14 @@ int pb200_paella_features_weighted(pb200_paella* m, const int64_t* tokens, const
                                    int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max,
                                    const float* attn_w, int n_w, int w_ld, const int* w_len, const int* w_row, int w_batch,
                                    float* features, void* workspace, int64_t workspace_bytes, void* stream) {
+    return pb200_paella_features_tiled(m, tokens, r, batch_total, n_pairs, h, w, cond_cache, cache_slots, kv_slot, s_max, attn_w, n_w,
+                                       w_ld, w_len, w_row, w_batch, nullptr, features, workspace, workspace_bytes, stream);
+}
+
+int pb200_paella_features_tiled(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h, int w,
+                                const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                                int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, float* features,
+                                void* workspace, int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
     PB_CHECK(w_ld >= 0, "features: attention-weight row stride %d < 0", w_ld);
     const pb200_paella_config& c = m->cfg;
@@ -649,6 +657,10 @@ int pb200_paella_features_weighted(pb200_paella* m, const int64_t* tokens, const
     // approximation.  Guided samples first keeps every replication one contiguous copy.
     PB_CHECK(n_pairs >= 0 && 2 * n_pairs <= Bt, "features: %d CFG pairs in a batch of %d", n_pairs, Bt);
     int Bc = Bt - n_pairs;                              // samples currently carried by x
+    // seamless tiling: wrap [Bt - n_pairs], one byte per sample; the unconditional row Bt - n_pairs + i reads byte i, before and
+    // after the replication below.  Only the ResBlocks' depthwise padding depends on it (no positional embedding, and
+    // h, w are multiples of every level's stride, so each level's grid tiles the torus)
+    const int n_base = Bt - n_pairs;
 
     // timestep embedding and every TimestepBlock's (a, b) at once
     PB_TRY(launch_r_embed(r, Bc, c.c_r, ws.r_emb, st));
@@ -721,7 +733,7 @@ int pb200_paella_features_weighted(pb200_paella* m, const int64_t* tokens, const
                 if (b.kind == BK_RES) {
                     const float* skip = b.c_skip ? ws.xd[l] : nullptr;
                     PB_TRY(launch_dwconv_ln(x, skip, m->w<float>(b.dw_w), m->w<float>(b.dw_b), Bc, gh[l], gw[l], ch,
-                                            c.kernel_size, ws.a16, st));
+                                            c.kernel_size, ws.a16, st, wrap, n_base));
                 } else {
                     PB_TRY(launch_ln_rows(x, M, ch, 1.0f, 0.0f, ws.a16, nullptr, st));
                 }

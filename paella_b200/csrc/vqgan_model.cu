@@ -270,10 +270,12 @@ __global__ void __launch_bounds__(256) vq_dec_head4_kernel(const float* __restri
     *reinterpret_cast<float4*>(out + pos * c1 + q * 4) = make_float4(dot(bv.x, w0), dot(bv.y, w1), dot(bv.z, w2), dot(bv.w, w3));
 }
 
-// ResBlock middle: x += (depthwise3x3(ReplicationPad(xt)) + bias) * g2; xt, x NHWC fp32; w9 [9][c]
+// ResBlock middle: x += (depthwise3x3(ReplicationPad(xt)) + bias) * g2; xt, x NHWC fp32; w9 [9][c].
+// WRAP: sample b pads circularly on the axes of wrap[b] (bit 0 x, bit 1 y) and by replication on the others.
+template <bool WRAP>
 __global__ void __launch_bounds__(256) vq_dw_residual_kernel(const float* __restrict__ xt, float* __restrict__ x,
                                                              const float* __restrict__ w9, const float* __restrict__ bias,
-                                                             float g2, int B, int h, int w, int c) {
+                                                             float g2, int B, int h, int w, int c, const uint8_t* __restrict__ wrap) {
     const int nq = c >> 2;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (int64_t)B * h * w * nq) return;
@@ -282,13 +284,14 @@ __global__ void __launch_bounds__(256) vq_dw_residual_kernel(const float* __rest
     const int b = (int)(pos / ((int64_t)h * w));
     const int rem = (int)(pos - (int64_t)b * h * w);
     const int y = rem / w, xx = rem - y * w;
+    const int wc = WRAP ? wrap[b] : 0;
     float4 acc = __ldg(reinterpret_cast<const float4*>(bias) + q);
 #pragma unroll
     for (int ky = 0; ky < 3; ++ky) {
-        const int iy = min(max(y + ky - 1, 0), h - 1);
+        const int iy = (WRAP && (wc & 2)) ? (y + ky - 1 + h) % h : min(max(y + ky - 1, 0), h - 1);
 #pragma unroll
         for (int kx = 0; kx < 3; ++kx) {
-            const int ix = min(max(xx + kx - 1, 0), w - 1);
+            const int ix = (WRAP && (wc & 1)) ? (xx + kx - 1 + w) % w : min(max(xx + kx - 1, 0), w - 1);
             const float4 v = *reinterpret_cast<const float4*>(xt + (((int64_t)b * h + iy) * w + ix) * c + q * 4);
             const float4 ww = __ldg(reinterpret_cast<const float4*>(w9 + (int64_t)(ky * 3 + kx) * c) + q);
             acc.x = fmaf(v.x, ww.x, acc.x); acc.y = fmaf(v.y, ww.y, acc.y);
@@ -404,10 +407,12 @@ static void vq_plan(const pb200_vqgan* m, int B, int H, int W, uint8_t* base, in
     };
     const int64_t M0 = (int64_t)B * (H / 2) * (W / 2), M1 = (int64_t)B * (H / 4) * (W / 4);
     const int64_t big = M0 * m->c0 > M1 * m->c1 ? M0 * m->c0 : M1 * m->c1;
+    // a16 also holds the bordered ConvTranspose2d input of a tiled decode, [B, H/4 + 2, W/4 + 2, c1]
+    const int64_t padded = (int64_t)B * (H / 4 + 2) * (W / 4 + 2) * m->c1;
     ws.xa = (float*)take(big * 4);
     ws.xb = (float*)take(big * 4);
     ws.tmp32 = (float*)take(big * 4);
-    ws.a16 = (__half*)take(big * 2);
+    ws.a16 = (__half*)take((big > padded ? big : padded) * 2);
     ws.h16 = (__half*)take(big * 4 * 2);
     ws.lat = (float*)take(M1 * m->cfg.c_latent * 4);
     ws.zq = (float*)take(M1 * m->cfg.c_latent * 4);
@@ -418,31 +423,38 @@ static void vq_plan(const pb200_vqgan* m, int B, int H, int W, uint8_t* base, in
 // a16 = fp16(LN(x')(1+g3)+g4).  x: NHWC fp32 [B,h,w,c].  *resid = where x' lives: `tmp32` on the fused path (one patch kernel +
 // a statistics pre-pass, ops.cu::launch_vq_front_fused; `scratch` = B*h*w float2), x itself (updated in place) on the three-launch
 // path that narrow widths (tiny test codecs) and in_place = true take.
+// wrap (optional, DEVICE uint8 [B]): circular padding on the axes of wrap[b] (bit 0 x, bit 1 y), seamless tiling.
 static int resblock_front(float* x, int B, int h, int w, int c, const float* dw_w9, const float* dw_b, const float* gam,
-                          float* tmp32, __half* a16, void* scratch, bool in_place, const float** resid, cudaStream_t st) {
+                          float* tmp32, __half* a16, void* scratch, bool in_place, const float** resid, cudaStream_t st,
+                          const uint8_t* wrap = nullptr) {
     const int64_t M = (int64_t)B * h * w;
     static const bool unfused = getenv("PB200_VQ_FRONT_UNFUSED") != nullptr;      // A/B knob
     if (!in_place && !unfused && vq_front_fused_ok(c, h, w)) {
         *resid = tmp32;
-        return launch_vq_front_fused(x, B, h, w, c, dw_w9, dw_b, gam, reinterpret_cast<float2*>(scratch), tmp32, a16, st);
+        return launch_vq_front_fused(x, B, h, w, c, dw_w9, dw_b, gam, reinterpret_cast<float2*>(scratch), tmp32, a16, st, wrap);
     }
     *resid = x;
     PB_TRY(launch_ln_rows(x, M, c, 1.0f + gam[0], gam[1], nullptr, tmp32, st));
     {
         ProfScope prof("vq_dwconv", (double)M * c * 12.0, st);
-        vq_dw_residual_kernel<<<ceil_div(M * (c / 4), 256), 256, 0, st>>>(tmp32, x, dw_w9, dw_b, gam[2], B, h, w, c);
+        if (wrap)
+            vq_dw_residual_kernel<true><<<ceil_div(M * (c / 4), 256), 256, 0, st>>>(tmp32, x, dw_w9, dw_b, gam[2], B, h, w, c, wrap);
+        else
+            vq_dw_residual_kernel<false><<<ceil_div(M * (c / 4), 256), 256, 0, st>>>(tmp32, x, dw_w9, dw_b, gam[2], B, h, w, c, wrap);
         PB_LAUNCH_CHECK();
     }
     return launch_ln_rows(x, M, c, 1.0f + gam[3], gam[4], a16, nullptr, st);
 }
 
 // x: NHWC fp32 [B,h,w,c], updated in place (ref/src/vqgan.py:36-42)
-static int run_resblock(pb200_vqgan* m, const VqResBlock& rb, float* x, int B, int h, int w, VqWs& ws, cudaStream_t st) {
+static int run_resblock(pb200_vqgan* m, const VqResBlock& rb, float* x, int B, int h, int w, VqWs& ws, cudaStream_t st,
+                        const uint8_t* wrap = nullptr) {
     const int c = rb.c;
     const int64_t M = (int64_t)B * h * w;
     const float* resid = x;
     // (h16 is idle until GEMM1 writes it: it lends its first bytes to the row statistics)
-    PB_TRY(resblock_front(x, B, h, w, c, m->w<float>(rb.dw_w), m->w<float>(rb.dw_b), rb.gam, ws.tmp32, ws.a16, ws.h16, false, &resid, st));
+    PB_TRY(resblock_front(x, B, h, w, c, m->w<float>(rb.dw_w), m->w<float>(rb.dw_b), rb.gam, ws.tmp32, ws.a16, ws.h16, false, &resid, st,
+                          wrap));
     pb200_gemm_epilogue e1 = vepi(PB200_EPI_GELU_F16, m->w<float>(rb.b1), ws.h16, 4 * c);
     PB_TRY(m->gemm(ws.a16, c, M, c, rb.w1, 4 * (int64_t)c, e1, st));
     pb200_gemm_epilogue e2 = vepi(PB200_EPI_RESID_F32, m->w<float>(rb.b2), x, c);
@@ -647,6 +659,11 @@ int pb200_vqgan_decode(pb200_vqgan* m, const int64_t* indices, const float* late
 
 int pb200_vqgan_decode_ex(pb200_vqgan* m, const int64_t* indices, const float* latents_nchw, int batch, int h, int w, void* img,
                           int img_mode, void* workspace, int64_t workspace_bytes, void* stream) {
+    return pb200_vqgan_decode_tiled(m, indices, latents_nchw, batch, h, w, img, img_mode, nullptr, workspace, workspace_bytes, stream);
+}
+
+int pb200_vqgan_decode_tiled(pb200_vqgan* m, const int64_t* indices, const float* latents_nchw, int batch, int h, int w, void* img,
+                             int img_mode, const uint8_t* wrap, void* workspace, int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "decode: weights not bound");
     PB_CHECK(img_mode >= 0 && img_mode <= 2, "decode: unknown image mode %d", img_mode);
     if (m->host_params_stale) PB_TRY(pb200_vqgan_sync_params(m, stream));
@@ -673,21 +690,27 @@ int pb200_vqgan_decode_ex(pb200_vqgan* m, const int64_t* indices, const float* l
                                                                             ws.xb);
         PB_LAUNCH_CHECK();
     }
-    for (const VqResBlock& rb : m->bottleneck) PB_TRY(run_resblock(m, rb, ws.xb, B, h1, w1, ws, st));
-    // ConvTranspose2d(c1 -> c0, k=4, s=2, p=1) as 4 sub-pixel phases of 2x2 taps
-    PB_TRY(launch_cast_f16(ws.xb, M1 * c1, ws.a16, st));
+    for (const VqResBlock& rb : m->bottleneck) PB_TRY(run_resblock(m, rb, ws.xb, B, h1, w1, ws, st, wrap));
+    // ConvTranspose2d(c1 -> c0, k=4, s=2, p=1) as 4 sub-pixel phases of 2x2 taps.  Tiled: the input gets a one-position border
+    // (circular copies on a wrapped axis, zeros otherwise -- the same sums as the map's zero fill) and the map reads it from +1
+    const int pad = wrap ? 1 : 0;
+    if (wrap)
+        PB_TRY(launch_pad_cast_f16(ws.xb, B, h1, w1, c1, wrap, ws.a16, st));
+    else
+        PB_TRY(launch_cast_f16(ws.xb, M1 * c1, ws.a16, st));
     {
         ConvGeom g;
         memset(&g, 0, sizeof(g));
         g.mode = 2; g.batch = B; g.gh = h1; g.gw = w1; g.cin = c1; g.n_cchunk = m->cpad1 / 64;
         conv_tile(w1, g.tw, g.th);
         g.tiles_x = ceil_div(w1, g.tw); g.tiles_y = ceil_div(h1, g.th);
-        g.oh = h0; g.ow = w0; g.sy = 2; g.sx = 2;
+        g.oh = h0; g.ow = w0; g.sy = 2; g.sx = 2; g.org = pad;
         const int64_t N = c0, K = 4 * (int64_t)m->cpad1;
         const int bn = gemm_pick_block_n((int64_t)B * g.tiles_x * g.tiles_y * 128, N, K);
         CUtensorMap ta;
-        const int64_t dims[4] = {c1, w1, h1, B};
-        const int64_t strides[3] = {(int64_t)c1 * 2, (int64_t)w1 * c1 * 2, (int64_t)h1 * w1 * c1 * 2};
+        const int64_t hp = h1 + 2 * pad, wp = w1 + 2 * pad;
+        const int64_t dims[4] = {c1, wp, hp, B};
+        const int64_t strides[3] = {(int64_t)c1 * 2, wp * c1 * 2, hp * wp * c1 * 2};
         const int box[4] = {64, g.tw, g.th, 1};
         PB_TRY(make_tmap_f16_nd(&ta, ws.a16, 4, dims, strides, box));
         for (int ph = 0; ph < 4; ++ph) {
@@ -698,7 +721,7 @@ int pb200_vqgan_decode_ex(pb200_vqgan* m, const int64_t* indices, const float* l
             PB_TRY(gemm_conv_launch(ta, *tb, bn, e, g, N, K, st));
         }
     }
-    PB_TRY(run_resblock(m, m->dec_last, ws.xa, B, h0, w0, ws, st));
+    PB_TRY(run_resblock(m, m->dec_last, ws.xa, B, h0, w0, ws, st, wrap));
     {
         ProfScope prof("vq_out_block", (double)M0 * (c0 * 4.0 + 48.0), st);
         const float *ow = m->w<float>(m->out_w), *ob = m->w<float>(m->out_b);

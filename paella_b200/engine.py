@@ -28,7 +28,9 @@ and generator offset are those of ``sample_notebook(model, inputs, (1, H, W), un
 cfg, mode, t_start, t_end, sampling_conditional_steps, sampling_quant_steps, attn_weights, vqmodel=vq, generator=[g],
 region=region)``: a step in argmax or quant mode draws nothing from ``g`` (only its mask draw, if it renoises).  With
 ``top_k`` / ``top_p`` a request's multinomial steps are truncated as in ``sample_notebook(..., top_k=k, top_p=p)``; the draws,
-and so the generator offsets, are those of the untruncated request.
+and so the generator offsets, are those of the untruncated request.  With ``tiling='x'``, ``'y'`` or ``'xy'`` a request's token
+grid wraps around as in ``sample_notebook(..., tiling=t)`` (seamless textures and panoramas), and ``decode=True`` decodes it
+with the same tiling; tiling draws nothing.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -38,7 +40,9 @@ one fused-sampler launch and one per-sample add-noise launch that writes every r
 in several sampling modes adds each row's mode to the table: the fused sampler skips the argmax and quant rows, which then go
 through the out_mapper GEMM to logits (a bounded number of samples at a time) and the argmax or quant kernel, one call per mode
 (Paella.sample_tokens_modes).  A step in which some request truncates adds each row's (k, p) to the table, and the fused sampler
-reads them there (0 and 1.0 for the rows that do not); a step in which none does launches exactly as without truncation.
+reads them there (0 and 1.0 for the rows that do not); a step in which none does launches exactly as without truncation.  A step
+in which some row tiles adds each row's wrap byte (0 for the rows that do not), read by the denoiser's depthwise convolutions; a
+step in which none does launches exactly as without tiling.
 The host knows which
 requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
 in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
@@ -66,7 +70,7 @@ class Request:
                  generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False,
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
                  region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
-                 top_k: int = 0, top_p: float = 1.0):
+                 top_k: int = 0, top_p: float = 1.0, wrap: int = 0):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -75,6 +79,7 @@ class Request:
         self.has_region = region is not None
         self.mode, self.quant_steps = mode, quant_steps      # sampling mode, and the step from which 'quant' is used (or None)
         self.top_k, self.top_p = top_k, top_p    # the truncation table's row: 0 and 1.0 are off
+        self.wrap = wrap                         # the wrap table's byte (ops.tiling_table): bit 0 x, bit 1 y; 0 is off
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -106,6 +111,9 @@ class StepPlan:
         self.truncates = any(dr and (q.top_k > 0 or q.top_p < 1.0) for q, dr in zip(order, self.draws))
         self.top_k = torch.tensor([q.top_k for q in order], dtype=torch.int32)
         self.top_p = torch.tensor([q.top_p for q in order], dtype=torch.float32)
+        # the wrap table, when some row tiles (otherwise the step launches the untiled kernels)
+        self.wraps = any(q.wrap for q in order)
+        self.wrap = torch.tensor([q.wrap for q in order], dtype=torch.uint8)
         # a row that does not renoise keeps its tokens (t < 0 never passes the mask test)
         self.t_next = torch.stack([q.r[q.k + 1] if rn else torch.tensor(-1.0) for q, rn in zip(order, self.renoise)])
         self.row_slot = torch.tensor([q.slot for q in order], dtype=torch.int32)
@@ -135,9 +143,10 @@ def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List
 
 def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tuple[torch.Tensor, Dict[str, Tuple[str, int, int]]]:
     """The step's one host-to-device buffer: int64 [(seed, offset) pairs of the sampler's draw, then of the mask draw], then the
-    float32 part [r, params (3 per row), t_next, (top_p)], then the int32 part [row_slot, kv_slot, (mode table), (top_k)], each
-    part padded to whole int64 words.  top_p / top_k are present only when ``plan.truncates``, the mode table only when the step
-    mixes modes.  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
+    float32 part [r, params (3 per row), t_next, (top_p)], then the int32 part [row_slot, kv_slot, (mode table), (top_k)], then
+    the uint8 part [(wrap)], each part padded to whole int64 words.  top_p / top_k are present only when ``plan.truncates``, the
+    mode table only when the step mixes modes, wrap (one byte per row) only when ``plan.wraps``.  Returns (buffer, {name: (dtype,
+    start, length)}), start and length in elements of that dtype within its part."""
     Bc, n_pairs = len(plan.order), plan.n_pairs
     mixed = not all(plan.draws)
     modes = ops.mode_table(plan.modes) if mixed else torch.zeros(0, dtype=torch.int32)
@@ -146,8 +155,9 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
     if plan.truncates:
         f32_parts.append(("top_p", plan.top_p))
         i32_parts.append(("top_k", plan.top_k))
+    u8_parts = [("wrap", plan.wrap)] if plan.wraps else []
     layout: Dict[str, Tuple[str, int, int]] = {}
-    for dt, parts in (("f32", f32_parts), ("i32", i32_parts)):
+    for dt, parts in (("f32", f32_parts), ("i32", i32_parts), ("u8", u8_parts)):
         o = 0
         for name, v in parts:
             layout[name] = (dt, o, v.numel())
@@ -156,9 +166,13 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
     i32 = torch.cat([v for _, v in i32_parts])
     f32 = torch.cat([f32, torch.zeros(f32.numel() % 2)])
     i32 = torch.cat([i32, torch.zeros(i32.numel() % 2, dtype=torch.int32)])
-    host = torch.cat([torch.tensor(draw + renoise, dtype=torch.int64), f32.view(torch.int64), i32.view(torch.int64)])
+    u8 = torch.cat([v for _, v in u8_parts] + [torch.zeros(0, dtype=torch.uint8)])
+    u8 = torch.cat([u8, torch.zeros(-u8.numel() % 8, dtype=torch.uint8)])
+    host = torch.cat([torch.tensor(draw + renoise, dtype=torch.int64), f32.view(torch.int64), i32.view(torch.int64),
+                      u8.view(torch.int64)])
     layout["f32"] = ("i64", 4 * Bc, f32.numel() // 2)
     layout["i32"] = ("i64", 4 * Bc + f32.numel() // 2, i32.numel() // 2)
+    layout["u8"] = ("i64", 4 * Bc + f32.numel() // 2 + i32.numel() // 2, u8.numel() // 8)
     return host, layout
 
 
@@ -250,7 +264,7 @@ class SamplingEngine:
     def submit(self, model_inputs, unconditional_inputs=None, *, generator=None, steps=12, renoise_steps=None,
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
-               sampling_quant_steps=None, top_k=None, top_p=None) -> Request:
+               sampling_quant_steps=None, top_k=None, top_p=None, tiling=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -263,7 +277,8 @@ class SamplingEngine:
         ``sampling_quant_steps`` choose each step's sampling mode as in sample_notebook (step k uses 'quant' if
         k >= sampling_quant_steps, ``mode`` otherwise; 'quant' reads the codebook of the engine's vqmodel).  ``top_k`` (None or
         an int >= 0) and ``top_p`` (None or a float in (0, 1]) truncate the request's multinomial steps as in sample_notebook;
-        ValueError for any other value.  The request's draws start when it is admitted."""
+        ValueError for any other value.  ``tiling`` (None, 'none', 'x', 'y' or 'xy') tiles the request as in sample_notebook, and
+        with ``decode=True`` its decode; ValueError for any other value.  The request's draws start when it is admitted."""
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
         g_idx = generator.device.index if generator.device.index is not None else torch.cuda.current_device()
@@ -277,6 +292,9 @@ class SamplingEngine:
             if torch.is_tensor(v):
                 raise ValueError(f"{name}: a request takes one value (got a tensor)")
         trunc = ops.truncation_table(top_k, top_p, 1, self.model.num_labels)
+        if isinstance(tiling, (list, tuple)):
+            raise ValueError("tiling: a request takes one value (got a list)")
+        wrap = ops.tiling_codes(tiling, 1)[0]
         renoise_steps = steps - 1 if renoise_steps is None else int(renoise_steps)
         cond_steps = steps if sampling_conditional_steps is None else int(sampling_conditional_steps)
         self._check_cond("model_inputs", model_inputs)
@@ -300,7 +318,7 @@ class SamplingEngine:
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
-                      sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)))
+                      sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap)
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
@@ -376,7 +394,8 @@ class SamplingEngine:
             buf = ops.to_device_async(host, dev)                 # the step's one host-to-device copy
             draw_d, renoise_d = buf[:2 * Bc].view(Bc, 2), buf[2 * Bc:4 * Bc].view(Bc, 2)
             parts = {"f32": buf[lay["f32"][1]:lay["f32"][1] + lay["f32"][2]].view(torch.float32),
-                     "i32": buf[lay["i32"][1]:lay["i32"][1] + lay["i32"][2]].view(torch.int32)}
+                     "i32": buf[lay["i32"][1]:lay["i32"][1] + lay["i32"][2]].view(torch.int32),
+                     "u8": buf[lay["u8"][1]:lay["u8"][1] + lay["u8"][2]].view(torch.uint8)}
 
             def part(name):
                 dt, o, n = lay[name]
@@ -384,13 +403,14 @@ class SamplingEngine:
             r_d, params_d, t_next_d = part("r"), part("params").view(Bc, 3), part("t_next")
             row_slot_d, kv_slot_d, modes_d = part("row_slot"), part("kv_slot"), part("modes")
             trunc_d = (part("top_k"), part("top_p")) if plan.truncates else None
+            wrap_d = part("wrap") if plan.wraps else None
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_pairs, self.s_max, self.n_slots, kv_slot_d)
             if any(q.attn_weights is not None for q in plan.order):       # row b reads the weights of its token slot
-                feats = m.features(x, r_d, cond, self.w_pool, Bc, n_pairs=n_pairs, w_len=self.w_len, w_row=row_slot_d)
+                feats = m.features(x, r_d, cond, self.w_pool, Bc, n_pairs=n_pairs, w_len=self.w_len, w_row=row_slot_d, wrap=wrap_d)
             else:
-                feats = m.features(x, r_d, cond, n_pairs=n_pairs)
+                feats = m.features(x, r_d, cond, n_pairs=n_pairs, wrap=wrap_d)
             if mixed:       # argmax and quant rows through the logits path, the multinomial rows in one fused-sampler launch
                 sampled = m.sample_tokens_modes(feats, Bc, n_pairs, H, W, params_d, draw_d, plan.modes, modes_d, self._codebook(),
                                                 out=self._sampled[:Bc], trunc=trunc_d)
@@ -416,7 +436,8 @@ class SamplingEngine:
                 return []
             dec = [q for q in done if q.decode]
             if dec:
-                imgs = self.vqmodel.decode_indices_u8(torch.cat([self.tokens[q.slot:q.slot + 1] for q in dec]))
+                tiling = [("none", "x", "y", "xy")[q.wrap] for q in dec]
+                imgs = self.vqmodel.decode_indices_u8(torch.cat([self.tokens[q.slot:q.slot + 1] for q in dec]), tiling)
                 for i, q in enumerate(dec):
                     q.result = imgs[i:i + 1]
             for q in done:

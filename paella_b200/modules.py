@@ -622,7 +622,8 @@ class Paella(nn.Module):
     # -------------------------------------------------------------- forward pieces
     def features(self, x: torch.Tensor, r: torch.Tensor, cond: ConditioningCache, attn_weights=None,
                  attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None,
-                 w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None,
+                 wrap: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
@@ -633,7 +634,10 @@ class Paella(nn.Module):
         ``attn_weights``: one vector for samples [0, attn_weights_batch), or with ``w_len`` a device float32 table [rows, w_ld]
         of per-sample vectors: sample b < attn_weights_batch reads row ``w_row[b]`` (int32 device [attn_weights_batch]; None:
         row b) and its first ``w_len[row]`` entries (int32 device [rows]; 0 = unweighted), pb200_paella_features_weighted.
-        Each length must not exceed the sample's max_attn_weights."""
+        Each length must not exceed the sample's max_attn_weights.
+        ``wrap``: seamless tiling, a device uint8 table of one byte per sample of x (ops.tiling_table; bit 0 wraps x, bit 1
+        wraps y): the ResBlocks' depthwise convolutions pad circularly on the wrapped axes, and sample B + i of a CFG batch reads
+        byte i (pb200_paella_features_tiled).  None launches exactly the untiled kernels."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -643,6 +647,8 @@ class Paella(nn.Module):
                 raise PaellaB200Error(f"features: n_pairs={n_pairs} for {Bt} samples (and not with cfg_pairs)")
         else:
             n_pairs = Bt if cfg_pairs else 0
+        if wrap is not None and (wrap.dtype != torch.uint8 or wrap.numel() != Bt or wrap.device != dev):
+            raise PaellaB200Error(f"features: wrap must be a uint8 table of {Bt} entries on {dev}")
         Bt += n_pairs
         if Bt != cond.batch_total:
             raise PaellaB200Error(f"batch {Bt} does not match the conditioning cache ({cond.batch_total})")
@@ -656,12 +662,24 @@ class Paella(nn.Module):
                         or w_len.numel() != attn_weights.shape[0] or (w_row is not None and w_row.numel() < attn_weights_batch):
                     raise PaellaB200Error("features: a per-sample weight table is float32 [rows, w_ld] with int32 w_len [rows] "
                                           "and an optional int32 w_row [attn_weights_batch]")
+                if wrap is not None:
+                    check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                        ptr(cond.slot_map), cond.s_max, ptr(attn_weights), 0, attn_weights.shape[1],
+                                                        ptr(w_len), ptr(w_row), attn_weights_batch, ptr(wrap), ptr(feats), ptr(ws),
+                                                        ws.numel(), current_stream()), "pb200_paella_features_tiled")
+                    return feats
                 check(L.pb200_paella_features_weighted(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
                                                        ptr(cond.slot_map), cond.s_max, ptr(attn_weights), 0, attn_weights.shape[1],
                                                        ptr(w_len), ptr(w_row), attn_weights_batch, ptr(feats), ptr(ws), ws.numel(),
                                                        current_stream()), "pb200_paella_features_weighted")
                 return feats
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
+            if wrap is not None:        # the single weight vector is the weighted call with w_ld = 0 and no w_len
+                check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                    ptr(cond.slot_map), cond.s_max, ptr(aw), aw.numel() if aw is not None else 0, 0,
+                                                    None, None, attn_weights_batch, ptr(wrap), ptr(feats), ptr(ws), ws.numel(),
+                                                    current_stream()), "pb200_paella_features_tiled")
+                return feats
             check(L.pb200_paella_features_pairs(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
                                                 ptr(cond.slot_map), cond.s_max, ptr(aw),
                                                 aw.numel() if aw is not None else 0, attn_weights_batch, ptr(feats), ptr(ws),
@@ -891,17 +909,25 @@ class Paella(nn.Module):
     def forward(self, x, r, byt5, clip=None, clip_image=None, x_cat=None, **kwargs):
         """ref/src/modules.py:263-275 / ref/utils/modules.py:268-282: logits [B, num_labels, H, W] fp32.
         ``attn_weights``: one vector for every sample, or a list or tuple of B entries, each None or a 1-D CPU float tensor
-        that weights sample b alone (ValueError for a bad entry, before anything is enqueued)."""
+        that weights sample b alone (ValueError for a bad entry, before anything is enqueued).
+        ``tiling``: seamless tiling (keyword only): None / 'none', 'x' (left and right edges wrap), 'y' (top and bottom wrap) or
+        'xy', one for every sample or a list or tuple of B values.  The ResBlocks' depthwise convolutions then pad circularly,
+        as the reference with ``padding_mode='circular'`` on those Conv2d modules does.  ValueError, before anything is
+        enqueued, for an unknown value, a list of the wrong length or a tensor."""
         if x_cat is not None:
             x = torch.cat([x, x_cat], dim=1)
         attn_weights = kwargs.pop("attn_weights", None)
+        tiling = kwargs.pop("tiling", None)
         if kwargs:
             raise TypeError(f"unexpected keyword arguments {sorted(kwargs)}")
         B, H, W = x.shape
+        wrap = ops.tiling_table(tiling, B)
         cond_len = self.conditioning_seq_len({"byt5": byt5, "clip": clip, "clip_image": clip_image})
         aw, w_len = self._attn_weights_table(attn_weights, B, (H, W), cond_len)
         cond = self._cond_for_forward(byt5, clip, clip_image, (H, W))
-        feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len)
+        if wrap is not None:
+            wrap = ops.to_device_async(wrap, self._device())
+        feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len, wrap=wrap)
         return self.logits_from_features(feats, B, H, W)
 
     def _cond_for_forward(self, byt5, clip, clip_image, hw):

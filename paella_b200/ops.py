@@ -266,6 +266,38 @@ def truncation_table(top_k, top_p, batch: int, num_labels: int) -> Optional[Tupl
     return k, p
 
 
+# ------------------------------------------------------------------ seamless tiling
+# The denoiser's ResBlock depthwise convolutions and the decoder's ReplicationPad2d / ConvTranspose2d read across a wrapped edge
+# (include/paella_b200.h, pb200_paella_features_tiled, pb200_vqgan_decode_tiled).  The kernels read a device table of one byte per
+# sample: bit 0 wraps x (left and right edges), bit 1 wraps y (top and bottom).
+TILINGS = {None: 0, "none": 0, "x": 1, "y": 2, "xy": 3}
+
+
+def _tiling_code(name: str, value) -> int:
+    if not (value is None or isinstance(value, str)) or value not in TILINGS:
+        raise ValueError(f"{name}={value!r}: expected None, 'none', 'x', 'y' or 'xy'")
+    return TILINGS[value]
+
+
+def tiling_codes(tiling, batch: int) -> list:
+    """``tiling`` (one value for every sample, or a list or tuple of ``batch`` values) -> the ``batch`` wrap codes.  ValueError,
+    before anything is enqueued, for an unknown value, a list of the wrong length, or a tensor."""
+    if isinstance(tiling, (list, tuple)):
+        if len(tiling) != batch:
+            raise ValueError(f"tiling: got {len(tiling)} entries for a batch of {batch} (one per sample)")
+        return [_tiling_code(f"tiling[{b}]", v) for b, v in enumerate(tiling)]
+    if torch.is_tensor(tiling):
+        raise ValueError("tiling: expected None, 'none', 'x', 'y', 'xy' or a list of them (got a tensor)")
+    return [_tiling_code("tiling", tiling)] * batch
+
+
+def tiling_table(tiling, batch: int) -> Optional[torch.Tensor]:
+    """``tiling`` as the host wrap table: uint8 [batch], or None when no sample wraps (the call then launches exactly the
+    zero- / replication-padding kernels).  ValueError as in ``tiling_codes``."""
+    codes = tiling_codes(tiling, batch)
+    return torch.tensor(codes, dtype=torch.uint8) if any(codes) else None
+
+
 # ------------------------------------------------------------------ per-sample sampling modes
 # The notebook's sampling modes (paella_inference.ipynb cell 3).  'multinomial' draws H*W*num_labels exponentials per step; 'argmax'
 # and 'quant' draw nothing.  A step with several modes sends one int32 table to the device: the mode code of every sample, then

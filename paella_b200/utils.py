@@ -35,6 +35,13 @@ multinomial draw to its k most likely codes, then to the smallest top set of the
 (ops.truncation_table; pb200_paella_sample_tokens_params_trunc).  The draw uses the same random numbers as without
 truncation, so every generator ends at the same offset and the per-sample guarantees above hold for truncated rows too.
 Argmax and quant steps are not truncated; ``exact=True`` does not take truncation.
+
+Seamless tiling: ``tiling`` (all three functions; None / 'none', 'x', 'y' or 'xy', one for the call or a list or tuple of B values)
+makes sample i's token grid wrap around on its axes: 'x' joins the left and right edges (a horizontal panorama), 'xy' all four (a
+texture that repeats without a seam).  The denoiser's ResBlock depthwise convolutions then pad circularly (ops.tiling_table;
+pb200_paella_features_tiled), the only place a Paella token grid meets its edges.  Tiling draws no random numbers, so every
+generator ends at the same offset, and the per-sample guarantees above hold for tiled rows too.  ``sample(..., decode=vqmodel)``
+decodes each image with its own tiling.
 """
 from __future__ import annotations
 
@@ -141,7 +148,7 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
-                 codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None):
+                 codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None):
     """``modes``: None, or per step the list of B mode names (sampling_modes) -- a step whose modes differ samples each row in
     its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the scalar path in that mode.  ``top_k`` /
     ``top_p``: the truncation of the multinomial draws (module docstring); a truncating call takes the per-sample table path."""
@@ -149,6 +156,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     dev = model._device()
     check_region(region, init_x, latent_shape, dev)
     trunc = ops.truncation_table(top_k, top_p, B, model.num_labels)
+    wrap = ops.tiling_table(tiling, B)
     if exact and trunc is not None:
         raise ValueError("exact=True restates the reference op for op, which has no top_k / top_p truncation")
     use_cfg_any = cfgs is not None
@@ -161,10 +169,12 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         ops.check_generators(generator, B, dev)
         ops.check_per_sample_numel(H * W * model.num_labels)
     with torch.inference_mode():
-        # one copy for the whole loop: [steps][B][3] params and [steps + 1][B] noise levels, and a CPU region
+        # one copy for the whole loop: [steps][B][3] params and [steps + 1][B] noise levels, a CPU region and the wrap table
         region_host = region is not None and region.device.type == "cpu"
         parts = (list(sched) if sched is not None else []) + (list(trunc) if trunc is not None else []) + ([region] if region_host else [])
+        parts += [wrap] if wrap is not None else []
         parts_d = ops.to_device_packed(parts, dev) if parts else []
+        wrap_d = parts_d.pop() if wrap is not None else None
         if sched is not None:
             params_d, r_d = parts_d[0], parts_d[1]
         trunc_d = (parts_d[2], parts_d[3]) if trunc is not None else None
@@ -209,7 +219,8 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 cfg_i, temp_i = (float(cfgs[i]) if guided else None), float(temperatures[i])
             else:
                 r, params_i = r_d[i], params_d[i]
-            feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided, w_len=w_len)
+            feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided, w_len=w_len,
+                                   wrap=wrap_d)
             if step_modes is not None:
                 sampled = _sample_modes_step(model, feats, B, H, W, guided, params_i, step_modes, generator, codebook, dev, trunc_d)
             elif mode == "multinomial" and not exact:
@@ -311,23 +322,23 @@ def load_conditional_models(byt5_model_name, vqgan_path, device):
     return vqgan, (byt5_tokenizer, byt5)
 
 
-def _decode_tail(tokens, decode, decode_output):
+def _decode_tail(tokens, decode, decode_output, tiling=None):
     """The step after the path (SURVEY.md §8 f2; ref/src_distributed/train.py:168-171, notebook nb:354-357): the final token
     grid goes straight into the f4 decoder on the same stream -- no host round trip, no separate clamp / byte pass."""
     if decode is None:
         return tokens
     if decode_output == "uint8":
-        return decode.decode_indices_u8(tokens)
+        return decode.decode_indices_u8(tokens, tiling)
     if decode_output == "clamp":
-        return decode.decode_indices_clamped(tokens)
+        return decode.decode_indices_clamped(tokens, tiling)
     if decode_output == "raw":
-        return decode.decode_indices(tokens)
+        return decode.decode_indices(tokens, tiling)
     raise ValueError(f"decode_output={decode_output!r}: expected 'uint8', 'clamp' or 'raw'")
 
 
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
            cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
-           top_k=None, top_p=None):
+           top_k=None, top_p=None, tiling=None):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -339,7 +350,10 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     Per-sample settings (module docstring): ``cfg`` [B], ``temperature`` [B, 2], ``t_start`` / ``t_end`` [B].  A per-sample cfg
     of 0 is unguided like the scalar ``cfg=0``; so is 1.0, and an all-zero tensor makes the whole call unguided.
     ``top_k`` / ``top_p`` (module docstring): None, a scalar, or a CPU tensor [B]; ValueError, before anything is enqueued and
-    before any generator advances, for a bad value and for truncation with exact=True."""
+    before any generator advances, for a bad value and for truncation with exact=True.
+    ``tiling`` (module docstring): seamless tiling per call or per sample; with ``decode`` each image is decoded with its own
+    tiling.  ValueError, before anything is enqueued and before any generator advances, for an unknown value, a list of the
+    wrong length or a tensor."""
     per_sample_cfg = torch.is_tensor(cfg)
     if per_sample_cfg:
         cfg_vals = [v if v else 1.0 for v in ops.per_sample_values("cfg", cfg, latent_shape[0])]   # f*1 + u*0 = f
@@ -351,20 +365,21 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
         raise TypeError("sample(): cfg is set but unconditional_inputs is None")
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, None, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
-                          per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p)
-    return _decode_tail(out, decode, decode_output)
+                          per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling)
+    return _decode_tail(out, decode, decode_output, tiling)
 
 
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
-                       exact=False, generator=None, region=None, top_k=None, top_p=None):
+                       exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
     docstring): bool [B, H, W] on the CPU or the model's device, True where tokens are generated; ``init_x`` then holds the
     tokens kept elsewhere.  ValueError, before anything is enqueued and before any generator advances, for a region without
     init_x, of another shape or dtype, or on another device.  ``top_k`` / ``top_p`` as in ``sample``; a shard given
-    ``top_k[lo:hi]`` computes what rows [lo, hi) compute."""
+    ``top_k[lo:hi]`` computes what rows [lo, hi) compute.  ``tiling`` as in ``sample``; a shard given ``tiling[lo:hi]`` computes
+    what rows [lo, hi) compute."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -372,14 +387,15 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     cfgs = _cfg_schedule(cfg, latent_shape[0], steps)
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
-                          generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p)
+                          generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
+                          tiling=tiling)
     return out
 
 
 def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None, init_x=None, steps=12, renoise_steps=None,
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
-                    generator=None, region=None, top_k=None, top_p=None):
+                    generator=None, region=None, top_k=None, top_p=None, tiling=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -392,7 +408,8 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     or an int >= 0; row i then equals row i of the call with mode i and quant step i for every sample, on per-sample
     generators.  A call whose modes differ within a step needs ``generator=[g_0, ..., g_{B-1}]`` (the argmax and quant rows draw
     nothing, the multinomial ones draw per sample); one whose entries are all equal is the scalar call (sampling_modes).
-    ``top_k`` / ``top_p`` as in ``sample``: they truncate the multinomial steps only."""
+    ``top_k`` / ``top_p`` as in ``sample``: they truncate the multinomial steps only.  ``tiling`` as in ``sample``: the
+    intermediates are those of the tiled call."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -409,4 +426,4 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     return _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                         temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, True,
                         sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes,
-                        top_k=top_k, top_p=top_p)
+                        top_k=top_k, top_p=top_p, tiling=tiling)

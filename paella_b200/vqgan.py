@@ -243,9 +243,11 @@ class VQModel(nn.Module):
         mse = torch.mean((qe - lat) ** 2)
         return qe / self.scale_factor, lat / self.scale_factor, idx, mse + mse * 0.25
 
-    def _decode(self, idx, lat, mode=_lib.IMG_F32_NCHW):
+    def _decode(self, idx, lat, mode=_lib.IMG_F32_NCHW, tiling=None):
         self._ensure_packed()
         L, dev = lib(), self._device()
+        B = idx.shape[0] if idx is not None else lat.shape[0]
+        wrap = ops.tiling_table(tiling, B)
         with torch.cuda.device(dev):
             if idx is not None:
                 idx = idx.to(device=dev, dtype=torch.int64).contiguous()
@@ -258,26 +260,36 @@ class VQModel(nn.Module):
             else:
                 img = torch.empty(B, 3, 4 * h, 4 * w, dtype=torch.float32, device=dev)
             ws = self._ws(L.pb200_vqgan_workspace_bytes(self._handle, B, 4 * h, 4 * w))
+            if wrap is not None:
+                wrap = ops.to_device_async(wrap, dev)
+                check(L.pb200_vqgan_decode_tiled(self._handle, ptr(idx), ptr(lat), B, h, w, ptr(img), mode, ptr(wrap), ptr(ws),
+                                                 ws.numel(), current_stream()), "pb200_vqgan_decode_tiled")
+                return img
             check(L.pb200_vqgan_decode_ex(self._handle, ptr(idx), ptr(lat), B, h, w, ptr(img), mode, ptr(ws), ws.numel(),
                                           current_stream()), "pb200_vqgan_decode_ex")
         return img
 
-    def decode(self, x):
+    # ``tiling`` (every decode below): seamless tiling, None / 'none', 'x', 'y' or 'xy' for every image or a list or tuple of B
+    # values.  On a wrapped axis the ResBlocks' ReplicationPad2d pads circularly and the ConvTranspose2d reads its input
+    # modulo the grid, so decoding tokens rolled by (a, b) gives the image rolled by (4a, 4b), and a tiled image repeats
+    # without a seam (pb200_vqgan_decode_tiled).  ValueError, before anything is enqueued, for an unknown value, a list of the
+    # wrong length or a tensor.
+    def decode(self, x, tiling=None):
         """ref/src/vqgan.py:97-101."""
-        return self._decode(None, x * self.scale_factor)
+        return self._decode(None, x * self.scale_factor, tiling=tiling)
 
-    def decode_indices(self, x):
+    def decode_indices(self, x, tiling=None):
         """ref/src/vqgan.py:103-107 (no scale_factor on this path, as in the reference)."""
-        return self._decode(x, None)
+        return self._decode(x, None, tiling=tiling)
 
-    def decode_indices_clamped(self, x):
+    def decode_indices_clamped(self, x, tiling=None):
         """``decode_indices(x).clamp(0, 1)`` (ref/src_distributed/train.py:168-171) with the clamp fused into the decoder's last kernel."""
-        return self._decode(x, None, _lib.IMG_F32_NCHW_CLAMP01)
+        return self._decode(x, None, _lib.IMG_F32_NCHW_CLAMP01, tiling)
 
-    def decode_indices_u8(self, x):
+    def decode_indices_u8(self, x, tiling=None):
         """uint8 NHWC images [B,4h,4w,3]: ``decode_indices(x).clamp(0,1)`` followed by torchvision save_image's byte conversion
         (``mul(255).add_(0.5).clamp_(0,255).to(uint8)`` on the HWC view), fused into the decoder's last kernel."""
-        return self._decode(x, None, _lib.IMG_U8_NHWC)
+        return self._decode(x, None, _lib.IMG_U8_NHWC, tiling)
 
     def forward(self, x, quantize=False):
         qe, x, _, vq_loss = self.encode(x, quantize)
