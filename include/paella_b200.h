@@ -250,6 +250,21 @@ int pb200_attention_slots(const void* qkv16, const void* ckv16, const int* kv_le
                           int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
                           int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
                           void* stream);
+/* pb200_attention_slots with regional prompts, for samples b < mask_batch:
+ *   q_mask       uint8 [mask_batch][positions]: bit k of query q's byte set = it sees the conditioning of prompt k;
+ *   region_slot  int32 [rows][max_regions]: the block of ckv16 (and entry of kv_len) of prompts 1..max_regions, -1 = none;
+ *   mask_row     int32 [mask_batch]: the region_slot row sample b reads, or NULL: row b;
+ *   max_regions  0..7.
+ * Prompt 0 is sample b's own block kv_slot[b].  A query attends, in one softmax, to every self key and to the conditioning
+ * keys of each prompt whose bit it has; a query must have at least one bit (or self_attn).  A tile of 64 queries loads no
+ * key of a prompt none of them sees.  Samples b >= mask_batch attend as in pb200_attention_slots, and a query whose byte is
+ * 1 (prompt 0 alone) gets the same bits as there.  attn_weights apply to [self ; prompt 0] and must not be combined with
+ * regions on one sample.  [ref/src/modules.py:7-19 with a boolean attn_mask on nn.MultiheadAttention] */
+int pb200_attention_regional(const void* qkv16, const void* ckv16, const int* kv_len, const int* kv_slot, int n_slots, void* out16,
+                             int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
+                             int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
+                             const uint8_t* q_mask, const int* region_slot, const int* mask_row, int max_regions, int mask_batch,
+                             void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Denoiser (ref/src/modules.py:109-283, ref/utils/modules.py) as an opaque handle.
@@ -357,6 +372,20 @@ int pb200_paella_features_tiled(pb200_paella* m, const int64_t* tokens, const fl
                                 const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
                                 int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, float* features,
                                 void* workspace, int64_t workspace_bytes, void* stream);
+/* pb200_paella_features_tiled with regional prompts on the conditional rows [0, batch_total - n_pairs):
+ *   prompt_mask  DEVICE uint8 [rows][h*w] token masks: bit k (k >= 1) set = the token lies in region k, bit 0 = in no region;
+ *   mask_row     DEVICE int32 [batch_total - n_pairs]: the prompt_mask / region_slot row of sample b, or NULL: row b;
+ *   region_slot  DEVICE int32 [rows][max_regions]: the cache slot of prompt k >= 1 (projected like any conditioning), -1 = none;
+ *   max_regions  0..7.
+ * A position of an AttnBlock level (stride patch_size * 2^level tokens) carries the OR of its footprint's token masks and attends
+ * to every self key and to the conditioning of each prompt it has a bit of, prompt 0 being the sample's own kv_slot (see
+ * pb200_attention_regional).  The unconditional rows are never masked.  attn weights must not be set on a regional sample.
+ * prompt_mask = NULL is pb200_paella_features_tiled, the same launches. */
+int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,
+                                   int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w,
+                                   int n_w, int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
+                                   const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
+                                   float* features, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* out_mapper on features -> logits fp32 NCHW [B, num_labels, H*W]   (ref/src/modules.py:184-187,274) */
 int pb200_paella_logits(pb200_paella* m, const float* features, int batch, int hw, float* logits_nchw,

@@ -95,6 +95,9 @@ SIGNATURES = {
                                 c_int, c_int, c_void_p]),
     "pb200_attention_slots": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                       c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]),
+    "pb200_attention_regional": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                         c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                         c_int, c_void_p]),
     "pb200_paella_create": (c_int, [POINTER(PaellaConfig), POINTER(c_void_p)]),
     "pb200_paella_destroy": (None, [c_void_p]),
     "pb200_paella_weight_bytes": (c_int64, [c_void_p]),
@@ -120,6 +123,9 @@ SIGNATURES = {
     "pb200_paella_features_tiled": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
                                             c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                             c_int64, c_void_p]),
+    "pb200_paella_features_regional": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                               c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                               c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_int64, c_void_p]),
     "pb200_paella_sample_tokens_pairs_skip": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,

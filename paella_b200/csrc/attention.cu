@@ -41,9 +41,12 @@ constexpr float NEG_BIG = -1e30f;
 
 // One CTA per (64 queries, head, sample); each warp owns 16 queries and walks the keys in 64-key chunks
 // (double-buffered cp.async).  It runs every head dim other than 80 (csrc/attention_wg.cu), and head_dim 80 with
-// PB200_ATTN_MMA_SYNC=1.
-template <int HD>
-__global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
+// PB200_ATTN_MMA_SYNC=1.  REG (attention_kernel_regional): regional prompts (AttnRegion): the tile walks [self ; prompt 0]
+// as above, then the chunks of every further prompt some query of it sees, each from the prompt's own first row
+// (attn_build_segs); a row's keys of a prompt it does not see are masked like keys past the end, so its softmax is exact over
+// the keys it sees.
+template <int HD, bool REG>
+__device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRegion& rg) {
     constexpr int LDS = HD + 8;           // padded row: (HD+8)*2 bytes is an odd multiple of 16 -> conflict-free ldmatrix
     constexpr int CPR = HD / 8;           // 16-byte chunks per row
     constexpr int QROWS = ATT_BM;
@@ -65,6 +68,14 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
     const int Nk = n_self + n_cond;
     const __half* qkv_b = p.qkv + (int64_t)b * p.P * ldq;
     const __half* ckv_b = p.ckv + (int64_t)slot * p.S_max * ldc;
+    AttnSegs* segs = reinterpret_cast<AttnSegs*>(sVb + n_buf * ATT_BN * LDS);
+    if constexpr (REG) {
+        if (warp == 0) {
+            const uint32_t u = attn_tile_union(p, rg, b, q0, lane);
+            if (lane == 0) attn_build_segs(p, rg, b, u, true, *segs);
+        }
+        __syncthreads();
+    }
 
     // K/V chunk j0.. -> buffer `buf` with 16-byte cp.async (zero-fill for keys past the end)
     auto load_chunk = [&](int j0, int buf) {
@@ -88,6 +99,32 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
             cp_async16(smem_u32(sV + r * LDS + cc * 8), vs, nbytes);
         }
     };
+    // chunk c of the regional walk -> buffer `buf`: keys before the segment's `from` are self keys, the rest its prompt's rows
+    auto load_chunk_reg = [&](int c, int buf) {
+        int si = 0;
+        while (c >= segs->first[si + 1]) ++si;
+        const int j0 = (c - segs->first[si]) * ATT_BN, len = segs->len[si], from = segs->from[si];
+        const __half* cb = p.ckv + (int64_t)segs->slot[si] * p.S_max * ldc;
+        __half* sK = sKb + buf * ATT_BN * LDS;
+        __half* sV = sVb + buf * ATT_BN * LDS;
+        for (int i = tid; i < ATT_BN * CPR; i += 128) {
+            const int r = i / CPR, cc = i - r * CPR;
+            const int j = j0 + r;
+            const __half *ks = qkv_b, *vs = qkv_b;
+            uint32_t nbytes = 0;
+            if (j < from) {
+                ks = qkv_b + (int64_t)j * ldq + h * HD + cc * 8 + E;
+                vs = ks + E;
+                nbytes = 16;
+            } else if (j < len) {
+                ks = cb + (int64_t)(j - from) * ldc + h * HD + cc * 8;
+                vs = ks + E;
+                nbytes = 16;
+            }
+            cp_async16(smem_u32(sK + r * LDS + cc * 8), ks, nbytes);
+            cp_async16(smem_u32(sV + r * LDS + cc * 8), vs, nbytes);
+        }
+    };
     // Q rides in the same cp.async group as the first K/V chunk (a register-staged Q load costs 5 serialised global
     // round trips before anything else can start)
     for (int c = tid; c < QROWS * CPR; c += 128) {
@@ -95,7 +132,13 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
         const bool ok = q0 + r < p.P;
         cp_async16(smem_u32(sQ + r * LDS + cc * 8), ok ? qkv_b + (int64_t)(q0 + r) * ldq + h * HD + cc * 8 : qkv_b, ok ? 16u : 0u);
     }
-    load_chunk(0, 0);
+    int n_chunks = 0;
+    if constexpr (REG) {
+        n_chunks = segs->first[segs->n];
+        if (n_chunks > 0) load_chunk_reg(0, 0);
+    } else {
+        load_chunk(0, 0);
+    }
     cp_async_commit();
 
     const int qrow0 = warp * 16;                              // this warp's 16 query rows inside the tile
@@ -109,6 +152,9 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
     const int n_w = attn_weight_row(p, b, w_row);
     const bool weighted = n_w > 0;
     const int w_start = Nk - n_w;
+    uint32_t row_mask[2] = {0u, 0u};
+    if constexpr (REG)
+        for (int r = 0; r < 2; ++r) row_mask[r] = attn_row_mask(p, rg, b, q0 + warp * 16 + g + 8 * r);
 
     auto load_q_frags = [&]() {
 #pragma unroll
@@ -116,16 +162,18 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
             ldmatrix_x4(qf[ks], smem_u32(sQ + (qrow0 + (lane & 15)) * LDS + ks * 16 + (lane >> 4) * 8));
     };
 
-    // one online-softmax pass of this warp's 16 query rows over the 64 keys j0.. held in (sK, sV)
-    auto process_chunk = [&](int j0, const __half* sK, const __half* sV) {
-        const bool full = j0 + ATT_BN <= Nk;      // warp-uniform: no key of this chunk is masked
+    // one online-softmax pass of this warp's 16 query rows over the 64 keys j0.. held in (sK, sV); regional: of a segment of
+    // seg_nk keys, bit `bit` of a row's mask gating its keys from `from` on
+    auto process_chunk = [&](int j0, const __half* sK, const __half* sV, int seg_nk, int from, int bit) {
+        auto visible = [&](int key, int r) { return key < seg_nk && (key < from || ((row_mask[r] >> bit) & 1u)); };
+        const bool full = !REG && j0 + ATT_BN <= Nk;      // warp-uniform: no key of this chunk is masked
         // ---- S = Q K^T
         float s[ATT_BN / 8][4];
 #pragma unroll
         for (int i = 0; i < ATT_BN / 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
 #pragma unroll
         for (int np = 0; np < ATT_BN / 16; ++np) {
-            if (j0 + np * 16 >= Nk) break;    // 16-key groups past the end are fully masked
+            if (j0 + np * 16 >= (REG ? seg_nk : Nk)) break;    // 16-key groups past the end are fully masked
 #pragma unroll
             for (int ks = 0; ks < HD / 16; ++ks) {
                 uint32_t kf[4];
@@ -148,7 +196,11 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
                 const int key = j0 + nt * 8 + 2 * t;
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                    if (key + (e & 1) >= Nk) s[nt][e] = NEG_BIG;
+                    if constexpr (REG) {
+                        if (!visible(key + (e & 1), e >> 1)) s[nt][e] = NEG_BIG;
+                    } else {
+                        if (key + (e & 1) >= Nk) s[nt][e] = NEG_BIG;
+                    }
                     mx[e >> 1] = fmaxf(mx[e >> 1], s[nt][e]);
                 }
             }
@@ -165,15 +217,17 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
         }
 #pragma unroll
         for (int nt = 0; nt < ATT_BN / 8; ++nt) {
-            if (!full && j0 + (nt >> 1) * 16 >= Nk) break;      // same groups the MMAs skip
+            if (!full && j0 + (nt >> 1) * 16 >= (REG ? seg_nk : Nk)) break;      // same groups the MMAs skip
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const float pv = exp2f(fmaf(s[nt][e], p.scale_log2, msc[e >> 1]));
+                float pv = exp2f(fmaf(s[nt][e], p.scale_log2, msc[e >> 1]));
+                // a row may see no key of this chunk yet: its running max is then the mask value itself
+                if constexpr (REG) pv = visible(j0 + nt * 8 + 2 * t + (e & 1), e >> 1) ? pv : 0.f;
                 rs[e >> 1] += pv;
                 s[nt][e] = pv;
             }
         }
-        if (weighted) {       // post-softmax, un-renormalised scaling of the last n_w key columns
+        if (weighted && (!REG || bit == 0)) {       // post-softmax, un-renormalised scaling of the last n_w key columns
 #pragma unroll
             for (int nt = 0; nt < ATT_BN / 8; ++nt) {
                 const int key = j0 + nt * 8 + 2 * t;
@@ -198,7 +252,7 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
         // ---- O += P V
 #pragma unroll
         for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-            if (j0 + kk * 16 >= Nk) break;    // P is zero there
+            if (j0 + kk * 16 >= (REG ? seg_nk : Nk)) break;    // P is zero there
             uint32_t a[4];
             a[0] = pack_half2(s[2 * kk][0], s[2 * kk][1]);
             a[1] = pack_half2(s[2 * kk][2], s[2 * kk][3]);
@@ -216,14 +270,29 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
 
     const bool warp_active = q0 + warp * 16 < p.P;       // warps past the last query only help with the loads
     int buf = 0;
-    for (int j0 = 0; j0 < Nk; j0 += ATT_BN, buf ^= 1) {
+    if constexpr (REG) {
+        for (int c = 0; c < n_chunks; ++c, buf ^= 1) {
+            if (c + 1 < n_chunks) load_chunk_reg(c + 1, buf ^ 1);
+            cp_async_commit();
+            cp_async_wait<1>();
+            __syncthreads();
+            if (c == 0) load_q_frags();
+            if (warp_active) {
+                int si = 0;
+                while (c >= segs->first[si + 1]) ++si;
+                process_chunk((c - segs->first[si]) * ATT_BN, sKb + buf * ATT_BN * LDS, sVb + buf * ATT_BN * LDS, segs->len[si],
+                              segs->from[si], segs->bit[si]);
+            }
+            __syncthreads();
+        }
+    } else for (int j0 = 0; j0 < Nk; j0 += ATT_BN, buf ^= 1) {
         // prefetch the next chunk into the other buffer (all warps finished reading it at the end of the last iteration)
         if (j0 + ATT_BN < Nk) load_chunk(j0 + ATT_BN, buf ^ 1);
         cp_async_commit();
         cp_async_wait<1>();               // this chunk has landed (the prefetch may still be in flight)
         __syncthreads();
         if (j0 == 0) load_q_frags();
-        if (warp_active) process_chunk(j0, sKb + buf * ATT_BN * LDS, sVb + buf * ATT_BN * LDS);
+        if (warp_active) process_chunk(j0, sKb + buf * ATT_BN * LDS, sVb + buf * ATT_BN * LDS, 0, 0, 0);
         __syncthreads();                  // everyone is done with this buffer before it is refilled
     }
     cp_async_wait<0>();
@@ -241,23 +310,36 @@ __global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
     }
 }
 
-int launch_attention(const AttnParams& p, cudaStream_t st) {
+template <int HD>
+__global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) { attention_body<HD, false>(p, AttnRegion{}); }
+template <int HD>
+__global__ void __launch_bounds__(128) attention_kernel_regional(const AttnParams p, const AttnRegion rg) { attention_body<HD, true>(p, rg); }
+
+int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg) {
     PB_CHECK(p.nhead > 0 && p.E % p.nhead == 0, "attention: E=%d not divisible by nhead=%d", p.E, p.nhead);
     const int hd = p.E / p.nhead;
     PB_CHECK(p.E % 8 == 0, "attention: E must be a multiple of 8");
     if (p.B == 0 || p.P == 0) return 0;
     {
-        const int rc = launch_attention_wgmma(p, st);
+        const int rc = launch_attention_wgmma(p, st, rg);
         if (rc >= 0) return rc;
     }
     // algorithmic bytes: q, self k/v, out once; conditioning k/v once per sample
     ProfScope prof("attention", 2.0 * ((double)p.B * p.P * 4.0 * p.E + (double)p.B * p.S_max * 2.0 * p.E), st);
     dim3 grid(ceil_div(p.P, ATT_BM), p.nhead, p.B);
     PB_CHECK(grid.y <= 65535 && grid.z <= 65535, "attention: grid too large");
-    const size_t smem = (size_t)(ATT_BM + 4 * ATT_BN) * (hd + 8) * sizeof(__half);
+    const bool reg = rg != nullptr;
+    const size_t smem = (size_t)(ATT_BM + 4 * ATT_BN) * (hd + 8) * sizeof(__half) + (reg ? sizeof(AttnSegs) : 0);
     switch (hd) {
 #define PB_ATT_CASE(H)                                                                                              \
     case H: {                                                                                                       \
+        if (reg) {                                                                                                  \
+            static DeviceOnce attr_reg;                                                                             \
+            if (attr_reg.first())                                                                                   \
+                PB_CUDA(cudaFuncSetAttribute(attention_kernel_regional<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            attention_kernel_regional<H><<<grid, 128, smem, st>>>(p, *rg);                                          \
+            break;                                                                                                  \
+        }                                                                                                           \
         static DeviceOnce attr;                                                                                   \
         if (attr.first()) {                                                                                                \
             PB_CUDA(cudaFuncSetAttribute(attention_kernel<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \

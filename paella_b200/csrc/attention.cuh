@@ -25,6 +25,77 @@ struct AttnParams {
     const int* w_row = nullptr;
 };
 
+// Regional prompts, for samples b < mask_batch (the conditional rows).  Query q of sample b sees the conditioning of prompt k
+// iff bit k of q_mask[b * P + q] is set: prompt 0 is the sample's own kv_slot[b], prompts 1..max_regions the cache slots
+// region_slot[row * max_regions + k - 1] (-1: none), row = mask_row[b] (NULL: b), each read from its row 0 with its own
+// kv_len.  Self keys stay visible to every query.  A separate kernel argument, so the plain instances keep their code.
+struct AttnRegion {
+    const uint8_t* q_mask;
+    const int* region_slot;
+    const int* mask_row;
+    int max_regions;
+    int mask_batch;
+};
+
+constexpr int ATT_MAX_REGIONS = 7;      // prompts 1..7: the mask bits above prompt 0's
+
+// The key walk of a regional tile: segments of keys, each cut into 64-key chunks from its own first key.  Bit `bit` of a
+// query's mask gates the segment's keys from `from` on (-1: none gated).
+struct AttnSegs {
+    int n;
+    int first[ATT_MAX_REGIONS + 3];     // first chunk of segment i; first[n] = the tile's chunk count
+    int slot[ATT_MAX_REGIONS + 2];      // cache slot the segment's conditioning keys come from
+    int len[ATT_MAX_REGIONS + 2];       // keys
+    int bit[ATT_MAX_REGIONS + 2];
+    int from[ATT_MAX_REGIONS + 2];
+};
+
+// The OR of the masks of queries [q0, q0 + 64) of sample b (one warp; every lane gets it).  Samples past mask_batch see
+// prompt 0 alone.
+__device__ __forceinline__ uint32_t attn_tile_union(const AttnParams& p, const AttnRegion& rg, int b, int q0, int lane) {
+    if (b >= rg.mask_batch) return 1u;
+    uint32_t u = 0;
+    for (int q = q0 + lane; q < q0 + 64 && q < p.P; q += 32) u |= rg.q_mask[(int64_t)b * p.P + q];
+    return __reduce_or_sync(0xffffffffu, u);
+}
+
+// The mask of query row `row` of sample b (rows past P: every prompt, their output is never stored).
+__device__ __forceinline__ uint32_t attn_row_mask(const AttnParams& p, const AttnRegion& rg, int b, int row) {
+    if (b >= rg.mask_batch) return 1u;
+    return row < p.P ? rg.q_mask[(int64_t)b * p.P + row] : 0xffu;
+}
+
+// One thread: the segments of a tile whose queries' masks OR to u.  concat_self: the self keys and prompt 0 form one segment
+// (the mma.sync kernel's [self ; cond] walk, prompt 0 gated from key n_self on), otherwise the self keys are a segment of their
+// own.  A prompt outside u gets no segment, so no chunk of it is loaded.
+__device__ __forceinline__ void attn_build_segs(const AttnParams& p, const AttnRegion& rg, int b, uint32_t u, bool concat_self, AttnSegs& s) {
+    const int n_self = p.self_attn ? p.P : 0;
+    int n = 0, c = 0;
+    auto add = [&](int slot, int len, int bit, int from) {
+        s.first[n] = c; s.slot[n] = slot; s.len[n] = len; s.bit[n] = bit; s.from[n] = from;
+        c += (len + 63) / 64;
+        ++n;
+    };
+    const int slot0 = p.kv_slot ? p.kv_slot[b] : b;
+    const int len0 = (u & 1u) ? (p.kv_len ? p.kv_len[slot0] : p.S_max) : 0;
+    if (concat_self) {
+        add(slot0, n_self + len0, 0, n_self);
+    } else {
+        if (n_self > 0) add(-1, n_self, -1, 0);
+        if (u & 1u) add(slot0, len0, 0, 0);
+    }
+    if (b < rg.mask_batch && rg.region_slot) {
+        const int row = rg.mask_row ? rg.mask_row[b] : b;
+        for (int k = 1; k <= rg.max_regions && k <= ATT_MAX_REGIONS; ++k) {
+            if (!((u >> k) & 1u)) continue;
+            const int sl = rg.region_slot[(int64_t)row * rg.max_regions + k - 1];
+            if (sl >= 0) add(sl, p.kv_len ? p.kv_len[sl] : p.S_max, k, 0);
+        }
+    }
+    s.first[n] = c;
+    s.n = n;
+}
+
 // The weight row of sample b and its length (0: unweighted), per the table layout above.
 __device__ __forceinline__ int attn_weight_row(const AttnParams& p, int b, const float*& w) {
     if (p.attn_w == nullptr || b >= p.w_batch) return 0;
@@ -34,7 +105,11 @@ __device__ __forceinline__ int attn_weight_row(const AttnParams& p, int b, const
 }
 
 // Dispatch: the wgmma + TMA kernel (attention_wg.cu) for head_dim 80, the mma.sync kernel (attention.cu) for other head dims
-int launch_attention(const AttnParams& p, cudaStream_t st);
-int launch_attention_wgmma(const AttnParams& p, cudaStream_t st);      // 0 launched, 1 error, -1 shape not handled
+// (rg: the regional table, or NULL for the plain instances)
+int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr);
+int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr);      // 0 launched, 1 error, -1 shape not handled
+// Every AttnBlock level's position masks from token masks (ops.cu, regional_masks)
+int launch_regional_masks(const uint8_t* tok_mask, const int* mask_row, int batch, int h, int w, int patch, int n_levels,
+                          uint8_t* out, cudaStream_t st);
 
 }  // namespace pb

@@ -30,13 +30,20 @@ constexpr int AW_OFF_STAGE = AW_OFF_Q16 + AW_BM * 32;    // 10240
 constexpr int AW_OFF_VT = AW_OFF_STAGE + 2 * AW_STAGE;   // [80 dims][64 keys], SWIZZLE_128B
 constexpr int AW_OFF_BAR = AW_OFF_VT + AW_HD * 128;
 constexpr int AW_SMEM = AW_OFF_BAR + 64 + 1024;          // + alignment slack
+constexpr int AW_OFF_SEGS = AW_OFF_BAR + 64;             // regional instance: the tile's AttnSegs
+constexpr int AW_SMEM_REG = AW_OFF_SEGS + 256 + 1024;
+static_assert(sizeof(AttnSegs) <= 256, "AttnSegs outgrew its shared-memory slot");
 
 struct AttnMaps {
     CUtensorMap q64, q16, qv;      // over qkv [B*P, 3E]: 64x64 SW128, 16x64 SW32, 80x64 unswizzled boxes
     CUtensorMap c64, c16, cv;      // the same over ckv [slots*S_max, 2E]
 };
 
-__global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_constant__ AttnMaps maps, const AttnParams p) {
+// REG (attention_wgmma_kernel_regional): regional prompts (AttnRegion).  The tile walks its self keys, then the chunks of every
+// prompt some query of it sees (attn_build_segs), each from the prompt's own first row; a row's keys of a prompt it does not
+// see are masked the way keys at or past `valid` are, so its softmax is exact over the keys it sees.
+template <bool REG>
+__device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const AttnParams& p, const AttnRegion& rg) {
     pdl_launch_dependents();
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -52,13 +59,32 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
     const int n_cond = p.kv_len ? p.kv_len[slot] : p.S_max;
     const int Nk = n_self + n_cond;
     const int n_sc = (n_self + AW_BN - 1) / AW_BN;
-    const int n_chunks = n_sc + (n_cond + AW_BN - 1) / AW_BN;
+    int n_chunks = n_sc + (n_cond + AW_BN - 1) / AW_BN;
+    AttnSegs* segs = reinterpret_cast<AttnSegs*>(gbase + AW_OFF_SEGS);
+    auto seg_of = [&](int c) {
+        int si = 0;
+        while (c >= segs->first[si + 1]) ++si;
+        return si;
+    };
 
     auto issue_chunk = [&](int c) {         // one thread
         const int st = c & 1;
         const uint32_t sb = base + AW_OFF_STAGE + st * AW_STAGE;
         ptx::mbar_arrive_expect_tx(full_bar(st), AW_STAGE);
-        if (c < n_sc) {
+        if constexpr (REG) {
+            const int si = seg_of(c), k0 = (c - segs->first[si]) * AW_BN;
+            if (segs->slot[si] < 0) {
+                const int row = b * p.P + k0;
+                ptx::tma_load_2d(&maps.q64, full_bar(st), sb, E + h * AW_HD, row);
+                ptx::tma_load_2d(&maps.q16, full_bar(st), sb + AW_K64, E + h * AW_HD + 64, row);
+                ptx::tma_load_2d(&maps.qv, full_bar(st), sb + AW_K64 + AW_K16, 2 * E + h * AW_HD, row);
+            } else {
+                const int row = segs->slot[si] * p.S_max + k0;
+                ptx::tma_load_2d(&maps.c64, full_bar(st), sb, h * AW_HD, row);
+                ptx::tma_load_2d(&maps.c16, full_bar(st), sb + AW_K64, h * AW_HD + 64, row);
+                ptx::tma_load_2d(&maps.cv, full_bar(st), sb + AW_K64 + AW_K16, E + h * AW_HD, row);
+            }
+        } else if (c < n_sc) {
             const int row = b * p.P + c * AW_BN;
             ptx::tma_load_2d(&maps.q64, full_bar(st), sb, E + h * AW_HD, row);
             ptx::tma_load_2d(&maps.q16, full_bar(st), sb + AW_K64, E + h * AW_HD + 64, row);
@@ -70,6 +96,14 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
             ptx::tma_load_2d(&maps.cv, full_bar(st), sb + AW_K64 + AW_K16, E + h * AW_HD, row);
         }
     };
+    if constexpr (REG) {
+        if (wq == 0) {
+            const uint32_t u = attn_tile_union(p, rg, b, q0, lane);
+            if (lane == 0) attn_build_segs(p, rg, b, u, false, *segs);
+            __syncwarp();
+            n_chunks = segs->first[segs->n];
+        }
+    }
     if (wq == 0 && ptx::elect_one()) {
         ptx::mbar_init(q_bar, 1);
         ptx::mbar_init(full_bar(0), 1);
@@ -81,6 +115,11 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
         for (int c = 0; c < 2 && c < n_chunks; ++c) issue_chunk(c);
     }
     __syncthreads();
+    uint32_t row_mask[2] = {0u, 0u};
+    if constexpr (REG) {
+        n_chunks = segs->first[segs->n];
+        for (int r = 0; r < 2; ++r) row_mask[r] = attn_row_mask(p, rg, b, q0 + wq * 16 + (lane >> 2) + 8 * r);
+    }
 
     const float* w_row = nullptr;
     const int n_w = attn_weight_row(p, b, w_row);
@@ -96,10 +135,24 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
 
     for (int c = 0; c < n_chunks; ++c) {
         const int st = c & 1;
-        const bool self = c < n_sc;
-        const int k0 = self ? c * AW_BN : (c - n_sc) * AW_BN;             // first key of the chunk inside its source
-        const int valid = min(AW_BN, (self ? n_self : n_cond) - k0);
-        const int key0 = self ? k0 : n_self + k0;                           // index in [self ; cond]
+        int k0, valid, key0, lim[2];
+        if constexpr (REG) {
+            const int si = seg_of(c), bit = segs->bit[si];
+            k0 = (c - segs->first[si]) * AW_BN;
+            valid = min(AW_BN, segs->len[si] - k0);
+            key0 = bit < 0 ? k0 : bit == 0 ? n_self + k0 : Nk;              // only [self ; prompt 0] is weighted
+            for (int r = 0; r < 2; ++r) lim[r] = (bit < 0 || ((row_mask[r] >> bit) & 1u)) ? valid : 0;
+        } else {
+            const bool self = c < n_sc;
+            k0 = self ? c * AW_BN : (c - n_sc) * AW_BN;                      // first key of the chunk inside its source
+            valid = min(AW_BN, (self ? n_self : n_cond) - k0);
+            key0 = self ? k0 : n_self + k0;                                   // index in [self ; cond]
+        }
+        // keys at or past lim(i) are masked for the row of accumulator element i
+        auto lim_of = [&](int i) {
+            if constexpr (REG) return lim[(i >> 1) & 1];
+            else return valid;
+        };
         const uint32_t sb = base + AW_OFF_STAGE + st * AW_STAGE;
         ptx::mbar_wait(full_bar(st), (c >> 1) & 1);
         // V [key][dim] -> Vt [dim][key] with the 128-byte swizzle: the 80 8x8 blocks (8 key blocks x 10 dim blocks) through
@@ -144,7 +197,7 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
 #pragma unroll
         for (int i = 0; i < AW_BN / 2; ++i) {
             const int col = (i >> 2) * 8 + 2 * (lane & 3) + (i & 1);
-            if (col >= valid) s[i] = -1e30f;
+            if (col >= lim_of(i)) s[i] = -1e30f;
             mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
         }
         float corr[2], rs[2] = {0.f, 0.f}, msc[2];
@@ -160,11 +213,11 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
 #pragma unroll
         for (int i = 0; i < AW_BN / 2; ++i) {
             const int col = (i >> 2) * 8 + 2 * (lane & 3) + (i & 1);
-            float pv = col < valid ? exp2f(fmaf(s[i], p.scale_log2, msc[(i >> 1) & 1])) : 0.f;
+            float pv = col < lim_of(i) ? exp2f(fmaf(s[i], p.scale_log2, msc[(i >> 1) & 1])) : 0.f;
             rs[(i >> 1) & 1] += pv;
             if (weighted) {       // post-softmax, un-renormalised scaling of the last n_w keys
                 const int kj = key0 + col;
-                if (kj >= w_start && col < valid) pv *= w_row[kj - w_start];
+                if (kj >= w_start && col < lim_of(i) && (!REG || kj < Nk)) pv *= w_row[kj - w_start];
             }
             s[i] = pv;
         }
@@ -206,8 +259,16 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_const
     }
 }
 
+__global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_constant__ AttnMaps maps, const AttnParams p) {
+    attention_wgmma_body<false>(maps, p, AttnRegion{});
+}
+__global__ void __launch_bounds__(128) attention_wgmma_kernel_regional(const __grid_constant__ AttnMaps maps, const AttnParams p,
+                                                                       const AttnRegion rg) {
+    attention_wgmma_body<true>(maps, p, rg);
+}
+
 // returns 0 = launched, 1 = error, -1 = shape not handled here (head_dim != 80: the caller runs the mma.sync kernel)
-int launch_attention_wgmma(const AttnParams& p, cudaStream_t st) {
+int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg) {
     static const bool off = getenv("PB200_ATTN_MMA_SYNC") != nullptr;      // A/B knob: the mma.sync kernel for every shape
     if (off || p.E != AW_HD * p.nhead) return -1;
     const int64_t q_rows = (int64_t)p.B * p.P;
@@ -223,12 +284,20 @@ int launch_attention_wgmma(const AttnParams& p, cudaStream_t st) {
     } else {
         m.c64 = m.q64; m.c16 = m.q16; m.cv = m.qv;      // never read: no conditioning keys
     }
-    static DeviceOnce attr;
-    if (attr.first()) PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM));
     ProfScope prof("attention", 2.0 * ((double)p.B * p.P * 4.0 * p.E + (double)p.B * p.S_max * 2.0 * p.E), st);
     dim3 grid(ceil_div(p.P, AW_BM), p.nhead, p.B);
     PB_CHECK(grid.y <= 65535 && grid.z <= 65535, "attention: grid too large");
-    attention_wgmma_kernel<<<grid, 128, AW_SMEM, st>>>(m, p);
+    if (rg != nullptr) {
+        static DeviceOnce attr_reg;
+        if (attr_reg.first())
+            PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel_regional, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM_REG));
+        attention_wgmma_kernel_regional<<<grid, 128, AW_SMEM_REG, st>>>(m, p, *rg);
+    } else {
+        static DeviceOnce attr;
+        if (attr.first())
+            PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM));
+        attention_wgmma_kernel<<<grid, 128, AW_SMEM, st>>>(m, p);
+    }
     PB_LAUNCH_CHECK();
     return 0;
 }

@@ -158,6 +158,16 @@ int pb200_attention_slots(const void* qkv16, const void* ckv16, const int* kv_le
                           int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
                           int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
                           void* stream) {
+    return pb200_attention_regional(qkv16, ckv16, kv_len, kv_slot, n_slots, out16, batch, positions, s_max, embed, nhead, self_attn,
+                                    attn_weights, n_weights, weights_ld, weights_len, weights_row, weighted_batch, nullptr, nullptr,
+                                    nullptr, 0, 0, stream);
+}
+
+int pb200_attention_regional(const void* qkv16, const void* ckv16, const int* kv_len, const int* kv_slot, int n_slots, void* out16,
+                             int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
+                             int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
+                             const uint8_t* q_mask, const int* region_slot, const int* mask_row, int max_regions, int mask_batch,
+                             void* stream) {
     PB_CHECK(qkv16 && out16 && (ckv16 || s_max == 0), "attention: null pointer");
     PB_CHECK(self_attn || s_max > 0, "attention: no keys");
     PB_CHECK(n_slots >= 0 && weights_ld >= 0, "attention: negative slot count or weight stride");
@@ -173,7 +183,12 @@ int pb200_attention_slots(const void* qkv16, const void* ckv16, const int* kv_le
     p.scale_log2 = 1.4426950408889634f / sqrtf((float)(embed / (nhead > 0 ? nhead : 1)));
     p.attn_w = attn_weights; p.n_w = attn_weights ? n_weights : 0; p.w_batch = weighted_batch;
     p.w_ld = weights_ld; p.w_len = weights_len; p.w_row = weights_row;
-    return launch_attention(p, (cudaStream_t)stream);
+    if (q_mask == nullptr) return launch_attention(p, (cudaStream_t)stream);
+    PB_CHECK(max_regions >= 0 && max_regions <= ATT_MAX_REGIONS, "attention: max_regions=%d (0..%d)", max_regions, ATT_MAX_REGIONS);
+    PB_CHECK(mask_batch >= 0 && mask_batch <= batch, "attention: mask_batch=%d for %d samples", mask_batch, batch);
+    PB_CHECK(region_slot != nullptr || max_regions == 0, "attention: regional prompts need region_slot");
+    const AttnRegion rg{q_mask, region_slot, mask_row, max_regions, mask_batch};
+    return launch_attention(p, (cudaStream_t)stream, &rg);
 }
 
 }  // extern "C"

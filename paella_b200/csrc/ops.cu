@@ -7,6 +7,7 @@
 //   r_embed / film gen_r_embedding + TimestepBlock.mapper                  ref/src/modules.py:212-221,99-106
 //   silu_cast      AttnBlock.kv_mapper's SiLU                              ref/src/modules.py:71-74
 #include "ops.cuh"
+#include "attention.cuh"
 
 namespace pb {
 
@@ -981,5 +982,43 @@ static int transpose(const float* in, int B, int R, int Cc, float* out, cudaStre
 
 int launch_nchw_to_nhwc(const float* in, int B, int C, int HW, float* out, cudaStream_t st) { return transpose(in, B, C, HW, out, st); }
 int launch_nhwc_to_nchw(const float* in, int B, int C, int HW, float* out, cudaStream_t st) { return transpose(in, B, HW, C, out, st); }
+
+// Regional prompts: the mask of every position of every level, the OR of its (patch << level)^2 footprint of token masks.  Output
+// level l holds [batch][P_l] at batch * (P_0 + ... + P_{l-1}); sample b reads token-mask row mask_row[b] (NULL: b).
+__global__ void __launch_bounds__(256) regional_masks_kernel(const uint8_t* __restrict__ tok, const int* __restrict__ mask_row,
+                                                             int batch, int h, int w, int patch, int n_levels, int per_sample,
+                                                             uint8_t* __restrict__ out) {
+    const int b = blockIdx.y;
+    int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= per_sample) return;
+    const uint8_t* t = tok + (int64_t)(mask_row ? mask_row[b] : b) * h * w;
+    int64_t base = 0;
+    for (int l = 0; l < n_levels; ++l) {
+        const int s = patch << l, gw = w / s, P = (h / s) * gw;
+        if (i < P) {
+            const int y = i / gw, x = i - y * gw;
+            uint32_t m = 0;
+            for (int dy = 0; dy < s; ++dy)
+                for (int dx = 0; dx < s; ++dx) m |= t[(y * s + dy) * w + x * s + dx];
+            out[base + (int64_t)b * P + i] = (uint8_t)m;
+            return;
+        }
+        i -= P;
+        base += (int64_t)batch * P;
+    }
+}
+
+int launch_regional_masks(const uint8_t* tok_mask, const int* mask_row, int batch, int h, int w, int patch, int n_levels,
+                          uint8_t* out, cudaStream_t st) {
+    if (batch == 0) return 0;
+    int per_sample = 0;
+    for (int l = 0; l < n_levels; ++l) per_sample += (h / (patch << l)) * (w / (patch << l));
+    ProfScope prof("regional_masks", (double)batch * (n_levels * h * w + per_sample), st);
+    PB_CHECK(batch <= 65535, "regional_masks: batch too large");
+    regional_masks_kernel<<<dim3(ceil_div(per_sample, 256), batch), 256, 0, st>>>(tok_mask, mask_row, batch, h, w, patch, n_levels,
+                                                                                 per_sample, out);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
 
 }  // namespace pb

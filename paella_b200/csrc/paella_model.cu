@@ -382,6 +382,7 @@ struct FeatWs {
     float* lnmean;               // per AttnBlock [M]: mean of its input rows (the next folded LayerNorm's per-row shift)
     int64_t lnmean_stride;
     float *r_emb, *film, *y;
+    uint8_t* qmask;              // regional prompts: every level's position masks (launch_regional_masks)
 };
 
 static void plan_features(const pb200_paella* m, int Bt, int H, int W, Arena& ar, FeatWs& ws) {
@@ -414,6 +415,9 @@ static void plan_features(const pb200_paella* m, int Bt, int H, int W, Arena& ar
     ws.r_emb = ar.take<float>((int64_t)Bt * c.c_r);
     ws.film = ar.take<float>((int64_t)Bt * (m->film_total > 0 ? m->film_total : 4));
     ws.y = ar.take<float>((int64_t)Bt * H * W * c.c_out);
+    int64_t n_pos = 0;
+    for (int l = 0; l < c.n_levels; ++l) n_pos += P >> (2 * l);
+    ws.qmask = ar.take<uint8_t>((int64_t)Bt * n_pos);
 }
 
 struct CondWs {
@@ -629,7 +633,19 @@ int pb200_paella_features_tiled(pb200_paella* m, const int64_t* tokens, const fl
                                 const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
                                 int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, float* features,
                                 void* workspace, int64_t workspace_bytes, void* stream) {
+    return pb200_paella_features_regional(m, tokens, r, batch_total, n_pairs, h, w, cond_cache, cache_slots, kv_slot, s_max, attn_w, n_w,
+                                          w_ld, w_len, w_row, w_batch, wrap, nullptr, nullptr, nullptr, 0, features, workspace,
+                                          workspace_bytes, stream);
+}
+
+int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,
+                                   int w, const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w,
+                                   int n_w, int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
+                                   const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
+                                   float* features, void* workspace, int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
+    PB_CHECK(max_regions >= 0 && max_regions <= ATT_MAX_REGIONS, "features: max_regions=%d (0..%d)", max_regions, ATT_MAX_REGIONS);
+    PB_CHECK(prompt_mask == nullptr || region_slot != nullptr || max_regions == 0, "features: regional prompts need region_slot");
     PB_CHECK(w_ld >= 0, "features: attention-weight row stride %d < 0", w_ld);
     const pb200_paella_config& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -661,6 +677,14 @@ int pb200_paella_features_tiled(pb200_paella* m, const int64_t* tokens, const fl
     // after the replication below.  Only the ResBlocks' depthwise padding depends on it (no positional embedding, and
     // h, w are multiples of every level's stride, so each level's grid tiles the torus)
     const int n_base = Bt - n_pairs;
+    // regional prompts: the position masks of every level for the conditional rows [0, n_base), once per call; level l's
+    // [n_base][P_l] table starts at qmask_off[l]
+    int64_t qmask_off[PB200_MAX_LEVELS];
+    {
+        int64_t off = 0;
+        for (int l = 0; l < L; ++l) { qmask_off[l] = off; off += (int64_t)n_base * gh[l] * gw[l]; }
+    }
+    if (prompt_mask) PB_TRY(launch_regional_masks(prompt_mask, mask_row, n_base, h, w, ps, L, ws.qmask, st));
 
     // timestep embedding and every TimestepBlock's (a, b) at once
     PB_TRY(launch_r_embed(r, Bc, c.c_r, ws.r_emb, st));
@@ -789,7 +813,12 @@ int pb200_paella_features_tiled(pb200_paella* m, const int64_t* tokens, const fl
                 ap.scale_log2 = 1.4426950408889634f / sqrtf((float)(ch / c.nhead[l]));
                 ap.attn_w = attn_w; ap.n_w = n_w; ap.w_batch = w_batch;
                 ap.w_ld = w_ld; ap.w_len = w_len; ap.w_row = w_row;
-                PB_TRY(launch_attention(ap, st));
+                if (prompt_mask) {
+                    const AttnRegion rg{ws.qmask + qmask_off[l], region_slot, mask_row, max_regions, n_base};
+                    PB_TRY(launch_attention(ap, st, &rg));
+                } else {
+                    PB_TRY(launch_attention(ap, st));
+                }
                 pb200_gemm_epilogue e2 = epi(PB200_EPI_RESID_F32, m->w<float>(b.outproj_b), x, ch);
                 e2.resid = x; e2.ldr = ch; e2.rows_per_sample = P;
                 PB_TRY(m->gemm(ws.o16, ch, M, ch, b.outproj_w, ch, e2, st));

@@ -30,7 +30,10 @@ region=region)``: a step in argmax or quant mode draws nothing from ``g`` (only 
 ``top_k`` / ``top_p`` a request's multinomial steps are truncated as in ``sample_notebook(..., top_k=k, top_p=p)``; the draws,
 and so the generator offsets, are those of the untruncated request.  With ``tiling='x'``, ``'y'`` or ``'xy'`` a request's token
 grid wraps around as in ``sample_notebook(..., tiling=t)`` (seamless textures and panoramas), and ``decode=True`` decodes it
-with the same tiling; tiling draws nothing.
+with the same tiling; tiling draws nothing.  With ``prompt_regions=[(inputs, region), ...]`` (an engine built with
+``max_prompt_regions`` > 0) a request carries regional prompts as ``sample_notebook(..., prompt_regions=[regions])`` does: their
+K/V are projected at admission into slots reserved for its token slot, and its token masks and region slots sit in device
+pools by token slot; regional prompts draw nothing.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -42,7 +45,9 @@ through the out_mapper GEMM to logits (a bounded number of samples at a time) an
 (Paella.sample_tokens_modes).  A step in which some request truncates adds each row's (k, p) to the table, and the fused sampler
 reads them there (0 and 1.0 for the rows that do not); a step in which none does launches exactly as without truncation.  A step
 in which some row tiles adds each row's wrap byte (0 for the rows that do not), read by the denoiser's depthwise convolutions; a
-step in which none does launches exactly as without tiling.
+step in which none does launches exactly as without tiling.  A step in which some row is regional launches the regional
+denoiser (pb200_paella_features_regional), each row reading its token slot's masks and region slots; a step in which none is
+launches exactly as without regional prompts.
 The host knows which
 requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
 in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
@@ -70,7 +75,7 @@ class Request:
                  generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False,
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
                  region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
-                 top_k: int = 0, top_p: float = 1.0, wrap: int = 0):
+                 top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -80,6 +85,8 @@ class Request:
         self.mode, self.quant_steps = mode, quant_steps      # sampling mode, and the step from which 'quant' is used (or None)
         self.top_k, self.top_p = top_k, top_p    # the truncation table's row: 0 and 1.0 are off
         self.wrap = wrap                         # the wrap table's byte (ops.tiling_table): bit 0 x, bit 1 y; 0 is off
+        self.regions = regions                   # regional prompts: (uint8 [H, W] token masks, [inputs, ...]) or None
+        self.regional = regions is not None
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -204,20 +211,29 @@ class SamplingEngine:
 
     ``max_batch`` requests are in flight at most; later ones queue and are admitted FIFO at step boundaries.  Conditioning of
     up to ``max_cond_len`` rows.  ``unconditional_inputs`` (batch 1) is projected once and used by every guided request that
-    brings no negative prompt of its own.  ``vqmodel`` decodes the requests submitted with ``decode=True``."""
+    brings no negative prompt of its own.  ``vqmodel`` decodes the requests submitted with ``decode=True``.
+    ``max_prompt_regions`` (0 .. 7): the regional prompts a request may carry.  The engine reserves that many K/V slots per token
+    slot, each of max_cond_len rows in every AttnBlock: about 30 MB per slot on the default model at max_cond_len 132 (44
+    AttnBlocks x 132 rows x 2 x 1280 fp16), so max_prompt_regions x max_batch such slots in all.  At 0 the engine allocates
+    what it does without regional prompts."""
 
     def __init__(self, model: Paella, latent_hw=(32, 32), max_batch: int = 64, max_cond_len: int = 140,
-                 unconditional_inputs: Optional[Dict[str, torch.Tensor]] = None, vqmodel=None):
+                 unconditional_inputs: Optional[Dict[str, torch.Tensor]] = None, vqmodel=None, max_prompt_regions: int = 0):
         self.model, self.vqmodel = model, vqmodel
         self.H, self.W = int(latent_hw[0]), int(latent_hw[1])
         self.max_batch, self.s_max = int(max_batch), int(max_cond_len)
         if not 1 <= self.max_batch <= 65535:
             raise ValueError(f"max_batch={max_batch}: expected 1 .. 65535")
+        if isinstance(max_prompt_regions, bool) or not isinstance(max_prompt_regions, int) \
+                or not 0 <= max_prompt_regions <= ops.MAX_PROMPT_REGIONS:
+            raise ValueError(f"max_prompt_regions={max_prompt_regions!r}: expected an int in 0 .. {ops.MAX_PROMPT_REGIONS}")
+        self.max_regions = max_prompt_regions
         ops.check_per_sample_numel(self.H * self.W * model.num_labels)
         self.dev = model._device()
         L = lib()
         model._ensure_packed()
-        self.n_slots = 2 * self.max_batch + 1        # conditional, own unconditional, and the shared unconditional slot
+        # conditional, own unconditional, the shared unconditional slot, then max_regions regional slots per token slot
+        self.n_slots = 2 * self.max_batch + 1 + self.max_regions * self.max_batch
         self.shared_slot = None
         # per-request attn_weights: a row per token slot, as long as the longest vector max_cond_len admits on this grid (bounded
         # for a model without AttnBlocks, where the weights have no effect)
@@ -233,6 +249,10 @@ class SamplingEngine:
             self.src = torch.zeros_like(self.tokens)
             self.region = torch.ones(self.max_batch, self.H, self.W, dtype=torch.bool, device=self.dev)
             self._neg_t = torch.full((self.max_batch,), -1.0, dtype=torch.float32, device=self.dev)   # composite-only t
+            if self.max_regions:
+                # per-request regional prompts by token slot: token masks (all bit 0 for a plain request) and region slots
+                self.prompt_mask = torch.ones(self.max_batch, self.H, self.W, dtype=torch.uint8, device=self.dev)
+                self.region_slot = torch.full((self.max_batch, self.max_regions), -1, dtype=torch.int32, device=self.dev)
             # zero-filled: K/V rows past a slot's kv_len are never attended to, but must be finite (see prepare_conditioning)
             self.cache = ConditioningCache(
                 torch.zeros(L.pb200_paella_cond_cache_bytes(model._handle, self.n_slots, self.s_max), dtype=torch.uint8,
@@ -264,7 +284,7 @@ class SamplingEngine:
     def submit(self, model_inputs, unconditional_inputs=None, *, generator=None, steps=12, renoise_steps=None,
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
-               sampling_quant_steps=None, top_k=None, top_p=None, tiling=None) -> Request:
+               sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -278,7 +298,10 @@ class SamplingEngine:
         k >= sampling_quant_steps, ``mode`` otherwise; 'quant' reads the codebook of the engine's vqmodel).  ``top_k`` (None or
         an int >= 0) and ``top_p`` (None or a float in (0, 1]) truncate the request's multinomial steps as in sample_notebook;
         ValueError for any other value.  ``tiling`` (None, 'none', 'x', 'y' or 'xy') tiles the request as in sample_notebook, and
-        with ``decode=True`` its decode; ValueError for any other value.  The request's draws start when it is admitted."""
+        with ``decode=True`` its decode; ValueError for any other value.  ``prompt_regions`` (None or a list of at most
+        max_prompt_regions (inputs, region) pairs: a batch-1 conditioning dict of at most max_cond_len rows and a bool [H, W]
+        region) gives the request regional prompts as in sample_notebook; ValueError for any other value, and with
+        ``attn_weights``.  The request's draws start when it is admitted."""
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
         g_idx = generator.device.index if generator.device.index is not None else torch.cuda.current_device()
@@ -311,6 +334,16 @@ class SamplingEngine:
         sampling_quant_steps = ops.check_quant_steps("sampling_quant_steps", sampling_quant_steps)
         if self.vqmodel is None and any(ops.mode_at(mode, sampling_quant_steps, k) == "quant" for k in range(steps)):
             raise ValueError("mode 'quant' (or sampling_quant_steps) needs the VQGAN codebook: build the engine with vqmodel=...")
+        regions = None
+        if prompt_regions is not None:
+            if not isinstance(prompt_regions, (list, tuple)) or len(prompt_regions) > self.max_regions:
+                raise ValueError(f"prompt_regions: at most max_prompt_regions={self.max_regions} (inputs, region) pairs per request")
+            regions = ops.regional_table([prompt_regions], 1, (self.H, self.W), self.dev)
+            ops.check_regions_unweighted(regions, attn_weights)
+            if regions is not None:
+                for k, inputs in enumerate(regions[1][0]):
+                    self._check_cond(f"prompt_regions[{k}]", inputs)
+                regions = (regions[0][0], regions[1][0])
         if attn_weights is not None:
             n_keys = self.model.max_attn_weights((self.H, self.W), self.model.conditioning_seq_len(model_inputs))
             attn_weights = ops.check_attn_weight_vector("attn_weights", attn_weights, min(n_keys, self.w_max))
@@ -318,7 +351,7 @@ class SamplingEngine:
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
-                      sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap)
+                      sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap, regions)
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
@@ -348,11 +381,26 @@ class SamplingEngine:
         host_src = [q for q in new if q.has_region and q.init_x.device.type == "cpu"]
         src_row = {id(q): j for j, q in enumerate(host_src)}
         srcs = torch.cat([q.init_x.to(torch.int64) for q in host_src]) if host_src else torch.zeros(0, dtype=torch.int64)
-        slots, w_lens_d, w_rows_d, regions_d, srcs_d = ops.to_device_packed(
-            [torch.tensor([q.slot for q in new], dtype=torch.int32), w_lens, w_rows, regions, srcs], self.dev)
+        # regional prompts: each request's token masks (all bit 0 without regions) and the K/V slots reserved for its token slot
+        R = self.max_regions
+        masks = torch.ones(n, self.H, self.W, dtype=torch.uint8)
+        rslots = torch.full((n, R), -1, dtype=torch.int32)
+        region_writes = []
+        for j, q in enumerate(new):
+            if q.regional:
+                masks[j] = q.regions[0]
+                for k, inputs in enumerate(q.regions[1]):
+                    rslots[j, k] = self._region_slot(q.slot, k)
+                    region_writes.append((self._region_slot(q.slot, k), inputs))
+        slots, w_lens_d, w_rows_d, regions_d, srcs_d, *regional_d = ops.to_device_packed(
+            [torch.tensor([q.slot for q in new], dtype=torch.int32), w_lens, w_rows, regions, srcs] + ([masks, rslots] if R else []),
+            self.dev)
         self.w_len.index_copy_(0, slots.long(), w_lens_d)
         self.w_pool.index_copy_(0, slots.long(), w_rows_d)
         self.region.index_copy_(0, slots.long(), regions_d)
+        if R:
+            self.prompt_mask.index_copy_(0, slots.long(), regional_d[0])
+            self.region_slot.index_copy_(0, slots.long(), regional_d[1])
         ops.randint_per_sample(self.noise, m.num_labels, table, slot=slots, batch=n)
         for q in new:
             s = q.slot
@@ -367,12 +415,16 @@ class SamplingEngine:
         # the conditional and own unconditional K/V of the admitted requests: one projection per run of contiguous slots with
         # one sequence layout (the rows equal per-request projections bit for bit: the conditioning path has no statistic
         # that spans rows)
-        writes = [(q.slot, q.inputs) for q in new] + [(q.uncond_slot, q.uncond) for q in new if q.uncond is not None]
+        writes = [(q.slot, q.inputs) for q in new] + [(q.uncond_slot, q.uncond) for q in new if q.uncond is not None] + region_writes
         for run in admission_runs([(slot, cond_layout(x)) for slot, x in writes]):
             m.write_conditioning(self.cache, writes[run[0]][0], _cat_inputs([writes[i][1] for i in run], self.dev), (self.H, self.W))
         for q in new:
-            q.inputs = q.uncond = q.init_x = q.region = None
+            q.inputs = q.uncond = q.init_x = q.region = q.regions = None
         self._active += new
+
+    def _region_slot(self, token_slot: int, k: int) -> int:
+        """The K/V slot of regional prompt k of the request in ``token_slot``."""
+        return 2 * self.max_batch + 1 + token_slot * self.max_regions + k
 
     def step(self) -> List[Request]:
         """Admit what fits, advance every active request by one of its own steps, and return the requests that finished
@@ -407,10 +459,13 @@ class SamplingEngine:
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_pairs, self.s_max, self.n_slots, kv_slot_d)
+            # row b reads the regional prompts of its token slot
+            regional = (self.prompt_mask, self.region_slot, row_slot_d) if any(q.regional for q in plan.order) else None
             if any(q.attn_weights is not None for q in plan.order):       # row b reads the weights of its token slot
-                feats = m.features(x, r_d, cond, self.w_pool, Bc, n_pairs=n_pairs, w_len=self.w_len, w_row=row_slot_d, wrap=wrap_d)
+                feats = m.features(x, r_d, cond, self.w_pool, Bc, n_pairs=n_pairs, w_len=self.w_len, w_row=row_slot_d, wrap=wrap_d,
+                                   regional=regional)
             else:
-                feats = m.features(x, r_d, cond, n_pairs=n_pairs, wrap=wrap_d)
+                feats = m.features(x, r_d, cond, n_pairs=n_pairs, wrap=wrap_d, regional=regional)
             if mixed:       # argmax and quant rows through the logits path, the multinomial rows in one fused-sampler launch
                 sampled = m.sample_tokens_modes(feats, Bc, n_pairs, H, W, params_d, draw_d, plan.modes, modes_d, self._codebook(),
                                                 out=self._sampled[:Bc], trunc=trunc_d)

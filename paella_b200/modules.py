@@ -264,12 +264,14 @@ class ConditioningCache:
     cond K/V for ``batch_total`` samples (conditional rows first, then unconditional rows)."""
 
     def __init__(self, cache: torch.Tensor, batch_total: int, s_max: int, slots: Optional[int] = None,
-                 slot_map: Optional[torch.Tensor] = None):
+                 slot_map: Optional[torch.Tensor] = None, extra_slot: int = 0):
         self.cache, self.batch_total, self.s_max = cache, batch_total, s_max
         # a group whose samples all carry the same conditioning (the unconditional half of a CFG batch) occupies ONE
         # slot of the cache; slot_map (int32 [batch_total], None = identity) names the slot each sample attends to
         self.slots = batch_total if slots is None else slots
         self.slot_map = slot_map
+        # regional prompts (prepare_conditioning's ``extra``) occupy slots [extra_slot, slots), in the order given
+        self.extra_slot = extra_slot
 
 
 class Paella(nn.Module):
@@ -513,10 +515,12 @@ class Paella(nn.Module):
 
     # -------------------------------------------------------------- conditioning
     def prepare_conditioning(self, groups: Sequence[Dict[str, torch.Tensor]], latent_hw=(32, 32),
-                             share_uniform: bool = True) -> ConditioningCache:
+                             share_uniform: bool = True, extra: Sequence[Dict[str, torch.Tensor]] = ()) -> ConditioningCache:
         """gen_c_embeddings (ref/src/modules.py:223-232) + every AttnBlock's kv_mapper and K/V projection of the
         conditioning rows, for the concatenation of ``groups`` (e.g. [conditional, unconditional]).  A group whose
-        samples all carry the same tensors (the usual unconditional group) is projected once and shared."""
+        samples all carry the same tensors (the usual unconditional group) is projected once and shared.  ``extra``: batch-1
+        conditioning dicts (regional prompts) projected into slots of their own after the groups' (cache.extra_slot on),
+        consecutive ones of one sequence layout in one projection; no sample's slot_map entry names them."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -528,7 +532,7 @@ class Paella(nn.Module):
             if ci is not None:
                 n += len(ci) if isinstance(ci, (list, tuple)) else 1
             return g["byt5"].shape[1] + seq * n
-        s_max = max(seqlen(g) for g in groups)
+        s_max = max(seqlen(g) for g in list(groups) + list(extra))
         bt = sum(g["byt5"].shape[0] for g in groups)
 
         def uniform(g):
@@ -541,11 +545,30 @@ class Paella(nn.Module):
             return all(bool((t == t[:1]).all()) for t in ts if t is not None)
         shared = [uniform(g) for g in groups]
         slots = sum(1 if sh else g["byt5"].shape[0] for g, sh in zip(groups, shared))
+        extra_slot = slots
+        if extra:
+            from .engine import cond_layout
+            runs = []          # consecutive extra prompts of one layout: one projection, as groups of batch > 1
+            for g in extra:
+                if runs and cond_layout(g) == cond_layout(runs[-1][0]):
+                    runs[-1].append(g)
+                else:
+                    runs.append([g])
+            for run in runs:
+                ci = run[0].get("clip_image")
+                groups = list(groups) + [{
+                    "byt5": torch.cat([g["byt5"] for g in run]),
+                    "clip": torch.cat([g["clip"] for g in run]) if run[0].get("clip") is not None else None,
+                    "clip_image": None if ci is None else
+                    [torch.cat([g["clip_image"][i] for g in run]) for i in range(len(ci))] if isinstance(ci, (list, tuple))
+                    else torch.cat([g["clip_image"] for g in run])}]
+                shared.append(False)
+            slots += len(extra)
         with torch.cuda.device(dev):
             # zero-filled: rows between a slot's own length and s_max are never written by the K/V GEMMs, and the attention
             # kernel multiplies them by exactly-zero probabilities -- they must be finite
             cache = torch.zeros(L.pb200_paella_cond_cache_bytes(self._handle, slots, s_max), dtype=torch.uint8, device=dev)
-            ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, bt, latent_hw[0], latent_hw[1], s_max))
+            ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, max(bt, slots), latent_hw[0], latent_hw[1], s_max))
             off = 0
             keep = []
             slot_of = []
@@ -576,8 +599,9 @@ class Paella(nn.Module):
                 check(L.pb200_paella_prepare_cond(self._handle, ctypes.byref(cond), B, off, slots, s_max, ptr(cache), ptr(ws),
                                                   ws.numel(), current_stream()), "pb200_paella_prepare_cond")
                 off += B
-            slot_map = torch.tensor(slot_of, dtype=torch.int32, device=dev) if slots != bt else None
-        return ConditioningCache(cache, bt, s_max, slots, slot_map)
+            identity = slots == bt and not extra          # (extra slots: slots may equal bt with a shared group)
+            slot_map = None if identity else torch.tensor(slot_of[:bt], dtype=torch.int32, device=dev)
+        return ConditioningCache(cache, bt, s_max, slots, slot_map, extra_slot)
 
     def gen_r_embedding(self, r, max_positions=10000):
         """ref/src/modules.py:212-221 -> [B, c_r]."""
@@ -623,7 +647,7 @@ class Paella(nn.Module):
     def features(self, x: torch.Tensor, r: torch.Tensor, cond: ConditioningCache, attn_weights=None,
                  attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None,
                  w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None,
-                 wrap: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 wrap: Optional[torch.Tensor] = None, regional=None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
@@ -637,7 +661,11 @@ class Paella(nn.Module):
         Each length must not exceed the sample's max_attn_weights.
         ``wrap``: seamless tiling, a device uint8 table of one byte per sample of x (ops.tiling_table; bit 0 wraps x, bit 1
         wraps y): the ResBlocks' depthwise convolutions pad circularly on the wrapped axes, and sample B + i of a CFG batch reads
-        byte i (pb200_paella_features_tiled).  None launches exactly the untiled kernels."""
+        byte i (pb200_paella_features_tiled).  None launches exactly the untiled kernels.
+        ``regional``: regional prompts, (token masks, region_slot, mask_row) on the device: uint8 [rows, H, W] masks (bit k >= 1:
+        in region k, bit 0: in none), int32 [rows, R] cache slots of prompts 1..R (-1: none) and int32 [B] rows of the samples
+        of x (None: row b); the unconditional rows are never masked (pb200_paella_features_regional).  None launches exactly the
+        kernels without it."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -662,6 +690,10 @@ class Paella(nn.Module):
                         or w_len.numel() != attn_weights.shape[0] or (w_row is not None and w_row.numel() < attn_weights_batch):
                     raise PaellaB200Error("features: a per-sample weight table is float32 [rows, w_ld] with int32 w_len [rows] "
                                           "and an optional int32 w_row [attn_weights_batch]")
+                if regional is not None:
+                    self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(attn_weights), 0, attn_weights.shape[1], ptr(w_len),
+                                                                            ptr(w_row)), attn_weights_batch, wrap, regional, feats, ws)
+                    return feats
                 if wrap is not None:
                     check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
                                                         ptr(cond.slot_map), cond.s_max, ptr(attn_weights), 0, attn_weights.shape[1],
@@ -674,6 +706,10 @@ class Paella(nn.Module):
                                                        current_stream()), "pb200_paella_features_weighted")
                 return feats
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
+            if regional is not None:
+                self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(aw), aw.numel() if aw is not None else 0, 0, None, None),
+                                        attn_weights_batch, wrap, regional, feats, ws)
+                return feats
             if wrap is not None:        # the single weight vector is the weighted call with w_ld = 0 and no w_len
                 check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
                                                     ptr(cond.slot_map), cond.s_max, ptr(aw), aw.numel() if aw is not None else 0, 0,
@@ -685,6 +721,33 @@ class Paella(nn.Module):
                                                 aw.numel() if aw is not None else 0, attn_weights_batch, ptr(feats), ptr(ws),
                                                 ws.numel(), current_stream()), "pb200_paella_features_pairs")
         return feats
+
+    def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws):
+        mask, region_slot, mask_row = regional
+        rows = mask.shape[0]
+        if mask.dtype != torch.uint8 or tuple(mask.shape[1:]) != (H, W) or region_slot.dtype != torch.int32 or region_slot.dim() != 2 \
+                or region_slot.shape[0] != rows or not 0 <= region_slot.shape[1] <= ops.MAX_PROMPT_REGIONS \
+                or (mask_row is None and rows < Bt - n_pairs) or (mask_row is not None and mask_row.numel() < Bt - n_pairs):
+            raise PaellaB200Error(f"features: regional prompts are uint8 masks [rows, {H}, {W}], int32 region_slot [rows, <= "
+                                  f"{ops.MAX_PROMPT_REGIONS}] and an optional int32 mask_row [{Bt - n_pairs}]")
+        check(lib().pb200_paella_features_regional(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                   ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
+                                                   ptr(mask_row), ptr(region_slot), region_slot.shape[1], ptr(feats), ptr(ws),
+                                                   ws.numel(), current_stream()), "pb200_paella_features_regional")
+
+    def regional_device(self, table, cond: ConditioningCache):
+        """The host table of ops.regional_table as features' ``regional`` argument for ``cond``, a cache whose extra slots are the
+        table's prompts in order (prepare_conditioning's ``extra``): (uint8 masks [B, H, W], int32 region_slot [B, R]) in one
+        asynchronous copy, and mask_row None."""
+        masks, prompts = table
+        R = max(len(p) for p in prompts)
+        slots = torch.full((len(prompts), R), -1, dtype=torch.int32)
+        k = cond.extra_slot
+        for b, own in enumerate(prompts):
+            slots[b, :len(own)] = torch.arange(k, k + len(own), dtype=torch.int32)
+            k += len(own)
+        mask_d, slot_d = ops.to_device_packed([masks, slots], self._device())
+        return mask_d, slot_d, None
 
     def logits_from_features(self, feats: torch.Tensor, batch: int, h: int, w: int) -> torch.Tensor:
         self._ensure_packed()
@@ -913,21 +976,35 @@ class Paella(nn.Module):
         ``tiling``: seamless tiling (keyword only): None / 'none', 'x' (left and right edges wrap), 'y' (top and bottom wrap) or
         'xy', one for every sample or a list or tuple of B values.  The ResBlocks' depthwise convolutions then pad circularly,
         as the reference with ``padding_mode='circular'`` on those Conv2d modules does.  ValueError, before anything is
-        enqueued, for an unknown value, a list of the wrong length or a tensor."""
+        enqueued, for an unknown value, a list of the wrong length or a tensor.
+        ``prompt_regions``: regional prompts (keyword only): None, or a list or tuple of B entries, each None or a list of at most
+        7 (inputs, region) pairs -- a batch-1 conditioning dict and a bool [H, W] token mask on the CPU or the model's device
+        (ops.regional_table).  Every AttnBlock position then attends to the self keys and to the conditioning of each region its
+        footprint touches, and to the sample's own conditioning where its footprint touches no region.  ValueError, before
+        anything is enqueued, for a bad entry and for regions on a sample that also has attn_weights."""
         if x_cat is not None:
             x = torch.cat([x, x_cat], dim=1)
         attn_weights = kwargs.pop("attn_weights", None)
         tiling = kwargs.pop("tiling", None)
+        prompt_regions = kwargs.pop("prompt_regions", None)
         if kwargs:
             raise TypeError(f"unexpected keyword arguments {sorted(kwargs)}")
         B, H, W = x.shape
         wrap = ops.tiling_table(tiling, B)
+        regions = ops.regional_table(prompt_regions, B, (H, W), self._device())
+        ops.check_regions_unweighted(regions, attn_weights)
         cond_len = self.conditioning_seq_len({"byt5": byt5, "clip": clip, "clip_image": clip_image})
         aw, w_len = self._attn_weights_table(attn_weights, B, (H, W), cond_len)
-        cond = self._cond_for_forward(byt5, clip, clip_image, (H, W))
+        regional = None
+        if regions is None:
+            cond = self._cond_for_forward(byt5, clip, clip_image, (H, W))
+        else:
+            cond = self.prepare_conditioning([{"byt5": byt5, "clip": clip, "clip_image": clip_image}], (H, W), share_uniform=False,
+                                             extra=[g for own in regions[1] for g in own])
+            regional = self.regional_device(regions, cond)
         if wrap is not None:
             wrap = ops.to_device_async(wrap, self._device())
-        feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len, wrap=wrap)
+        feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len, wrap=wrap, regional=regional)
         return self.logits_from_features(feats, B, H, W)
 
     def _cond_for_forward(self, byt5, clip, clip_image, hw):

@@ -298,7 +298,79 @@ def tiling_table(tiling, batch: int) -> Optional[torch.Tensor]:
     return torch.tensor(codes, dtype=torch.uint8) if any(codes) else None
 
 
-# ------------------------------------------------------------------ per-sample sampling modes
+# ------------------------------------------------------------------ regional prompts
+# Each sample may carry up to MAX_PROMPT_REGIONS (inputs, region) pairs.  Token t of a sample gets a mask byte: bit k >= 1 set iff
+# t lies in region k, bit 0 iff it lies in no region.  The denoiser's AttnBlock positions OR their footprint's bytes and attend to
+# the conditioning of every prompt they have a bit of, prompt 0 being the sample's own (include/paella_b200.h,
+# pb200_paella_features_regional).
+MAX_PROMPT_REGIONS = 7
+
+
+def check_conditioning_inputs(name: str, inputs) -> None:
+    """ValueError unless ``inputs`` is a batch-1 conditioning dict: ``byt5`` [1, L, byt5_embd] with L >= 1, and optional ``clip``
+    and ``clip_image`` (a tensor or a list or tuple of tensors) whose first dimension is 1."""
+    if not isinstance(inputs, dict) or not torch.is_tensor(inputs.get("byt5")):
+        raise ValueError(f"{name}: expected a conditioning dict with a 'byt5' tensor (got {type(inputs).__name__})")
+    byt5 = inputs["byt5"]
+    if byt5.dim() != 3 or byt5.shape[0] != 1 or byt5.shape[1] < 1:
+        raise ValueError(f"{name}: byt5 of shape {list(byt5.shape)}; expected [1, L, byt5_embd] with L >= 1")
+    ci = inputs.get("clip_image")
+    extra = [("clip", inputs.get("clip"))] + [("clip_image", t) for t in (ci if isinstance(ci, (list, tuple)) else [ci])]
+    for key, t in extra:
+        if t is not None and (not torch.is_tensor(t) or t.dim() < 1 or t.shape[0] != 1):
+            raise ValueError(f"{name}: {key} must be None or a tensor of batch 1")
+
+
+def regional_table(prompt_regions, batch: int, hw, device=None):
+    """``prompt_regions`` (None, or a list or tuple of ``batch`` entries, each None or a list or tuple of at most
+    MAX_PROMPT_REGIONS (inputs, region) pairs) -> None when no sample has a region, otherwise (uint8 [batch, H, W] token masks,
+    the list of each sample's region inputs in order).  ``inputs``: a batch-1 conditioning dict; ``region``: a bool [H, W]
+    tensor on the CPU or on ``device`` (copied to the host).  A single pair or list of pairs is not broadcast.  ValueError
+    for any other shape of the argument, before anything is enqueued."""
+    if prompt_regions is None:
+        return None
+    if not isinstance(prompt_regions, (list, tuple)):
+        raise ValueError(f"prompt_regions: expected None or a list of {batch} entries (got {type(prompt_regions).__name__})")
+    if len(prompt_regions) != batch:
+        raise ValueError(f"prompt_regions: got {len(prompt_regions)} entries for a batch of {batch} (one per sample, None for none)")
+    H, W = int(hw[0]), int(hw[1])
+    masks = torch.zeros(batch, H, W, dtype=torch.uint8)
+    prompts = []
+    for b, entry in enumerate(prompt_regions):
+        if entry is None:
+            entry = []
+        if not isinstance(entry, (list, tuple)):
+            raise ValueError(f"prompt_regions[{b}]: expected None or a list of (inputs, region) pairs (got {type(entry).__name__})")
+        if len(entry) > MAX_PROMPT_REGIONS:
+            raise ValueError(f"prompt_regions[{b}]: {len(entry)} regions; at most {MAX_PROMPT_REGIONS}")
+        own = []
+        for k, pair in enumerate(entry, start=1):
+            name = f"prompt_regions[{b}][{k - 1}]"
+            if not isinstance(pair, (list, tuple)) or len(pair) != 2:
+                raise ValueError(f"{name}: expected an (inputs, region) pair")
+            inputs, region = pair
+            check_conditioning_inputs(name, inputs)
+            if not torch.is_tensor(region) or region.dtype != torch.bool or tuple(region.shape) != (H, W):
+                raise ValueError(f"{name}: region must be a bool tensor of shape [{H}, {W}]")
+            if region.device.type != "cpu" and (device is None or region.device != torch.device(device)):
+                raise ValueError(f"{name}: region is on {region.device}, the model on {device}")
+            masks[b] |= region.cpu().to(torch.uint8) << k
+            own.append(inputs)
+        masks[b][masks[b] == 0] = 1
+        prompts.append(own)
+    if not any(prompts):
+        return None
+    return masks, prompts
+
+
+def check_regions_unweighted(table, attn_weights) -> None:
+    """ValueError if a sample of regional_table's ``table`` has regions and ``attn_weights`` (one vector for every sample, or a
+    list with an entry per sample) weights it: the two are not defined together."""
+    if table is None or attn_weights is None:
+        return
+    for b, own in enumerate(table[1]):
+        if own and (not isinstance(attn_weights, (list, tuple)) or attn_weights[b] is not None):
+            raise ValueError(f"prompt_regions[{b}]: regional prompts and attn_weights on one sample are not supported")
 # The notebook's sampling modes (paella_inference.ipynb cell 3).  'multinomial' draws H*W*num_labels exponentials per step; 'argmax'
 # and 'quant' draw nothing.  A step with several modes sends one int32 table to the device: the mode code of every sample, then
 # the samples in argmax mode, then the samples in quant mode, each list ascending.

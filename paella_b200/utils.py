@@ -42,6 +42,16 @@ texture that repeats without a seam).  The denoiser's ResBlock depthwise convolu
 pb200_paella_features_tiled), the only place a Paella token grid meets its edges.  Tiling draws no random numbers, so every
 generator ends at the same offset, and the per-sample guarantees above hold for tiled rows too.  ``sample(..., decode=vqmodel)``
 decodes each image with its own tiling.
+
+Regional prompts: ``prompt_regions`` (all three functions; None, or a list or tuple of B entries, each None or a list of at most 7
+(inputs, region) pairs) gives sample i further prompts, each on a region of its token grid: ``inputs`` is a batch-1 conditioning
+dict like ``model_inputs`` and ``region`` a bool [H, W] tensor (``token_region`` makes one from a pixel mask).  In the conditional
+forward, every AttnBlock position attends to all self keys and, in one softmax, to the conditioning of each region its footprint
+(patch_size * 2^level tokens square) touches, and to the sample's own ``model_inputs`` row where it touches no region; regions may
+overlap or leave tokens uncovered.  The unconditional forward is unchanged, so negative prompts stay global.  Regional prompts draw
+no random numbers, so every generator ends at the same offset, and the per-sample guarantees above hold for regional rows too
+(ops.regional_table; pb200_paella_features_regional).  ValueError, before anything is enqueued and before any generator advances,
+for a bad entry and for regions on a sample that also has ``attn_weights``.
 """
 from __future__ import annotations
 
@@ -148,7 +158,8 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
-                 codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None):
+                 codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None,
+                 prompt_regions=None):
     """``modes``: None, or per step the list of B mode names (sampling_modes) -- a step whose modes differ samples each row in
     its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the scalar path in that mode.  ``top_k`` /
     ``top_p``: the truncation of the multinomial draws (module docstring); a truncating call takes the per-sample table path."""
@@ -157,6 +168,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     check_region(region, init_x, latent_shape, dev)
     trunc = ops.truncation_table(top_k, top_p, B, model.num_labels)
     wrap = ops.tiling_table(tiling, B)
+    regions = ops.regional_table(prompt_regions, B, (H, W), dev)
+    ops.check_regions_unweighted(regions, attn_weights)
+    extra = [g for own in regions[1] for g in own] if regions is not None else []
     if exact and trunc is not None:
         raise ValueError("exact=True restates the reference op for op, which has no top_k / top_p truncation")
     use_cfg_any = cfgs is not None
@@ -195,8 +209,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             t_list = torch.linspace(t_start, t_end, steps + 1)
             temperatures = torch.linspace(temperature[0], temperature[1], steps)
         groups = [model_inputs] + ([unconditional_inputs] if use_cfg_any else [])
-        cond_full = model.prepare_conditioning(groups, (H, W))
-        cond_only = None
+        cond_full = model.prepare_conditioning(groups, (H, W), extra=extra)
+        regional_full = model.regional_device(regions, cond_full) if regions is not None else None
+        cond_only = regional_only = None
         intermediates = []
         for i in range(steps):
             step_modes = None
@@ -210,7 +225,8 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 cond, tokens = cond_full, sampled          # one (tokens, r) per CFG pair, see Paella.features
             elif use_cfg_any:
                 if cond_only is None:
-                    cond_only = model.prepare_conditioning([model_inputs], (H, W))
+                    cond_only = model.prepare_conditioning([model_inputs], (H, W), extra=extra)
+                    regional_only = model.regional_device(regions, cond_only) if regions is not None else None
                 cond, tokens = cond_only, sampled
             else:
                 cond, tokens = cond_full, sampled
@@ -220,7 +236,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             else:
                 r, params_i = r_d[i], params_d[i]
             feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided, w_len=w_len,
-                                   wrap=wrap_d)
+                                   wrap=wrap_d, regional=regional_only if cond is cond_only else regional_full)
             if step_modes is not None:
                 sampled = _sample_modes_step(model, feats, B, H, W, guided, params_i, step_modes, generator, codebook, dev, trunc_d)
             elif mode == "multinomial" and not exact:
@@ -338,7 +354,7 @@ def _decode_tail(tokens, decode, decode_output, tiling=None):
 
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
            cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
-           top_k=None, top_p=None, tiling=None):
+           top_k=None, top_p=None, tiling=None, prompt_regions=None):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -353,7 +369,7 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     before any generator advances, for a bad value and for truncation with exact=True.
     ``tiling`` (module docstring): seamless tiling per call or per sample; with ``decode`` each image is decoded with its own
     tiling.  ValueError, before anything is enqueued and before any generator advances, for an unknown value, a list of the
-    wrong length or a tensor."""
+    wrong length or a tensor.  ``prompt_regions`` (module docstring): regional prompts per sample."""
     per_sample_cfg = torch.is_tensor(cfg)
     if per_sample_cfg:
         cfg_vals = [v if v else 1.0 for v in ops.per_sample_values("cfg", cfg, latent_shape[0])]   # f*1 + u*0 = f
@@ -365,13 +381,13 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
         raise TypeError("sample(): cfg is set but unconditional_inputs is None")
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, None, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
-                          per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling)
+                          per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling, prompt_regions=prompt_regions)
     return _decode_tail(out, decode, decode_output, tiling)
 
 
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
-                       exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None):
+                       exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
@@ -379,6 +395,7 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     tokens kept elsewhere.  ValueError, before anything is enqueued and before any generator advances, for a region without
     init_x, of another shape or dtype, or on another device.  ``top_k`` / ``top_p`` as in ``sample``; a shard given
     ``top_k[lo:hi]`` computes what rows [lo, hi) compute.  ``tiling`` as in ``sample``; a shard given ``tiling[lo:hi]`` computes
+    what rows [lo, hi) compute.  ``prompt_regions`` (module docstring) likewise: a shard given ``prompt_regions[lo:hi]`` computes
     what rows [lo, hi) compute."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -388,14 +405,14 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
                           generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
-                          tiling=tiling)
+                          tiling=tiling, prompt_regions=prompt_regions)
     return out
 
 
 def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None, init_x=None, steps=12, renoise_steps=None,
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
-                    generator=None, region=None, top_k=None, top_p=None, tiling=None):
+                    generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -409,7 +426,8 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     generators.  A call whose modes differ within a step needs ``generator=[g_0, ..., g_{B-1}]`` (the argmax and quant rows draw
     nothing, the multinomial ones draw per sample); one whose entries are all equal is the scalar call (sampling_modes).
     ``top_k`` / ``top_p`` as in ``sample``: they truncate the multinomial steps only.  ``tiling`` as in ``sample``: the
-    intermediates are those of the tiled call."""
+    intermediates are those of the tiled call.  ``prompt_regions`` as in ``sample``; regional samples' rows may not also
+    have ``attn_weights``."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -426,4 +444,4 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     return _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                         temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, True,
                         sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes,
-                        top_k=top_k, top_p=top_p, tiling=tiling)
+                        top_k=top_k, top_p=top_p, tiling=tiling, prompt_regions=prompt_regions)
