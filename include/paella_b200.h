@@ -386,6 +386,29 @@ int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const
                                    int n_w, int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
                                    const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
                                    float* features, void* workspace, int64_t workspace_bytes, void* stream);
+/* pb200_paella_features_regional with an arbitrary tail: the batch is [batch_total - n_tail base samples; n_tail tail rows], and
+ * tail row batch_total - n_tail + i carries the tokens and r of base sample tail_src[i] (DEVICE int32 [n_tail], each in
+ * [0, batch_total - n_tail)) under its own kv_slot entry.  The conditioning-free prefix (everything before the first AttnBlock)
+ * runs once on the base samples and is gathered to the tail rows, so a tail row's features equal those of its source's tokens
+ * and r run as an ordinary row with that K/V slot.  A sample may own several tail rows (guidance prompts: one conditional
+ * forward per extra prompt); n_tail < batch_total.  A tail row reads its source's wrap byte, and is never masked (prompt_mask
+ * covers the base rows only) nor weighted (attn weights cover rows [0, w_batch), w_batch <= batch_total - n_tail).
+ * tail_src = NULL is [0, n_tail), the unconditional rows of a CFG batch: pb200_paella_features_regional, the same launches. */
+int pb200_paella_features_tail(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                               const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                               int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, const uint8_t* prompt_mask,
+                               const int* mask_row, const int* region_slot, int max_regions, const int* tail_src, float* features,
+                               void* workspace, int64_t workspace_bytes, void* stream);
+
+/* Guidance prompts: the K-way guided mix, in place on fp32 features [samples][hw][c_out] (pb200_paella_features_tail's output).
+ * Composed sample y reads rows[y * ld .. + ld) (DEVICE int32 sample indices: its conditional row c, its unconditional row u,
+ * then its term rows t_1 .. t_J, -1 after its last term) and coef[y * ld .. + ld) (DEVICE fp32 a_c, a_u, a_1 .. a_J), and
+ * writes t = fmaf(f_c, a_c, f_u * a_u), then t = fmaf(f_j, a_j, t) for each term in order, over row c.  With coefficients that
+ * sum to 1 this is the mix of the logits (the out_mapper is linear after its LayerNorm); a sampler then takes row c with the
+ * params (1, 0, 1/T).  2 <= ld <= 2 + PB200_MAX_GUIDANCE_PROMPTS; no two composed samples share a row c. */
+#define PB200_MAX_GUIDANCE_PROMPTS 7
+int pb200_paella_guidance_mix(pb200_paella* m, float* features, int hw, const int* rows, const float* coef, int n_composed, int ld,
+                              void* stream);
 
 /* out_mapper on features -> logits fp32 NCHW [B, num_labels, H*W]   (ref/src/modules.py:184-187,274) */
 int pb200_paella_logits(pb200_paella* m, const float* features, int batch, int hw, float* logits_nchw,

@@ -126,6 +126,10 @@ SIGNATURES = {
     "pb200_paella_features_regional": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
                                                c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                                c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_features_tail": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                           c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_guidance_mix": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_int64, c_void_p]),
     "pb200_paella_sample_tokens_pairs_skip": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -952,6 +952,68 @@ int launch_gather_cast_f16(const float* a, const int* samples, int n_list, int n
     return 0;
 }
 
+// ------------------------------------------------------------------ tail rows and guidance prompts
+// Row gather of a tail: block y copies the `per` bytes of sample src[y] of `base` to sample n_base + y.  V is the widest word
+// that divides `per` (the buffers are 256-byte aligned), so each launch moves whole words.
+template <typename V>
+__global__ void replicate_rows_kernel(uint8_t* __restrict__ base, int64_t words, int n_base, const int* __restrict__ src) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= words) return;
+    const int y = blockIdx.y;
+    const V* from = reinterpret_cast<const V*>(base) + (int64_t)src[y] * words;
+    V* to = reinterpret_cast<V*>(base) + (int64_t)(n_base + y) * words;
+    to[i] = from[i];
+}
+
+int launch_replicate_rows(void* base, int64_t per, int n_base, const int* src, int n_tail, cudaStream_t st) {
+    ProfScope prof("replicate_rows", (double)n_tail * per * 2.0, st);
+    if (n_tail == 0 || per == 0) return 0;
+    PB_CHECK(src != nullptr && n_tail <= 65535 && ((uintptr_t)base & 15) == 0, "replicate_rows: %d rows", n_tail);
+    uint8_t* b = reinterpret_cast<uint8_t*>(base);
+    if (per % 16 == 0) {
+        replicate_rows_kernel<uint4><<<dim3((unsigned)ceil_div(per / 16, 256), n_tail), 256, 0, st>>>(b, per / 16, n_base, src);
+    } else if (per % 4 == 0) {
+        replicate_rows_kernel<uint32_t><<<dim3((unsigned)ceil_div(per / 4, 256), n_tail), 256, 0, st>>>(b, per / 4, n_base, src);
+    } else {
+        replicate_rows_kernel<uint8_t><<<dim3((unsigned)ceil_div(per, 256), n_tail), 256, 0, st>>>(b, per, n_base, src);
+    }
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
+// The K-way guidance mix, in place on fp32 features: composed sample y reads its row of `ld` int32 sample indices [c, u, t_1 ..]
+// and `ld` fp32 coefficients, evaluates cast_kernel<3>'s t = fmaf(f_c, a_c, f_u * a_u), then t = fmaf(f_j, a_j, t) in term order
+// up to the first index < 0, and writes t over sample c.  per4 = float4 words per sample.
+__global__ void __launch_bounds__(256) guidance_mix_kernel(float* __restrict__ f, int64_t per4, const int* __restrict__ rows,
+                                                           const float* __restrict__ coef, int ld) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= per4) return;
+    const int* idx = rows + (int64_t)blockIdx.y * ld;
+    const float* a = coef + (int64_t)blockIdx.y * ld;
+    float4* f4 = reinterpret_cast<float4*>(f);
+    const float4 c = f4[(int64_t)idx[0] * per4 + i], u = f4[(int64_t)idx[1] * per4 + i];
+    const float ac = a[0], au = a[1];
+    float4 t = make_float4(fmaf(c.x, ac, u.x * au), fmaf(c.y, ac, u.y * au), fmaf(c.z, ac, u.z * au), fmaf(c.w, ac, u.w * au));
+    for (int j = 2; j < ld; ++j) {
+        const int s = idx[j];
+        if (s < 0) break;
+        const float4 v = f4[(int64_t)s * per4 + i];
+        const float aj = a[j];
+        t = make_float4(fmaf(v.x, aj, t.x), fmaf(v.y, aj, t.y), fmaf(v.z, aj, t.z), fmaf(v.w, aj, t.w));
+    }
+    f4[(int64_t)idx[0] * per4 + i] = t;
+}
+
+int launch_guidance_mix(float* features, int64_t per, const int* rows, const float* coef, int n_composed, int ld, cudaStream_t st) {
+    ProfScope prof("guidance_mix", (double)n_composed * per * 4.0 * (ld + 1), st);
+    if (n_composed == 0 || per == 0) return 0;
+    PB_CHECK(per % 4 == 0 && ld >= 2 && n_composed <= 65535 && ((uintptr_t)features & 15) == 0,
+             "guidance_mix: %d samples of %lld elements, %d entries per row", n_composed, (long long)per, ld);
+    guidance_mix_kernel<<<dim3((unsigned)ceil_div(per / 4, 256), n_composed), 256, 0, st>>>(features, per / 4, rows, coef, ld);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
 // ------------------------------------------------------------------ layout
 // [B, R, Cc] -> [B, Cc, R] through a 32x33 shared tile
 __global__ void transpose_kernel(const float* __restrict__ in, int R, int Cc, float* __restrict__ out) {

@@ -64,6 +64,12 @@ int launch_gather_cast_f16(const float* a, const int* samples, int n_list, int n
 int launch_resample_mapped(const float* logits_c, const float* logits_u, int64_t batch, int64_t k, int64_t hw, const float* params,
                            const int* map, int mode, const float* codebook, int c_latent, int64_t* out, cudaStream_t st);
 
+// tail rows: sample n_base + i of `base` (per bytes per sample) becomes a copy of sample src[i] (src: DEVICE int32 [n_tail])
+int launch_replicate_rows(void* base, int64_t per, int n_base, const int* src, int n_tail, cudaStream_t st);
+// guidance prompts, in place: per composed sample y, rows[y][0..ld) (DEVICE int32: c, u, then term samples, -1 = none) and
+// coef[y][0..ld) (DEVICE fp32); sample c becomes fmaf(f_c, a_c, f_u*a_u), then fmaf(f_j, a_j, .) per term.  per % 4 == 0
+int launch_guidance_mix(float* features, int64_t per, const int* rows, const float* coef, int n_composed, int ld, cudaStream_t st);
+
 // [B, C, HW] <-> [B, HW, C] fp32
 int launch_nchw_to_nhwc(const float* in, int B, int C, int HW, float* out, cudaStream_t st);
 int launch_nhwc_to_nchw(const float* in, int B, int C, int HW, float* out, cudaStream_t st);

@@ -383,6 +383,7 @@ struct FeatWs {
     int64_t lnmean_stride;
     float *r_emb, *film, *y;
     uint8_t* qmask;              // regional prompts: every level's position masks (launch_regional_masks)
+    uint8_t* wrap;               // tiling with a tail map: the wrap byte of every row [Bt]
 };
 
 static void plan_features(const pb200_paella* m, int Bt, int H, int W, Arena& ar, FeatWs& ws) {
@@ -418,6 +419,7 @@ static void plan_features(const pb200_paella* m, int Bt, int H, int W, Arena& ar
     int64_t n_pos = 0;
     for (int l = 0; l < c.n_levels; ++l) n_pos += P >> (2 * l);
     ws.qmask = ar.take<uint8_t>((int64_t)Bt * n_pos);
+    ws.wrap = ar.take<uint8_t>(Bt);
 }
 
 struct CondWs {
@@ -643,6 +645,16 @@ int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const
                                    int n_w, int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
                                    const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
                                    float* features, void* workspace, int64_t workspace_bytes, void* stream) {
+    return pb200_paella_features_tail(m, tokens, r, batch_total, n_pairs, h, w, cond_cache, cache_slots, kv_slot, s_max, attn_w, n_w,
+                                      w_ld, w_len, w_row, w_batch, wrap, prompt_mask, mask_row, region_slot, max_regions, nullptr,
+                                      features, workspace, workspace_bytes, stream);
+}
+
+int pb200_paella_features_tail(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                               const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                               int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, const uint8_t* prompt_mask,
+                               const int* mask_row, const int* region_slot, int max_regions, const int* tail_src, float* features,
+                               void* workspace, int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
     PB_CHECK(max_regions >= 0 && max_regions <= ATT_MAX_REGIONS, "features: max_regions=%d (0..%d)", max_regions, ATT_MAX_REGIONS);
     PB_CHECK(prompt_mask == nullptr || region_slot != nullptr || max_regions == 0, "features: regional prompts need region_slot");
@@ -665,18 +677,32 @@ int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const
     int gh[PB200_MAX_LEVELS], gw[PB200_MAX_LEVELS];
     for (int l = 0; l < L; ++l) { gh[l] = (h / ps) >> l; gw[l] = (w / ps) >> l; }
 
-    // Classifier-free-guidance pairs: the batch is [Bc samples; the unconditional rows of the first n_pairs of them], and
-    // sample i < n_pairs and sample Bc + i carry the same (tokens, r) and differ only in their conditioning rows, which
+    // The tail: the batch is [Bc samples; n_tail rows], and tail row Bc + i carries the (tokens, r) of sample tail_src[i]
+    // (NULL: sample i, the unconditional rows of a CFG batch) and differs from it only in its conditioning rows, which
     // enter through the AttnBlocks alone.  Everything before the first AttnBlock (the whole level-0 down stack of the
-    // reference config, 'CT') is therefore computed ONCE for the Bc samples, and the first n_pairs samples' rows are
+    // reference config, 'CT') is therefore computed ONCE for the Bc samples, and the source samples' rows are
     // replicated to the tail when the first AttnBlock is reached -- the same arithmetic on the same inputs, not an
-    // approximation.  Guided samples first keeps every replication one contiguous copy.
-    PB_CHECK(n_pairs >= 0 && 2 * n_pairs <= Bt, "features: %d CFG pairs in a batch of %d", n_pairs, Bt);
+    // approximation.  Without a map, guided samples first keeps every replication one contiguous copy; with one, a sample
+    // may own several tail rows (guidance prompts) and replicate_rows_kernel gathers them.
+    const int n_pairs = n_tail;
+    if (tail_src)
+        PB_CHECK(n_tail >= 0 && n_tail < Bt, "features: %d tail rows in a batch of %d", n_tail, Bt);
+    else
+        PB_CHECK(n_pairs >= 0 && 2 * n_pairs <= Bt, "features: %d CFG pairs in a batch of %d", n_pairs, Bt);
     int Bc = Bt - n_pairs;                              // samples currently carried by x
-    // seamless tiling: wrap [Bt - n_pairs], one byte per sample; the unconditional row Bt - n_pairs + i reads byte i, before and
-    // after the replication below.  Only the ResBlocks' depthwise padding depends on it (no positional embedding, and
-    // h, w are multiples of every level's stride, so each level's grid tiles the torus)
+    // seamless tiling: wrap [Bt - n_pairs], one byte per sample; the tail row Bt - n_pairs + i reads the byte of its source
+    // sample, before and after the replication below.  Only the ResBlocks' depthwise padding depends on it (no positional
+    // embedding, and h, w are multiples of every level's stride, so each level's grid tiles the torus)
     const int n_base = Bt - n_pairs;
+    // with a map, the depthwise kernels read a per-row table [Bt] (their n_base = Bt): the base bytes, then the sources' bytes
+    const uint8_t* wrap_dw = wrap;
+    int n_base_dw = n_base;
+    if (wrap && tail_src) {
+        PB_CUDA(cudaMemcpyAsync(ws.wrap, wrap, (size_t)n_base, cudaMemcpyDeviceToDevice, st));
+        PB_TRY(launch_replicate_rows(ws.wrap, 1, n_base, tail_src, n_tail, st));
+        wrap_dw = ws.wrap;
+        n_base_dw = Bt;
+    }
     // regional prompts: the position masks of every level for the conditional rows [0, n_base), once per call; level l's
     // [n_base][P_l] table starts at qmask_off[l]
     int64_t qmask_off[PB200_MAX_LEVELS];
@@ -689,9 +715,13 @@ int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const
     // timestep embedding and every TimestepBlock's (a, b) at once
     PB_TRY(launch_r_embed(r, Bc, c.c_r, ws.r_emb, st));
     PB_TRY(launch_film_table(ws.r_emb, Bc, c.c_r, m->w<float>(m->film_w), m->w<float>(m->film_b), m->film_total, ws.film, st));
-    if (Bc < Bt)
-        PB_CUDA(cudaMemcpyAsync(ws.film + (size_t)Bc * m->film_total, ws.film, (size_t)n_pairs * m->film_total * sizeof(float),
-                                cudaMemcpyDeviceToDevice, st));
+    // replicate the first n_pairs samples' rows of a buffer (bytes per sample each) to the tail, or gather the sources' rows
+    auto tail_copy = [&](void* base, size_t per) -> int {
+        if (tail_src) return launch_replicate_rows(base, (int64_t)per, Bc, tail_src, n_tail, st);
+        PB_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(base) + Bc * per, base, n_pairs * per, cudaMemcpyDeviceToDevice, st));
+        return 0;
+    };
+    if (Bc < Bt) PB_TRY(tail_copy(ws.film, (size_t)m->film_total * sizeof(float)));
     PB_CUDA(cudaMemsetAsync(ws.gsq, 0, (size_t)Bt * 4 * m->max_c * sizeof(uint64_t), st));
     if (Bc < Bt) PB_CUDA(cudaMemsetAsync(ws.gscale, 0, (size_t)Bt * 4 * m->max_c * sizeof(uint64_t), st));
     if (m->n_attn > 0) PB_CUDA(cudaMemsetAsync(ws.lnstat, 0, (size_t)ws.lnstat_stride * m->n_attn * sizeof(int64_t), st));
@@ -712,16 +742,11 @@ int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const
     bool up_phase = false;
     // replicate the shared prefix: x (= xd[l] on the down path) and every saved level output below it
     auto replicate = [&](int level, int attn_index) -> int {
-        for (int q = 0; q <= level; ++q) {
-            const size_t per = (size_t)gh[q] * gw[q] * c.c_hidden[q];
-            PB_CUDA(cudaMemcpyAsync(ws.xd[q] + Bc * per, ws.xd[q], n_pairs * per * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        }
+        for (int q = 0; q <= level; ++q) PB_TRY(tail_copy(ws.xd[q], (size_t)gh[q] * gw[q] * c.c_hidden[q] * sizeof(float)));
         if (attn_index >= 0 && ln_ready == attn_index) {   // the folded-LayerNorm inputs of the AttnBlock that starts here
-            const size_t rows = (size_t)Bc * gh[level] * gw[level], pair_rows = (size_t)n_pairs * gh[level] * gw[level];
-            PB_CUDA(cudaMemcpyAsync(ws.a16 + rows * c.c_hidden[level], ws.a16, pair_rows * c.c_hidden[level] * sizeof(__half),
-                                    cudaMemcpyDeviceToDevice, st));
-            int64_t* stat = ws.lnstat + ws.lnstat_stride * ln_ready;
-            PB_CUDA(cudaMemcpyAsync(stat + 2 * rows, stat, 2 * pair_rows * sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+            const size_t P = (size_t)gh[level] * gw[level];
+            PB_TRY(tail_copy(ws.a16, P * c.c_hidden[level] * sizeof(__half)));
+            PB_TRY(tail_copy(ws.lnstat + ws.lnstat_stride * ln_ready, 2 * P * sizeof(int64_t)));
         }
         Bc = Bt;
         return 0;
@@ -757,7 +782,7 @@ int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const
                 if (b.kind == BK_RES) {
                     const float* skip = b.c_skip ? ws.xd[l] : nullptr;
                     PB_TRY(launch_dwconv_ln(x, skip, m->w<float>(b.dw_w), m->w<float>(b.dw_b), Bc, gh[l], gw[l], ch,
-                                            c.kernel_size, ws.a16, st, wrap, n_base));
+                                            c.kernel_size, ws.a16, st, wrap_dw, n_base_dw));
                 } else {
                     PB_TRY(launch_ln_rows(x, M, ch, 1.0f, 0.0f, ws.a16, nullptr, st));
                 }
@@ -836,12 +861,19 @@ int pb200_paella_features_regional(pb200_paella* m, const int64_t* tokens, const
         e.up_h = gh[0]; e.up_w = gw[0]; e.up_cout = c.c_out;
         PB_TRY(m->gemm(ws.a16, ch, M0, ch, m->clf_w, 4 * (int64_t)c.c_out, e, st));
         PB_TRY(launch_ln_rows(ws.y, (int64_t)Bc * h * w, c.c_out, 1.0f, 0.0f, nullptr, features, st));
-        if (Bc < Bt) {      // a model without any AttnBlock or up path: the pairs are identical to the end
-            const size_t per = (size_t)h * w * c.c_out;
-            PB_CUDA(cudaMemcpyAsync(features + Bc * per, features, n_pairs * per * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        }
+        // a model without any AttnBlock or up path: the tail rows equal their sources to the end
+        if (Bc < Bt) PB_TRY(tail_copy(features, (size_t)h * w * c.c_out * sizeof(float)));
     }
     return 0;
+}
+
+int pb200_paella_guidance_mix(pb200_paella* m, float* features, int hw, const int* rows, const float* coef, int n_composed, int ld,
+                              void* stream) {
+    PB_CHECK(m != nullptr && features != nullptr && (n_composed == 0 || (rows != nullptr && coef != nullptr)),
+             "guidance_mix: features, rows and coef are required");
+    PB_CHECK(hw >= 0 && n_composed >= 0 && ld >= 2 && ld <= 2 + PB200_MAX_GUIDANCE_PROMPTS,
+             "guidance_mix: %d composed samples with %d entries per row (2 .. %d)", n_composed, ld, 2 + PB200_MAX_GUIDANCE_PROMPTS);
+    return launch_guidance_mix(features, (int64_t)hw * m->cfg.c_out, rows, coef, n_composed, ld, (cudaStream_t)stream);
 }
 
 int pb200_paella_features_pairs(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_pairs, int h,

@@ -33,7 +33,10 @@ grid wraps around as in ``sample_notebook(..., tiling=t)`` (seamless textures an
 with the same tiling; tiling draws nothing.  With ``prompt_regions=[(inputs, region), ...]`` (an engine built with
 ``max_prompt_regions`` > 0) a request carries regional prompts as ``sample_notebook(..., prompt_regions=[regions])`` does: their
 K/V are projected at admission into slots reserved for its token slot, and its token masks and region slots sit in device
-pools by token slot; regional prompts draw nothing.
+pools by token slot; regional prompts draw nothing.  With ``guidance_prompts=[(inputs, weight), ...]`` (an engine built with
+``max_guidance_prompts`` > 0) a guided request mixes further weighted prompts into its guidance as ``sample_notebook(...,
+guidance_prompts=[terms])`` does: their K/V are projected at admission into slots reserved for its token slot, and each of its
+guided steps runs one more denoiser row per term; terms draw nothing.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -47,7 +50,10 @@ reads them there (0 and 1.0 for the rows that do not); a step in which none does
 in which some row tiles adds each row's wrap byte (0 for the rows that do not), read by the denoiser's depthwise convolutions; a
 step in which none does launches exactly as without tiling.  A step in which some row is regional launches the regional
 denoiser (pb200_paella_features_regional), each row reading its token slot's masks and region slots; a step in which none is
-launches exactly as without regional prompts.
+launches exactly as without regional prompts.  A step in which some guided row has guidance prompts appends their term rows after
+the unconditional rows, ordered by request, then term (pb200_paella_features_tail, each term row reading its own K/V slot), mixes
+each such request's rows into its conditional row (pb200_paella_guidance_mix) and samples that row with the params (1, 0, 1/T); the
+tail map, mix rows and coefficients ride in the step's table.  A step with no such row launches exactly as without them.
 The host knows which
 requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
 in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
@@ -75,7 +81,7 @@ class Request:
                  generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False,
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
                  region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
-                 top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None):
+                 top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None, terms=None, mix_coef=None):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -87,6 +93,10 @@ class Request:
         self.wrap = wrap                         # the wrap table's byte (ops.tiling_table): bit 0 x, bit 1 y; 0 is off
         self.regions = regions                   # regional prompts: (uint8 [H, W] token masks, [inputs, ...]) or None
         self.regional = regions is not None
+        self.terms = terms                       # guidance prompts: [(inputs, weight), ...] until admission, or None
+        self.n_terms = len(terms) if terms is not None else 0
+        self.mix_coef = mix_coef                 # CPU float32 [cond_steps, 2 + n_terms]: the guided steps' mix coefficients
+        self.term_slot: List[int] = []           # the K/V slots of the terms
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -109,6 +119,19 @@ class StepPlan:
     def __init__(self, order: List[Request]):
         self.order = order
         self.n_pairs = sum(1 for q in order if q.guided and q.k < q.cond_steps)
+        # guidance prompts: the guided rows with terms (composed), their term rows after the unconditional rows
+        self.composed = [i for i, q in enumerate(order[:self.n_pairs]) if q.n_terms]
+        Bc, n_pairs = len(order), self.n_pairs
+        J = max((order[i].n_terms for i in self.composed), default=0)
+        self.tail = torch.tensor(list(range(n_pairs)) + [i for i in self.composed for _ in range(order[i].n_terms)], dtype=torch.int32)
+        self.mix_rows = torch.full((len(self.composed), 2 + J), -1, dtype=torch.int32)
+        self.mix_coef = torch.zeros(len(self.composed), 2 + J, dtype=torch.float32)
+        t = Bc + n_pairs
+        for y, i in enumerate(self.composed):
+            q = order[i]
+            self.mix_rows[y, :2 + q.n_terms] = torch.tensor([i, Bc + i] + list(range(t, t + q.n_terms)), dtype=torch.int32)
+            self.mix_coef[y, :2 + q.n_terms] = q.mix_coef[q.k]
+            t += q.n_terms
         self.r = torch.stack([q.r[q.k] for q in order])
         self.params = torch.stack([q.params[q.k] for q in order])
         self.renoise = [q.k < q.renoise_steps for q in order]
@@ -124,7 +147,8 @@ class StepPlan:
         # a row that does not renoise keeps its tokens (t < 0 never passes the mask test)
         self.t_next = torch.stack([q.r[q.k + 1] if rn else torch.tensor(-1.0) for q, rn in zip(order, self.renoise)])
         self.row_slot = torch.tensor([q.slot for q in order], dtype=torch.int32)
-        self.kv_slot = torch.tensor([q.slot for q in order] + [q.uncond_slot for q in order[:self.n_pairs]], dtype=torch.int32)
+        self.kv_slot = torch.tensor([q.slot for q in order] + [q.uncond_slot for q in order[:self.n_pairs]] +
+                                    [s for i in self.composed for s in order[i].term_slot], dtype=torch.int32)
 
 
 def cond_layout(inputs: Dict[str, torch.Tensor]) -> Tuple[int, bool, int]:
@@ -150,9 +174,10 @@ def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List
 
 def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tuple[torch.Tensor, Dict[str, Tuple[str, int, int]]]:
     """The step's one host-to-device buffer: int64 [(seed, offset) pairs of the sampler's draw, then of the mask draw], then the
-    float32 part [r, params (3 per row), t_next, (top_p)], then the int32 part [row_slot, kv_slot, (mode table), (top_k)], then
-    the uint8 part [(wrap)], each part padded to whole int64 words.  top_p / top_k are present only when ``plan.truncates``, the
-    mode table only when the step mixes modes, wrap (one byte per row) only when ``plan.wraps``.  Returns (buffer, {name: (dtype,
+    float32 part [r, params (3 per row), t_next, (top_p), (mix_coef)], then the int32 part [row_slot, kv_slot, (mode table), (top_k),
+    (tail, mix_rows)], then the uint8 part [(wrap)], each part padded to whole int64 words.  top_p / top_k are present only when
+    ``plan.truncates``, the mode table only when the step mixes modes, wrap (one byte per row) only when ``plan.wraps``, the tail
+    map and the mix table only when some row of the step is composed (guidance prompts).  Returns (buffer, {name: (dtype,
     start, length)}), start and length in elements of that dtype within its part."""
     Bc, n_pairs = len(plan.order), plan.n_pairs
     mixed = not all(plan.draws)
@@ -162,6 +187,9 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
     if plan.truncates:
         f32_parts.append(("top_p", plan.top_p))
         i32_parts.append(("top_k", plan.top_k))
+    if plan.composed:
+        f32_parts.append(("mix_coef", plan.mix_coef.view(-1)))
+        i32_parts += [("tail", plan.tail), ("mix_rows", plan.mix_rows.view(-1))]
     u8_parts = [("wrap", plan.wrap)] if plan.wraps else []
     layout: Dict[str, Tuple[str, int, int]] = {}
     for dt, parts in (("f32", f32_parts), ("i32", i32_parts), ("u8", u8_parts)):
@@ -215,10 +243,13 @@ class SamplingEngine:
     ``max_prompt_regions`` (0 .. 7): the regional prompts a request may carry.  The engine reserves that many K/V slots per token
     slot, each of max_cond_len rows in every AttnBlock: about 30 MB per slot on the default model at max_cond_len 132 (44
     AttnBlocks x 132 rows x 2 x 1280 fp16), so max_prompt_regions x max_batch such slots in all.  At 0 the engine allocates
-    what it does without regional prompts."""
+    what it does without regional prompts.  ``max_guidance_prompts`` (0 .. 7): the guidance prompts a request may carry, with K/V
+    slots reserved the same way: max_guidance_prompts x max_batch slots of about 30 MB each on the default model at max_cond_len
+    132 (about 1.9 GB per prompt at max_batch 64).  At 0 the engine allocates what it does without guidance prompts."""
 
     def __init__(self, model: Paella, latent_hw=(32, 32), max_batch: int = 64, max_cond_len: int = 140,
-                 unconditional_inputs: Optional[Dict[str, torch.Tensor]] = None, vqmodel=None, max_prompt_regions: int = 0):
+                 unconditional_inputs: Optional[Dict[str, torch.Tensor]] = None, vqmodel=None, max_prompt_regions: int = 0,
+                 max_guidance_prompts: int = 0):
         self.model, self.vqmodel = model, vqmodel
         self.H, self.W = int(latent_hw[0]), int(latent_hw[1])
         self.max_batch, self.s_max = int(max_batch), int(max_cond_len)
@@ -228,12 +259,17 @@ class SamplingEngine:
                 or not 0 <= max_prompt_regions <= ops.MAX_PROMPT_REGIONS:
             raise ValueError(f"max_prompt_regions={max_prompt_regions!r}: expected an int in 0 .. {ops.MAX_PROMPT_REGIONS}")
         self.max_regions = max_prompt_regions
+        if isinstance(max_guidance_prompts, bool) or not isinstance(max_guidance_prompts, int) \
+                or not 0 <= max_guidance_prompts <= ops.MAX_GUIDANCE_PROMPTS:
+            raise ValueError(f"max_guidance_prompts={max_guidance_prompts!r}: expected an int in 0 .. {ops.MAX_GUIDANCE_PROMPTS}")
+        self.max_terms = max_guidance_prompts
         ops.check_per_sample_numel(self.H * self.W * model.num_labels)
         self.dev = model._device()
         L = lib()
         model._ensure_packed()
-        # conditional, own unconditional, the shared unconditional slot, then max_regions regional slots per token slot
-        self.n_slots = 2 * self.max_batch + 1 + self.max_regions * self.max_batch
+        # conditional, own unconditional, the shared unconditional slot, then max_regions regional slots per token slot, then
+        # max_terms guidance-prompt slots per token slot
+        self.n_slots = 2 * self.max_batch + 1 + (self.max_regions + self.max_terms) * self.max_batch
         self.shared_slot = None
         # per-request attn_weights: a row per token slot, as long as the longest vector max_cond_len admits on this grid (bounded
         # for a model without AttnBlocks, where the weights have no effect)
@@ -257,7 +293,7 @@ class SamplingEngine:
             self.cache = ConditioningCache(
                 torch.zeros(L.pb200_paella_cond_cache_bytes(model._handle, self.n_slots, self.s_max), dtype=torch.uint8,
                             device=self.dev), self.n_slots, self.s_max, self.n_slots, None)
-            model._ws(L.pb200_paella_workspace_bytes(model._handle, 2 * self.max_batch, self.H, self.W, self.s_max))
+            model._ws(L.pb200_paella_workspace_bytes(model._handle, (2 + self.max_terms) * self.max_batch, self.H, self.W, self.s_max))
             if unconditional_inputs is not None:
                 self._check_cond("unconditional_inputs", unconditional_inputs)
                 self.shared_slot = 2 * self.max_batch
@@ -284,7 +320,7 @@ class SamplingEngine:
     def submit(self, model_inputs, unconditional_inputs=None, *, generator=None, steps=12, renoise_steps=None,
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
-               sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None) -> Request:
+               sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -301,7 +337,10 @@ class SamplingEngine:
         with ``decode=True`` its decode; ValueError for any other value.  ``prompt_regions`` (None or a list of at most
         max_prompt_regions (inputs, region) pairs: a batch-1 conditioning dict of at most max_cond_len rows and a bool [H, W]
         region) gives the request regional prompts as in sample_notebook; ValueError for any other value, and with
-        ``attn_weights``.  The request's draws start when it is admitted."""
+        ``attn_weights``.  ``guidance_prompts`` (None or a list of at most max_guidance_prompts (inputs, weight) pairs: a batch-1
+        conditioning dict of at most max_cond_len rows and a finite real weight) mixes further prompts into a guided request's
+        guidance as in sample_notebook; ValueError for any other value, and on a request without cfg.  The request's draws start
+        when it is admitted."""
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
         g_idx = generator.device.index if generator.device.index is not None else torch.cuda.current_device()
@@ -344,14 +383,34 @@ class SamplingEngine:
                 for k, inputs in enumerate(regions[1][0]):
                     self._check_cond(f"prompt_regions[{k}]", inputs)
                 regions = (regions[0][0], regions[1][0])
+        terms = None
+        if guidance_prompts is not None:
+            if not isinstance(guidance_prompts, (list, tuple)) or len(guidance_prompts) > self.max_terms:
+                raise ValueError(f"guidance_prompts: at most max_guidance_prompts={self.max_terms} (inputs, weight) pairs per request")
+            table = ops.guidance_table([guidance_prompts], 1)
+            if table is not None:
+                terms = table[0]
+                for j, (inputs, _) in enumerate(terms):
+                    self._check_cond(f"guidance_prompts[{j}]", inputs)
+                if cfg is None:
+                    raise ValueError("guidance_prompts need a guided request (cfg is None)")
         if attn_weights is not None:
             n_keys = self.model.max_attn_weights((self.H, self.W), self.model.conditioning_seq_len(model_inputs))
             attn_weights = ops.check_attn_weight_vector("attn_weights", attn_weights, min(n_keys, self.w_max))
         cfgs = U._cfg_schedule(cfg, 1, steps)
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
+        mix_coef = None
+        if terms is not None:      # the guided steps' mix coefficients; their params rows become (1, 0, 1/T): f*1 + u*0 = f
+            n_guided = min(steps, cond_steps)
+            step_cfg = cfgs[0] if torch.is_tensor(cfg) else cfgs
+            mix_coef = torch.tensor([ops.guidance_coefficients(step_cfg[i], [w for _, w in terms]) for i in range(n_guided)],
+                                    dtype=torch.float32).view(n_guided, 2 + len(terms))
+            params[:n_guided, 0, 0] = 1.0
+            params[:n_guided, 0, 1] = 0.0
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
-                      sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap, regions)
+                      sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap, regions,
+                      terms, mix_coef)
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
@@ -415,16 +474,24 @@ class SamplingEngine:
         # the conditional and own unconditional K/V of the admitted requests: one projection per run of contiguous slots with
         # one sequence layout (the rows equal per-request projections bit for bit: the conditioning path has no statistic
         # that spans rows)
-        writes = [(q.slot, q.inputs) for q in new] + [(q.uncond_slot, q.uncond) for q in new if q.uncond is not None] + region_writes
+        for q in new:
+            q.term_slot = [self._term_slot(q.slot, j) for j in range(q.n_terms)]
+        term_writes = [(s, inputs) for q in new for s, (inputs, _) in zip(q.term_slot, q.terms or [])]
+        writes = [(q.slot, q.inputs) for q in new] + [(q.uncond_slot, q.uncond) for q in new if q.uncond is not None] + region_writes \
+            + term_writes
         for run in admission_runs([(slot, cond_layout(x)) for slot, x in writes]):
             m.write_conditioning(self.cache, writes[run[0]][0], _cat_inputs([writes[i][1] for i in run], self.dev), (self.H, self.W))
         for q in new:
-            q.inputs = q.uncond = q.init_x = q.region = q.regions = None
+            q.inputs = q.uncond = q.init_x = q.region = q.regions = q.terms = None
         self._active += new
 
     def _region_slot(self, token_slot: int, k: int) -> int:
         """The K/V slot of regional prompt k of the request in ``token_slot``."""
         return 2 * self.max_batch + 1 + token_slot * self.max_regions + k
+
+    def _term_slot(self, token_slot: int, j: int) -> int:
+        """The K/V slot of guidance prompt j of the request in ``token_slot``."""
+        return 2 * self.max_batch + 1 + self.max_regions * self.max_batch + token_slot * self.max_terms + j
 
     def step(self) -> List[Request]:
         """Admit what fits, advance every active request by one of its own steps, and return the requests that finished
@@ -456,16 +523,21 @@ class SamplingEngine:
             row_slot_d, kv_slot_d, modes_d = part("row_slot"), part("kv_slot"), part("modes")
             trunc_d = (part("top_k"), part("top_p")) if plan.truncates else None
             wrap_d = part("wrap") if plan.wraps else None
+            n_tail = plan.tail.numel() if plan.composed else n_pairs
+            tail = dict(tail_src=part("tail")) if plan.composed else dict(n_pairs=n_pairs)
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
-            cond = ConditioningCache(self.cache.cache, Bc + n_pairs, self.s_max, self.n_slots, kv_slot_d)
+            cond = ConditioningCache(self.cache.cache, Bc + n_tail, self.s_max, self.n_slots, kv_slot_d)
             # row b reads the regional prompts of its token slot
             regional = (self.prompt_mask, self.region_slot, row_slot_d) if any(q.regional for q in plan.order) else None
             if any(q.attn_weights is not None for q in plan.order):       # row b reads the weights of its token slot
-                feats = m.features(x, r_d, cond, self.w_pool, Bc, n_pairs=n_pairs, w_len=self.w_len, w_row=row_slot_d, wrap=wrap_d,
-                                   regional=regional)
+                feats = m.features(x, r_d, cond, self.w_pool, Bc, w_len=self.w_len, w_row=row_slot_d, wrap=wrap_d, regional=regional,
+                                   **tail)
             else:
-                feats = m.features(x, r_d, cond, n_pairs=n_pairs, wrap=wrap_d, regional=regional)
+                feats = m.features(x, r_d, cond, wrap=wrap_d, regional=regional, **tail)
+            if plan.composed:       # each composed row becomes its guided mix, sampled with (1, 0, 1/T)
+                J2 = plan.mix_rows.shape[1]
+                m.guidance_mix(feats, hw, part("mix_rows").view(-1, J2), part("mix_coef").view(-1, J2))
             if mixed:       # argmax and quant rows through the logits path, the multinomial rows in one fused-sampler launch
                 sampled = m.sample_tokens_modes(feats, Bc, n_pairs, H, W, params_d, draw_d, plan.modes, modes_d, self._codebook(),
                                                 out=self._sampled[:Bc], trunc=trunc_d)

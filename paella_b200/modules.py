@@ -515,12 +515,15 @@ class Paella(nn.Module):
 
     # -------------------------------------------------------------- conditioning
     def prepare_conditioning(self, groups: Sequence[Dict[str, torch.Tensor]], latent_hw=(32, 32),
-                             share_uniform: bool = True, extra: Sequence[Dict[str, torch.Tensor]] = ()) -> ConditioningCache:
+                             share_uniform: bool = True, extra: Sequence[Dict[str, torch.Tensor]] = (),
+                             tail: Sequence[int] = ()) -> ConditioningCache:
         """gen_c_embeddings (ref/src/modules.py:223-232) + every AttnBlock's kv_mapper and K/V projection of the
         conditioning rows, for the concatenation of ``groups`` (e.g. [conditional, unconditional]).  A group whose
         samples all carry the same tensors (the usual unconditional group) is projected once and shared.  ``extra``: batch-1
-        conditioning dicts (regional prompts) projected into slots of their own after the groups' (cache.extra_slot on),
-        consecutive ones of one sequence layout in one projection; no sample's slot_map entry names them."""
+        conditioning dicts (regional and guidance prompts) projected into slots of their own after the groups'
+        (cache.extra_slot on), consecutive ones of one sequence layout in one projection.  ``tail``: indices into ``extra``; the
+        cache then has len(tail) more samples after the groups', sample k of them attending to extra prompt tail[k] (the term
+        rows of features' ``tail_src``).  No other sample's slot_map entry names an extra slot."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -600,8 +603,8 @@ class Paella(nn.Module):
                                                   ws.numel(), current_stream()), "pb200_paella_prepare_cond")
                 off += B
             identity = slots == bt and not extra          # (extra slots: slots may equal bt with a shared group)
-            slot_map = None if identity else torch.tensor(slot_of[:bt], dtype=torch.int32, device=dev)
-        return ConditioningCache(cache, bt, s_max, slots, slot_map, extra_slot)
+            slot_map = None if identity else torch.tensor(slot_of[:bt] + [extra_slot + k for k in tail], dtype=torch.int32, device=dev)
+        return ConditioningCache(cache, bt + len(tail), s_max, slots, slot_map, extra_slot)
 
     def gen_r_embedding(self, r, max_positions=10000):
         """ref/src/modules.py:212-221 -> [B, c_r]."""
@@ -647,7 +650,7 @@ class Paella(nn.Module):
     def features(self, x: torch.Tensor, r: torch.Tensor, cond: ConditioningCache, attn_weights=None,
                  attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None,
                  w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None,
-                 wrap: Optional[torch.Tensor] = None, regional=None) -> torch.Tensor:
+                 wrap: Optional[torch.Tensor] = None, regional=None, tail_src: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
@@ -665,12 +668,21 @@ class Paella(nn.Module):
         ``regional``: regional prompts, (token masks, region_slot, mask_row) on the device: uint8 [rows, H, W] masks (bit k >= 1:
         in region k, bit 0: in none), int32 [rows, R] cache slots of prompts 1..R (-1: none) and int32 [B] rows of the samples
         of x (None: row b); the unconditional rows are never masked (pb200_paella_features_regional).  None launches exactly the
-        kernels without it."""
+        kernels without it.
+        ``tail_src``: an arbitrary tail instead of ``cfg_pairs`` / ``n_pairs``, a device int32 [n_tail] of samples of x: the
+        result has B + n_tail samples, sample B + i being sample tail_src[i]'s tokens and r under conditioning row B + i of
+        ``cond`` (guidance prompts: the unconditional rows, then the term rows).  Tail rows read their source's wrap byte and are
+        never masked nor weighted (pb200_paella_features_tail)."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
         Bt, H, W = x.shape
-        if n_pairs is not None:
+        if tail_src is not None:
+            if cfg_pairs or n_pairs is not None or tail_src.dtype != torch.int32 or tail_src.dim() != 1 or tail_src.device != dev \
+                    or tail_src.numel() > 65535:
+                raise PaellaB200Error(f"features: tail_src must be an int32 vector on {dev} (and not with cfg_pairs or n_pairs)")
+            n_pairs = tail_src.numel()
+        elif n_pairs is not None:
             if cfg_pairs or not 0 <= n_pairs <= Bt:
                 raise PaellaB200Error(f"features: n_pairs={n_pairs} for {Bt} samples (and not with cfg_pairs)")
         else:
@@ -690,9 +702,10 @@ class Paella(nn.Module):
                         or w_len.numel() != attn_weights.shape[0] or (w_row is not None and w_row.numel() < attn_weights_batch):
                     raise PaellaB200Error("features: a per-sample weight table is float32 [rows, w_ld] with int32 w_len [rows] "
                                           "and an optional int32 w_row [attn_weights_batch]")
-                if regional is not None:
+                if regional is not None or tail_src is not None:
                     self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(attn_weights), 0, attn_weights.shape[1], ptr(w_len),
-                                                                            ptr(w_row)), attn_weights_batch, wrap, regional, feats, ws)
+                                                                            ptr(w_row)), attn_weights_batch, wrap, regional, feats, ws,
+                                            tail_src)
                     return feats
                 if wrap is not None:
                     check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -706,9 +719,9 @@ class Paella(nn.Module):
                                                        current_stream()), "pb200_paella_features_weighted")
                 return feats
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
-            if regional is not None:
+            if regional is not None or tail_src is not None:
                 self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(aw), aw.numel() if aw is not None else 0, 0, None, None),
-                                        attn_weights_batch, wrap, regional, feats, ws)
+                                        attn_weights_batch, wrap, regional, feats, ws, tail_src)
                 return feats
             if wrap is not None:        # the single weight vector is the weighted call with w_ld = 0 and no w_len
                 check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -722,18 +735,44 @@ class Paella(nn.Module):
                                                 ws.numel(), current_stream()), "pb200_paella_features_pairs")
         return feats
 
-    def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws):
-        mask, region_slot, mask_row = regional
-        rows = mask.shape[0]
-        if mask.dtype != torch.uint8 or tuple(mask.shape[1:]) != (H, W) or region_slot.dtype != torch.int32 or region_slot.dim() != 2 \
-                or region_slot.shape[0] != rows or not 0 <= region_slot.shape[1] <= ops.MAX_PROMPT_REGIONS \
-                or (mask_row is None and rows < Bt - n_pairs) or (mask_row is not None and mask_row.numel() < Bt - n_pairs):
-            raise PaellaB200Error(f"features: regional prompts are uint8 masks [rows, {H}, {W}], int32 region_slot [rows, <= "
-                                  f"{ops.MAX_PROMPT_REGIONS}] and an optional int32 mask_row [{Bt - n_pairs}]")
+    def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws, tail_src=None):
+        """pb200_paella_features_regional, or with ``tail_src`` pb200_paella_features_tail (``regional`` may then be None)."""
+        mask = region_slot = mask_row = None
+        if regional is not None:
+            mask, region_slot, mask_row = regional
+            rows = mask.shape[0]
+            if mask.dtype != torch.uint8 or tuple(mask.shape[1:]) != (H, W) or region_slot.dtype != torch.int32 \
+                    or region_slot.dim() != 2 or region_slot.shape[0] != rows or not 0 <= region_slot.shape[1] <= ops.MAX_PROMPT_REGIONS \
+                    or (mask_row is None and rows < Bt - n_pairs) or (mask_row is not None and mask_row.numel() < Bt - n_pairs):
+                raise PaellaB200Error(f"features: regional prompts are uint8 masks [rows, {H}, {W}], int32 region_slot [rows, <= "
+                                      f"{ops.MAX_PROMPT_REGIONS}] and an optional int32 mask_row [{Bt - n_pairs}]")
+        if w_batch > Bt - n_pairs:
+            raise PaellaB200Error(f"features: {w_batch} weighted samples of {Bt - n_pairs}")
+        n_regions = region_slot.shape[1] if region_slot is not None else 0
+        if tail_src is not None:
+            check(lib().pb200_paella_features_tail(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                   ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
+                                                   ptr(mask_row), ptr(region_slot), n_regions, ptr(tail_src), ptr(feats), ptr(ws),
+                                                   ws.numel(), current_stream()), "pb200_paella_features_tail")
+            return
         check(lib().pb200_paella_features_regional(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
                                                    ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
-                                                   ptr(mask_row), ptr(region_slot), region_slot.shape[1], ptr(feats), ptr(ws),
+                                                   ptr(mask_row), ptr(region_slot), n_regions, ptr(feats), ptr(ws),
                                                    ws.numel(), current_stream()), "pb200_paella_features_regional")
+
+    def guidance_mix(self, feats: torch.Tensor, hw: int, rows: torch.Tensor, coef: torch.Tensor) -> torch.Tensor:
+        """Guidance prompts: the K-way guided mix in place on ``feats`` (fp32 [samples * hw, c_out], features' output), one
+        launch: composed sample y's row rows[y, 0] becomes the mix of its rows ``rows[y]`` (device int32 [n, 2 + J]: c, u, then
+        its term rows, -1 after the last) with the coefficients ``coef[y]`` (device float32 [n, 2 + J],
+        ops.guidance_coefficients) -- pb200_paella_guidance_mix.  A sampler then takes row c with params (1, 0, 1/T)."""
+        self._ensure_packed()
+        if rows.dtype != torch.int32 or coef.dtype != torch.float32 or rows.dim() != 2 or tuple(coef.shape) != tuple(rows.shape) \
+                or feats.dtype != torch.float32 or not feats.is_contiguous():
+            raise PaellaB200Error("guidance_mix: int32 rows and float32 coef of one shape [n, 2 + J] on contiguous fp32 features")
+        with torch.cuda.device(self._device()):
+            check(lib().pb200_paella_guidance_mix(self._handle, ptr(feats), hw, ptr(rows), ptr(coef), rows.shape[0], rows.shape[1],
+                                                  current_stream()), "pb200_paella_guidance_mix")
+        return feats
 
     def regional_device(self, table, cond: ConditioningCache):
         """The host table of ops.regional_table as features' ``regional`` argument for ``cond``, a cache whose extra slots are the

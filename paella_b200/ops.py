@@ -6,6 +6,7 @@ what the torch kernel would have consumed (ATen/native/cuda/DistributionTemplate
 """
 from __future__ import annotations
 
+import math
 from typing import Optional, Tuple
 
 import torch
@@ -371,6 +372,79 @@ def check_regions_unweighted(table, attn_weights) -> None:
     for b, own in enumerate(table[1]):
         if own and (not isinstance(attn_weights, (list, tuple)) or attn_weights[b] is not None):
             raise ValueError(f"prompt_regions[{b}]: regional prompts and attn_weights on one sample are not supported")
+
+
+# ------------------------------------------------------------------ guidance prompts
+# Each sample of a guided call may carry up to MAX_GUIDANCE_PROMPTS (inputs, weight) terms.  On a guided step with scale cfg its
+# logits are l_u + cfg * [(l_c - l_u) + sum_j w_j (l_j - l_u)], l_j being the conditional forward under term j's inputs.  The
+# coefficients (a_c, a_u, a_1 ..) sum to 1, so the mix runs on the features before the out_mapper GEMM
+# (pb200_paella_guidance_mix), and the sampler then takes the mixed row with (1, 0, 1/T).
+MAX_GUIDANCE_PROMPTS = 7
+
+
+def guidance_table(guidance_prompts, batch: int):
+    """``guidance_prompts`` (None, or a list or tuple of ``batch`` entries, each None or a list or tuple of at most
+    MAX_GUIDANCE_PROMPTS (inputs, weight) pairs) -> None when no sample has a term, otherwise the ``batch`` lists of (inputs,
+    float weight) pairs.  ``inputs``: a batch-1 conditioning dict (check_conditioning_inputs); ``weight``: a finite real number,
+    negative for a further negative prompt.  ValueError for any other shape of the argument, before anything is enqueued."""
+    if guidance_prompts is None:
+        return None
+    if not isinstance(guidance_prompts, (list, tuple)):
+        raise ValueError(f"guidance_prompts: expected None or a list of {batch} entries (got {type(guidance_prompts).__name__})")
+    if len(guidance_prompts) != batch:
+        raise ValueError(f"guidance_prompts: got {len(guidance_prompts)} entries for a batch of {batch} (one per sample, None for none)")
+    terms = []
+    for b, entry in enumerate(guidance_prompts):
+        if entry is None:
+            entry = []
+        if not isinstance(entry, (list, tuple)):
+            raise ValueError(f"guidance_prompts[{b}]: expected None or a list of (inputs, weight) pairs (got {type(entry).__name__})")
+        if len(entry) > MAX_GUIDANCE_PROMPTS:
+            raise ValueError(f"guidance_prompts[{b}]: {len(entry)} terms; at most {MAX_GUIDANCE_PROMPTS}")
+        own = []
+        for j, pair in enumerate(entry):
+            name = f"guidance_prompts[{b}][{j}]"
+            if not isinstance(pair, (list, tuple)) or len(pair) != 2:
+                raise ValueError(f"{name}: expected an (inputs, weight) pair")
+            inputs, weight = pair
+            check_conditioning_inputs(name, inputs)
+            if isinstance(weight, bool) or not isinstance(weight, (int, float)) or not math.isfinite(weight):
+                raise ValueError(f"{name}: weight must be a finite real number (got {weight!r})")
+            own.append((inputs, float(weight)))
+        terms.append(own)
+    if not any(terms):
+        return None
+    return terms
+
+
+def guidance_coefficients(cfg: float, weights) -> list:
+    """The mix coefficients of one guided step as fp32 values: (float)cfg, (float)(1 - cfg (1 + sum w)), then (float)(cfg w_j)
+    per term, from doubles.  With no terms they are (cfg, 1 - cfg) of sampling_params, bit for bit."""
+    c = float(cfg)
+    total = 0.0
+    for w in weights:
+        total += w
+    vals = [c, 1.0 - c * (1.0 + total)] + [c * w for w in weights]
+    return torch.tensor(vals, dtype=torch.float64).float().tolist()
+
+
+def guidance_mix_table(terms, cond_row, uncond_row, term_rows, cfgs) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The per-call mix table of the composed samples (those with terms, in ``terms`` order of the samples given): int32
+    [n_composed, 2 + J] row indices [c, u, t_1 .. t_J] (-1 after a sample's last term) and float32 [steps, n_composed, 2 + J]
+    coefficients (guidance_coefficients, 0 after the last term).  ``terms``: each composed sample's weights; ``cond_row``,
+    ``uncond_row``: its rows; ``term_rows``: its term rows; ``cfgs``: per step, each composed sample's cfg."""
+    n = len(terms)
+    J = max(len(w) for w in terms)
+    rows = torch.full((n, 2 + J), -1, dtype=torch.int32)
+    coef = torch.zeros(len(cfgs), n, 2 + J, dtype=torch.float32)
+    for y, ws in enumerate(terms):
+        rows[y, 0], rows[y, 1] = cond_row[y], uncond_row[y]
+        rows[y, 2:2 + len(ws)] = torch.tensor(term_rows[y], dtype=torch.int32)
+        for i, step_cfgs in enumerate(cfgs):
+            coef[i, y, :2 + len(ws)] = torch.tensor(guidance_coefficients(step_cfgs[y], ws))
+    return rows, coef
+
+
 # The notebook's sampling modes (paella_inference.ipynb cell 3).  'multinomial' draws H*W*num_labels exponentials per step; 'argmax'
 # and 'quant' draw nothing.  A step with several modes sends one int32 table to the device: the mode code of every sample, then
 # the samples in argmax mode, then the samples in quant mode, each list ascending.

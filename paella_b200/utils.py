@@ -52,6 +52,20 @@ overlap or leave tokens uncovered.  The unconditional forward is unchanged, so n
 no random numbers, so every generator ends at the same offset, and the per-sample guarantees above hold for regional rows too
 (ops.regional_table; pb200_paella_features_regional).  ValueError, before anything is enqueued and before any generator advances,
 for a bad entry and for regions on a sample that also has ``attn_weights``.
+
+Guidance prompts: ``guidance_prompts`` (all three functions; None, or a list or tuple of B entries, each None or a list of at most 7
+(inputs, weight) pairs) gives sample i further global prompts in its guided mix: ``inputs`` is a batch-1 conditioning dict like
+``model_inputs`` and ``weight`` a finite real number, negative for a further negative prompt.  On a guided step with scale cfg_i the
+sample's logits are l_u + cfg_i * [(l_c - l_u) + sum_j w_j (l_j - l_u)], l_j being the conditional forward under term j's inputs:
+one more denoiser row per term, which shares the conditioning-free prefix with its sample (pb200_paella_features_tail).  The
+coefficients cfg_i, 1 - cfg_i (1 + sum w) and cfg_i w_j are computed in double from the step's torch.linspace cfg and rounded to fp32;
+they sum to 1, so the mix runs on the features before the out_mapper GEMM (pb200_paella_guidance_mix), and the sample is then drawn
+from the mixed row as an unguided one.  Terms act on guided steps only and draw no random numbers, so every generator ends at the
+same offset, and the per-sample guarantees above hold for such rows too.  Term prompts are global: regional prompts and
+``attn_weights`` apply to the sample's conditional row only.  Argmax and quant steps, truncation, tiling and regions see the mixed
+row.  ValueError, before anything is enqueued and before any generator advances, for the wrong number of entries, more than 7
+terms, bad inputs or a non-finite weight, terms in a call that is not guided (cfg None; in ``sample`` a cfg of 0, or a per-sample
+cfg of 0 on a sample with terms), and terms with ``exact=True``.
 """
 from __future__ import annotations
 
@@ -159,10 +173,11 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
                  codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None,
-                 prompt_regions=None):
+                 prompt_regions=None, guidance_prompts=None):
     """``modes``: None, or per step the list of B mode names (sampling_modes) -- a step whose modes differ samples each row in
     its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the scalar path in that mode.  ``top_k`` /
-    ``top_p``: the truncation of the multinomial draws (module docstring); a truncating call takes the per-sample table path."""
+    ``top_p``: the truncation of the multinomial draws (module docstring); a truncating call takes the per-sample table path,
+    and so does a call with ``guidance_prompts`` (module docstring)."""
     B, H, W = latent_shape
     dev = model._device()
     check_region(region, init_x, latent_shape, dev)
@@ -170,12 +185,36 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     wrap = ops.tiling_table(tiling, B)
     regions = ops.regional_table(prompt_regions, B, (H, W), dev)
     ops.check_regions_unweighted(regions, attn_weights)
+    terms = ops.guidance_table(guidance_prompts, B)
     extra = [g for own in regions[1] for g in own] if regions is not None else []
     if exact and trunc is not None:
         raise ValueError("exact=True restates the reference op for op, which has no top_k / top_p truncation")
     use_cfg_any = cfgs is not None
+    if terms is not None and exact:
+        raise ValueError("exact=True restates the reference op for op, which has no guidance prompts")
+    if terms is not None and not use_cfg_any:
+        raise ValueError("guidance_prompts need a guided call (cfg is None or 0)")
     mixed_steps = modes is not None and any(len(set(ms)) > 1 for ms in modes)
-    sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg, always=mixed_steps or trunc is not None)
+    sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg,
+                              always=mixed_steps or trunc is not None or terms is not None)
+    mix = None
+    if terms is not None:
+        # the composed samples' mix table over the guided steps; their params rows there become (1, 0, 1/T): f*1 + u*0 = f
+        comp = [b for b in range(B) if terms[b]]
+        n_reg = len(extra)
+        term_src, term_rows, k = [], [], 2 * B
+        for b in comp:
+            term_rows.append(list(range(k, k + len(terms[b]))))
+            term_src += [b] * len(terms[b])
+            k += len(terms[b])
+        extra = extra + [inputs for b in comp for inputs, _ in terms[b]]
+        n_guided = min(steps, sampling_conditional_steps)
+        step_cfgs = [[(cfgs[b] if per_sample_cfg else cfgs)[i] for b in comp] for i in range(n_guided)]
+        mix_rows, mix_coef = ops.guidance_mix_table([[w for _, w in terms[b]] for b in comp], comp, [B + b for b in comp], term_rows,
+                                                    step_cfgs)
+        sched[0][:n_guided, comp, 0] = 1.0
+        sched[0][:n_guided, comp, 1] = 0.0
+        mix = (list(range(B)) + term_src, [n_reg + j for j in range(len(term_src))], mix_rows, mix_coef)
     w_table = None
     if isinstance(attn_weights, (list, tuple)):       # per-sample vectors, for the conditional rows only
         w_table = ops.attn_weights_table(attn_weights, B, [model.max_attn_weights((H, W), model.conditioning_seq_len(model_inputs))] * B)
@@ -187,7 +226,10 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         region_host = region is not None and region.device.type == "cpu"
         parts = (list(sched) if sched is not None else []) + (list(trunc) if trunc is not None else []) + ([region] if region_host else [])
         parts += [wrap] if wrap is not None else []
+        parts += [torch.tensor(mix[0], dtype=torch.int32), mix[2], mix[3]] if mix is not None else []
         parts_d = ops.to_device_packed(parts, dev) if parts else []
+        if mix is not None:
+            mix_coef_d, mix_rows_d, tail_d = parts_d.pop(), parts_d.pop(), parts_d.pop()
         wrap_d = parts_d.pop() if wrap is not None else None
         if sched is not None:
             params_d, r_d = parts_d[0], parts_d[1]
@@ -209,8 +251,10 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             t_list = torch.linspace(t_start, t_end, steps + 1)
             temperatures = torch.linspace(temperature[0], temperature[1], steps)
         groups = [model_inputs] + ([unconditional_inputs] if use_cfg_any else [])
-        cond_full = model.prepare_conditioning(groups, (H, W), extra=extra)
+        # with guidance prompts the guided batch is [B conditional; B unconditional; term rows by sample, then term]
+        cond_full = model.prepare_conditioning(groups, (H, W), extra=extra, tail=mix[1] if mix is not None else ())
         regional_full = model.regional_device(regions, cond_full) if regions is not None else None
+        extra_only = extra[:len(extra) - len(mix[1])] if mix is not None else extra
         cond_only = regional_only = None
         intermediates = []
         for i in range(steps):
@@ -225,7 +269,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 cond, tokens = cond_full, sampled          # one (tokens, r) per CFG pair, see Paella.features
             elif use_cfg_any:
                 if cond_only is None:
-                    cond_only = model.prepare_conditioning([model_inputs], (H, W), extra=extra)
+                    cond_only = model.prepare_conditioning([model_inputs], (H, W), extra=extra_only)
                     regional_only = model.regional_device(regions, cond_only) if regions is not None else None
                 cond, tokens = cond_only, sampled
             else:
@@ -235,8 +279,12 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 cfg_i, temp_i = (float(cfgs[i]) if guided else None), float(temperatures[i])
             else:
                 r, params_i = r_d[i], params_d[i]
-            feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided, w_len=w_len,
-                                   wrap=wrap_d, regional=regional_only if cond is cond_only else regional_full)
+            composed = guided and mix is not None
+            feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided and not composed,
+                                   w_len=w_len, wrap=wrap_d, regional=regional_only if cond is cond_only else regional_full,
+                                   tail_src=tail_d if composed else None)
+            if composed:
+                model.guidance_mix(feats, H * W, mix_rows_d, mix_coef_d[i])
             if step_modes is not None:
                 sampled = _sample_modes_step(model, feats, B, H, W, guided, params_i, step_modes, generator, codebook, dev, trunc_d)
             elif mode == "multinomial" and not exact:
@@ -354,7 +402,7 @@ def _decode_tail(tokens, decode, decode_output, tiling=None):
 
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
            cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
-           top_k=None, top_p=None, tiling=None, prompt_regions=None):
+           top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -369,8 +417,14 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     before any generator advances, for a bad value and for truncation with exact=True.
     ``tiling`` (module docstring): seamless tiling per call or per sample; with ``decode`` each image is decoded with its own
     tiling.  ValueError, before anything is enqueued and before any generator advances, for an unknown value, a list of the
-    wrong length or a tensor.  ``prompt_regions`` (module docstring): regional prompts per sample."""
+    wrong length or a tensor.  ``prompt_regions`` (module docstring): regional prompts per sample.  ``guidance_prompts`` (module
+    docstring): weighted extra and negative prompts per sample in the guided mix; a sample with terms needs a cfg other than 0."""
     per_sample_cfg = torch.is_tensor(cfg)
+    terms = ops.guidance_table(guidance_prompts, latent_shape[0])
+    if terms is not None and per_sample_cfg:
+        for b, v in enumerate(ops.per_sample_values("cfg", cfg, latent_shape[0])):
+            if terms[b] and not v:
+                raise ValueError(f"guidance_prompts[{b}]: a sample with guidance prompts needs a cfg other than 0 (unguided)")
     if per_sample_cfg:
         cfg_vals = [v if v else 1.0 for v in ops.per_sample_values("cfg", cfg, latent_shape[0])]   # f*1 + u*0 = f
         cfgs = [[v] * steps for v in cfg_vals] if any(cfg.tolist()) else None
@@ -381,13 +435,15 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
         raise TypeError("sample(): cfg is set but unconditional_inputs is None")
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, None, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
-                          per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling, prompt_regions=prompt_regions)
+                          per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling, prompt_regions=prompt_regions,
+                          guidance_prompts=guidance_prompts)
     return _decode_tail(out, decode, decode_output, tiling)
 
 
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
-                       exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None):
+                       exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None,
+                       guidance_prompts=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
@@ -396,7 +452,8 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     init_x, of another shape or dtype, or on another device.  ``top_k`` / ``top_p`` as in ``sample``; a shard given
     ``top_k[lo:hi]`` computes what rows [lo, hi) compute.  ``tiling`` as in ``sample``; a shard given ``tiling[lo:hi]`` computes
     what rows [lo, hi) compute.  ``prompt_regions`` (module docstring) likewise: a shard given ``prompt_regions[lo:hi]`` computes
-    what rows [lo, hi) compute."""
+    what rows [lo, hi) compute.  ``guidance_prompts`` (module docstring) likewise: a shard given ``guidance_prompts[lo:hi]``
+    computes what rows [lo, hi) compute."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -405,14 +462,14 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                           temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
                           generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
-                          tiling=tiling, prompt_regions=prompt_regions)
+                          tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts)
     return out
 
 
 def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None, init_x=None, steps=12, renoise_steps=None,
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
-                    generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None):
+                    generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -427,7 +484,8 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     nothing, the multinomial ones draw per sample); one whose entries are all equal is the scalar call (sampling_modes).
     ``top_k`` / ``top_p`` as in ``sample``: they truncate the multinomial steps only.  ``tiling`` as in ``sample``: the
     intermediates are those of the tiled call.  ``prompt_regions`` as in ``sample``; regional samples' rows may not also
-    have ``attn_weights``."""
+    have ``attn_weights``.  ``guidance_prompts`` as in ``sample``: the argmax and quant steps of a sample with terms see its mixed
+    features, and ``attn_weights`` weight its conditional row only."""
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -444,4 +502,4 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     return _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
                         temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, True,
                         sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes,
-                        top_k=top_k, top_p=top_p, tiling=tiling, prompt_regions=prompt_regions)
+                        top_k=top_k, top_p=top_p, tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts)
