@@ -265,6 +265,16 @@ int pb200_attention_regional(const void* qkv16, const void* ckv16, const int* kv
                              int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
                              const uint8_t* q_mask, const int* region_slot, const int* mask_row, int max_regions, int mask_batch,
                              void* stream);
+/* pb200_attention_slots with attention maps, for samples b < map_batch whose map row mr = map_row[b] (NULL: b) is >= 0:
+ *   scores  fp32 [rows][nhead][positions][s_max]: query q's scaled score s * log2(e) / sqrt(head_dim) on each of the sample's
+ *           conditioning keys j < kv_len (entries past kv_len are not written);
+ *   lse2    fp32 [rows][nhead][positions]: query q's log2 of the softmax denominator over [self ; cond] keys, in the same units.
+ * exp2(score - lse2) is then the softmax probability of the key before attn_weights.  out16 gets the bits of
+ * pb200_attention_slots on the same inputs.  [ref/utils/alter_attention.py:4-43 with need_weights=True] */
+int pb200_attention_maps(const void* qkv16, const void* ckv16, const int* kv_len, const int* kv_slot, int n_slots, void* out16,
+                         int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
+                         int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
+                         float* scores, float* lse2, const int* map_row, int map_batch, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Denoiser (ref/src/modules.py:109-283, ref/utils/modules.py) as an opaque handle.
@@ -399,6 +409,30 @@ int pb200_paella_features_tail(pb200_paella* m, const int64_t* tokens, const flo
                                int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, const uint8_t* prompt_mask,
                                const int* mask_row, const int* region_slot, int max_regions, const int* tail_src, float* features,
                                void* workspace, int64_t workspace_bytes, void* stream);
+/* Attention maps: pb200_paella_features_tail that also accumulates, for base samples b < map_batch whose map row
+ * mr = map_row[b] (DEVICE int32 [map_batch], NULL: b) is >= 0, each AttnBlock's cross-attention map into
+ *   map_acc  DEVICE fp32 [map_rows][map_len][n_pos], n_pos = the sum over levels l of (h / (patch << l)) * (w / (patch << l)),
+ *            caller-owned and caller-zeroed:
+ *            map_acc[mr][s][off_l + p] += (1 / nhead_l) * sum over heads of P[p, n_self + s], level l's block positions p at
+ *            off_l (level 0 first), for every conditioning key s < min(kv_len, map_len).
+ * P is the softmax over [self ; cond] keys times the sample's attn weights (post-softmax, not renormalised), so the sums are the
+ * probabilities ref/utils/alter_attention.py returns with need_weights=True.  Each AttnBlock then runs the maps instance of the
+ * attention kernel and an accumulate kernel; features are bit-identical to the call without maps, and each map row's sums depend
+ * on its sample alone (no atomics).  The workspace must hold pb200_paella_workspace_bytes + pb200_paella_maps_workspace_bytes
+ * (map_rows).  With prompt_mask, a map row's keys are its own prompt 0's, and its token masks should all be 1 (no region):
+ * maps of a regional sample are not defined.  map_batch = 0 is pb200_paella_features_tail, the same launches. */
+int64_t pb200_paella_maps_workspace_bytes(const pb200_paella* m, int map_rows, int h, int w, int s_max);
+int pb200_paella_features_maps(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                               const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                               int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, const uint8_t* prompt_mask,
+                               const int* mask_row, const int* region_slot, int max_regions, const int* tail_src, const int* map_row,
+                               int map_batch, float* map_acc, int map_rows, int map_len, float* features, void* workspace,
+                               int64_t workspace_bytes, void* stream);
+/* maps fp32 [rows][s][h][w] from rows consecutive accumulator rows of pb200_paella_features_maps accumulated over n_steps
+ * forwards: maps[row][j][y][x] = (1 / (n_steps * n_attn)) * sum over levels l, ascending, of
+ * map_acc[row][j][off_l + (y / (patch << l)) * gw_l + x / (patch << l)] (nearest-neighbour upsampling); s <= map_len. */
+int pb200_paella_attention_maps_finalize(pb200_paella* m, const float* map_acc, int rows, int map_len, int h, int w, int s, int n_steps,
+                                         float* maps, void* stream);
 
 /* Guidance prompts: the K-way guided mix, in place on fp32 features [samples][hw][c_out] (pb200_paella_features_tail's output).
  * Composed sample y reads rows[y * ld .. + ld) (DEVICE int32 sample indices: its conditional row c, its unconditional row u,

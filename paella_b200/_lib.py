@@ -98,6 +98,9 @@ SIGNATURES = {
     "pb200_attention_regional": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                          c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                          c_int, c_void_p]),
+    "pb200_attention_maps": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                     c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                     c_void_p]),
     "pb200_paella_create": (c_int, [POINTER(PaellaConfig), POINTER(c_void_p)]),
     "pb200_paella_destroy": (None, [c_void_p]),
     "pb200_paella_weight_bytes": (c_int64, [c_void_p]),
@@ -130,6 +133,12 @@ SIGNATURES = {
                                            c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_guidance_mix": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "pb200_paella_maps_workspace_bytes": (c_int64, [c_void_p, c_int, c_int, c_int, c_int]),
+    "pb200_paella_features_maps": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                           c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                           c_int64, c_void_p]),
+    "pb200_paella_attention_maps_finalize": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_int64, c_void_p]),
     "pb200_paella_sample_tokens_pairs_skip": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,

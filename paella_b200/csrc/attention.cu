@@ -44,9 +44,11 @@ constexpr float NEG_BIG = -1e30f;
 // PB200_ATTN_MMA_SYNC=1.  REG (attention_kernel_regional): regional prompts (AttnRegion): the tile walks [self ; prompt 0]
 // as above, then the chunks of every further prompt some query of it sees, each from the prompt's own first row
 // (attn_build_segs); a row's keys of a prompt it does not see are masked like keys past the end, so its softmax is exact over
-// the keys it sees.
-template <int HD, bool REG>
-__device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRegion& rg) {
+// the keys it sees.  MAPS (attention_kernel_maps, and with REG attention_kernel_regional_maps): attention maps (AttnMapOut); a map
+// row also stores the scaled scores of its own conditioning keys (prompt 0's) and, at the end, its rows' log2-sum-exp, and O takes
+// the same arithmetic as the instance without maps.
+template <int HD, bool REG, bool MAPS>
+__device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRegion& rg, const AttnMapOut& mo) {
     constexpr int LDS = HD + 8;           // padded row: (HD+8)*2 bytes is an odd multiple of 16 -> conflict-free ldmatrix
     constexpr int CPR = HD / 8;           // 16-byte chunks per row
     constexpr int QROWS = ATT_BM;
@@ -66,6 +68,7 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
     const int slot = p.kv_slot ? p.kv_slot[b] : b;            // samples with identical conditioning share one K/V block
     const int n_cond = p.kv_len ? p.kv_len[slot] : p.S_max;
     const int Nk = n_self + n_cond;
+    const int mr = MAPS ? attn_map_row(mo, b) : -1;
     const __half* qkv_b = p.qkv + (int64_t)b * p.P * ldq;
     const __half* ckv_b = p.ckv + (int64_t)slot * p.S_max * ldc;
     AttnSegs* segs = reinterpret_cast<AttnSegs*>(sVb + n_buf * ATT_BN * LDS);
@@ -180,6 +183,25 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
                 ldmatrix_x4(kf, smem_u32(sK + (np * 16 + (lane & 7) + ((lane >> 4) << 3)) * LDS + ks * 16 + ((lane >> 3) & 1) * 8));
                 mma_16816(s[2 * np], qf[ks], kf[0], kf[1]);
                 mma_16816(s[2 * np + 1], qf[ks], kf[2], kf[3]);
+            }
+        }
+        if constexpr (MAPS) {
+            // the chunk's own conditioning keys j - c_from: [n_self, Nk), or regional prompt 0's part of segment 0
+            const int c_from = REG ? from : n_self, c_end = REG ? seg_nk : Nk;
+            if (mr >= 0 && (!REG || bit == 0) && j0 + ATT_BN > c_from) {
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int row = q0 + warp * 16 + g + 8 * r;
+                    if (row >= p.P) continue;
+                    float* dst = mo.scores + (((int64_t)mr * p.nhead + h) * p.P + row) * p.S_max;
+#pragma unroll
+                    for (int nt = 0; nt < ATT_BN / 8; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int key = j0 + nt * 8 + 2 * t + e;
+                            if (key >= c_from && key < c_end) dst[key - c_from] = s[nt][2 * r + e] * p.scale_log2;
+                        }
+                }
             }
         }
         // ---- mask, online softmax (rows g and g+8 of the warp's 16).  The running max is kept in the scaled log2
@@ -306,22 +328,35 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
 #pragma unroll
             for (int nt = 0; nt < HD / 8; ++nt)
                 *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack_half2(o[nt][2 * r] * inv, o[nt][2 * r + 1] * inv);
+            if constexpr (MAPS)
+                if (mr >= 0 && t == 0) mo.lse2[((int64_t)mr * p.nhead + h) * p.P + row] = m_run[r] + log2f(l_run[r]);
         }
     }
 }
 
 template <int HD>
-__global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) { attention_body<HD, false>(p, AttnRegion{}); }
+__global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) { attention_body<HD, false, false>(p, AttnRegion{}, AttnMapOut{}); }
 template <int HD>
-__global__ void __launch_bounds__(128) attention_kernel_regional(const AttnParams p, const AttnRegion rg) { attention_body<HD, true>(p, rg); }
+__global__ void __launch_bounds__(128) attention_kernel_regional(const AttnParams p, const AttnRegion rg) {
+    attention_body<HD, true, false>(p, rg, AttnMapOut{});
+}
+template <int HD>
+__global__ void __launch_bounds__(128) attention_kernel_maps(const AttnParams p, const AttnMapOut mo) {
+    attention_body<HD, false, true>(p, AttnRegion{}, mo);
+}
+// (min blocks 1: at head_dim 80 the default register target spills)
+template <int HD>
+__global__ void __launch_bounds__(128, 1) attention_kernel_regional_maps(const AttnParams p, const AttnRegion rg, const AttnMapOut mo) {
+    attention_body<HD, true, true>(p, rg, mo);
+}
 
-int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg) {
+int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo) {
     PB_CHECK(p.nhead > 0 && p.E % p.nhead == 0, "attention: E=%d not divisible by nhead=%d", p.E, p.nhead);
     const int hd = p.E / p.nhead;
     PB_CHECK(p.E % 8 == 0, "attention: E must be a multiple of 8");
     if (p.B == 0 || p.P == 0) return 0;
     {
-        const int rc = launch_attention_wgmma(p, st, rg);
+        const int rc = launch_attention_wgmma(p, st, rg, mo);
         if (rc >= 0) return rc;
     }
     // algorithmic bytes: q, self k/v, out once; conditioning k/v once per sample
@@ -333,6 +368,20 @@ int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg)
     switch (hd) {
 #define PB_ATT_CASE(H)                                                                                              \
     case H: {                                                                                                       \
+        if (mo != nullptr && reg) {                                                                                 \
+            static DeviceOnce attr_reg_maps;                                                                        \
+            if (attr_reg_maps.first())                                                                              \
+                PB_CUDA(cudaFuncSetAttribute(attention_kernel_regional_maps<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            attention_kernel_regional_maps<H><<<grid, 128, smem, st>>>(p, *rg, *mo);                                \
+            break;                                                                                                  \
+        }                                                                                                           \
+        if (mo != nullptr) {                                                                                        \
+            static DeviceOnce attr_maps;                                                                            \
+            if (attr_maps.first())                                                                                  \
+                PB_CUDA(cudaFuncSetAttribute(attention_kernel_maps<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            attention_kernel_maps<H><<<grid, 128, smem, st>>>(p, *mo);                                              \
+            break;                                                                                                  \
+        }                                                                                                           \
         if (reg) {                                                                                                  \
             static DeviceOnce attr_reg;                                                                             \
             if (attr_reg.first())                                                                                   \

@@ -37,6 +37,23 @@ struct AttnRegion {
     int mask_batch;
 };
 
+// Attention maps, for samples b < map_batch with map_row[b] >= 0 (NULL: row b): the instance writes, per head, the scaled scores
+// s * scale_log2 of the sample's conditioning keys to scores [rows][nhead][P][S_max] (keys past kv_len untouched) and each query's
+// m_run + log2(l_run) to lse2 [rows][nhead][P], so that exp2(score - lse2) is the softmax probability before attn_weights.  A
+// separate kernel argument, so the plain instances keep their code.
+struct AttnMapOut {
+    float* scores;
+    float* lse2;
+    const int* map_row;
+    int map_batch;
+};
+
+// The map row of sample b, or -1
+__device__ __forceinline__ int attn_map_row(const AttnMapOut& mo, int b) {
+    if (b >= mo.map_batch) return -1;
+    return mo.map_row ? mo.map_row[b] : b;
+}
+
 constexpr int ATT_MAX_REGIONS = 7;      // prompts 1..7: the mask bits above prompt 0's
 
 // The key walk of a regional tile: segments of keys, each cut into 64-key chunks from its own first key.  Bit `bit` of a
@@ -106,8 +123,18 @@ __device__ __forceinline__ int attn_weight_row(const AttnParams& p, int b, const
 
 // Dispatch: the wgmma + TMA kernel (attention_wg.cu) for head_dim 80, the mma.sync kernel (attention.cu) for other head dims
 // (rg: the regional table, or NULL for the plain instances)
-int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr);
-int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr);      // 0 launched, 1 error, -1 shape not handled
+// (mo: the map outputs, or NULL.  With rg too, a map row's keys are its prompt 0's; its queries should all see prompt 0 alone.)
+int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr, const AttnMapOut* mo = nullptr);
+int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr,
+                           const AttnMapOut* mo = nullptr);      // 0 launched, 1 error, -1 shape not handled
+// Attention maps (ops.cu): acc [rows][acc_ld][acc_pos] += (1/nhead) * sum over heads h in ascending order of
+// w_s * exp2(score - lse2) at columns [acc_off, acc_off + P), for every map row of p's batch and every conditioning key s < kv_len
+int launch_attention_maps_accumulate(const AttnParams& p, const AttnMapOut& mo, float* acc, int acc_ld, int acc_pos, int acc_off,
+                                     cudaStream_t st);
+// maps [rows][S][h][w] = scale * sum over levels l, ascending, of acc[row][s][off_l + (y / (patch << l)) * gw_l + x / (patch << l)],
+// off_l = sum of the grids (h / patch >> k) * (w / patch >> k) of the levels k < l
+int launch_attention_maps_finalize(const float* acc, int rows, int acc_ld, int acc_pos, int S, int h, int w, int patch, int n_levels,
+                                   float scale, float* maps, cudaStream_t st);
 // Every AttnBlock level's position masks from token masks (ops.cu, regional_masks)
 int launch_regional_masks(const uint8_t* tok_mask, const int* mask_row, int batch, int h, int w, int patch, int n_levels,
                           uint8_t* out, cudaStream_t st);

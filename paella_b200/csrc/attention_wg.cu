@@ -42,8 +42,12 @@ struct AttnMaps {
 // REG (attention_wgmma_kernel_regional): regional prompts (AttnRegion).  The tile walks its self keys, then the chunks of every
 // prompt some query of it sees (attn_build_segs), each from the prompt's own first row; a row's keys of a prompt it does not
 // see are masked the way keys at or past `valid` are, so its softmax is exact over the keys it sees.
-template <bool REG>
-__device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const AttnParams& p, const AttnRegion& rg) {
+// MAPS (attention_wgmma_kernel_maps, and with REG attention_wgmma_kernel_regional_maps): attention maps (AttnMapOut).  A map row
+// also stores the scaled scores of its own conditioning's chunks (prompt 0's) and, at the end, its rows' log2-sum-exp; O takes the
+// same arithmetic as the instance without maps.
+template <bool REG, bool MAPS>
+__device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const AttnParams& p, const AttnRegion& rg,
+                                                     const AttnMapOut& mo) {
     pdl_launch_dependents();
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -59,6 +63,7 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
     const int n_cond = p.kv_len ? p.kv_len[slot] : p.S_max;
     const int Nk = n_self + n_cond;
     const int n_sc = (n_self + AW_BN - 1) / AW_BN;
+    const int mr = MAPS ? attn_map_row(mo, b) : -1;
     int n_chunks = n_sc + (n_cond + AW_BN - 1) / AW_BN;
     AttnSegs* segs = reinterpret_cast<AttnSegs*>(gbase + AW_OFF_SEGS);
     auto seg_of = [&](int c) {
@@ -136,14 +141,17 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
     for (int c = 0; c < n_chunks; ++c) {
         const int st = c & 1;
         int k0, valid, key0, lim[2];
+        bool own_cond;                      // a chunk of the sample's own conditioning keys (the map's keys)
         if constexpr (REG) {
             const int si = seg_of(c), bit = segs->bit[si];
+            own_cond = bit == 0;
             k0 = (c - segs->first[si]) * AW_BN;
             valid = min(AW_BN, segs->len[si] - k0);
             key0 = bit < 0 ? k0 : bit == 0 ? n_self + k0 : Nk;              // only [self ; prompt 0] is weighted
             for (int r = 0; r < 2; ++r) lim[r] = (bit < 0 || ((row_mask[r] >> bit) & 1u)) ? valid : 0;
         } else {
             const bool self = c < n_sc;
+            own_cond = !self;
             k0 = self ? c * AW_BN : (c - n_sc) * AW_BN;                      // first key of the chunk inside its source
             valid = min(AW_BN, (self ? n_self : n_cond) - k0);
             key0 = self ? k0 : n_self + k0;                                   // index in [self ; cond]
@@ -191,6 +199,21 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         ptx::fence_regs(s);
+        if constexpr (MAPS) {
+            if (mr >= 0 && own_cond) {       // the conditioning keys k0 + col of rows lane/4 and lane/4 + 8 of the warp's 16
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int row = q0 + wq * 16 + (lane >> 2) + 8 * r;
+                    if (row >= p.P) continue;
+                    float* dst = mo.scores + (((int64_t)mr * p.nhead + h) * p.P + row) * p.S_max + k0;
+#pragma unroll
+                    for (int i = 0; i < AW_BN / 2; ++i) {
+                        const int col = (i >> 2) * 8 + 2 * (lane & 3) + (i & 1);
+                        if (((i >> 1) & 1) == r && col < valid) dst[col] = s[i] * p.scale_log2;
+                    }
+                }
+            }
+        }
 
         // ---- mask, online softmax (rows lane/4 and lane/4 + 8 of the warp's 16; key column 8n + 2(lane%4) + i%2)
         float mx[2] = {-1e30f, -1e30f};
@@ -255,20 +278,30 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
 #pragma unroll
             for (int n = 0; n < AW_HD / 8; ++n)
                 *reinterpret_cast<uint32_t*>(dst + n * 8) = pack_half2(o[4 * n + 2 * r] * inv, o[4 * n + 2 * r + 1] * inv);
+            if constexpr (MAPS)
+                if (mr >= 0 && (lane & 3) == 0) mo.lse2[((int64_t)mr * p.nhead + h) * p.P + row] = m_run[r] + log2f(l_run[r]);
         }
     }
 }
 
 __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_constant__ AttnMaps maps, const AttnParams p) {
-    attention_wgmma_body<false>(maps, p, AttnRegion{});
+    attention_wgmma_body<false, false>(maps, p, AttnRegion{}, AttnMapOut{});
 }
 __global__ void __launch_bounds__(128) attention_wgmma_kernel_regional(const __grid_constant__ AttnMaps maps, const AttnParams p,
                                                                        const AttnRegion rg) {
-    attention_wgmma_body<true>(maps, p, rg);
+    attention_wgmma_body<true, false>(maps, p, rg, AttnMapOut{});
+}
+__global__ void __launch_bounds__(128) attention_wgmma_kernel_maps(const __grid_constant__ AttnMaps maps, const AttnParams p,
+                                                                   const AttnMapOut mo) {
+    attention_wgmma_body<false, true>(maps, p, AttnRegion{}, mo);
+}
+__global__ void __launch_bounds__(128) attention_wgmma_kernel_regional_maps(const __grid_constant__ AttnMaps maps, const AttnParams p,
+                                                                            const AttnRegion rg, const AttnMapOut mo) {
+    attention_wgmma_body<true, true>(maps, p, rg, mo);
 }
 
 // returns 0 = launched, 1 = error, -1 = shape not handled here (head_dim != 80: the caller runs the mma.sync kernel)
-int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg) {
+int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo) {
     static const bool off = getenv("PB200_ATTN_MMA_SYNC") != nullptr;      // A/B knob: the mma.sync kernel for every shape
     if (off || p.E != AW_HD * p.nhead) return -1;
     const int64_t q_rows = (int64_t)p.B * p.P;
@@ -287,7 +320,17 @@ int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegio
     ProfScope prof("attention", 2.0 * ((double)p.B * p.P * 4.0 * p.E + (double)p.B * p.S_max * 2.0 * p.E), st);
     dim3 grid(ceil_div(p.P, AW_BM), p.nhead, p.B);
     PB_CHECK(grid.y <= 65535 && grid.z <= 65535, "attention: grid too large");
-    if (rg != nullptr) {
+    if (mo != nullptr && rg != nullptr) {
+        static DeviceOnce attr_reg_maps;
+        if (attr_reg_maps.first())
+            PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel_regional_maps, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM_REG));
+        attention_wgmma_kernel_regional_maps<<<grid, 128, AW_SMEM_REG, st>>>(m, p, *rg, *mo);
+    } else if (mo != nullptr) {
+        static DeviceOnce attr_maps;
+        if (attr_maps.first())
+            PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel_maps, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM));
+        attention_wgmma_kernel_maps<<<grid, 128, AW_SMEM, st>>>(m, p, *mo);
+    } else if (rg != nullptr) {
         static DeviceOnce attr_reg;
         if (attr_reg.first())
             PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel_regional, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM_REG));

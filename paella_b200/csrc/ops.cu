@@ -1083,4 +1083,70 @@ int launch_regional_masks(const uint8_t* tok_mask, const int* mask_row, int batc
     return 0;
 }
 
+// Attention maps: one thread per (sample, query position, conditioning key), keys fastest so that the heads' score rows are read
+// coalesced.  Every (map row, key, position) has one writer per launch, so the accumulator needs no atomics and a row's sums depend
+// on that row alone.
+__global__ void __launch_bounds__(256) attention_maps_accumulate_kernel(const AttnParams p, const AttnMapOut mo, float* __restrict__ acc,
+                                                                        int acc_ld, int acc_pos, int acc_off) {
+    const int b = blockIdx.y;
+    const int mr = attn_map_row(mo, b);
+    if (mr < 0) return;
+    const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= (int64_t)p.P * p.S_max) return;
+    const int pos = (int)(i / p.S_max), s = (int)(i - (int64_t)pos * p.S_max);
+    const int slot = p.kv_slot ? p.kv_slot[b] : b;
+    const int n_cond = p.kv_len ? p.kv_len[slot] : p.S_max;
+    if (s >= n_cond || s >= acc_ld) return;
+    const float* sc = mo.scores + ((int64_t)mr * p.nhead * p.P + pos) * p.S_max + s;
+    const float* ls = mo.lse2 + (int64_t)mr * p.nhead * p.P + pos;
+    float sum = 0.f;
+    for (int h = 0; h < p.nhead; ++h) sum += exp2f(sc[(int64_t)h * p.P * p.S_max] - ls[(int64_t)h * p.P]);
+    const float* w = nullptr;
+    const int n_w = attn_weight_row(p, b, w);
+    const int n_self = p.self_attn ? p.P : 0, kj = n_self + s, w_start = n_self + n_cond - n_w;
+    if (n_w > 0 && kj >= w_start) sum *= w[kj - w_start];
+    acc[((int64_t)mr * acc_ld + s) * acc_pos + acc_off + pos] += sum * (1.0f / (float)p.nhead);
+}
+
+int launch_attention_maps_accumulate(const AttnParams& p, const AttnMapOut& mo, float* acc, int acc_ld, int acc_pos, int acc_off,
+                                     cudaStream_t st) {
+    if (mo.map_batch == 0 || p.P == 0 || p.S_max == 0) return 0;
+    ProfScope prof("attention_maps", (double)mo.map_batch * p.P * p.S_max * (p.nhead + 2) * 4.0, st);
+    PB_CHECK(mo.map_batch <= 65535, "attention_maps: map batch too large");
+    attention_maps_accumulate_kernel<<<dim3((unsigned)ceil_div((int64_t)p.P * p.S_max, 256), mo.map_batch), 256, 0, st>>>(
+        p, mo, acc, acc_ld, acc_pos, acc_off);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
+// one thread per (row, key, token); the levels are summed in ascending order
+__global__ void __launch_bounds__(256) attention_maps_finalize_kernel(const float* __restrict__ acc, int acc_ld, int acc_pos, int S,
+                                                                      int h, int w, int patch, int n_levels, float scale,
+                                                                      float* __restrict__ maps) {
+    const int row = blockIdx.z, s = blockIdx.y;
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= h * w) return;
+    const int y = i / w, x = i - y * w;
+    const float* a = acc + ((int64_t)row * acc_ld + s) * acc_pos;
+    float t = 0.f;
+    int off = 0;
+    for (int l = 0; l < n_levels; ++l) {
+        const int st = patch << l, gw = w / st;
+        t += a[off + (y / st) * gw + x / st];
+        off += (h / st) * gw;
+    }
+    maps[((int64_t)row * S + s) * h * w + i] = t * scale;
+}
+
+int launch_attention_maps_finalize(const float* acc, int rows, int acc_ld, int acc_pos, int S, int h, int w, int patch, int n_levels,
+                                   float scale, float* maps, cudaStream_t st) {
+    if (rows == 0 || S == 0 || h * w == 0) return 0;
+    ProfScope prof("attention_maps", (double)rows * S * h * w * (n_levels + 1) * 4.0, st);
+    PB_CHECK(rows <= 65535 && S <= 65535, "attention_maps: %d rows of %d keys", rows, S);
+    attention_maps_finalize_kernel<<<dim3(ceil_div(h * w, 256), S, rows), 256, 0, st>>>(acc, acc_ld, acc_pos, S, h, w, patch, n_levels,
+                                                                                          scale, maps);
+    PB_LAUNCH_CHECK();
+    return 0;
+}
+
 }  // namespace pb

@@ -384,9 +384,12 @@ struct FeatWs {
     float *r_emb, *film, *y;
     uint8_t* qmask;              // regional prompts: every level's position masks (launch_regional_masks)
     uint8_t* wrap;               // tiling with a tail map: the wrap byte of every row [Bt]
+    float *map_scores, *map_lse2;     // attention maps (map_rows > 0): one AttnBlock's AttnMapOut workspace, reused by every block
 };
 
-static void plan_features(const pb200_paella* m, int Bt, int H, int W, Arena& ar, FeatWs& ws) {
+// map_rows > 0: also the attention-map workspace of map_rows rows at conditioning length s_max, after everything else so that the
+// rest of the plan is the same with and without it
+static void plan_features(const pb200_paella* m, int Bt, int H, int W, Arena& ar, FeatWs& ws, int map_rows = 0, int s_max = 0) {
     const pb200_paella_config& c = m->cfg;
     const int ps = c.patch_size;
     int64_t max_mc = 0, P = (int64_t)(H / ps) * (W / ps);
@@ -420,6 +423,21 @@ static void plan_features(const pb200_paella* m, int Bt, int H, int W, Arena& ar
     for (int l = 0; l < c.n_levels; ++l) n_pos += P >> (2 * l);
     ws.qmask = ar.take<uint8_t>((int64_t)Bt * n_pos);
     ws.wrap = ar.take<uint8_t>(Bt);
+    ws.map_scores = ws.map_lse2 = nullptr;
+    if (map_rows > 0) {
+        int64_t hp = 0;       // the largest nhead * P of an AttnBlock
+        for (const BlockPlan& b : m->blocks)
+            if (b.kind == BK_ATTN) hp = std::max(hp, (int64_t)c.nhead[b.level] * (P >> (2 * b.level)));
+        ws.map_scores = ar.take<float>((int64_t)map_rows * hp * s_max);
+        ws.map_lse2 = ar.take<float>((int64_t)map_rows * hp);
+    }
+}
+
+// attention-map accumulator columns: every level's positions, level 0 first
+static int map_positions(const pb200_paella* m, int h, int w) {
+    int n = 0;
+    for (int l = 0; l < m->cfg.n_levels; ++l) n += (h / (m->cfg.patch_size << l)) * (w / (m->cfg.patch_size << l));
+    return n;
 }
 
 struct CondWs {
@@ -655,7 +673,32 @@ int pb200_paella_features_tail(pb200_paella* m, const int64_t* tokens, const flo
                                int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, const uint8_t* prompt_mask,
                                const int* mask_row, const int* region_slot, int max_regions, const int* tail_src, float* features,
                                void* workspace, int64_t workspace_bytes, void* stream) {
+    return pb200_paella_features_maps(m, tokens, r, batch_total, n_tail, h, w, cond_cache, cache_slots, kv_slot, s_max, attn_w, n_w, w_ld,
+                                      w_len, w_row, w_batch, wrap, prompt_mask, mask_row, region_slot, max_regions, tail_src, nullptr, 0,
+                                      nullptr, 0, 0, features, workspace, workspace_bytes, stream);
+}
+
+int64_t pb200_paella_maps_workspace_bytes(const pb200_paella* m, int map_rows, int h, int w, int s_max) {
+    if (m == nullptr || map_rows < 0) { set_error("maps_workspace_bytes: null model handle or negative row count"); return -1; }
+    Arena a{nullptr}, b{nullptr};
+    FeatWs f;
+    plan_features(m, 1, h, w, a, f);
+    plan_features(m, 1, h, w, b, f, map_rows, s_max);
+    return b.off - a.off + 256;
+}
+
+int pb200_paella_features_maps(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                               const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                               int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap, const uint8_t* prompt_mask,
+                               const int* mask_row, const int* region_slot, int max_regions, const int* tail_src, const int* map_row,
+                               int map_batch, float* map_acc, int map_rows, int map_len, float* features, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
+    PB_CHECK(map_batch == 0 || (map_acc != nullptr && map_rows > 0 && map_len > 0 && map_batch <= batch_total - n_tail),
+             "features: attention maps of %d samples need an accumulator of rows x keys (%d x %d) and at most the %d base samples",
+             map_batch, map_rows, map_len, batch_total - n_tail);
+    PB_CHECK(map_batch == 0 || map_row != nullptr || map_batch <= map_rows, "features: %d map samples for %d accumulator rows",
+             map_batch, map_rows);
     PB_CHECK(max_regions >= 0 && max_regions <= ATT_MAX_REGIONS, "features: max_regions=%d (0..%d)", max_regions, ATT_MAX_REGIONS);
     PB_CHECK(prompt_mask == nullptr || region_slot != nullptr || max_regions == 0, "features: regional prompts need region_slot");
     PB_CHECK(w_ld >= 0, "features: attention-weight row stride %d < 0", w_ld);
@@ -667,9 +710,14 @@ int pb200_paella_features_tail(pb200_paella* m, const int64_t* tokens, const flo
     PB_CHECK(m->n_attn == 0 || cond_cache != nullptr, "features: conditioning cache required");
     Arena ar{reinterpret_cast<uint8_t*>(workspace)};
     FeatWs ws;
-    plan_features(m, Bt, h, w, ar, ws);
+    plan_features(m, Bt, h, w, ar, ws, map_batch > 0 ? map_rows : 0, s_max);
     PB_CHECK(ar.off <= workspace_bytes, "features: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)ar.off);
     const uint8_t* cache = reinterpret_cast<const uint8_t*>(cond_cache);
+    // attention maps: the map rows' accumulator columns of level l start at map_off[l]
+    const AttnMapOut mo{ws.map_scores, ws.map_lse2, map_row, map_batch};
+    const int map_pos = map_positions(m, h, w);
+    int map_off[PB200_MAX_LEVELS];
+    for (int l = 0, off = 0; l < L; ++l) { map_off[l] = off; off += ((h / ps) >> l) * ((w / ps) >> l); }
     PB_CHECK(cache_slots > 0 && (kv_slot != nullptr || cache_slots == Bt), "features: %d cache slots for %d samples need a slot map",
              cache_slots, Bt);
     const int* kv_len = reinterpret_cast<const int*>(cache + cond_block_off(m, m->n_attn, cache_slots, s_max));
@@ -838,12 +886,9 @@ int pb200_paella_features_tail(pb200_paella* m, const int64_t* tokens, const flo
                 ap.scale_log2 = 1.4426950408889634f / sqrtf((float)(ch / c.nhead[l]));
                 ap.attn_w = attn_w; ap.n_w = n_w; ap.w_batch = w_batch;
                 ap.w_ld = w_ld; ap.w_len = w_len; ap.w_row = w_row;
-                if (prompt_mask) {
-                    const AttnRegion rg{ws.qmask + qmask_off[l], region_slot, mask_row, max_regions, n_base};
-                    PB_TRY(launch_attention(ap, st, &rg));
-                } else {
-                    PB_TRY(launch_attention(ap, st));
-                }
+                const AttnRegion rg{ws.qmask + qmask_off[l], region_slot, mask_row, max_regions, n_base};
+                PB_TRY(launch_attention(ap, st, prompt_mask ? &rg : nullptr, map_batch > 0 ? &mo : nullptr));
+                if (map_batch > 0) PB_TRY(launch_attention_maps_accumulate(ap, mo, map_acc, map_len, map_pos, map_off[l], st));
                 pb200_gemm_epilogue e2 = epi(PB200_EPI_RESID_F32, m->w<float>(b.outproj_b), x, ch);
                 e2.resid = x; e2.ldr = ch; e2.rows_per_sample = P;
                 PB_TRY(m->gemm(ws.o16, ch, M, ch, b.outproj_w, ch, e2, st));
@@ -865,6 +910,17 @@ int pb200_paella_features_tail(pb200_paella* m, const int64_t* tokens, const flo
         if (Bc < Bt) PB_TRY(tail_copy(features, (size_t)h * w * c.c_out * sizeof(float)));
     }
     return 0;
+}
+
+int pb200_paella_attention_maps_finalize(pb200_paella* m, const float* map_acc, int rows, int map_len, int h, int w, int s, int n_steps,
+                                         float* maps, void* stream) {
+    PB_CHECK(m != nullptr && (rows == 0 || (map_acc != nullptr && maps != nullptr)), "attention_maps_finalize: null argument");
+    PB_CHECK(rows >= 0 && n_steps > 0 && s >= 0 && s <= map_len, "attention_maps_finalize: %d rows, %d of %d keys, %d steps", rows, s,
+             map_len, n_steps);
+    const int ps = m->cfg.patch_size, L = m->cfg.n_levels;
+    PB_CHECK(h % (ps << (L - 1)) == 0 && w % (ps << (L - 1)) == 0, "latent grid %dx%d not divisible by %d", h, w, ps << (L - 1));
+    const float scale = 1.0f / (float)((int64_t)n_steps * (m->n_attn > 0 ? m->n_attn : 1));
+    return launch_attention_maps_finalize(map_acc, rows, map_len, map_positions(m, h, w), s, h, w, ps, L, scale, maps, (cudaStream_t)stream);
 }
 
 int pb200_paella_guidance_mix(pb200_paella* m, float* features, int hw, const int* rows, const float* coef, int n_composed, int ld,

@@ -36,7 +36,9 @@ K/V are projected at admission into slots reserved for its token slot, and its t
 pools by token slot; regional prompts draw nothing.  With ``guidance_prompts=[(inputs, weight), ...]`` (an engine built with
 ``max_guidance_prompts`` > 0) a guided request mixes further weighted prompts into its guidance as ``sample_notebook(...,
 guidance_prompts=[terms])`` does: their K/V are projected at admission into slots reserved for its token slot, and each of its
-guided steps runs one more denoiser row per term; terms draw nothing.
+guided steps runs one more denoiser row per term; terms draw nothing.  With ``attention_maps=True`` a request's
+``req.attention_maps`` (float32 [S, H, W], S its conditioning length) is set when it retires, equal bit for bit to the maps of
+``sample_notebook(..., attention_maps=True)`` on the same request; its tokens are unchanged, and maps draw nothing.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -53,7 +55,11 @@ denoiser (pb200_paella_features_regional), each row reading its token slot's mas
 launches exactly as without regional prompts.  A step in which some guided row has guidance prompts appends their term rows after
 the unconditional rows, ordered by request, then term (pb200_paella_features_tail, each term row reading its own K/V slot), mixes
 each such request's rows into its conditional row (pb200_paella_guidance_mix) and samples that row with the params (1, 0, 1/T); the
-tail map, mix rows and coefficients ride in the step's table.  A step with no such row launches exactly as without them.
+tail map, mix rows and coefficients ride in the step's table.  A step with no such row launches exactly as without them.  A
+step in which some row wants attention maps adds each row's map row (its token slot, -1 for the rows that do not) to the table and
+runs the maps denoiser (pb200_paella_features_maps), which accumulates into a pool of per-slot accumulators, allocated when the
+first such request is admitted and zeroed per request at admission; a request's maps are finalized with its own step count when it
+retires.  A step with no such row launches exactly as without maps.
 The host knows which
 requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
 in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
@@ -81,7 +87,8 @@ class Request:
                  generator=None, inputs=None, uncond=None, init_x=None, decode: bool = False,
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
                  region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
-                 top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None, terms=None, mix_coef=None):
+                 top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None, terms=None, mix_coef=None,
+                 attention_maps: bool = False, maps_len: int = 0):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -97,6 +104,8 @@ class Request:
         self.n_terms = len(terms) if terms is not None else 0
         self.mix_coef = mix_coef                 # CPU float32 [cond_steps, 2 + n_terms]: the guided steps' mix coefficients
         self.term_slot: List[int] = []           # the K/V slots of the terms
+        self.want_maps, self.maps_len = attention_maps, maps_len      # attention maps, over maps_len conditioning keys
+        self.attention_maps: Optional[torch.Tensor] = None            # float32 [maps_len, H, W], set at retirement
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -149,6 +158,9 @@ class StepPlan:
         self.row_slot = torch.tensor([q.slot for q in order], dtype=torch.int32)
         self.kv_slot = torch.tensor([q.slot for q in order] + [q.uncond_slot for q in order[:self.n_pairs]] +
                                     [s for i in self.composed for s in order[i].term_slot], dtype=torch.int32)
+        # attention maps: each row's accumulator row (its token slot), -1 for the rows without maps
+        self.maps = any(q.want_maps for q in order)
+        self.map_row = torch.tensor([q.slot if q.want_maps else -1 for q in order], dtype=torch.int32)
 
 
 def cond_layout(inputs: Dict[str, torch.Tensor]) -> Tuple[int, bool, int]:
@@ -175,10 +187,10 @@ def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List
 def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tuple[torch.Tensor, Dict[str, Tuple[str, int, int]]]:
     """The step's one host-to-device buffer: int64 [(seed, offset) pairs of the sampler's draw, then of the mask draw], then the
     float32 part [r, params (3 per row), t_next, (top_p), (mix_coef)], then the int32 part [row_slot, kv_slot, (mode table), (top_k),
-    (tail, mix_rows)], then the uint8 part [(wrap)], each part padded to whole int64 words.  top_p / top_k are present only when
-    ``plan.truncates``, the mode table only when the step mixes modes, wrap (one byte per row) only when ``plan.wraps``, the tail
-    map and the mix table only when some row of the step is composed (guidance prompts).  Returns (buffer, {name: (dtype,
-    start, length)}), start and length in elements of that dtype within its part."""
+    (tail, mix_rows), (map_row)], then the uint8 part [(wrap)], each part padded to whole int64 words.  top_p / top_k are present
+    only when ``plan.truncates``, the mode table only when the step mixes modes, wrap (one byte per row) only when ``plan.wraps``,
+    the tail map and the mix table only when some row of the step is composed (guidance prompts), map_row only when some row wants
+    attention maps.  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
     Bc, n_pairs = len(plan.order), plan.n_pairs
     mixed = not all(plan.draws)
     modes = ops.mode_table(plan.modes) if mixed else torch.zeros(0, dtype=torch.int32)
@@ -190,6 +202,8 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
     if plan.composed:
         f32_parts.append(("mix_coef", plan.mix_coef.view(-1)))
         i32_parts += [("tail", plan.tail), ("mix_rows", plan.mix_rows.view(-1))]
+    if plan.maps:
+        i32_parts.append(("map_row", plan.map_row))
     u8_parts = [("wrap", plan.wrap)] if plan.wraps else []
     layout: Dict[str, Tuple[str, int, int]] = {}
     for dt, parts in (("f32", f32_parts), ("i32", i32_parts), ("u8", u8_parts)):
@@ -299,6 +313,7 @@ class SamplingEngine:
                 self.shared_slot = 2 * self.max_batch
                 with torch.inference_mode():
                     model.write_conditioning(self.cache, self.shared_slot, unconditional_inputs, (self.H, self.W))
+        self.map_acc: Optional[torch.Tensor] = None      # attention maps: [max_batch, max_cond_len, positions], on first use
         self._free = list(range(self.max_batch))
         self._queue: collections.deque = collections.deque()
         self._active: List[Request] = []
@@ -320,7 +335,8 @@ class SamplingEngine:
     def submit(self, model_inputs, unconditional_inputs=None, *, generator=None, steps=12, renoise_steps=None,
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
-               sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None) -> Request:
+               sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
+               attention_maps=False) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -339,8 +355,10 @@ class SamplingEngine:
         region) gives the request regional prompts as in sample_notebook; ValueError for any other value, and with
         ``attn_weights``.  ``guidance_prompts`` (None or a list of at most max_guidance_prompts (inputs, weight) pairs: a batch-1
         conditioning dict of at most max_cond_len rows and a finite real weight) mixes further prompts into a guided request's
-        guidance as in sample_notebook; ValueError for any other value, and on a request without cfg.  The request's draws start
-        when it is admitted."""
+        guidance as in sample_notebook; ValueError for any other value, and on a request without cfg.  ``attention_maps=True`` sets
+        ``req.attention_maps`` at retirement (module docstring); ValueError for a flag that is not a bool and with
+        ``prompt_regions``.  The request's draws start when it is admitted."""
+        attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
         g_idx = generator.device.index if generator.device.index is not None else torch.cuda.current_device()
@@ -410,7 +428,7 @@ class SamplingEngine:
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
                       sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap, regions,
-                      terms, mix_coef)
+                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs))
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
@@ -460,6 +478,12 @@ class SamplingEngine:
         if R:
             self.prompt_mask.index_copy_(0, slots.long(), regional_d[0])
             self.region_slot.index_copy_(0, slots.long(), regional_d[1])
+        if any(q.want_maps for q in new):
+            if self.map_acc is None:
+                self.map_acc = m.map_accumulator(self.max_batch, self.s_max, (self.H, self.W))
+            for q in new:
+                if q.want_maps:
+                    self.map_acc[q.slot].zero_()
         ops.randint_per_sample(self.noise, m.num_labels, table, slot=slots, batch=n)
         for q in new:
             s = q.slot
@@ -525,6 +549,8 @@ class SamplingEngine:
             wrap_d = part("wrap") if plan.wraps else None
             n_tail = plan.tail.numel() if plan.composed else n_pairs
             tail = dict(tail_src=part("tail")) if plan.composed else dict(n_pairs=n_pairs)
+            if plan.maps:       # row b accumulates into its token slot's maps
+                tail["maps"] = (part("map_row"), Bc, self.map_acc)
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_tail, self.s_max, self.n_slots, kv_slot_d)
@@ -568,6 +594,8 @@ class SamplingEngine:
                 for i, q in enumerate(dec):
                     q.result = imgs[i:i + 1]
             for q in done:
+                if q.want_maps:
+                    q.attention_maps = m.finalize_attention_maps(self.map_acc[q.slot:q.slot + 1], (H, W), q.maps_len, q.steps)[0]
                 if not q.decode:
                     q.result = self.tokens[q.slot:q.slot + 1].clone()
                 self._free.append(q.slot)

@@ -650,7 +650,8 @@ class Paella(nn.Module):
     def features(self, x: torch.Tensor, r: torch.Tensor, cond: ConditioningCache, attn_weights=None,
                  attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None,
                  w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None,
-                 wrap: Optional[torch.Tensor] = None, regional=None, tail_src: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 wrap: Optional[torch.Tensor] = None, regional=None, tail_src: Optional[torch.Tensor] = None,
+                 maps=None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
@@ -672,7 +673,11 @@ class Paella(nn.Module):
         ``tail_src``: an arbitrary tail instead of ``cfg_pairs`` / ``n_pairs``, a device int32 [n_tail] of samples of x: the
         result has B + n_tail samples, sample B + i being sample tail_src[i]'s tokens and r under conditioning row B + i of
         ``cond`` (guidance prompts: the unconditional rows, then the term rows).  Tail rows read their source's wrap byte and are
-        never masked nor weighted (pb200_paella_features_tail)."""
+        never masked nor weighted (pb200_paella_features_tail).
+        ``maps``: attention maps, (map_row, map_batch, acc): sample b < map_batch of x adds its AttnBlocks' cross-attention maps to
+        accumulator row map_row[b] (a device int32 [map_batch], -1: none; None: row b) of ``acc`` (map_accumulator), so that
+        finalize_attention_maps turns it into the map of the forwards summed there (pb200_paella_features_maps).  The features are
+        those of the call without it, bit for bit.  None launches exactly the kernels without it."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -695,17 +700,27 @@ class Paella(nn.Module):
         with torch.cuda.device(dev):
             x = x.to(device=dev, dtype=torch.int64).contiguous()
             r = r.to(device=dev, dtype=torch.float32).contiguous()
-            ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, Bt, H, W, cond.s_max))
+            ws_bytes = L.pb200_paella_workspace_bytes(self._handle, Bt, H, W, cond.s_max)
+            if maps is not None:
+                map_row, map_batch, acc = maps
+                if acc.dtype != torch.float32 or acc.dim() != 3 or not acc.is_contiguous() or acc.device != dev \
+                        or acc.shape[2] != self.map_positions((H, W)) or not 0 <= map_batch <= Bt - n_pairs \
+                        or (map_row is not None and (map_row.dtype != torch.int32 or map_row.numel() < map_batch)) \
+                        or (map_row is None and map_batch > acc.shape[0]):
+                    raise PaellaB200Error(f"features: attention maps need a contiguous float32 accumulator [rows, keys, "
+                                          f"{self.map_positions((H, W))}] on {dev} and an optional int32 map_row [map_batch]")
+                ws_bytes += L.pb200_paella_maps_workspace_bytes(self._handle, acc.shape[0], H, W, cond.s_max)
+            ws = self._ws(ws_bytes)
             feats = torch.empty(Bt * H * W, self._cfg["c_out"], dtype=torch.float32, device=dev)
             if w_len is not None:
                 if attn_weights is None or attn_weights.dim() != 2 or attn_weights.dtype != torch.float32 or w_len.dtype != torch.int32 \
                         or w_len.numel() != attn_weights.shape[0] or (w_row is not None and w_row.numel() < attn_weights_batch):
                     raise PaellaB200Error("features: a per-sample weight table is float32 [rows, w_ld] with int32 w_len [rows] "
                                           "and an optional int32 w_row [attn_weights_batch]")
-                if regional is not None or tail_src is not None:
+                if regional is not None or tail_src is not None or maps is not None:
                     self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(attn_weights), 0, attn_weights.shape[1], ptr(w_len),
                                                                             ptr(w_row)), attn_weights_batch, wrap, regional, feats, ws,
-                                            tail_src)
+                                            tail_src, maps)
                     return feats
                 if wrap is not None:
                     check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -719,9 +734,9 @@ class Paella(nn.Module):
                                                        current_stream()), "pb200_paella_features_weighted")
                 return feats
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
-            if regional is not None or tail_src is not None:
+            if regional is not None or tail_src is not None or maps is not None:
                 self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(aw), aw.numel() if aw is not None else 0, 0, None, None),
-                                        attn_weights_batch, wrap, regional, feats, ws, tail_src)
+                                        attn_weights_batch, wrap, regional, feats, ws, tail_src, maps)
                 return feats
             if wrap is not None:        # the single weight vector is the weighted call with w_ld = 0 and no w_len
                 check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -735,8 +750,9 @@ class Paella(nn.Module):
                                                 ws.numel(), current_stream()), "pb200_paella_features_pairs")
         return feats
 
-    def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws, tail_src=None):
-        """pb200_paella_features_regional, or with ``tail_src`` pb200_paella_features_tail (``regional`` may then be None)."""
+    def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws, tail_src=None, maps=None):
+        """pb200_paella_features_regional, or with ``tail_src`` pb200_paella_features_tail, or with ``maps``
+        pb200_paella_features_maps (``regional`` may then be None)."""
         mask = region_slot = mask_row = None
         if regional is not None:
             mask, region_slot, mask_row = regional
@@ -749,6 +765,14 @@ class Paella(nn.Module):
         if w_batch > Bt - n_pairs:
             raise PaellaB200Error(f"features: {w_batch} weighted samples of {Bt - n_pairs}")
         n_regions = region_slot.shape[1] if region_slot is not None else 0
+        if maps is not None:
+            map_row, map_batch, acc = maps
+            check(lib().pb200_paella_features_maps(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                   ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
+                                                   ptr(mask_row), ptr(region_slot), n_regions, ptr(tail_src), ptr(map_row), map_batch,
+                                                   ptr(acc), acc.shape[0], acc.shape[1], ptr(feats), ptr(ws), ws.numel(),
+                                                   current_stream()), "pb200_paella_features_maps")
+            return
         if tail_src is not None:
             check(lib().pb200_paella_features_tail(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
                                                    ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
@@ -759,6 +783,32 @@ class Paella(nn.Module):
                                                    ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
                                                    ptr(mask_row), ptr(region_slot), n_regions, ptr(feats), ptr(ws),
                                                    ws.numel(), current_stream()), "pb200_paella_features_regional")
+
+    def map_positions(self, latent_hw) -> int:
+        """Columns of an attention-map accumulator on a ``latent_hw`` token grid: every level's block positions, level 0 first."""
+        ps = self._cfg["patch_size"]
+        return sum((int(latent_hw[0]) // (ps << l)) * (int(latent_hw[1]) // (ps << l)) for l in range(len(self._cfg["c_hidden"])))
+
+    def map_accumulator(self, rows: int, cond_len: int, latent_hw) -> torch.Tensor:
+        """A zeroed attention-map accumulator for features' ``maps``: float32 [rows, cond_len, map_positions] on the model's device."""
+        return torch.zeros(rows, cond_len, self.map_positions(latent_hw), dtype=torch.float32, device=self._device())
+
+    def finalize_attention_maps(self, acc: torch.Tensor, latent_hw, cond_len: int, n_steps: int) -> torch.Tensor:
+        """Attention maps float32 [rows, cond_len, H, W] from accumulator rows ``acc`` (a contiguous run of map_accumulator rows)
+        summed over ``n_steps`` forwards: every level upsampled by nearest neighbour, the levels summed and the result scaled by
+        1 / (n_steps * number of AttnBlocks) -- pb200_paella_attention_maps_finalize."""
+        self._ensure_packed()
+        H, W = int(latent_hw[0]), int(latent_hw[1])
+        if acc.dtype != torch.float32 or acc.dim() != 3 or not acc.is_contiguous() or acc.shape[2] != self.map_positions((H, W)) \
+                or not 0 <= cond_len <= acc.shape[1]:
+            raise PaellaB200Error(f"finalize_attention_maps: a contiguous float32 accumulator [rows, >= {cond_len}, "
+                                  f"{self.map_positions((H, W))}] is required")
+        with torch.cuda.device(self._device()):
+            out = torch.empty(acc.shape[0], cond_len, H, W, dtype=torch.float32, device=self._device())
+            check(lib().pb200_paella_attention_maps_finalize(self._handle, ptr(acc), acc.shape[0], acc.shape[1], H, W, cond_len,
+                                                             int(n_steps), ptr(out), current_stream()),
+                  "pb200_paella_attention_maps_finalize")
+        return out
 
     def guidance_mix(self, feats: torch.Tensor, hw: int, rows: torch.Tensor, coef: torch.Tensor) -> torch.Tensor:
         """Guidance prompts: the K-way guided mix in place on ``feats`` (fp32 [samples * hw, c_out], features' output), one
@@ -1020,12 +1070,18 @@ class Paella(nn.Module):
         7 (inputs, region) pairs -- a batch-1 conditioning dict and a bool [H, W] token mask on the CPU or the model's device
         (ops.regional_table).  Every AttnBlock position then attends to the self keys and to the conditioning of each region its
         footprint touches, and to the sample's own conditioning where its footprint touches no region.  ValueError, before
-        anything is enqueued, for a bad entry and for regions on a sample that also has attn_weights."""
+        anything is enqueued, for a bad entry and for regions on a sample that also has attn_weights.
+        ``attention_maps=True`` (keyword only): returns (logits, maps), maps float32 [B, S, H, W] on the model's device: for key s
+        of the sample's conditioning sequence (gen_c_embeddings order) and token (y, x), the mean over every AttnBlock and its
+        heads of the post-softmax, post-attn_weights probability the block position holding the token gives the key -- what the
+        reference's CustomMultiheadAttention returns with need_weights=True.  The logits are those of the call without it, bit
+        for bit.  ValueError, before anything is enqueued, for a flag that is not a bool and for maps with prompt_regions."""
         if x_cat is not None:
             x = torch.cat([x, x_cat], dim=1)
         attn_weights = kwargs.pop("attn_weights", None)
         tiling = kwargs.pop("tiling", None)
         prompt_regions = kwargs.pop("prompt_regions", None)
+        attention_maps = ops.check_attention_maps(kwargs.pop("attention_maps", False), prompt_regions)
         if kwargs:
             raise TypeError(f"unexpected keyword arguments {sorted(kwargs)}")
         B, H, W = x.shape
@@ -1043,8 +1099,13 @@ class Paella(nn.Module):
             regional = self.regional_device(regions, cond)
         if wrap is not None:
             wrap = ops.to_device_async(wrap, self._device())
-        feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len, wrap=wrap, regional=regional)
-        return self.logits_from_features(feats, B, H, W)
+        acc = self.map_accumulator(B, cond_len, (H, W)) if attention_maps else None
+        feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len, wrap=wrap, regional=regional,
+                              maps=(None, B, acc) if attention_maps else None)
+        logits = self.logits_from_features(feats, B, H, W)
+        if attention_maps:
+            return logits, self.finalize_attention_maps(acc, (H, W), cond_len, 1)
+        return logits
 
     def _cond_for_forward(self, byt5, clip, clip_image, hw):
         """The reference's own loop calls ``model(x, t, **inputs)`` twice per step with the SAME conditioning tensors

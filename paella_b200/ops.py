@@ -374,6 +374,17 @@ def check_regions_unweighted(table, attn_weights) -> None:
             raise ValueError(f"prompt_regions[{b}]: regional prompts and attn_weights on one sample are not supported")
 
 
+def check_attention_maps(attention_maps, prompt_regions=None) -> bool:
+    """``attention_maps`` -> the flag.  ValueError, before anything is enqueued, unless it is a bool, and for maps on a call or
+    request that also has ``prompt_regions``: regional tiles gate the sample's own prompt keys per query, and maps are not
+    defined there."""
+    if not isinstance(attention_maps, bool):
+        raise ValueError(f"attention_maps: expected a bool (got {type(attention_maps).__name__})")
+    if attention_maps and prompt_regions is not None:
+        raise ValueError("attention_maps: not defined together with prompt_regions")
+    return attention_maps
+
+
 # ------------------------------------------------------------------ guidance prompts
 # Each sample of a guided call may carry up to MAX_GUIDANCE_PROMPTS (inputs, weight) terms.  On a guided step with scale cfg its
 # logits are l_u + cfg * [(l_c - l_u) + sum_j w_j (l_j - l_u)], l_j being the conditional forward under term j's inputs.  The

@@ -66,6 +66,15 @@ same offset, and the per-sample guarantees above hold for such rows too.  Term p
 row.  ValueError, before anything is enqueued and before any generator advances, for the wrong number of entries, more than 7
 terms, bad inputs or a non-finite weight, terms in a call that is not guided (cfg None; in ``sample`` a cfg of 0, or a per-sample
 cfg of 0 on a sample with terms), and terms with ``exact=True``.
+
+Attention maps: ``attention_maps=True`` (all three functions) also returns maps, float32 [B, S, H, W] on the model's device: for
+key s of sample i's conditioning sequence (gen_c_embeddings order: the byt5 rows, then clip_seq_len rows per clip and per clip_image
+embedding) and token (y, x), the mean over the call's steps, every AttnBlock and its heads of the post-softmax, post-attn_weights
+probability that the block position holding the token gives the key, as the reference's CustomMultiheadAttention returns it with
+need_weights=True (pb200_paella_features_maps).  Only the sample's own conditional row contributes, on every step, guided or not.
+Maps draw no random numbers and change no token: tokens, intermediates and generator offsets are those of the call without them,
+and a sample's maps depend only on its own request where the forward is batch-invariant.  ValueError, before anything is enqueued
+and before any generator advances, for a flag that is not a bool and for maps together with ``prompt_regions``.
 """
 from __future__ import annotations
 
@@ -173,13 +182,15 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
                  codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None,
-                 prompt_regions=None, guidance_prompts=None):
-    """``modes``: None, or per step the list of B mode names (sampling_modes) -- a step whose modes differ samples each row in
-    its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the scalar path in that mode.  ``top_k`` /
-    ``top_p``: the truncation of the multinomial draws (module docstring); a truncating call takes the per-sample table path,
-    and so does a call with ``guidance_prompts`` (module docstring)."""
+                 prompt_regions=None, guidance_prompts=None, attention_maps=False):
+    """Returns (tokens, intermediates, maps or None).  ``modes``: None, or per step the list of B mode names (sampling_modes) --
+    a step whose modes differ samples each row in its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the
+    scalar path in that mode.  ``top_k`` / ``top_p``: the truncation of the multinomial draws (module docstring); a truncating
+    call takes the per-sample table path, and so does a call with ``guidance_prompts`` (module docstring).  ``attention_maps``:
+    the maps of the conditional rows (module docstring)."""
     B, H, W = latent_shape
     dev = model._device()
+    attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
     check_region(region, init_x, latent_shape, dev)
     trunc = ops.truncation_table(top_k, top_p, B, model.num_labels)
     wrap = ops.tiling_table(tiling, B)
@@ -256,6 +267,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         regional_full = model.regional_device(regions, cond_full) if regions is not None else None
         extra_only = extra[:len(extra) - len(mix[1])] if mix is not None else extra
         cond_only = regional_only = None
+        # attention maps: the conditional rows [0, B) accumulate into rows [0, B), finalized once after the loop
+        maps_len = model.conditioning_seq_len(model_inputs) if attention_maps else 0
+        acc = model.map_accumulator(B, maps_len, (H, W)) if attention_maps else None
         intermediates = []
         for i in range(steps):
             step_modes = None
@@ -282,7 +296,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             composed = guided and mix is not None
             feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided and not composed,
                                    w_len=w_len, wrap=wrap_d, regional=regional_only if cond is cond_only else regional_full,
-                                   tail_src=tail_d if composed else None)
+                                   tail_src=tail_d if composed else None, maps=(None, B, acc) if attention_maps else None)
             if composed:
                 model.guidance_mix(feats, H * W, mix_rows_d, mix_coef_d[i])
             if step_modes is not None:
@@ -324,7 +338,8 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                     sampled = model.add_noise(sampled, t_next, random_x=init_noise, generator=generator, src=src_d, region=region_d)[0]
                 if collect:
                     intermediates.append(sampled)
-    return sampled, intermediates
+        maps = model.finalize_attention_maps(acc, (H, W), maps_len, steps) if attention_maps else None
+    return sampled, intermediates, maps
 
 
 def _sample_modes_step(model, feats, B, H, W, guided, params, step_modes, generators, codebook, dev, trunc=None):
@@ -402,7 +417,7 @@ def _decode_tail(tokens, decode, decode_output, tiling=None):
 
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
            cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
-           top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None):
+           top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None, attention_maps=False):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -418,7 +433,9 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     ``tiling`` (module docstring): seamless tiling per call or per sample; with ``decode`` each image is decoded with its own
     tiling.  ValueError, before anything is enqueued and before any generator advances, for an unknown value, a list of the
     wrong length or a tensor.  ``prompt_regions`` (module docstring): regional prompts per sample.  ``guidance_prompts`` (module
-    docstring): weighted extra and negative prompts per sample in the guided mix; a sample with terms needs a cfg other than 0."""
+    docstring): weighted extra and negative prompts per sample in the guided mix; a sample with terms needs a cfg other than 0.
+    ``attention_maps=True`` (module docstring): returns (tokens or images, maps)."""
+    ops.check_attention_maps(attention_maps, prompt_regions)
     per_sample_cfg = torch.is_tensor(cfg)
     terms = ops.guidance_table(guidance_prompts, latent_shape[0])
     if terms is not None and per_sample_cfg:
@@ -433,17 +450,18 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
         cfgs = [cfg] * steps if cfg else None
     if cfgs is not None and unconditional_inputs is None:
         raise TypeError("sample(): cfg is set but unconditional_inputs is None")
-    out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, None, steps, renoise_steps,
-                          temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
-                          per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling, prompt_regions=prompt_regions,
-                          guidance_prompts=guidance_prompts)
-    return _decode_tail(out, decode, decode_output, tiling)
+    out, _, maps = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, None, steps, renoise_steps,
+                                temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
+                                per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling,
+                                prompt_regions=prompt_regions, guidance_prompts=guidance_prompts, attention_maps=attention_maps)
+    out = _decode_tail(out, decode, decode_output, tiling)
+    return (out, maps) if attention_maps else out
 
 
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
                        exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None,
-                       guidance_prompts=None):
+                       guidance_prompts=None, attention_maps=False):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
@@ -453,23 +471,26 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     ``top_k[lo:hi]`` computes what rows [lo, hi) compute.  ``tiling`` as in ``sample``; a shard given ``tiling[lo:hi]`` computes
     what rows [lo, hi) compute.  ``prompt_regions`` (module docstring) likewise: a shard given ``prompt_regions[lo:hi]`` computes
     what rows [lo, hi) compute.  ``guidance_prompts`` (module docstring) likewise: a shard given ``guidance_prompts[lo:hi]``
-    computes what rows [lo, hi) compute."""
+    computes what rows [lo, hi) compute.  ``attention_maps=True`` (module docstring): returns (tokens, maps) for the shard's rows."""
+    ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
         renoise_steps = steps - 1
     cfgs = _cfg_schedule(cfg, latent_shape[0], steps)
-    out, _ = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
-                          temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
-                          generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
-                          tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts)
-    return out
+    out, _, maps = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
+                                temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
+                                generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
+                                tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts,
+                                attention_maps=attention_maps)
+    return (out, maps) if attention_maps else out
 
 
 def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None, init_x=None, steps=12, renoise_steps=None,
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
-                    generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None):
+                    generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
+                    attention_maps=False):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -485,7 +506,9 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     ``top_k`` / ``top_p`` as in ``sample``: they truncate the multinomial steps only.  ``tiling`` as in ``sample``: the
     intermediates are those of the tiled call.  ``prompt_regions`` as in ``sample``; regional samples' rows may not also
     have ``attn_weights``.  ``guidance_prompts`` as in ``sample``: the argmax and quant steps of a sample with terms see its mixed
-    features, and ``attn_weights`` weight its conditional row only."""
+    features, and ``attn_weights`` weight its conditional row only.  ``attention_maps=True`` (module docstring): returns
+    (sampled, intermediate_images, maps)."""
+    ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
     if renoise_steps is None:
@@ -499,7 +522,10 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
         mode = mode[0]
     if modes is None and isinstance(sampling_quant_steps, (list, tuple)):
         sampling_quant_steps = sampling_quant_steps[0]
-    return _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps, renoise_steps,
-                        temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, True,
-                        sampling_quant_steps, codebook, generator, per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes,
-                        top_k=top_k, top_p=top_p, tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts)
+    sampled, intermediates, maps = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, init_x, steps,
+                                                renoise_steps, temperature, cfgs, t_start, t_end, sampling_conditional_steps, mode,
+                                                attn_weights, exact, True, sampling_quant_steps, codebook, generator,
+                                                per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes, top_k=top_k,
+                                                top_p=top_p, tiling=tiling, prompt_regions=prompt_regions,
+                                                guidance_prompts=guidance_prompts, attention_maps=attention_maps)
+    return (sampled, intermediates, maps) if attention_maps else (sampled, intermediates)
