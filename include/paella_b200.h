@@ -275,6 +275,20 @@ int pb200_attention_maps(const void* qkv16, const void* ckv16, const int* kv_len
                          int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
                          int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
                          float* scores, float* lse2, const int* map_row, int map_batch, void* stream);
+/* Prompt-to-prompt injection: pb200_attention_regional (q_mask NULL: no regions) with optional attention maps
+ * (pb200_attention_maps; map_batch 0: none), where sample b < inj_batch with a = inj_src[b] >= 0 (DEVICE int32 [inj_batch], -1:
+ * none) replays sample a's attention probabilities:
+ *   out[b] = (softmax(scale * Q_a [K_a,self ; K_a,cond]^T) * w_b) [V_b,self ; V_b,cond]
+ * Q_a and K_a,self are sample a's rows of qkv16, K_a,cond its slot kv_slot[a]'s; the values, kv_len and the weights w_b are
+ * sample b's own.  The caller keeps kv_len of b's and a's slots equal.  With q_mask, an injected sample and its source must see
+ * prompt 0 alone at every query.  inj_src[b] == b gives the bits of the call without injection.  A map row of an injected
+ * sample holds the replayed probabilities.  [prompt-to-prompt editing, Hertz et al. 2022, on ref/utils/alter_attention.py] */
+int pb200_attention_inject(const void* qkv16, const void* ckv16, const int* kv_len, const int* kv_slot, int n_slots, void* out16,
+                           int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
+                           int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
+                           const uint8_t* q_mask, const int* region_slot, const int* mask_row, int max_regions, int mask_batch,
+                           float* scores, float* lse2, const int* map_row, int map_batch, const int* inj_src, int inj_batch,
+                           void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Denoiser (ref/src/modules.py:109-283, ref/utils/modules.py) as an opaque handle.
@@ -428,6 +442,18 @@ int pb200_paella_features_maps(pb200_paella* m, const int64_t* tokens, const flo
                                const int* mask_row, const int* region_slot, int max_regions, const int* tail_src, const int* map_row,
                                int map_batch, float* map_acc, int map_rows, int map_len, float* features, void* workspace,
                                int64_t workspace_bytes, void* stream);
+/* Prompt-to-prompt injection: pb200_paella_features_maps where, in every AttnBlock and every head, base sample b < inj_batch
+ * with a = inj_src[b] >= 0 (DEVICE int32 [inj_batch], -1: none; a < batch_total - n_tail, a != b) attends with sample a's
+ * attention probabilities and its own values (pb200_attention_inject).  The caller keeps the conditioning lengths of b and a
+ * equal, and neither is regional.  Rows that are not injected, the source rows among them, get the bits of the call without
+ * injection.  inj_batch = 0 is pb200_paella_features_maps, the same launches. */
+int pb200_paella_features_inject(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                                 const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                                 int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
+                                 const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
+                                 const int* tail_src, const int* map_row, int map_batch, float* map_acc, int map_rows, int map_len,
+                                 const int* inj_src, int inj_batch, float* features, void* workspace, int64_t workspace_bytes,
+                                 void* stream);
 /* maps fp32 [rows][s][h][w] from rows consecutive accumulator rows of pb200_paella_features_maps accumulated over n_steps
  * forwards: maps[row][j][y][x] = (1 / (n_steps * n_attn)) * sum over levels l, ascending, of
  * map_acc[row][j][off_l + (y / (patch << l)) * gw_l + x / (patch << l)] (nearest-neighbour upsampling); s <= map_len. */

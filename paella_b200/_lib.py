@@ -101,6 +101,9 @@ SIGNATURES = {
     "pb200_attention_maps": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                      c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                      c_void_p]),
+    "pb200_attention_inject": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                       c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                       c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "pb200_paella_create": (c_int, [POINTER(PaellaConfig), POINTER(c_void_p)]),
     "pb200_paella_destroy": (None, [c_void_p]),
     "pb200_paella_weight_bytes": (c_int64, [c_void_p]),
@@ -138,6 +141,10 @@ SIGNATURES = {
                                            c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                            c_int64, c_void_p]),
+    "pb200_paella_features_inject": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                             c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int,
+                                             c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_attention_maps_finalize": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_int64, c_void_p]),

@@ -46,9 +46,11 @@ constexpr float NEG_BIG = -1e30f;
 // (attn_build_segs); a row's keys of a prompt it does not see are masked like keys past the end, so its softmax is exact over
 // the keys it sees.  MAPS (attention_kernel_maps, and with REG attention_kernel_regional_maps): attention maps (AttnMapOut); a map
 // row also stores the scaled scores of its own conditioning keys (prompt 0's) and, at the end, its rows' log2-sum-exp, and O takes
-// the same arithmetic as the instance without maps.
-template <int HD, bool REG, bool MAPS>
-__device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRegion& rg, const AttnMapOut& mo) {
+// the same arithmetic as the instance without maps.  INJ (the _inject instances): prompt-to-prompt injection (AttnInject); Q and
+// the K rows come from the source sample's row (self keys) or slot (its prompt 0's conditioning keys), the V rows from the
+// sample's own, so ks and vs have separate bases.
+template <int HD, bool REG, bool MAPS, bool INJ>
+__device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRegion& rg, const AttnMapOut& mo, const AttnInject& inj) {
     constexpr int LDS = HD + 8;           // padded row: (HD+8)*2 bytes is an odd multiple of 16 -> conflict-free ldmatrix
     constexpr int CPR = HD / 8;           // 16-byte chunks per row
     constexpr int QROWS = ATT_BM;
@@ -71,6 +73,9 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
     const int mr = MAPS ? attn_map_row(mo, b) : -1;
     const __half* qkv_b = p.qkv + (int64_t)b * p.P * ldq;
     const __half* ckv_b = p.ckv + (int64_t)slot * p.S_max * ldc;
+    const int qb = INJ ? attn_inj_src(inj, b) : b;            // the sample whose Q and K this one uses
+    const __half* qkv_k = INJ ? p.qkv + (int64_t)qb * p.P * ldq : qkv_b;
+    const __half* ckv_k = INJ ? p.ckv + (int64_t)(p.kv_slot ? p.kv_slot[qb] : qb) * p.S_max * ldc : ckv_b;
     AttnSegs* segs = reinterpret_cast<AttnSegs*>(sVb + n_buf * ATT_BN * LDS);
     if constexpr (REG) {
         if (warp == 0) {
@@ -90,12 +95,12 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
             const __half *ks = qkv_b, *vs = qkv_b;
             uint32_t nbytes = 0;
             if (j < n_self) {
-                ks = qkv_b + (int64_t)j * ldq + h * HD + cc * 8 + E;
-                vs = ks + E;
+                ks = qkv_k + (int64_t)j * ldq + h * HD + cc * 8 + E;
+                vs = INJ ? qkv_b + (int64_t)j * ldq + h * HD + cc * 8 + 2 * E : ks + E;
                 nbytes = 16;
             } else if (j < Nk) {
-                ks = ckv_b + (int64_t)(j - n_self) * ldc + h * HD + cc * 8;
-                vs = ks + E;
+                ks = ckv_k + (int64_t)(j - n_self) * ldc + h * HD + cc * 8;
+                vs = INJ ? ckv_b + (int64_t)(j - n_self) * ldc + h * HD + cc * 8 + E : ks + E;
                 nbytes = 16;
             }
             cp_async16(smem_u32(sK + r * LDS + cc * 8), ks, nbytes);
@@ -108,6 +113,7 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
         while (c >= segs->first[si + 1]) ++si;
         const int j0 = (c - segs->first[si]) * ATT_BN, len = segs->len[si], from = segs->from[si];
         const __half* cb = p.ckv + (int64_t)segs->slot[si] * p.S_max * ldc;
+        const __half* cb_k = INJ && segs->bit[si] == 0 ? ckv_k : cb;
         __half* sK = sKb + buf * ATT_BN * LDS;
         __half* sV = sVb + buf * ATT_BN * LDS;
         for (int i = tid; i < ATT_BN * CPR; i += 128) {
@@ -116,12 +122,12 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
             const __half *ks = qkv_b, *vs = qkv_b;
             uint32_t nbytes = 0;
             if (j < from) {
-                ks = qkv_b + (int64_t)j * ldq + h * HD + cc * 8 + E;
-                vs = ks + E;
+                ks = qkv_k + (int64_t)j * ldq + h * HD + cc * 8 + E;
+                vs = INJ ? qkv_b + (int64_t)j * ldq + h * HD + cc * 8 + 2 * E : ks + E;
                 nbytes = 16;
             } else if (j < len) {
-                ks = cb + (int64_t)(j - from) * ldc + h * HD + cc * 8;
-                vs = ks + E;
+                ks = cb_k + (int64_t)(j - from) * ldc + h * HD + cc * 8;
+                vs = INJ ? cb + (int64_t)(j - from) * ldc + h * HD + cc * 8 + E : ks + E;
                 nbytes = 16;
             }
             cp_async16(smem_u32(sK + r * LDS + cc * 8), ks, nbytes);
@@ -133,7 +139,7 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
     for (int c = tid; c < QROWS * CPR; c += 128) {
         const int r = c / CPR, cc = c - r * CPR;
         const bool ok = q0 + r < p.P;
-        cp_async16(smem_u32(sQ + r * LDS + cc * 8), ok ? qkv_b + (int64_t)(q0 + r) * ldq + h * HD + cc * 8 : qkv_b, ok ? 16u : 0u);
+        cp_async16(smem_u32(sQ + r * LDS + cc * 8), ok ? qkv_k + (int64_t)(q0 + r) * ldq + h * HD + cc * 8 : qkv_k, ok ? 16u : 0u);
     }
     int n_chunks = 0;
     if constexpr (REG) {
@@ -335,28 +341,47 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
 }
 
 template <int HD>
-__global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) { attention_body<HD, false, false>(p, AttnRegion{}, AttnMapOut{}); }
+__global__ void __launch_bounds__(128) attention_kernel(const AttnParams p) {
+    attention_body<HD, false, false, false>(p, AttnRegion{}, AttnMapOut{}, AttnInject{});
+}
 template <int HD>
 __global__ void __launch_bounds__(128) attention_kernel_regional(const AttnParams p, const AttnRegion rg) {
-    attention_body<HD, true, false>(p, rg, AttnMapOut{});
+    attention_body<HD, true, false, false>(p, rg, AttnMapOut{}, AttnInject{});
 }
 template <int HD>
 __global__ void __launch_bounds__(128) attention_kernel_maps(const AttnParams p, const AttnMapOut mo) {
-    attention_body<HD, false, true>(p, AttnRegion{}, mo);
+    attention_body<HD, false, true, false>(p, AttnRegion{}, mo, AttnInject{});
 }
-// (min blocks 1: at head_dim 80 the default register target spills)
+// (min blocks 1 on the regional maps and regional inject instances: at head_dim 80 the default register target spills)
 template <int HD>
 __global__ void __launch_bounds__(128, 1) attention_kernel_regional_maps(const AttnParams p, const AttnRegion rg, const AttnMapOut mo) {
-    attention_body<HD, true, true>(p, rg, mo);
+    attention_body<HD, true, true, false>(p, rg, mo, AttnInject{});
+}
+template <int HD>
+__global__ void __launch_bounds__(128) attention_kernel_inject(const AttnParams p, const AttnInject inj) {
+    attention_body<HD, false, false, true>(p, AttnRegion{}, AttnMapOut{}, inj);
+}
+template <int HD>
+__global__ void __launch_bounds__(128, 1) attention_kernel_regional_inject(const AttnParams p, const AttnRegion rg, const AttnInject inj) {
+    attention_body<HD, true, false, true>(p, rg, AttnMapOut{}, inj);
+}
+template <int HD>
+__global__ void __launch_bounds__(128) attention_kernel_maps_inject(const AttnParams p, const AttnMapOut mo, const AttnInject inj) {
+    attention_body<HD, false, true, true>(p, AttnRegion{}, mo, inj);
+}
+template <int HD>
+__global__ void __launch_bounds__(128, 1) attention_kernel_regional_maps_inject(const AttnParams p, const AttnRegion rg,
+                                                                                const AttnMapOut mo, const AttnInject inj) {
+    attention_body<HD, true, true, true>(p, rg, mo, inj);
 }
 
-int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo) {
+int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo, const AttnInject* inj) {
     PB_CHECK(p.nhead > 0 && p.E % p.nhead == 0, "attention: E=%d not divisible by nhead=%d", p.E, p.nhead);
     const int hd = p.E / p.nhead;
     PB_CHECK(p.E % 8 == 0, "attention: E must be a multiple of 8");
     if (p.B == 0 || p.P == 0) return 0;
     {
-        const int rc = launch_attention_wgmma(p, st, rg, mo);
+        const int rc = launch_attention_wgmma(p, st, rg, mo, inj);
         if (rc >= 0) return rc;
     }
     // algorithmic bytes: q, self k/v, out once; conditioning k/v once per sample
@@ -365,9 +390,20 @@ int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg,
     PB_CHECK(grid.y <= 65535 && grid.z <= 65535, "attention: grid too large");
     const bool reg = rg != nullptr;
     const size_t smem = (size_t)(ATT_BM + 4 * ATT_BN) * (hd + 8) * sizeof(__half) + (reg ? sizeof(AttnSegs) : 0);
+#define PB_ATT_LAUNCH(KERNEL, ...)                                                                                  \
+    {                                                                                                               \
+        static DeviceOnce attr_once;                                                                                \
+        if (attr_once.first()) PB_CUDA(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        KERNEL<<<grid, 128, smem, st>>>(p, __VA_ARGS__);                                                            \
+        break;                                                                                                      \
+    }
     switch (hd) {
 #define PB_ATT_CASE(H)                                                                                              \
     case H: {                                                                                                       \
+        if (inj != nullptr && mo != nullptr && reg) PB_ATT_LAUNCH(attention_kernel_regional_maps_inject<H>, *rg, *mo, *inj) \
+        if (inj != nullptr && mo != nullptr) PB_ATT_LAUNCH(attention_kernel_maps_inject<H>, *mo, *inj)              \
+        if (inj != nullptr && reg) PB_ATT_LAUNCH(attention_kernel_regional_inject<H>, *rg, *inj)                    \
+        if (inj != nullptr) PB_ATT_LAUNCH(attention_kernel_inject<H>, *inj)                                         \
         if (mo != nullptr && reg) {                                                                                 \
             static DeviceOnce attr_reg_maps;                                                                        \
             if (attr_reg_maps.first())                                                                              \
@@ -398,6 +434,7 @@ int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg,
     }
         PB_ATT_CASE(16) PB_ATT_CASE(32) PB_ATT_CASE(64) PB_ATT_CASE(80) PB_ATT_CASE(96)
 #undef PB_ATT_CASE
+#undef PB_ATT_LAUNCH
         default: PB_CHECK(false, "attention: head_dim %d unsupported (16/32/64/80/96)", hd);
     }
     PB_LAUNCH_CHECK();

@@ -54,6 +54,23 @@ __device__ __forceinline__ int attn_map_row(const AttnMapOut& mo, int b) {
     return mo.map_row ? mo.map_row[b] : b;
 }
 
+// Prompt-to-prompt injection, for samples b < batch with src[b] >= 0: sample b replays sample src[b]'s attention probabilities.
+// It loads Q and its self K from row src[b] and its conditioning K from slot kv_slot[src[b]], and its self V and conditioning V
+// from its own row and slot; key counts come from its own kv_len (the caller keeps them equal to the source's).  attn_weights
+// stay the sample's own.  With src[b] == b the instance computes what the instance without injection computes.  A separate
+// kernel argument, so the plain instances keep their code.
+struct AttnInject {
+    const int* src;
+    int batch;
+};
+
+// The sample whose queries and keys sample b uses: src[b], or b itself
+__device__ __forceinline__ int attn_inj_src(const AttnInject& inj, int b) {
+    if (b >= inj.batch) return b;
+    const int a = inj.src[b];
+    return a >= 0 ? a : b;
+}
+
 constexpr int ATT_MAX_REGIONS = 7;      // prompts 1..7: the mask bits above prompt 0's
 
 // The key walk of a regional tile: segments of keys, each cut into 64-key chunks from its own first key.  Bit `bit` of a
@@ -124,9 +141,12 @@ __device__ __forceinline__ int attn_weight_row(const AttnParams& p, int b, const
 // Dispatch: the wgmma + TMA kernel (attention_wg.cu) for head_dim 80, the mma.sync kernel (attention.cu) for other head dims
 // (rg: the regional table, or NULL for the plain instances)
 // (mo: the map outputs, or NULL.  With rg too, a map row's keys are its prompt 0's; its queries should all see prompt 0 alone.)
-int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr, const AttnMapOut* mo = nullptr);
-int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr,
-                           const AttnMapOut* mo = nullptr);      // 0 launched, 1 error, -1 shape not handled
+// (inj: the injection table, or NULL.  With rg too, only samples whose queries all see prompt 0 alone may be injected or be
+// sources: an injected sample's prompt 0 keys come from its source's slot, further prompts' from their own.)
+int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr, const AttnMapOut* mo = nullptr,
+                     const AttnInject* inj = nullptr);
+int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr, const AttnMapOut* mo = nullptr,
+                           const AttnInject* inj = nullptr);      // 0 launched, 1 error, -1 shape not handled
 // Attention maps (ops.cu): acc [rows][acc_ld][acc_pos] += (1/nhead) * sum over heads h in ascending order of
 // w_s * exp2(score - lse2) at columns [acc_off, acc_off + P), for every map row of p's batch and every conditioning key s < kv_len
 int launch_attention_maps_accumulate(const AttnParams& p, const AttnMapOut& mo, float* acc, int acc_ld, int acc_pos, int acc_off,

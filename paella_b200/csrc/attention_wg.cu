@@ -45,9 +45,12 @@ struct AttnMaps {
 // MAPS (attention_wgmma_kernel_maps, and with REG attention_wgmma_kernel_regional_maps): attention maps (AttnMapOut).  A map row
 // also stores the scaled scores of its own conditioning's chunks (prompt 0's) and, at the end, its rows' log2-sum-exp; O takes the
 // same arithmetic as the instance without maps.
-template <bool REG, bool MAPS>
+// INJ (the _inject instances): prompt-to-prompt injection (AttnInject).  Q and the K boxes of every stage come from the source
+// sample's row (self keys) or slot (its prompt 0's conditioning keys), the V box from the sample's own; the bytes of a stage are
+// the same, so expect_tx is too.
+template <bool REG, bool MAPS, bool INJ>
 __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const AttnParams& p, const AttnRegion& rg,
-                                                     const AttnMapOut& mo) {
+                                                     const AttnMapOut& mo, const AttnInject& inj) {
     pdl_launch_dependents();
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -64,6 +67,8 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
     const int Nk = n_self + n_cond;
     const int n_sc = (n_self + AW_BN - 1) / AW_BN;
     const int mr = MAPS ? attn_map_row(mo, b) : -1;
+    const int qb = INJ ? attn_inj_src(inj, b) : b;                           // the sample whose Q and K this one uses
+    const int kslot = INJ ? (p.kv_slot ? p.kv_slot[qb] : qb) : slot;
     int n_chunks = n_sc + (n_cond + AW_BN - 1) / AW_BN;
     AttnSegs* segs = reinterpret_cast<AttnSegs*>(gbase + AW_OFF_SEGS);
     auto seg_of = [&](int c) {
@@ -79,25 +84,26 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
         if constexpr (REG) {
             const int si = seg_of(c), k0 = (c - segs->first[si]) * AW_BN;
             if (segs->slot[si] < 0) {
-                const int row = b * p.P + k0;
-                ptx::tma_load_2d(&maps.q64, full_bar(st), sb, E + h * AW_HD, row);
-                ptx::tma_load_2d(&maps.q16, full_bar(st), sb + AW_K64, E + h * AW_HD + 64, row);
+                const int row = b * p.P + k0, krow = INJ ? qb * p.P + k0 : row;
+                ptx::tma_load_2d(&maps.q64, full_bar(st), sb, E + h * AW_HD, krow);
+                ptx::tma_load_2d(&maps.q16, full_bar(st), sb + AW_K64, E + h * AW_HD + 64, krow);
                 ptx::tma_load_2d(&maps.qv, full_bar(st), sb + AW_K64 + AW_K16, 2 * E + h * AW_HD, row);
             } else {
                 const int row = segs->slot[si] * p.S_max + k0;
-                ptx::tma_load_2d(&maps.c64, full_bar(st), sb, h * AW_HD, row);
-                ptx::tma_load_2d(&maps.c16, full_bar(st), sb + AW_K64, h * AW_HD + 64, row);
+                const int krow = INJ && segs->bit[si] == 0 ? kslot * p.S_max + k0 : row;
+                ptx::tma_load_2d(&maps.c64, full_bar(st), sb, h * AW_HD, krow);
+                ptx::tma_load_2d(&maps.c16, full_bar(st), sb + AW_K64, h * AW_HD + 64, krow);
                 ptx::tma_load_2d(&maps.cv, full_bar(st), sb + AW_K64 + AW_K16, E + h * AW_HD, row);
             }
         } else if (c < n_sc) {
-            const int row = b * p.P + c * AW_BN;
-            ptx::tma_load_2d(&maps.q64, full_bar(st), sb, E + h * AW_HD, row);
-            ptx::tma_load_2d(&maps.q16, full_bar(st), sb + AW_K64, E + h * AW_HD + 64, row);
+            const int row = b * p.P + c * AW_BN, krow = INJ ? qb * p.P + c * AW_BN : row;
+            ptx::tma_load_2d(&maps.q64, full_bar(st), sb, E + h * AW_HD, krow);
+            ptx::tma_load_2d(&maps.q16, full_bar(st), sb + AW_K64, E + h * AW_HD + 64, krow);
             ptx::tma_load_2d(&maps.qv, full_bar(st), sb + AW_K64 + AW_K16, 2 * E + h * AW_HD, row);
         } else {
-            const int row = slot * p.S_max + (c - n_sc) * AW_BN;
-            ptx::tma_load_2d(&maps.c64, full_bar(st), sb, h * AW_HD, row);
-            ptx::tma_load_2d(&maps.c16, full_bar(st), sb + AW_K64, h * AW_HD + 64, row);
+            const int row = slot * p.S_max + (c - n_sc) * AW_BN, krow = INJ ? kslot * p.S_max + (c - n_sc) * AW_BN : row;
+            ptx::tma_load_2d(&maps.c64, full_bar(st), sb, h * AW_HD, krow);
+            ptx::tma_load_2d(&maps.c16, full_bar(st), sb + AW_K64, h * AW_HD + 64, krow);
             ptx::tma_load_2d(&maps.cv, full_bar(st), sb + AW_K64 + AW_K16, E + h * AW_HD, row);
         }
     };
@@ -115,8 +121,8 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
         ptx::mbar_init(full_bar(1), 1);
         ptx::fence_barrier_init();
         ptx::mbar_arrive_expect_tx(q_bar, AW_BM * 160);
-        ptx::tma_load_2d(&maps.q64, q_bar, base, h * AW_HD, b * p.P + q0);
-        ptx::tma_load_2d(&maps.q16, q_bar, base + AW_OFF_Q16, h * AW_HD + 64, b * p.P + q0);
+        ptx::tma_load_2d(&maps.q64, q_bar, base, h * AW_HD, qb * p.P + q0);
+        ptx::tma_load_2d(&maps.q16, q_bar, base + AW_OFF_Q16, h * AW_HD + 64, qb * p.P + q0);
         for (int c = 0; c < 2 && c < n_chunks; ++c) issue_chunk(c);
     }
     __syncthreads();
@@ -285,23 +291,40 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
 }
 
 __global__ void __launch_bounds__(128) attention_wgmma_kernel(const __grid_constant__ AttnMaps maps, const AttnParams p) {
-    attention_wgmma_body<false, false>(maps, p, AttnRegion{}, AttnMapOut{});
+    attention_wgmma_body<false, false, false>(maps, p, AttnRegion{}, AttnMapOut{}, AttnInject{});
 }
 __global__ void __launch_bounds__(128) attention_wgmma_kernel_regional(const __grid_constant__ AttnMaps maps, const AttnParams p,
                                                                        const AttnRegion rg) {
-    attention_wgmma_body<true, false>(maps, p, rg, AttnMapOut{});
+    attention_wgmma_body<true, false, false>(maps, p, rg, AttnMapOut{}, AttnInject{});
 }
 __global__ void __launch_bounds__(128) attention_wgmma_kernel_maps(const __grid_constant__ AttnMaps maps, const AttnParams p,
                                                                    const AttnMapOut mo) {
-    attention_wgmma_body<false, true>(maps, p, AttnRegion{}, mo);
+    attention_wgmma_body<false, true, false>(maps, p, AttnRegion{}, mo, AttnInject{});
 }
 __global__ void __launch_bounds__(128) attention_wgmma_kernel_regional_maps(const __grid_constant__ AttnMaps maps, const AttnParams p,
                                                                             const AttnRegion rg, const AttnMapOut mo) {
-    attention_wgmma_body<true, true>(maps, p, rg, mo);
+    attention_wgmma_body<true, true, false>(maps, p, rg, mo, AttnInject{});
+}
+__global__ void __launch_bounds__(128) attention_wgmma_kernel_inject(const __grid_constant__ AttnMaps maps, const AttnParams p,
+                                                                     const AttnInject inj) {
+    attention_wgmma_body<false, false, true>(maps, p, AttnRegion{}, AttnMapOut{}, inj);
+}
+__global__ void __launch_bounds__(128) attention_wgmma_kernel_regional_inject(const __grid_constant__ AttnMaps maps, const AttnParams p,
+                                                                              const AttnRegion rg, const AttnInject inj) {
+    attention_wgmma_body<true, false, true>(maps, p, rg, AttnMapOut{}, inj);
+}
+__global__ void __launch_bounds__(128) attention_wgmma_kernel_maps_inject(const __grid_constant__ AttnMaps maps, const AttnParams p,
+                                                                          const AttnMapOut mo, const AttnInject inj) {
+    attention_wgmma_body<false, true, true>(maps, p, AttnRegion{}, mo, inj);
+}
+__global__ void __launch_bounds__(128) attention_wgmma_kernel_regional_maps_inject(const __grid_constant__ AttnMaps maps,
+                                                                                   const AttnParams p, const AttnRegion rg,
+                                                                                   const AttnMapOut mo, const AttnInject inj) {
+    attention_wgmma_body<true, true, true>(maps, p, rg, mo, inj);
 }
 
 // returns 0 = launched, 1 = error, -1 = shape not handled here (head_dim != 80: the caller runs the mma.sync kernel)
-int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo) {
+int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo, const AttnInject* inj) {
     static const bool off = getenv("PB200_ATTN_MMA_SYNC") != nullptr;      // A/B knob: the mma.sync kernel for every shape
     if (off || p.E != AW_HD * p.nhead) return -1;
     const int64_t q_rows = (int64_t)p.B * p.P;
@@ -320,7 +343,18 @@ int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegio
     ProfScope prof("attention", 2.0 * ((double)p.B * p.P * 4.0 * p.E + (double)p.B * p.S_max * 2.0 * p.E), st);
     dim3 grid(ceil_div(p.P, AW_BM), p.nhead, p.B);
     PB_CHECK(grid.y <= 65535 && grid.z <= 65535, "attention: grid too large");
-    if (mo != nullptr && rg != nullptr) {
+#define PB_AW_LAUNCH(KERNEL, SMEM, ...)                                                                 \
+    {                                                                                                   \
+        static DeviceOnce attr_once;                                                                    \
+        if (attr_once.first()) PB_CUDA(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM)); \
+        KERNEL<<<grid, 128, SMEM, st>>>(m, p, __VA_ARGS__);                                             \
+    }
+    if (inj != nullptr) {
+        if (mo != nullptr && rg != nullptr) PB_AW_LAUNCH(attention_wgmma_kernel_regional_maps_inject, AW_SMEM_REG, *rg, *mo, *inj)
+        else if (mo != nullptr) PB_AW_LAUNCH(attention_wgmma_kernel_maps_inject, AW_SMEM, *mo, *inj)
+        else if (rg != nullptr) PB_AW_LAUNCH(attention_wgmma_kernel_regional_inject, AW_SMEM_REG, *rg, *inj)
+        else PB_AW_LAUNCH(attention_wgmma_kernel_inject, AW_SMEM, *inj)
+    } else if (mo != nullptr && rg != nullptr) {
         static DeviceOnce attr_reg_maps;
         if (attr_reg_maps.first())
             PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel_regional_maps, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM_REG));
@@ -341,6 +375,7 @@ int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegio
             PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AW_SMEM));
         attention_wgmma_kernel<<<grid, 128, AW_SMEM, st>>>(m, p);
     }
+#undef PB_AW_LAUNCH
     PB_LAUNCH_CHECK();
     return 0;
 }

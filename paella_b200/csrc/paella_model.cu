@@ -693,7 +693,22 @@ int pb200_paella_features_maps(pb200_paella* m, const int64_t* tokens, const flo
                                const int* mask_row, const int* region_slot, int max_regions, const int* tail_src, const int* map_row,
                                int map_batch, float* map_acc, int map_rows, int map_len, float* features, void* workspace,
                                int64_t workspace_bytes, void* stream) {
+    return pb200_paella_features_inject(m, tokens, r, batch_total, n_tail, h, w, cond_cache, cache_slots, kv_slot, s_max, attn_w, n_w,
+                                        w_ld, w_len, w_row, w_batch, wrap, prompt_mask, mask_row, region_slot, max_regions, tail_src,
+                                        map_row, map_batch, map_acc, map_rows, map_len, nullptr, 0, features, workspace,
+                                        workspace_bytes, stream);
+}
+
+int pb200_paella_features_inject(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                                 const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                                 int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
+                                 const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
+                                 const int* tail_src, const int* map_row, int map_batch, float* map_acc, int map_rows, int map_len,
+                                 const int* inj_src, int inj_batch, float* features, void* workspace, int64_t workspace_bytes,
+                                 void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
+    PB_CHECK(inj_batch == 0 || (inj_src != nullptr && inj_batch > 0 && inj_batch <= batch_total - n_tail),
+             "features: injection table of %d samples for %d base samples", inj_batch, batch_total - n_tail);
     PB_CHECK(map_batch == 0 || (map_acc != nullptr && map_rows > 0 && map_len > 0 && map_batch <= batch_total - n_tail),
              "features: attention maps of %d samples need an accumulator of rows x keys (%d x %d) and at most the %d base samples",
              map_batch, map_rows, map_len, batch_total - n_tail);
@@ -887,7 +902,8 @@ int pb200_paella_features_maps(pb200_paella* m, const int64_t* tokens, const flo
                 ap.attn_w = attn_w; ap.n_w = n_w; ap.w_batch = w_batch;
                 ap.w_ld = w_ld; ap.w_len = w_len; ap.w_row = w_row;
                 const AttnRegion rg{ws.qmask + qmask_off[l], region_slot, mask_row, max_regions, n_base};
-                PB_TRY(launch_attention(ap, st, prompt_mask ? &rg : nullptr, map_batch > 0 ? &mo : nullptr));
+                const AttnInject inj{inj_src, inj_batch};
+                PB_TRY(launch_attention(ap, st, prompt_mask ? &rg : nullptr, map_batch > 0 ? &mo : nullptr, inj_batch > 0 ? &inj : nullptr));
                 if (map_batch > 0) PB_TRY(launch_attention_maps_accumulate(ap, mo, map_acc, map_len, map_pos, map_off[l], st));
                 pb200_gemm_epilogue e2 = epi(PB200_EPI_RESID_F32, m->w<float>(b.outproj_b), x, ch);
                 e2.resid = x; e2.ldr = ch; e2.rows_per_sample = P;

@@ -38,7 +38,10 @@ pools by token slot; regional prompts draw nothing.  With ``guidance_prompts=[(i
 guidance_prompts=[terms])`` does: their K/V are projected at admission into slots reserved for its token slot, and each of its
 guided steps runs one more denoiser row per term; terms draw nothing.  With ``attention_maps=True`` a request's
 ``req.attention_maps`` (float32 [S, H, W], S its conditioning length) is set when it retires, equal bit for bit to the maps of
-``sample_notebook(..., attention_maps=True)`` on the same request; its tokens are unchanged, and maps draw nothing.
+``sample_notebook(..., attention_maps=True)`` on the same request; its tokens are unchanged, and maps draw nothing.  With
+``attention_source=(src, k)`` a request is a prompt-to-prompt edit of the queued request ``src``: the edit and its source are
+admitted together and advance in lockstep, and on its steps i < k the edit's conditional forward replays the source's attention
+probabilities, as ``sample_notebook(..., attention_source=[None, (0, k)])`` does on the pair; injection draws nothing.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -59,7 +62,9 @@ tail map, mix rows and coefficients ride in the step's table.  A step with no su
 step in which some row wants attention maps adds each row's map row (its token slot, -1 for the rows that do not) to the table and
 runs the maps denoiser (pb200_paella_features_maps), which accumulates into a pool of per-slot accumulators, allocated when the
 first such request is admitted and zeroed per request at admission; a request's maps are finalized with its own step count when it
-retires.  A step with no such row launches exactly as without maps.
+retires.  A step with no such row launches exactly as without maps.  A step in which some edit is inside its window adds each
+row's source row in this step's order (-1 for the other rows) to the table and runs the injecting denoiser
+(pb200_paella_features_inject); a step with no such row launches exactly as without edits.
 The host knows which
 requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
 in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
@@ -88,7 +93,7 @@ class Request:
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
                  region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
                  top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None, terms=None, mix_coef=None,
-                 attention_maps: bool = False, maps_len: int = 0):
+                 attention_maps: bool = False, maps_len: int = 0, attention_source=None):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -106,6 +111,9 @@ class Request:
         self.term_slot: List[int] = []           # the K/V slots of the terms
         self.want_maps, self.maps_len = attention_maps, maps_len      # attention maps, over maps_len conditioning keys
         self.attention_maps: Optional[torch.Tensor] = None            # float32 [maps_len, H, W], set at retirement
+        # prompt-to-prompt: the source request and the steps it is replayed on, or None; a source lists its edits
+        self.inj_src, self.inj_k = attention_source if attention_source is not None else (None, 0)
+        self.edits: List["Request"] = []
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -161,6 +169,11 @@ class StepPlan:
         # attention maps: each row's accumulator row (its token slot), -1 for the rows without maps
         self.maps = any(q.want_maps for q in order)
         self.map_row = torch.tensor([q.slot if q.want_maps else -1 for q in order], dtype=torch.int32)
+        # prompt-to-prompt: each edit inside its window reads its source's row of this step's order, -1 for the other rows
+        row = {id(q): i for i, q in enumerate(order)}
+        self.inj_src = torch.tensor([row[id(q.inj_src)] if q.inj_src is not None and q.k < q.inj_k else -1 for q in order],
+                                    dtype=torch.int32)
+        self.injects = bool((self.inj_src >= 0).any())
 
 
 def cond_layout(inputs: Dict[str, torch.Tensor]) -> Tuple[int, bool, int]:
@@ -187,10 +200,10 @@ def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List
 def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tuple[torch.Tensor, Dict[str, Tuple[str, int, int]]]:
     """The step's one host-to-device buffer: int64 [(seed, offset) pairs of the sampler's draw, then of the mask draw], then the
     float32 part [r, params (3 per row), t_next, (top_p), (mix_coef)], then the int32 part [row_slot, kv_slot, (mode table), (top_k),
-    (tail, mix_rows), (map_row)], then the uint8 part [(wrap)], each part padded to whole int64 words.  top_p / top_k are present
-    only when ``plan.truncates``, the mode table only when the step mixes modes, wrap (one byte per row) only when ``plan.wraps``,
-    the tail map and the mix table only when some row of the step is composed (guidance prompts), map_row only when some row wants
-    attention maps.  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
+    (tail, mix_rows), (map_row), (inj_src)], then the uint8 part [(wrap)], each part padded to whole int64 words.  top_p / top_k
+    are present only when ``plan.truncates``, the mode table only when the step mixes modes, wrap (one byte per row) only when
+    ``plan.wraps``, the tail map and the mix table only when some row of the step is composed (guidance prompts), map_row only
+    when some row wants attention maps, inj_src only when some edit is inside its window.  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
     Bc, n_pairs = len(plan.order), plan.n_pairs
     mixed = not all(plan.draws)
     modes = ops.mode_table(plan.modes) if mixed else torch.zeros(0, dtype=torch.int32)
@@ -204,6 +217,8 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
         i32_parts += [("tail", plan.tail), ("mix_rows", plan.mix_rows.view(-1))]
     if plan.maps:
         i32_parts.append(("map_row", plan.map_row))
+    if plan.injects:
+        i32_parts.append(("inj_src", plan.inj_src))
     u8_parts = [("wrap", plan.wrap)] if plan.wraps else []
     layout: Dict[str, Tuple[str, int, int]] = {}
     for dt, parts in (("f32", f32_parts), ("i32", i32_parts), ("u8", u8_parts)):
@@ -239,6 +254,19 @@ def _cat_inputs(inputs: List[Dict[str, torch.Tensor]], dev) -> Dict[str, torch.T
         per = [list(ci) if isinstance(ci, (list, tuple)) else [ci] for ci in (x["clip_image"] for x in inputs)]
         out["clip_image"] = [cat([p[j] for p in per]) for j in range(len(per[0]))]
     return out
+
+
+def admit_from_queue(queue: "collections.deque[Request]", n_free: int) -> List[Request]:
+    """Take the requests one admission starts from ``queue``, FIFO, into at most ``n_free`` slots.  A source comes in with
+    every edit queued for it (its edits are queued after it), or it and everything behind it waits until enough slots are
+    free."""
+    new: List[Request] = []
+    while queue and n_free - len(new) >= 1 + len(queue[0].edits):
+        group = [queue[0]] + queue[0].edits
+        for q in group:
+            queue.remove(q)
+        new += group
+    return new
 
 
 def build_step_plan(active: List[Request]) -> StepPlan:
@@ -336,7 +364,7 @@ class SamplingEngine:
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
                sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
-               attention_maps=False) -> Request:
+               attention_maps=False, attention_source=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -357,7 +385,11 @@ class SamplingEngine:
         conditioning dict of at most max_cond_len rows and a finite real weight) mixes further prompts into a guided request's
         guidance as in sample_notebook; ValueError for any other value, and on a request without cfg.  ``attention_maps=True`` sets
         ``req.attention_maps`` at retirement (module docstring); ValueError for a flag that is not a bool and with
-        ``prompt_regions``.  The request's draws start when it is admitted."""
+        ``prompt_regions``.  ``attention_source=(src, k)`` makes the request a prompt-to-prompt edit of ``src`` (module
+        docstring): ``src`` must be a request of this engine that is still queued and not itself an edit, neither may have
+        ``prompt_regions``, both need the same conditioning length, ``steps``, ``renoise_steps`` and ``sampling_conditional_steps``,
+        k is an int in 0 .. steps, and the source with all its edits must fit in max_batch; ValueError otherwise.  Give the edit a
+        generator seeded like its source's.  The request's draws start when it is admitted."""
         attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
@@ -415,6 +447,8 @@ class SamplingEngine:
         if attn_weights is not None:
             n_keys = self.model.max_attn_weights((self.H, self.W), self.model.conditioning_seq_len(model_inputs))
             attn_weights = ops.check_attn_weight_vector("attn_weights", attn_weights, min(n_keys, self.w_max))
+        if attention_source is not None:
+            self._check_attention_source(attention_source, model_inputs, steps, renoise_steps, cond_steps, prompt_regions)
         cfgs = U._cfg_schedule(cfg, 1, steps)
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         mix_coef = None
@@ -428,18 +462,40 @@ class SamplingEngine:
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
                       sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap, regions,
-                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs))
+                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs), attention_source)
+        if attention_source is not None:
+            attention_source[0].edits.append(req)
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
 
+    def _check_attention_source(self, attention_source, model_inputs, steps, renoise_steps, cond_steps, prompt_regions):
+        """submit's rules for ``attention_source`` (ValueError)."""
+        if not isinstance(attention_source, (list, tuple)) or len(attention_source) != 2 or not isinstance(attention_source[0], Request) \
+                or isinstance(attention_source[1], bool) or not isinstance(attention_source[1], int):
+            raise ValueError(f"attention_source: expected a (Request, int steps) pair (got {attention_source!r})")
+        src, k = attention_source
+        if not any(q is src for q in self._queue):
+            raise ValueError("attention_source: the source must be a request of this engine that is still queued")
+        if src.inj_src is not None:
+            raise ValueError("attention_source: the source is itself an edit (no chains)")
+        if src.regional or prompt_regions:
+            raise ValueError("attention_source: prompt_regions on an edit or on its source are not supported")
+        if src.maps_len != self.model.conditioning_seq_len(model_inputs):
+            raise ValueError(f"attention_source: the source's conditioning has {src.maps_len} rows, the edit's "
+                             f"{self.model.conditioning_seq_len(model_inputs)}")
+        if (src.steps, src.renoise_steps, src.cond_steps) != (steps, renoise_steps, cond_steps):
+            raise ValueError("attention_source: the edit needs its source's steps, renoise_steps and sampling_conditional_steps")
+        if not 0 <= k <= steps:
+            raise ValueError(f"attention_source: {k} injected steps; expected 0..{steps}")
+        if len(src.edits) + 2 > self.max_batch:
+            raise ValueError(f"attention_source: a source and its {len(src.edits) + 1} edits exceed max_batch={self.max_batch}")
+
     def _admit(self):
-        new = []
-        while self._queue and self._free:
-            q = self._queue.popleft()
+        new = admit_from_queue(self._queue, len(self._free))
+        for q in new:
             q.slot = self._free.pop(0)
             q.uncond_slot = self.max_batch + q.slot if q.uncond is not None else self.shared_slot
-            new.append(q)
         if not new:
             return
         m = self.model
@@ -551,6 +607,8 @@ class SamplingEngine:
             tail = dict(tail_src=part("tail")) if plan.composed else dict(n_pairs=n_pairs)
             if plan.maps:       # row b accumulates into its token slot's maps
                 tail["maps"] = (part("map_row"), Bc, self.map_acc)
+            if plan.injects:    # row b replays the attention of row inj_src[b]
+                tail["inject"] = part("inj_src")
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_tail, self.s_max, self.n_slots, kv_slot_d)

@@ -651,7 +651,7 @@ class Paella(nn.Module):
                  attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None,
                  w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None,
                  wrap: Optional[torch.Tensor] = None, regional=None, tail_src: Optional[torch.Tensor] = None,
-                 maps=None) -> torch.Tensor:
+                 maps=None, inject: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
@@ -677,7 +677,11 @@ class Paella(nn.Module):
         ``maps``: attention maps, (map_row, map_batch, acc): sample b < map_batch of x adds its AttnBlocks' cross-attention maps to
         accumulator row map_row[b] (a device int32 [map_batch], -1: none; None: row b) of ``acc`` (map_accumulator), so that
         finalize_attention_maps turns it into the map of the forwards summed there (pb200_paella_features_maps).  The features are
-        those of the call without it, bit for bit.  None launches exactly the kernels without it."""
+        those of the call without it, bit for bit.  None launches exactly the kernels without it.
+        ``inject``: prompt-to-prompt injection, a device int32 [n] (n <= B): sample b < n of x with a = inject[b] >= 0 (-1: none)
+        attends in every AttnBlock with sample a's attention probabilities and its own values and attn_weights
+        (pb200_paella_features_inject).  Sample a and sample b must have the same conditioning length and no regions.  Every
+        other row is that of the call without it, bit for bit.  None launches exactly the kernels without it."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -694,6 +698,9 @@ class Paella(nn.Module):
             n_pairs = Bt if cfg_pairs else 0
         if wrap is not None and (wrap.dtype != torch.uint8 or wrap.numel() != Bt or wrap.device != dev):
             raise PaellaB200Error(f"features: wrap must be a uint8 table of {Bt} entries on {dev}")
+        if inject is not None and (inject.dtype != torch.int32 or inject.dim() != 1 or not 0 < inject.numel() <= Bt
+                                   or inject.device != dev or not inject.is_contiguous()):
+            raise PaellaB200Error(f"features: inject must be a contiguous int32 vector of at most {Bt} entries on {dev}")
         Bt += n_pairs
         if Bt != cond.batch_total:
             raise PaellaB200Error(f"batch {Bt} does not match the conditioning cache ({cond.batch_total})")
@@ -717,10 +724,10 @@ class Paella(nn.Module):
                         or w_len.numel() != attn_weights.shape[0] or (w_row is not None and w_row.numel() < attn_weights_batch):
                     raise PaellaB200Error("features: a per-sample weight table is float32 [rows, w_ld] with int32 w_len [rows] "
                                           "and an optional int32 w_row [attn_weights_batch]")
-                if regional is not None or tail_src is not None or maps is not None:
+                if regional is not None or tail_src is not None or maps is not None or inject is not None:
                     self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(attn_weights), 0, attn_weights.shape[1], ptr(w_len),
                                                                             ptr(w_row)), attn_weights_batch, wrap, regional, feats, ws,
-                                            tail_src, maps)
+                                            tail_src, maps, inject)
                     return feats
                 if wrap is not None:
                     check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -734,9 +741,9 @@ class Paella(nn.Module):
                                                        current_stream()), "pb200_paella_features_weighted")
                 return feats
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
-            if regional is not None or tail_src is not None or maps is not None:
+            if regional is not None or tail_src is not None or maps is not None or inject is not None:
                 self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(aw), aw.numel() if aw is not None else 0, 0, None, None),
-                                        attn_weights_batch, wrap, regional, feats, ws, tail_src, maps)
+                                        attn_weights_batch, wrap, regional, feats, ws, tail_src, maps, inject)
                 return feats
             if wrap is not None:        # the single weight vector is the weighted call with w_ld = 0 and no w_len
                 check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -750,9 +757,10 @@ class Paella(nn.Module):
                                                 ws.numel(), current_stream()), "pb200_paella_features_pairs")
         return feats
 
-    def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws, tail_src=None, maps=None):
+    def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws, tail_src=None, maps=None,
+                           inject=None):
         """pb200_paella_features_regional, or with ``tail_src`` pb200_paella_features_tail, or with ``maps``
-        pb200_paella_features_maps (``regional`` may then be None)."""
+        pb200_paella_features_maps, or with ``inject`` pb200_paella_features_inject (``regional`` may then be None)."""
         mask = region_slot = mask_row = None
         if regional is not None:
             mask, region_slot, mask_row = regional
@@ -765,6 +773,15 @@ class Paella(nn.Module):
         if w_batch > Bt - n_pairs:
             raise PaellaB200Error(f"features: {w_batch} weighted samples of {Bt - n_pairs}")
         n_regions = region_slot.shape[1] if region_slot is not None else 0
+        if inject is not None:
+            map_row, map_batch, acc = maps if maps is not None else (None, 0, None)
+            check(lib().pb200_paella_features_inject(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                     ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
+                                                     ptr(mask_row), ptr(region_slot), n_regions, ptr(tail_src), ptr(map_row), map_batch,
+                                                     ptr(acc), acc.shape[0] if acc is not None else 0,
+                                                     acc.shape[1] if acc is not None else 0, ptr(inject), inject.numel(), ptr(feats),
+                                                     ptr(ws), ws.numel(), current_stream()), "pb200_paella_features_inject")
+            return
         if maps is not None:
             map_row, map_batch, acc = maps
             check(lib().pb200_paella_features_maps(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -1075,19 +1092,27 @@ class Paella(nn.Module):
         of the sample's conditioning sequence (gen_c_embeddings order) and token (y, x), the mean over every AttnBlock and its
         heads of the post-softmax, post-attn_weights probability the block position holding the token gives the key -- what the
         reference's CustomMultiheadAttention returns with need_weights=True.  The logits are those of the call without it, bit
-        for bit.  ValueError, before anything is enqueued, for a flag that is not a bool and for maps with prompt_regions."""
+        for bit.  ValueError, before anything is enqueued, for a flag that is not a bool and for maps with prompt_regions.
+        ``attention_source``: prompt-to-prompt injection (keyword only): None, or a list or tuple of B entries, each None or the
+        int index a of another sample of the call.  Sample b then attends, in every AttnBlock and head, with sample a's attention
+        probabilities over [self ; conditioning] keys (from a's queries and keys), times its own attn_weights, applied to its own
+        values.  Every other sample's logits are those of the call without it, bit for bit.  ValueError, before anything is
+        enqueued, for a bad entry, a source that is itself injected, and prompt_regions on an injected sample or its source
+        (ops.attention_source_table)."""
         if x_cat is not None:
             x = torch.cat([x, x_cat], dim=1)
         attn_weights = kwargs.pop("attn_weights", None)
         tiling = kwargs.pop("tiling", None)
         prompt_regions = kwargs.pop("prompt_regions", None)
         attention_maps = ops.check_attention_maps(kwargs.pop("attention_maps", False), prompt_regions)
+        attention_source = kwargs.pop("attention_source", None)
         if kwargs:
             raise TypeError(f"unexpected keyword arguments {sorted(kwargs)}")
         B, H, W = x.shape
         wrap = ops.tiling_table(tiling, B)
         regions = ops.regional_table(prompt_regions, B, (H, W), self._device())
         ops.check_regions_unweighted(regions, attn_weights)
+        inject = ops.attention_source_table(attention_source, B, 1, regions, forward=True)
         cond_len = self.conditioning_seq_len({"byt5": byt5, "clip": clip, "clip_image": clip_image})
         aw, w_len = self._attn_weights_table(attn_weights, B, (H, W), cond_len)
         regional = None
@@ -1099,9 +1124,11 @@ class Paella(nn.Module):
             regional = self.regional_device(regions, cond)
         if wrap is not None:
             wrap = ops.to_device_async(wrap, self._device())
+        if inject is not None:
+            inject = ops.to_device_async(inject[0], self._device())
         acc = self.map_accumulator(B, cond_len, (H, W)) if attention_maps else None
         feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len, wrap=wrap, regional=regional,
-                              maps=(None, B, acc) if attention_maps else None)
+                              maps=(None, B, acc) if attention_maps else None, inject=inject)
         logits = self.logits_from_features(feats, B, H, W)
         if attention_maps:
             return logits, self.finalize_attention_maps(acc, (H, W), cond_len, 1)

@@ -385,6 +385,62 @@ def check_attention_maps(attention_maps, prompt_regions=None) -> bool:
     return attention_maps
 
 
+# ------------------------------------------------------------------ prompt-to-prompt editing
+# Sample b with attention_source[b] = (a, k) replays sample a's attention probabilities in its conditional forward on steps i < k,
+# in every AttnBlock and head, with its own values and attn_weights (pb200_paella_features_inject).  The table holds, per step, the
+# source of each sample or -1.
+def _is_int(v) -> bool:
+    return isinstance(v, int) and not isinstance(v, bool)
+
+
+def attention_source_table(attention_source, batch: int, steps: int, regions=None, exact: bool = False,
+                           forward: bool = False) -> Optional[torch.Tensor]:
+    """``attention_source`` (None, or a list or tuple of ``batch`` entries, each None or an (a, k) pair of ints; with ``forward``
+    each None or an int a, injected in that single forward) -> None when no sample is injected on any step, otherwise int32 CPU
+    [steps, batch]: entry [i, b] is a when i < k, else -1.  ``regions``: regional_table's result, whose samples with regions may be
+    neither sources nor edits.  ValueError, before anything is enqueued, for the wrong length, a bad entry (a bool is not an int),
+    a source out of range or equal to its sample, a source that is itself injected, k outside [0, steps], regions on an edit or
+    its source, and ``exact=True``."""
+    if attention_source is None:
+        return None
+    if not isinstance(attention_source, (list, tuple)):
+        raise ValueError(f"attention_source: expected None or a list of {batch} entries (got {type(attention_source).__name__})")
+    if len(attention_source) != batch:
+        raise ValueError(f"attention_source: got {len(attention_source)} entries for a batch of {batch} (one per sample, None for none)")
+    pairs = []
+    for b, entry in enumerate(attention_source):
+        if entry is None:
+            pairs.append(None)
+            continue
+        if forward:
+            if not _is_int(entry):
+                raise ValueError(f"attention_source[{b}]: expected None or the int index of a source sample (got {entry!r})")
+            a, k = entry, steps
+        else:
+            if not isinstance(entry, (list, tuple)) or len(entry) != 2 or not _is_int(entry[0]) or not _is_int(entry[1]):
+                raise ValueError(f"attention_source[{b}]: expected None or an (int source, int steps) pair (got {entry!r})")
+            a, k = entry
+        if not 0 <= a < batch or a == b:
+            raise ValueError(f"attention_source[{b}]: source {a} is not another sample of the call (0..{batch - 1})")
+        if not 0 <= k <= steps:
+            raise ValueError(f"attention_source[{b}]: {k} injected steps; expected 0..{steps}")
+        pairs.append((a, k))
+    for b, p in enumerate(pairs):
+        if p is not None and pairs[p[0]] is not None:
+            raise ValueError(f"attention_source[{b}]: source {p[0]} is itself injected (no chains)")
+        if p is not None and regions is not None and (regions[1][b] or regions[1][p[0]]):
+            raise ValueError(f"attention_source[{b}]: prompt_regions on an injected sample or on its source are not supported")
+    if all(p is None for p in pairs):
+        return None
+    if exact:
+        raise ValueError("exact=True restates the reference op for op, which has no attention injection")
+    table = torch.full((steps, batch), -1, dtype=torch.int32)
+    for b, p in enumerate(pairs):
+        if p is not None:
+            table[:p[1], b] = p[0]
+    return table
+
+
 # ------------------------------------------------------------------ guidance prompts
 # Each sample of a guided call may carry up to MAX_GUIDANCE_PROMPTS (inputs, weight) terms.  On a guided step with scale cfg its
 # logits are l_u + cfg * [(l_c - l_u) + sum_j w_j (l_j - l_u)], l_j being the conditional forward under term j's inputs.  The

@@ -75,6 +75,21 @@ need_weights=True (pb200_paella_features_maps).  Only the sample's own condition
 Maps draw no random numbers and change no token: tokens, intermediates and generator offsets are those of the call without them,
 and a sample's maps depend only on its own request where the forward is batch-invariant.  ValueError, before anything is enqueued
 and before any generator advances, for a flag that is not a bool and for maps together with ``prompt_regions``.
+
+Prompt-to-prompt editing: ``attention_source`` (all three functions; None, or a list or tuple of B entries, each None or an (a, k)
+pair of ints) makes sample i an edit of sample a of the same call: on steps s < k, sample i's conditional forward (guided or not)
+attends in every AttnBlock and head with sample a's attention probabilities, the joint softmax over self and conditioning keys of
+a's own queries and keys in that forward, times sample i's own ``attn_weights``, applied to sample i's own values.  Run an edit from
+its source's noise, by giving it its own generator seeded like the source's (``generator=[g_0, ..., g_{B-1}]``); the call does not
+check it.  With the same prompt and seed an edit returns its source's tokens for any k; with another prompt it keeps the
+source's layout for the first k steps (Hertz et al. 2022, "Prompt-to-Prompt Image Editing with Cross Attention Control"), and an
+edit with the source's prompt and its own ``attn_weights`` is their attention re-weighting.  Unconditional rows, guidance-prompt
+term rows, the source's own row and every step s >= k are never injected.  Injection draws no random numbers, so every generator
+ends at the same offset, and rows that are not edits, the sources among them, are those of the call without it, bit for bit.  A
+source and its edits must sit in the same shard; indices are relative to the call.  ValueError, before anything is enqueued and
+before any generator advances, for the wrong length, a bad entry (a bool is not an int), a source out of range or equal to its
+sample, a source that is itself injected, k outside [0, steps], ``prompt_regions`` on an edit or its source, and ``exact=True``
+(ops.attention_source_table; pb200_paella_features_inject).
 """
 from __future__ import annotations
 
@@ -182,12 +197,13 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
                  codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None,
-                 prompt_regions=None, guidance_prompts=None, attention_maps=False):
+                 prompt_regions=None, guidance_prompts=None, attention_maps=False, attention_source=None):
     """Returns (tokens, intermediates, maps or None).  ``modes``: None, or per step the list of B mode names (sampling_modes) --
     a step whose modes differ samples each row in its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the
     scalar path in that mode.  ``top_k`` / ``top_p``: the truncation of the multinomial draws (module docstring); a truncating
     call takes the per-sample table path, and so does a call with ``guidance_prompts`` (module docstring).  ``attention_maps``:
-    the maps of the conditional rows (module docstring)."""
+    the maps of the conditional rows (module docstring).  ``attention_source``: prompt-to-prompt injection (module docstring);
+    step i passes row i of the table to the denoiser, or nothing when no sample is injected there."""
     B, H, W = latent_shape
     dev = model._device()
     attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
@@ -197,6 +213,8 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     regions = ops.regional_table(prompt_regions, B, (H, W), dev)
     ops.check_regions_unweighted(regions, attn_weights)
     terms = ops.guidance_table(guidance_prompts, B)
+    inj = ops.attention_source_table(attention_source, B, steps, regions, exact)
+    inj_steps = [bool((row >= 0).any()) for row in inj] if inj is not None else [False] * steps
     extra = [g for own in regions[1] for g in own] if regions is not None else []
     if exact and trunc is not None:
         raise ValueError("exact=True restates the reference op for op, which has no top_k / top_p truncation")
@@ -238,7 +256,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         parts = (list(sched) if sched is not None else []) + (list(trunc) if trunc is not None else []) + ([region] if region_host else [])
         parts += [wrap] if wrap is not None else []
         parts += [torch.tensor(mix[0], dtype=torch.int32), mix[2], mix[3]] if mix is not None else []
+        parts += [inj] if any(inj_steps) else []
         parts_d = ops.to_device_packed(parts, dev) if parts else []
+        inj_d = parts_d.pop() if any(inj_steps) else None
         if mix is not None:
             mix_coef_d, mix_rows_d, tail_d = parts_d.pop(), parts_d.pop(), parts_d.pop()
         wrap_d = parts_d.pop() if wrap is not None else None
@@ -296,7 +316,8 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             composed = guided and mix is not None
             feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided and not composed,
                                    w_len=w_len, wrap=wrap_d, regional=regional_only if cond is cond_only else regional_full,
-                                   tail_src=tail_d if composed else None, maps=(None, B, acc) if attention_maps else None)
+                                   tail_src=tail_d if composed else None, maps=(None, B, acc) if attention_maps else None,
+                                   inject=inj_d[i] if inj_steps[i] else None)
             if composed:
                 model.guidance_mix(feats, H * W, mix_rows_d, mix_coef_d[i])
             if step_modes is not None:
@@ -417,7 +438,8 @@ def _decode_tail(tokens, decode, decode_output, tiling=None):
 
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
            cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
-           top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None, attention_maps=False):
+           top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None, attention_maps=False,
+           attention_source=None):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -434,7 +456,8 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     tiling.  ValueError, before anything is enqueued and before any generator advances, for an unknown value, a list of the
     wrong length or a tensor.  ``prompt_regions`` (module docstring): regional prompts per sample.  ``guidance_prompts`` (module
     docstring): weighted extra and negative prompts per sample in the guided mix; a sample with terms needs a cfg other than 0.
-    ``attention_maps=True`` (module docstring): returns (tokens or images, maps)."""
+    ``attention_maps=True`` (module docstring): returns (tokens or images, maps).  ``attention_source`` (module docstring):
+    prompt-to-prompt edits of other samples of the call; give each edit its own generator seeded like its source's."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     per_sample_cfg = torch.is_tensor(cfg)
     terms = ops.guidance_table(guidance_prompts, latent_shape[0])
@@ -453,7 +476,8 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     out, _, maps = _sample_core(model, model_inputs, tuple(latent_shape), unconditional_inputs, None, steps, renoise_steps,
                                 temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
                                 per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling,
-                                prompt_regions=prompt_regions, guidance_prompts=guidance_prompts, attention_maps=attention_maps)
+                                prompt_regions=prompt_regions, guidance_prompts=guidance_prompts, attention_maps=attention_maps,
+                                attention_source=attention_source)
     out = _decode_tail(out, decode, decode_output, tiling)
     return (out, maps) if attention_maps else out
 
@@ -461,7 +485,7 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
                        exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None,
-                       guidance_prompts=None, attention_maps=False):
+                       guidance_prompts=None, attention_maps=False, attention_source=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
@@ -471,7 +495,8 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     ``top_k[lo:hi]`` computes what rows [lo, hi) compute.  ``tiling`` as in ``sample``; a shard given ``tiling[lo:hi]`` computes
     what rows [lo, hi) compute.  ``prompt_regions`` (module docstring) likewise: a shard given ``prompt_regions[lo:hi]`` computes
     what rows [lo, hi) compute.  ``guidance_prompts`` (module docstring) likewise: a shard given ``guidance_prompts[lo:hi]``
-    computes what rows [lo, hi) compute.  ``attention_maps=True`` (module docstring): returns (tokens, maps) for the shard's rows."""
+    computes what rows [lo, hi) compute.  ``attention_maps=True`` (module docstring): returns (tokens, maps) for the shard's rows.
+    ``attention_source`` (module docstring): a source and its edits sit in the same shard, with indices relative to the shard."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -482,7 +507,7 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
                                 temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
                                 generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
                                 tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts,
-                                attention_maps=attention_maps)
+                                attention_maps=attention_maps, attention_source=attention_source)
     return (out, maps) if attention_maps else out
 
 
@@ -490,7 +515,7 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
                     generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
-                    attention_maps=False):
+                    attention_maps=False, attention_source=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -507,7 +532,8 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     intermediates are those of the tiled call.  ``prompt_regions`` as in ``sample``; regional samples' rows may not also
     have ``attn_weights``.  ``guidance_prompts`` as in ``sample``: the argmax and quant steps of a sample with terms see its mixed
     features, and ``attn_weights`` weight its conditional row only.  ``attention_maps=True`` (module docstring): returns
-    (sampled, intermediate_images, maps)."""
+    (sampled, intermediate_images, maps).  ``attention_source`` (module docstring): prompt-to-prompt edits; an edit's
+    ``attn_weights`` reweight the replayed probabilities."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -527,5 +553,6 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                                                 attn_weights, exact, True, sampling_quant_steps, codebook, generator,
                                                 per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes, top_k=top_k,
                                                 top_p=top_p, tiling=tiling, prompt_regions=prompt_regions,
-                                                guidance_prompts=guidance_prompts, attention_maps=attention_maps)
+                                                guidance_prompts=guidance_prompts, attention_maps=attention_maps,
+                                                attention_source=attention_source)
     return (sampled, intermediates, maps) if attention_maps else (sampled, intermediates)
