@@ -555,6 +555,25 @@ int pb200_paella_resample_samples(pb200_paella* m, const float* features, int ba
                                   int n_guided, const float* params, int mode, const float* codebook, int c_latent, int chunk,
                                   int64_t* tokens_out, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* Token scoring: per-token log-likelihood statistics of given codes under the denoiser, from one fused out_mapper +
+ * log-softmax kernel; the logits never reach HBM.  Replaces ref/utils/modules.py:268-280 (the out_mapper of Paella.forward)
+ * followed by src/train.py:36,64,71 (nn.CrossEntropyLoss(label_smoothing, reduction='none')(pred, latents) and
+ * pred.argmax(1) == latents).
+ *   features  fp32 [(batch + n_pairs)*hw, c_out] in pb200_paella_features_pairs layout: the first n_pairs samples are mixed
+ *             with their unconditional rows at (batch + s)*hw using params' (cfg, 1 - cfg) (the A operand
+ *             pb200_paella_sample_tokens_pairs draws from at T = 1), the others are taken as they are;
+ *   params    fp32 [batch][3] of per-sample (cfg, 1 - cfg, 1/T), only the first two columns read; NULL when n_pairs = 0;
+ *   targets   int64 [batch*hw] codes.
+ * Per row, with l the logits and y the target: nll_out = logsumexp(l) - l_y, smooth_out = logsumexp(l) - mean_j l_j (fp32
+ * [batch*hw] each; the label-smoothed loss is (1 - eps) nll + eps smooth) and argmax_out = the lowest j with l_j = max l
+ * (int64 [batch*hw]).  A target outside [0, num_labels) gives a NaN nll in its row and nothing else: it is never used as an
+ * index.  Each row's results depend only on its own features.  workspace: pb200_paella_token_scores_workspace_bytes(batch, hw)
+ * bytes (the fp16 A operand). */
+int64_t pb200_paella_token_scores_workspace_bytes(const pb200_paella* m, int batch, int hw);
+int pb200_paella_token_scores(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                              const int64_t* targets, float* nll_out, float* smooth_out, int64_t* argmax_out, void* workspace,
+                              int64_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * VQGAN (ref/src/vqgan.py:45-107).
  * ------------------------------------------------------------------------------------------ */

@@ -16,6 +16,7 @@
 #include "gemm.cuh"
 #include "ops.cuh"
 #include "sampler.cuh"
+#include "score.cuh"
 
 namespace pb {
 
@@ -1091,6 +1092,32 @@ int pb200_paella_sample_tokens_pairs_trunc(pb200_paella* m, const float* feature
     PB_TRY(launch_cast_f16(features + mixed, rows * c.c_out - mixed, a16 + mixed, st));
     return launch_fused_sampler_params(a16, batch, hw, c.c_out, m->w<__half>(m->out_w), c.num_labels, 1.0f, params, 0, 0,
                                        seed_offset, tokens_out, st, skip, top_k, top_p);
+}
+
+int64_t pb200_paella_token_scores_workspace_bytes(const pb200_paella* m, int batch, int hw) {
+    if (m == nullptr || batch < 0 || hw < 0) { set_error("token_scores_workspace_bytes: null model handle or negative shape"); return -1; }
+    return ((int64_t)batch * hw * m->cfg.c_out * 2 + 255) / 256 * 256;
+}
+
+int pb200_paella_token_scores(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                              const int64_t* targets, float* nll_out, float* smooth_out, int64_t* argmax_out, void* workspace,
+                              int64_t workspace_bytes, void* stream) {
+    PB_CHECK(m != nullptr && m->blob != nullptr, "token_scores: weights not bound");
+    PB_CHECK(batch >= 0 && hw >= 0 && n_pairs >= 0 && n_pairs <= batch, "token_scores: %d pairs among %d samples", n_pairs, batch);
+    PB_CHECK(n_pairs == 0 || params != nullptr, "token_scores: guided samples need params");
+    const pb200_paella_config& c = m->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t rows = (int64_t)batch * hw;
+    if (rows == 0) return 0;
+    PB_CHECK(features != nullptr && targets != nullptr && nll_out != nullptr && smooth_out != nullptr && argmax_out != nullptr,
+             "token_scores: features, targets and the three outputs are required");
+    PB_CHECK(rows * c.c_out * 2 <= workspace_bytes, "token_scores: workspace too small (use pb200_paella_token_scores_workspace_bytes)");
+    __half* a16 = reinterpret_cast<__half*>(workspace);
+    // the A operand pb200_paella_sample_tokens_pairs feeds the sampler: guided samples mixed with their unconditional rows
+    const int64_t mixed = (int64_t)n_pairs * hw * c.c_out;
+    PB_TRY(launch_mix_cast_rows_f16(features, features + rows * c.c_out, params, (int64_t)hw * c.c_out, mixed, a16, st));
+    PB_TRY(launch_cast_f16(features + mixed, rows * c.c_out - mixed, a16 + mixed, st));
+    return launch_token_scores(a16, rows, c.c_out, m->w<__half>(m->out_w), c.num_labels, targets, nll_out, smooth_out, argmax_out, st);
 }
 
 // scratch of pb200_paella_resample_samples: fp16 features and fp32 logits of 2 * chunk sample blocks

@@ -11,6 +11,7 @@ from __future__ import annotations
 import ctypes
 import math
 import os
+from collections import namedtuple
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -259,6 +260,10 @@ class TimestepBlock(nn.Module):
 
 
 # ------------------------------------------------------------------------------------------------
+# Paella.token_scores: fp32 [B, H, W] negative log-likelihood and label-smoothed loss, int64 [B, H, W] arg-max code
+TokenScores = namedtuple("TokenScores", ["nll", "loss", "argmax"])
+
+
 class ConditioningCache:
     """x- and t-independent conditioning work of one sample() call: c_embed and every AttnBlock's
     cond K/V for ``batch_total`` samples (conditional rows first, then unconditional rows)."""
@@ -1133,6 +1138,87 @@ class Paella(nn.Module):
         if attention_maps:
             return logits, self.finalize_attention_maps(acc, (H, W), cond_len, 1)
         return logits
+
+    def token_scores(self, x, r, targets, byt5, clip=None, clip_image=None, *, label_smoothing=0.0, cfg=None,
+                     unconditional_inputs=None, attn_weights=None, tiling=None, prompt_regions=None) -> TokenScores:
+        """How likely the denoiser finds ``targets`` given the noised tokens ``x`` at noise level ``r``: per token the statistics
+        of train.py's objective (src/train.py:36,64,71), from one fused out_mapper + log-softmax kernel whose logits never reach
+        HBM (pb200_paella_token_scores).  Returns TokenScores(nll, loss, argmax):
+          nll     fp32 [B, H, W]  -log_softmax(logits)[target] = logsumexp(l) - l_y;
+          loss    fp32 [B, H, W]  (1 - eps) nll + eps (logsumexp(l) - mean_j l_j), which is
+                                  nn.CrossEntropyLoss(label_smoothing=eps, reduction='none'); at eps = 0 the nll tensor itself;
+          argmax  int64 [B, H, W] the lowest code with the largest logit (pred.argmax(1)).
+        ``targets``: int64 [B, H, W] on the model's device; a code outside [0, num_labels) gives a NaN nll and loss in its token
+        only.  ``cfg``: None (the conditional logits), a number, or a CPU tensor [B] of per-sample scales: each sample is then
+        scored under the guided logits u + cfg (c - u) of the CFG pair batch the sampling loop builds, the distribution sample()
+        draws from at temperature 1, with ``unconditional_inputs`` (default: zeros like the conditioning, as in sample_notebook).
+        ``attn_weights``, ``tiling`` and ``prompt_regions`` mean what they mean in ``forward`` and apply to the conditional rows.
+        ValueError, before anything is enqueued, for bad targets, an eps outside [0, 1] and a bad cfg, attn_weights, tiling or
+        prompt_regions; TypeError for any other keyword argument."""
+        B, H, W = x.shape
+        eps = ops.check_label_smoothing(label_smoothing)
+        self._check_score_targets(targets, x.shape)
+        setup = self._score_setup(B, (H, W), {"byt5": byt5, "clip": clip, "clip_image": clip_image}, unconditional_inputs, cfg,
+                                  attn_weights, tiling, prompt_regions)
+        return self._score_tokens(setup, x, r, targets, eps)
+
+    def _check_score_targets(self, targets, shape, name: str = "targets") -> None:
+        if not torch.is_tensor(targets) or targets.dtype != torch.int64 or targets.device != self._device() \
+                or tuple(targets.shape) != tuple(shape):
+            got = f"{targets.dtype} {list(targets.shape)} on {targets.device}" if torch.is_tensor(targets) else type(targets).__name__
+            raise ValueError(f"{name}: expected int64 codes of shape {list(shape)} on {self._device()} (got {got})")
+
+    def _score_setup(self, batch: int, latent_hw, model_inputs, unconditional_inputs, cfg, attn_weights, tiling, prompt_regions):
+        """token_scores' per-call state, reused by every forward of utils.score: validates the arguments (ValueError before
+        anything is enqueued), then builds the conditioning and the device tables of the conditional rows."""
+        H, W = int(latent_hw[0]), int(latent_hw[1])
+        params = ops.score_cfg_params(cfg, batch)
+        wrap = ops.tiling_table(tiling, batch)
+        regions = ops.regional_table(prompt_regions, batch, (H, W), self._device())
+        ops.check_regions_unweighted(regions, attn_weights)
+        cond_len = self.conditioning_seq_len(model_inputs)
+        w_table = None
+        if isinstance(attn_weights, (list, tuple)):
+            w_table = ops.attn_weights_table(attn_weights, batch, [self.max_attn_weights((H, W), cond_len)] * batch)
+        if params is not None and unconditional_inputs is None:
+            unconditional_inputs = {k: (torch.zeros_like(v) if torch.is_tensor(v) else [torch.zeros_like(t) for t in v])
+                                    for k, v in model_inputs.items() if v is not None}
+        dev = self._device()
+        aw, w_len = attn_weights, None
+        if w_table is not None:
+            aw, w_len = ops.attn_weights_to_device(*w_table, dev)
+        extra = [g for own in regions[1] for g in own] if regions is not None else []
+        regional = None
+        if params is None and regions is None:
+            cond = self._cond_for_forward(model_inputs["byt5"], model_inputs.get("clip"), model_inputs.get("clip_image"), (H, W))
+        else:
+            groups = [model_inputs] + ([unconditional_inputs] if params is not None else [])
+            cond = self.prepare_conditioning(groups, (H, W), extra=extra)
+            regional = self.regional_device(regions, cond) if regions is not None else None
+        return {"batch": batch, "hw": (H, W), "cond": cond, "aw": aw, "w_len": w_len, "regional": regional,
+                "wrap": ops.to_device_async(wrap, dev) if wrap is not None else None,
+                "params": ops.to_device_async(params, dev) if params is not None else None}
+
+    def _score_tokens(self, setup, x, r, targets, eps: float) -> TokenScores:
+        """One scoring forward on ``_score_setup``'s state: the features of the conditional (and, with cfg, unconditional) rows,
+        then pb200_paella_token_scores."""
+        B, (H, W) = setup["batch"], setup["hw"]
+        if tuple(x.shape) != (B, H, W):
+            raise ValueError(f"x of shape {list(x.shape)}; expected {[B, H, W]}")
+        params, aw = setup["params"], setup["aw"]
+        guided = params is not None
+        feats = self.features(x, r, setup["cond"], aw, B if aw is not None else 0, cfg_pairs=guided, w_len=setup["w_len"],
+                              wrap=setup["wrap"], regional=setup["regional"])
+        L, dev = lib(), self._device()
+        with torch.cuda.device(dev):
+            nll = torch.empty(B, H, W, dtype=torch.float32, device=dev)
+            smooth = torch.empty_like(nll)
+            argmax = torch.empty(B, H, W, dtype=torch.int64, device=dev)
+            ws = self._ws(L.pb200_paella_token_scores_workspace_bytes(self._handle, B, H * W))
+            check(L.pb200_paella_token_scores(self._handle, ptr(feats), B, B if guided else 0, H * W, ptr(params),
+                                              ptr(targets.contiguous()), ptr(nll), ptr(smooth), ptr(argmax), ptr(ws), ws.numel(),
+                                              current_stream()), "pb200_paella_token_scores")
+        return TokenScores(nll, ops.smoothed_loss(nll, smooth, eps), argmax)
 
     def _cond_for_forward(self, byt5, clip, clip_image, hw):
         """The reference's own loop calls ``model(x, t, **inputs)`` twice per step with the SAME conditioning tensors

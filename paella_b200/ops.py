@@ -515,6 +515,54 @@ def guidance_mix_table(terms, cond_row, uncond_row, term_rows, cfgs) -> Tuple[to
 # The notebook's sampling modes (paella_inference.ipynb cell 3).  'multinomial' draws H*W*num_labels exponentials per step; 'argmax'
 # and 'quant' draw nothing.  A step with several modes sends one int32 table to the device: the mode code of every sample, then
 # the samples in argmax mode, then the samples in quant mode, each list ascending.
+# ------------------------------------------------------------------ token scoring
+# pb200_paella_token_scores returns per token nll = lse - l_y and smooth = lse - mean_j l_j; the label-smoothed cross entropy
+# torch.nn.CrossEntropyLoss(label_smoothing=eps, reduction='none') computes is (1 - eps) nll + eps smooth.
+def check_label_smoothing(eps) -> float:
+    """``label_smoothing`` -> the float.  ValueError unless it is a real number in [0, 1] (a bool is not one)."""
+    if isinstance(eps, bool) or not isinstance(eps, (int, float)) or not 0.0 <= float(eps) <= 1.0:
+        raise ValueError(f"label_smoothing: expected a number in [0, 1] (got {eps!r})")
+    return float(eps)
+
+
+def smoothed_loss(nll: torch.Tensor, smooth: torch.Tensor, eps: float) -> torch.Tensor:
+    """(1 - eps) nll + eps smooth in the tensors' dtype; ``nll`` itself (the same tensor) at eps = 0."""
+    if eps == 0.0:
+        return nll
+    return nll.mul(1.0 - eps).add_(smooth, alpha=eps)
+
+
+def score_cfg_params(cfg, batch: int) -> Optional[torch.Tensor]:
+    """``cfg`` of Paella.token_scores (None, a real number, or a CPU float tensor [batch]) -> None or the CPU params table
+    float32 [batch, 3] of (cfg, 1 - cfg, 1) that sampling_params_table builds at temperature 1.  ValueError (nothing enqueued)
+    for a bad value."""
+    if cfg is None:
+        return None
+    if torch.is_tensor(cfg):
+        cfgs = per_sample_values("cfg", cfg, batch)
+    elif isinstance(cfg, bool) or not isinstance(cfg, (int, float)) or not math.isfinite(cfg):
+        raise ValueError(f"cfg: expected None, a finite number or a CPU tensor [{batch}] (got {cfg!r})")
+    else:
+        cfgs = [float(cfg)] * batch
+    return sampling_params(cfgs, [1.0] * batch)
+
+
+def check_score_levels(levels) -> list:
+    """``levels`` of utils.score -> a list of floats.  ValueError unless it is a non-empty list, tuple or 1-D CPU tensor of
+    finite numbers in [0, 1] (a bool is not one)."""
+    if torch.is_tensor(levels):
+        if levels.device.type != "cpu" or levels.dim() != 1 or not levels.is_floating_point():
+            raise ValueError(f"levels: expected a 1-D CPU floating-point tensor (got {levels.dtype} of shape {list(levels.shape)} "
+                             f"on {levels.device})")
+        levels = levels.tolist()
+    if not isinstance(levels, (list, tuple)) or not levels:
+        raise ValueError("levels: expected a non-empty sequence of noise levels in [0, 1]")
+    for i, v in enumerate(levels):
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not 0.0 <= float(v) <= 1.0:
+            raise ValueError(f"levels[{i}]: expected a number in [0, 1] (got {v!r})")
+    return [float(v) for v in levels]
+
+
 SAMPLING_MODES = ("multinomial", "argmax", "quant")
 RESAMPLE_CHUNK = 8      # guided samples per out_mapper GEMM of pb200_paella_resample_samples (bounds its logits scratch)
 

@@ -90,9 +90,15 @@ source and its edits must sit in the same shard; indices are relative to the cal
 before any generator advances, for the wrong length, a bad entry (a bool is not an int), a source out of range or equal to its
 sample, a source that is itself injected, k outside [0, steps], ``prompt_regions`` on an edit or its source, and ``exact=True``
 (ops.attention_source_table; pb200_paella_features_inject).
+
+Scoring: ``score`` asks the denoiser how likely a given token grid is under a prompt -- held-out evaluation of a checkpoint with
+train.py's objective, reranking of candidates, or picking the prompt that best explains an image.  It noises the tokens at each
+of a list of noise levels, as add_noise does, and scores each noised grid against the clean tokens with Paella.token_scores
+(pb200_paella_token_scores), whose fused kernel never writes the logits.
 """
 from __future__ import annotations
 
+from collections import namedtuple
 from typing import Dict, Optional, Sequence, Tuple
 
 import torch
@@ -402,6 +408,68 @@ def sampling_modes(mode, sampling_quant_steps, batch: int, steps: int, generator
         if exact:
             raise ValueError("exact=True is the multinomial parity path; it does not take per-sample modes")
     return table
+
+
+# utils.score: fp32 [B] mean nll, loss and argmax accuracy over the scored tokens, and the fp32 [B, H, W] per-token nll averaged
+# over the levels
+Scores = namedtuple("Scores", ["nll", "loss", "acc", "nll_map"])
+
+
+def score(model, tokens, model_inputs, unconditional_inputs=None, levels=None, cfg=None, label_smoothing=0.0, generator=None,
+          region=None, attn_weights=None, tiling=None, prompt_regions=None) -> Scores:
+    """The Monte-Carlo denoising score of ``tokens`` (int64 [B, H, W] on the model's device) under ``model_inputs``.
+
+    For each noise level t_k of ``levels`` in order (default torch.linspace(1.0, 0.0, 9)[:8], the levels at which an 8-step
+    sample() calls the model) the tokens are noised with exactly the draws of ``model.add_noise(tokens, t_k * ones(B),
+    generator=generator)`` -- a mask, then the replacement codes, on the default CUDA generator, one generator, or per sample on
+    a list of B -- and the noised grid is scored against ``tokens`` by ``model.token_scores`` at r = t_k, with ``cfg``,
+    ``unconditional_inputs``, ``label_smoothing``, ``attn_weights``, ``tiling`` and ``prompt_regions`` as there.  ``region`` (bool
+    [B, H, W] on the CPU or the model's device) keeps the tokens outside it from ever being noised (add_noise's ``src=tokens,
+    region=region``) and restricts the means to the tokens inside it.
+
+    Returns Scores(nll, loss, acc, nll_map): nll_map fp32 [B, H, W] is the levels' nll summed in level order in fp32 and divided by
+    K = len(levels); nll and loss fp32 [B] are the means over the scored tokens of nll_map and of the levels' mean loss, and acc
+    fp32 [B] is train.py's accuracy, the fraction of scored tokens and levels whose arg-max code is the token.  Rows with equal
+    tokens, prompt and seed get equal scores where the forward is batch-invariant (DESIGN.md §3), so per-sample generators
+    seeded alike compare prompts on common noise.  ValueError, before anything is enqueued and before any generator advances,
+    for tokens that are not int64 [B, H, W] on the model's device, bad levels, an eps outside [0, 1], and a bad cfg,
+    generator list, region, attn_weights, tiling or prompt_regions."""
+    dev = model._device()
+    if not torch.is_tensor(tokens) or tokens.dim() != 3:
+        raise ValueError("tokens: expected int64 codes [B, H, W] on the model's device")
+    model._check_score_targets(tokens, tokens.shape, "tokens")
+    B, H, W = tokens.shape
+    levels = ops.check_score_levels(torch.linspace(1.0, 0.0, 9)[:8] if levels is None else levels)
+    eps = ops.check_label_smoothing(label_smoothing)
+    if ops.per_sample(generator):
+        ops.check_generators(generator, B, dev)
+        ops.check_per_sample_numel(H * W)
+    check_region(region, tokens, tokens.shape, dev)
+    setup = model._score_setup(B, (H, W), model_inputs, unconditional_inputs, cfg, attn_weights, tiling, prompt_regions)
+    region_d = region.to(dev) if region is not None else None
+    nll_sum = loss_sum = hits = None
+    for t_k in levels:
+        t = torch.full((B,), t_k, dtype=torch.float32, device=dev)
+        if region_d is None:
+            noised = model.add_noise(tokens, t, generator=generator)[0]
+        else:
+            noised = model.add_noise(tokens, t, generator=generator, src=tokens, region=region_d)[0]
+        s = model._score_tokens(setup, noised, t, tokens, eps)
+        hit = (s.argmax == tokens).to(torch.float32)
+        if nll_sum is None:
+            nll_sum, loss_sum, hits = s.nll.clone(), s.loss.clone(), hit
+        else:
+            nll_sum += s.nll
+            loss_sum += s.loss
+            hits += hit
+    K = len(levels)
+    nll_map = nll_sum / K
+    w = region_d.to(torch.float64) if region_d is not None else torch.ones(B, H, W, dtype=torch.float64, device=dev)
+    n = w.sum((1, 2))
+
+    def mean(m):
+        return ((m.double() * w).sum((1, 2)) / n).float()
+    return Scores(mean(nll_map), mean(loss_sum / K), mean(hits / K), nll_map)
 
 
 def load_conditional_models(byt5_model_name, vqgan_path, device):
