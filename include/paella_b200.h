@@ -454,6 +454,74 @@ int pb200_paella_features_inject(pb200_paella* m, const int64_t* tokens, const f
                                  const int* tail_src, const int* map_row, int map_batch, float* map_acc, int map_rows, int map_len,
                                  const int* inj_src, int inj_batch, float* features, void* workspace, int64_t workspace_bytes,
                                  void* stream);
+/* ------------------------------------------------------------------------------------------
+ * LoRA adapters per sample on every AttnBlock: a sample with adapter (A, B, alpha) of rank r at scale s is computed as the
+ * reference model with W' = W + s * (alpha / r) * B A on the adapter's targets, which are the projections of
+ *   Attention2D / nn.MultiheadAttention in_proj (q, k, v packed) and out_proj   ref/src/modules.py:12-19
+ *   AttnBlock.kv_mapper[1]                                                       ref/src/modules.py:76-79
+ * Each delta is added after the layer's own GEMM by a segmented shrink (U = x A^T) + expand (y += s (alpha/r) U B^T) kernel.
+ * ------------------------------------------------------------------------------------------ */
+#define PB200_LORA_MAX_ADAPTERS 32        /* distinct adapters in one call */
+#define PB200_LORA_MAX_ATTN_BLOCKS 128
+#define PB200_LORA_WORKSPACE_PER_ROW 256  /* bytes of scratch per row: the shrink's fp32 U, up to 64 ranks */
+enum { PB200_LORA_IN_PROJ = 1, PB200_LORA_OUT_PROJ = 2, PB200_LORA_KV_MAPPER = 4 };   /* target bits */
+
+/* One adapter operand of the kernel-level entry point:
+ *   a    fp16 [rank_pad][k] (rows >= r zero), b fp16 [n][rank_pad] (columns >= r zero), both 16-byte aligned;
+ *   aux  fp32 [rank_pad + 1]: the row sums of the fp16 rows of a (read in folded-LayerNorm mode), then alpha / r;
+ *   rank_pad  r rounded up to a multiple of 8 (8..64), 0 = absent. */
+typedef struct pb200_lora_operand {
+    const void* a;
+    const void* b;
+    const float* aux;
+    int rank_pad;
+} pb200_lora_operand;
+
+/* For rows i < m with id = row_adapter[i / rows_per_entry] >= 0 (< n_ops) and s = row_scale[i / rows_per_entry] != 0 (DEVICE int32 /
+ * fp32 tables):  u = x[i] a_id^T, or with ln_stat (DEVICE int64 [m][2], the PB200_EPI_F16_LN statistics over k columns of the
+ * shifted fp16 rows x) u_j = rstd_i (x[i] a_id[j]^T - mean'_i aux[j]);  then y[o] += s * aux[rank_pad] * u b_id^T with
+ * o = (i / remap_in) * remap_out + i % remap_in (remap_in = 0: o = i).  y: fp16 (y_f32 = 0, rounded once) or fp32, ldy elements
+ * per row.  Rows with id -1 or scale 0 are neither read nor written.  Each row's result depends on its own row, adapter and scale
+ * only (no split-K, no atomics, one summation order).  k % 8 == 0, ldx % 8 == 0, n and ldy even.  ops: HOST array of n_ops <= 32
+ * operands.  workspace: m * PB200_LORA_WORKSPACE_PER_ROW bytes. */
+int pb200_lora_shrink_expand(const void* x, int64_t ldx, int64_t m, int k, int n, int rows_per_entry, const int* row_adapter,
+                             const float* row_scale, const pb200_lora_operand* ops, int n_ops, const int64_t* ln_stat, void* y,
+                             int64_t ldy, int y_f32, int remap_in, int remap_out, void* workspace, int64_t workspace_bytes,
+                             void* stream);
+
+/* A packed adapter of a model (paella_b200/lora.py builds it).  blob: DEVICE, 256-byte aligned; rank 1..64; targets[i]: the target
+ * bits AttnBlock i (plan order, i < n_attn) carries.  Blob layout, with rp = rank rounded up to a multiple of 8: for each AttnBlock in
+ * plan order, for each target it carries in the order in_proj, out_proj, kv_mapper, three parts, each starting on a 256-byte boundary:
+ *   A    fp16 [rp][in]     lora_A rows, rows >= rank zero
+ *   B    fp16 [out][rp]    lora_B rows, columns >= rank zero
+ *   aux  fp32 [rp + 1]     row sums of the fp16 A rows, then alpha / rank
+ * with (in, out) = (c, 3c) for in_proj, (c, c) for out_proj and (c_cond, c) for kv_mapper, c the block's width. */
+typedef struct pb200_lora_adapter {
+    const void* blob;
+    int rank;
+    unsigned char targets[PB200_LORA_MAX_ATTN_BLOCKS];
+} pb200_lora_adapter;
+
+/* pb200_paella_prepare_cond with adapters: slot batch_offset + b is projected under adapter row_adapter[b] (DEVICE int32 [batch],
+ * -1: none, else an index into the HOST array adapters[n_adapters]) at scale row_scale[b] (DEVICE fp32 [batch]): kv_mapper[1] and
+ * the K/V rows of in_proj get the adapter's deltas.  n_adapters = 0 is pb200_paella_prepare_cond, the same launches. */
+int pb200_paella_prepare_cond_lora(pb200_paella* m, const pb200_cond* cond, int batch, int batch_offset, int batch_total, int s_max,
+                                   void* cond_cache, void* workspace, int64_t workspace_bytes, const pb200_lora_adapter* adapters,
+                                   int n_adapters, const int* row_adapter, const float* row_scale, void* stream);
+/* pb200_paella_features_inject with adapters: base sample b (< batch_total - n_tail) runs every AttnBlock's in_proj and out_proj
+ * under adapter row_adapter[b] (DEVICE int32 [batch_total - n_tail], -1: none) at scale row_scale[b] (DEVICE fp32), and so does
+ * each tail row, under its source sample's entry (the unconditional and guidance-prompt term rows of that sample).  Nothing runs
+ * before the first AttnBlock, so the shared prefix is unchanged.  Rows without an adapter get the bits of the call without
+ * adapters.  n_adapters = 0 is pb200_paella_features_inject, the same launches. */
+int pb200_paella_features_lora(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                               const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                               int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
+                               const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
+                               const int* tail_src, const int* map_row, int map_batch, float* map_acc, int map_rows, int map_len,
+                               const int* inj_src, int inj_batch, const pb200_lora_adapter* adapters, int n_adapters,
+                               const int* row_adapter, const float* row_scale, float* features, void* workspace,
+                               int64_t workspace_bytes, void* stream);
+
 /* maps fp32 [rows][s][h][w] from rows consecutive accumulator rows of pb200_paella_features_maps accumulated over n_steps
  * forwards: maps[row][j][y][x] = (1 / (n_steps * n_attn)) * sum over levels l, ascending, of
  * map_acc[row][j][off_l + (y / (patch << l)) * gw_l + x / (patch << l)] (nearest-neighbour upsampling); s <= map_len. */

@@ -12,6 +12,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpaella_b200.so")
 
 PB200_MAX_LEVELS = 4
+PB200_LORA_MAX_ADAPTERS = 32
+PB200_LORA_MAX_ATTN_BLOCKS = 128
+PB200_LORA_WORKSPACE_PER_ROW = 256
 
 EPI_F16, EPI_F32, EPI_GELU_F16, EPI_RESID_F32, EPI_UNPATCH_F32, EPI_NCHW_F32, EPI_RESID_LN_F32, EPI_F16_LN, EPI_RESID_LN_INV_F32 = range(9)
 
@@ -44,6 +47,14 @@ class Cond(ctypes.Structure):
 class VqganConfig(ctypes.Structure):
     _fields_ = [("levels", c_int), ("bottleneck_blocks", c_int), ("c_hidden", c_int), ("c_latent", c_int),
                 ("codebook_size", c_int), ("scale_factor", c_float)]
+
+
+class LoraOperand(ctypes.Structure):
+    _fields_ = [("a", c_void_p), ("b", c_void_p), ("aux", c_void_p), ("rank_pad", c_int)]
+
+
+class LoraAdapter(ctypes.Structure):
+    _fields_ = [("blob", c_void_p), ("rank", c_int), ("targets", ctypes.c_ubyte * PB200_LORA_MAX_ATTN_BLOCKS)]
 
 
 # name -> (restype, argtypes); mirrors include/paella_b200.h one to one
@@ -145,6 +156,14 @@ SIGNATURES = {
                                              c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                              c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int,
                                              c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_lora_shrink_expand": (c_int, [c_void_p, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, POINTER(LoraOperand), c_int,
+                                         c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_prepare_cond_lora": (c_int, [c_void_p, POINTER(Cond), c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int64,
+                                               POINTER(LoraAdapter), c_int, c_void_p, c_void_p, c_void_p]),
+    "pb200_paella_features_lora": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                           c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int,
+                                           POINTER(LoraAdapter), c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_attention_maps_finalize": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_int64, c_void_p]),

@@ -84,6 +84,17 @@ __device__ __forceinline__ float warp_max(float v) {
     return v;
 }
 
+// (-mean, rstd) of a row from the folded LayerNorm's fixed-point row statistics st = (sum x * 2^20, sum x^2 * 2^16) over c columns
+// (PB200_EPI_RESID_LN*): the PB200_EPI_F16_LN epilogue and the LoRA shrink's fold both normalise with exactly these values
+__device__ __forceinline__ void ln_stat_moments(const int64_t* st_row, int c, float& neg_mean, float& rstd) {
+    const longlong2 st = *reinterpret_cast<const longlong2*>(st_row);
+    const float inv_c = 1.0f / (float)c;
+    const float mean = (float)st.x * (1.0f / 1048576.0f) * inv_c;
+    const float ex2 = (float)st.y * (1.0f / 65536.0f) * inv_c;
+    neg_mean = -mean;
+    rstd = 1.0f / sqrtf(fmaxf(ex2 - mean * mean, 0.f) + 1e-6f);
+}
+
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
 // Exact-erf GELU for the GEMM epilogue: erfc by Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7, far below the fp16

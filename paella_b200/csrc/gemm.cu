@@ -207,14 +207,9 @@ __device__ __forceinline__ void epilogue_preload(const pb200_gemm_epilogue& ep, 
                                                  EpiPre<MODE>& pre, int lane, bool first_chunk) {
     if constexpr (MODE == PB200_EPI_F16_LN) {
         if (first_chunk && row < M) {      // row statistics -> (mean, rstd), once per tile
-            const longlong2 st = *reinterpret_cast<const longlong2*>(ep.ln_stat + 2 * (int64_t)row);
-            const float inv_c = 1.0f / (float)ep.ln_c;
-            const float mean = (float)st.x * (1.0f / 1048576.0f) * inv_c;
-            const float ex2 = (float)st.y * (1.0f / 65536.0f) * inv_c;
-            pre.neg_mean = -mean;
-            pre.rstd = 1.0f / sqrtf(fmaxf(ex2 - mean * mean, 0.f) + 1e-6f);
+            ln_stat_moments(ep.ln_stat + 2 * (int64_t)row, ep.ln_c, pre.neg_mean, pre.rstd);
             // the true row mean, for the next producer's shift (every N-tile writes the same value: benign)
-            if (ep.ln_mean_out) ep.ln_mean_out[row] = (ep.ln_shift ? ep.ln_shift[row] : 0.f) + mean;
+            if (ep.ln_mean_out) ep.ln_mean_out[row] = (ep.ln_shift ? ep.ln_shift[row] : 0.f) - pre.neg_mean;
         }
     }
     if constexpr (is_resid_ln<MODE>) {

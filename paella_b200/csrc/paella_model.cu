@@ -14,6 +14,7 @@
 
 #include "attention.cuh"
 #include "gemm.cuh"
+#include "lora.cuh"
 #include "ops.cuh"
 #include "sampler.cuh"
 #include "score.cuh"
@@ -386,6 +387,9 @@ struct FeatWs {
     uint8_t* qmask;              // regional prompts: every level's position masks (launch_regional_masks)
     uint8_t* wrap;               // tiling with a tail map: the wrap byte of every row [Bt]
     float *map_scores, *map_lse2;     // attention maps (map_rows > 0): one AttnBlock's AttnMapOut workspace, reused by every block
+    int* lora_id;                // LoRA: every row's adapter [Bt] (the base samples', then each tail row's source's)
+    float* lora_scale;           // LoRA: every row's scale [Bt]
+    float* lora_u;               // LoRA: the shrink's output of an AttnBlock's rows
 };
 
 // map_rows > 0: also the attention-map workspace of map_rows rows at conditioning length s_max, after everything else so that the
@@ -432,6 +436,10 @@ static void plan_features(const pb200_paella* m, int Bt, int H, int W, Arena& ar
         ws.map_scores = ar.take<float>((int64_t)map_rows * hp * s_max);
         ws.map_lse2 = ar.take<float>((int64_t)map_rows * hp);
     }
+    // last, so that the rest of the plan (and the map workspace size) is the same with and without them
+    ws.lora_id = ar.take<int>(Bt);
+    ws.lora_scale = ar.take<float>(Bt);
+    ws.lora_u = reinterpret_cast<float*>(ar.take<uint8_t>(ws.lnmean_stride * PB200_LORA_WORKSPACE_PER_ROW));
 }
 
 // attention-map accumulator columns: every level's positions, level 0 first
@@ -444,6 +452,7 @@ static int map_positions(const pb200_paella* m, int h, int w) {
 struct CondWs {
     __half *byt5_16, *clip_16, *silu16, *kvm16;
     float* seq;
+    float* lora_u;      // LoRA: the shrink's output of the conditioning rows (last, so the rest of the plan does not move)
 };
 
 static void plan_cond(const pb200_paella* m, int B, int L, int S, Arena& ar, CondWs& ws) {
@@ -453,6 +462,7 @@ static void plan_cond(const pb200_paella* m, int B, int L, int S, Arena& ar, Con
     ws.seq = ar.take<float>((int64_t)B * S * c.c_cond);
     ws.silu16 = ar.take<__half>((int64_t)B * S * c.c_cond);
     ws.kvm16 = ar.take<__half>((int64_t)B * S * m->max_c);
+    ws.lora_u = reinterpret_cast<float*>(ar.take<uint8_t>((int64_t)B * S * PB200_LORA_WORKSPACE_PER_ROW));
 }
 
 // cond cache: per attention block [Bt, s_max, 2c] fp16, then kv_len int32 [Bt]
@@ -469,6 +479,51 @@ static int64_t cond_block_off(const pb200_paella* m, int attn_index, int Bt, int
 __global__ void fill_int_kernel(int* p, int n, int v) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) p[i] = v;
+}
+
+// The operands of every adapter of one call, per AttnBlock and target (pb200_lora_adapter's blob layout, include/paella_b200.h)
+struct LoraPlan {
+    std::vector<LoraOperands> in_proj, out_proj, kv_mapper;      // [n_attn]
+    bool any = false;
+};
+
+static int lora_plan(const pb200_paella* m, const pb200_lora_adapter* ad, int n, LoraPlan& lp) {
+    PB_CHECK(n >= 0 && n <= PB200_LORA_MAX_ADAPTERS && (n == 0 || ad != nullptr), "lora: %d adapters (0..%d)", n, PB200_LORA_MAX_ADAPTERS);
+    if (n == 0) return 0;
+    PB_CHECK(m->n_attn <= PB200_LORA_MAX_ATTN_BLOCKS, "lora: %d AttnBlocks (at most %d)", m->n_attn, PB200_LORA_MAX_ATTN_BLOCKS);
+    LoraOperands none;
+    memset(&none, 0, sizeof(none));
+    lp.in_proj.assign(m->n_attn, none);
+    lp.out_proj.assign(m->n_attn, none);
+    lp.kv_mapper.assign(m->n_attn, none);
+    auto al = [](int64_t b) { return (b + 255) / 256 * 256; };
+    for (int i = 0; i < n; ++i) {
+        PB_CHECK(ad[i].blob != nullptr && ((uintptr_t)ad[i].blob & 255) == 0 && ad[i].rank >= 1 && ad[i].rank <= LORA_MAX_RANK,
+                 "lora: adapter %d: rank %d (1..%d) and a 256-byte aligned blob", i, ad[i].rank, LORA_MAX_RANK);
+        const int rp = (ad[i].rank + 7) / 8 * 8;
+        const uint8_t* base = reinterpret_cast<const uint8_t*>(ad[i].blob);
+        int64_t off = 0;
+        for (const BlockPlan& b : m->blocks) {
+            if (b.kind != BK_ATTN) continue;
+            const int mask = ad[i].targets[b.attn_index];
+            PB_CHECK((mask & ~7) == 0, "lora: adapter %d: target bits %#x on AttnBlock %d", i, mask, b.attn_index);
+            for (int t = 0; t < 3; ++t) {
+                if (!(mask & (1 << t))) continue;
+                const int64_t in = t == 2 ? m->cfg.c_cond : b.c, out = t == 0 ? 3 * b.c : b.c;
+                LoraOperand op;
+                op.a = reinterpret_cast<const __half*>(base + off);
+                off += al(rp * in * 2);
+                op.b = reinterpret_cast<const __half*>(base + off);
+                off += al(out * rp * 2);
+                op.aux = reinterpret_cast<const float*>(base + off);
+                off += al((int64_t)(rp + 1) * 4);
+                op.rank_pad = rp;
+                (t == 0 ? lp.in_proj : t == 1 ? lp.out_proj : lp.kv_mapper)[b.attn_index].op[i] = op;
+                lp.any = true;
+            }
+        }
+    }
+    return 0;
 }
 
 }  // namespace pb
@@ -606,7 +661,17 @@ int pb200_paella_c_embeddings(pb200_paella* m, const pb200_cond* cond, int batch
 
 int pb200_paella_prepare_cond(pb200_paella* m, const pb200_cond* cond, int batch, int batch_offset, int batch_total,
                               int s_max, void* cond_cache, void* workspace, int64_t workspace_bytes, void* stream) {
+    return pb200_paella_prepare_cond_lora(m, cond, batch, batch_offset, batch_total, s_max, cond_cache, workspace, workspace_bytes,
+                                          nullptr, 0, nullptr, nullptr, stream);
+}
+
+int pb200_paella_prepare_cond_lora(pb200_paella* m, const pb200_cond* cond, int batch, int batch_offset, int batch_total, int s_max,
+                                   void* cond_cache, void* workspace, int64_t workspace_bytes, const pb200_lora_adapter* adapters,
+                                   int n_adapters, const int* row_adapter, const float* row_scale, void* stream) {
     PB_CHECK(m->blob != nullptr, "prepare_cond: weights not bound");
+    LoraPlan lp;
+    PB_TRY(lora_plan(m, adapters, n_adapters, lp));
+    PB_CHECK(!lp.any || (row_adapter != nullptr && row_scale != nullptr), "prepare_cond: adapters need row_adapter and row_scale");
     PB_CHECK(cond && cond->byt5 && cond->byt5_len > 0, "prepare_cond: byt5 embeddings are required");
     const pb200_paella_config& c = m->cfg;
     cudaStream_t st = (cudaStream_t)stream;
@@ -630,11 +695,21 @@ int pb200_paella_prepare_cond(pb200_paella* m, const pb200_cond* cond, int batch
         const int ch = b.c;
         pb200_gemm_epilogue e1 = epi(PB200_EPI_F16, m->w<float>(b.kvm_b), ws.kvm16, ch);
         PB_TRY(m->gemm(ws.silu16, c.c_cond, (int64_t)B * S, c.c_cond, b.kvm_w, ch, e1, st));
+        if (lp.any)
+            PB_TRY(launch_lora(ws.silu16, c.c_cond, (int64_t)B * S, c.c_cond, ch, S, row_adapter, row_scale, lp.kv_mapper[b.attn_index],
+                               nullptr, ws.kvm16, ch, false, 0, 0, ws.lora_u, st));
         __half* dst = reinterpret_cast<__half*>(cache + cond_block_off(m, b.attn_index, batch_total, s_max)) +
                       (int64_t)batch_offset * s_max * 2 * ch;
         pb200_gemm_epilogue e2 = epi(PB200_EPI_F16, m->w<float>(b.inproj_b) + ch, dst, 2 * ch);
         e2.remap_in = S; e2.remap_out = s_max;
         PB_TRY(m->gemm(ws.kvm16, ch, (int64_t)B * S, ch, b.inproj_w + (int64_t)ch * ch * 2, 2 * ch, e2, st));
+        if (lp.any) {       // the K/V rows [c, 3c) of in_proj's B
+            LoraOperands kv = lp.in_proj[b.attn_index];
+            for (LoraOperand& o : kv.op)
+                if (o.rank_pad) o.b += (int64_t)ch * o.rank_pad;
+            PB_TRY(launch_lora(ws.kvm16, ch, (int64_t)B * S, ch, 2 * ch, S, row_adapter, row_scale, kv, nullptr, dst, 2 * ch, false, S,
+                               s_max, ws.lora_u, st));
+        }
     }
     int* kv_len = reinterpret_cast<int*>(cache + cond_block_off(m, m->n_attn, batch_total, s_max));
     fill_int_kernel<<<ceil_div(B, 128), 128, 0, st>>>(kv_len + batch_offset, B, S);
@@ -707,7 +782,24 @@ int pb200_paella_features_inject(pb200_paella* m, const int64_t* tokens, const f
                                  const int* tail_src, const int* map_row, int map_batch, float* map_acc, int map_rows, int map_len,
                                  const int* inj_src, int inj_batch, float* features, void* workspace, int64_t workspace_bytes,
                                  void* stream) {
+    return pb200_paella_features_lora(m, tokens, r, batch_total, n_tail, h, w, cond_cache, cache_slots, kv_slot, s_max, attn_w, n_w, w_ld,
+                                      w_len, w_row, w_batch, wrap, prompt_mask, mask_row, region_slot, max_regions, tail_src, map_row,
+                                      map_batch, map_acc, map_rows, map_len, inj_src, inj_batch, nullptr, 0, nullptr, nullptr, features,
+                                      workspace, workspace_bytes, stream);
+}
+
+int pb200_paella_features_lora(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                               const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                               int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
+                               const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
+                               const int* tail_src, const int* map_row, int map_batch, float* map_acc, int map_rows, int map_len,
+                               const int* inj_src, int inj_batch, const pb200_lora_adapter* adapters, int n_adapters,
+                               const int* row_adapter, const float* row_scale, float* features, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
+    LoraPlan lp;
+    PB_TRY(lora_plan(m, adapters, n_adapters, lp));
+    PB_CHECK(!lp.any || (row_adapter != nullptr && row_scale != nullptr), "features: adapters need row_adapter and row_scale");
     PB_CHECK(inj_batch == 0 || (inj_src != nullptr && inj_batch > 0 && inj_batch <= batch_total - n_tail),
              "features: injection table of %d samples for %d base samples", inj_batch, batch_total - n_tail);
     PB_CHECK(map_batch == 0 || (map_acc != nullptr && map_rows > 0 && map_len > 0 && map_batch <= batch_total - n_tail),
@@ -766,6 +858,18 @@ int pb200_paella_features_inject(pb200_paella* m, const int64_t* tokens, const f
         PB_TRY(launch_replicate_rows(ws.wrap, 1, n_base, tail_src, n_tail, st));
         wrap_dw = ws.wrap;
         n_base_dw = Bt;
+    }
+    // LoRA: every row's (adapter, scale), [Bt] -- the base samples' entries, then each tail row's source's
+    if (lp.any) {
+        PB_CUDA(cudaMemcpyAsync(ws.lora_id, row_adapter, (size_t)n_base * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        PB_CUDA(cudaMemcpyAsync(ws.lora_scale, row_scale, (size_t)n_base * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        if (tail_src) {
+            PB_TRY(launch_replicate_rows(ws.lora_id, sizeof(int), n_base, tail_src, n_tail, st));
+            PB_TRY(launch_replicate_rows(ws.lora_scale, sizeof(float), n_base, tail_src, n_tail, st));
+        } else if (n_pairs > 0) {
+            PB_CUDA(cudaMemcpyAsync(ws.lora_id + n_base, ws.lora_id, (size_t)n_pairs * sizeof(int), cudaMemcpyDeviceToDevice, st));
+            PB_CUDA(cudaMemcpyAsync(ws.lora_scale + n_base, ws.lora_scale, (size_t)n_pairs * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        }
     }
     // regional prompts: the position masks of every level for the conditional rows [0, n_base), once per call; level l's
     // [n_base][P_l] table starts at qmask_off[l]
@@ -890,6 +994,9 @@ int pb200_paella_features_inject(pb200_paella* m, const int64_t* tokens, const f
                     PB_TRY(launch_ln_rows(x, M, ch, 1.0f, 0.0f, ws.a16, nullptr, st, mean_out));
                 }
                 PB_TRY(m->gemm(ws.a16, ch, M, ch, b.inproj_w, 3 * (int64_t)ch, e1, st));
+                if (lp.any)
+                    PB_TRY(launch_lora(ws.a16, ch, M, ch, 3 * ch, P, ws.lora_id, ws.lora_scale, lp.in_proj[b.attn_index],
+                                       folded ? e1.ln_stat : nullptr, ws.qkv16, 3 * ch, false, 0, 0, ws.lora_u, st));
                 AttnParams ap;
                 ap.qkv = ws.qkv16;
                 ap.ckv = reinterpret_cast<const __half*>(cache + cond_block_off(m, b.attn_index, cache_slots, s_max));
@@ -909,6 +1016,9 @@ int pb200_paella_features_inject(pb200_paella* m, const int64_t* tokens, const f
                 pb200_gemm_epilogue e2 = epi(PB200_EPI_RESID_F32, m->w<float>(b.outproj_b), x, ch);
                 e2.resid = x; e2.ldr = ch; e2.rows_per_sample = P;
                 PB_TRY(m->gemm(ws.o16, ch, M, ch, b.outproj_w, ch, e2, st));
+                if (lp.any)
+                    PB_TRY(launch_lora(ws.o16, ch, M, ch, ch, P, ws.lora_id, ws.lora_scale, lp.out_proj[b.attn_index], nullptr, x, ch,
+                                       true, 0, 0, ws.lora_u, st));
                 break;
             }
         }

@@ -41,7 +41,12 @@ guided steps runs one more denoiser row per term; terms draw nothing.  With ``at
 ``sample_notebook(..., attention_maps=True)`` on the same request; its tokens are unchanged, and maps draw nothing.  With
 ``attention_source=(src, k)`` a request is a prompt-to-prompt edit of the queued request ``src``: the edit and its source are
 admitted together and advance in lockstep, and on its steps i < k the edit's conditional forward replays the source's attention
-probabilities, as ``sample_notebook(..., attention_source=[None, (0, k)])`` does on the pair; injection draws nothing.
+probabilities, as ``sample_notebook(..., attention_source=[None, (0, k)])`` does on the pair; injection draws nothing.  With
+``lora=adapter`` or ``(adapter, scale)`` a request runs under a LoRA adapter as ``sample_notebook(..., lora=[entry])`` does: its
+K/V slots are projected under the adapter at admission, and a guided request without a negative prompt of its own gets its own
+unconditional slot, holding the engine-wide unconditional inputs projected under its adapter (the shared slot is the model's
+without an adapter); adapters draw nothing.  One step's launches take at most 32 distinct adapters (ops.MAX_LORA_ADAPTERS):
+admission holds a request whose adapter would be the 33rd in flight, and everything queued behind it, until a request retires.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -64,7 +69,9 @@ runs the maps denoiser (pb200_paella_features_maps), which accumulates into a po
 first such request is admitted and zeroed per request at admission; a request's maps are finalized with its own step count when it
 retires.  A step with no such row launches exactly as without maps.  A step in which some edit is inside its window adds each
 row's source row in this step's order (-1 for the other rows) to the table and runs the injecting denoiser
-(pb200_paella_features_inject); a step with no such row launches exactly as without edits.
+(pb200_paella_features_inject); a step with no such row launches exactly as without edits.  A step in which some row has a LoRA
+adapter adds each row's adapter index and scale to the table and runs the adapted denoiser (pb200_paella_features_lora); a step
+with no such row launches exactly as without adapters.  No adapter memory is reserved: an adapter lives in its LoraAdapter.
 The host knows which
 requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
 in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
@@ -93,7 +100,7 @@ class Request:
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
                  region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
                  top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None, terms=None, mix_coef=None,
-                 attention_maps: bool = False, maps_len: int = 0, attention_source=None):
+                 attention_maps: bool = False, maps_len: int = 0, attention_source=None, lora=None):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -114,6 +121,7 @@ class Request:
         # prompt-to-prompt: the source request and the steps it is replayed on, or None; a source lists its edits
         self.inj_src, self.inj_k = attention_source if attention_source is not None else (None, 0)
         self.edits: List["Request"] = []
+        self.lora = lora                         # LoRA: (adapter, scale) or None, held until retirement
         # with keep_intermediates: what sample_notebook returns as its second value, device tensors [1, H, W]
         self.intermediates: Optional[List[torch.Tensor]] = [] if keep_intermediates else None
         self.k = 0                               # steps done
@@ -174,6 +182,9 @@ class StepPlan:
         self.inj_src = torch.tensor([row[id(q.inj_src)] if q.inj_src is not None and q.k < q.inj_k else -1 for q in order],
                                     dtype=torch.int32)
         self.injects = bool((self.inj_src >= 0).any())
+        # LoRA: each row's index into the step's distinct adapters (-1: none) and its scale, when some row has an adapter
+        self.adapters, self.lora_id, self.lora_scale = ops.lora_rows([q.lora for q in order])
+        self.loras = bool(self.adapters)
 
 
 def cond_layout(inputs: Dict[str, torch.Tensor]) -> Tuple[int, bool, int]:
@@ -199,11 +210,12 @@ def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List
 
 def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tuple[torch.Tensor, Dict[str, Tuple[str, int, int]]]:
     """The step's one host-to-device buffer: int64 [(seed, offset) pairs of the sampler's draw, then of the mask draw], then the
-    float32 part [r, params (3 per row), t_next, (top_p), (mix_coef)], then the int32 part [row_slot, kv_slot, (mode table), (top_k),
-    (tail, mix_rows), (map_row), (inj_src)], then the uint8 part [(wrap)], each part padded to whole int64 words.  top_p / top_k
-    are present only when ``plan.truncates``, the mode table only when the step mixes modes, wrap (one byte per row) only when
-    ``plan.wraps``, the tail map and the mix table only when some row of the step is composed (guidance prompts), map_row only
-    when some row wants attention maps, inj_src only when some edit is inside its window.  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
+    float32 part [r, params (3 per row), t_next, (top_p), (mix_coef), (lora_scale)], then the int32 part [row_slot, kv_slot, (mode
+    table), (top_k), (tail, mix_rows), (map_row), (inj_src), (lora_id)], then the uint8 part [(wrap)], each part padded to whole
+    int64 words.  top_p / top_k are present only when ``plan.truncates``, the mode table only when the step mixes modes, wrap (one
+    byte per row) only when ``plan.wraps``, the tail map and the mix table only when some row of the step is composed (guidance
+    prompts), map_row only when some row wants attention maps, inj_src only when some edit is inside its window, lora_id and
+    lora_scale only when some row has a LoRA adapter (the adapters' blob pointers travel as kernel arguments).  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
     Bc, n_pairs = len(plan.order), plan.n_pairs
     mixed = not all(plan.draws)
     modes = ops.mode_table(plan.modes) if mixed else torch.zeros(0, dtype=torch.int32)
@@ -219,6 +231,9 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
         i32_parts.append(("map_row", plan.map_row))
     if plan.injects:
         i32_parts.append(("inj_src", plan.inj_src))
+    if plan.loras:
+        f32_parts.append(("lora_scale", plan.lora_scale))
+        i32_parts.append(("lora_id", plan.lora_id))
     u8_parts = [("wrap", plan.wrap)] if plan.wraps else []
     layout: Dict[str, Tuple[str, int, int]] = {}
     for dt, parts in (("f32", f32_parts), ("i32", i32_parts), ("u8", u8_parts)):
@@ -256,13 +271,19 @@ def _cat_inputs(inputs: List[Dict[str, torch.Tensor]], dev) -> Dict[str, torch.T
     return out
 
 
-def admit_from_queue(queue: "collections.deque[Request]", n_free: int) -> List[Request]:
+def admit_from_queue(queue: "collections.deque[Request]", n_free: int, active: List[Request] = ()) -> List[Request]:
     """Take the requests one admission starts from ``queue``, FIFO, into at most ``n_free`` slots.  A source comes in with
     every edit queued for it (its edits are queued after it), or it and everything behind it waits until enough slots are
-    free."""
+    free.  Likewise a request whose LoRA adapter would take the adapters in flight (``active``'s and the admitted ones') past
+    ops.MAX_LORA_ADAPTERS, the most one step's launches take, waits with everything behind it until a request retires."""
     new: List[Request] = []
+    adapters = ops.distinct_adapters([q.lora for q in active])
     while queue and n_free - len(new) >= 1 + len(queue[0].edits):
         group = [queue[0]] + queue[0].edits
+        grown = adapters + [a for a in ops.distinct_adapters([q.lora for q in group]) if not any(a is b for b in adapters)]
+        if len(grown) > ops.MAX_LORA_ADAPTERS:
+            break
+        adapters = grown
         for q in group:
             queue.remove(q)
         new += group
@@ -336,6 +357,8 @@ class SamplingEngine:
                 torch.zeros(L.pb200_paella_cond_cache_bytes(model._handle, self.n_slots, self.s_max), dtype=torch.uint8,
                             device=self.dev), self.n_slots, self.s_max, self.n_slots, None)
             model._ws(L.pb200_paella_workspace_bytes(model._handle, (2 + self.max_terms) * self.max_batch, self.H, self.W, self.s_max))
+            # a request with a LoRA adapter projects these under its adapter into its own unconditional slot
+            self._uncond_inputs = unconditional_inputs
             if unconditional_inputs is not None:
                 self._check_cond("unconditional_inputs", unconditional_inputs)
                 self.shared_slot = 2 * self.max_batch
@@ -364,7 +387,7 @@ class SamplingEngine:
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
                sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
-               attention_maps=False, attention_source=None) -> Request:
+               attention_maps=False, attention_source=None, lora=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -389,7 +412,11 @@ class SamplingEngine:
         docstring): ``src`` must be a request of this engine that is still queued and not itself an edit, neither may have
         ``prompt_regions``, both need the same conditioning length, ``steps``, ``renoise_steps`` and ``sampling_conditional_steps``,
         k is an int in 0 .. steps, and the source with all its edits must fit in max_batch; ValueError otherwise.  Give the edit a
-        generator seeded like its source's.  The request's draws start when it is admitted."""
+        generator seeded like its source's.  ``lora`` (None, an adapter or (adapter, scale)) runs the request under a LoRA adapter
+        as in sample_notebook, its conditional, unconditional, regional and guidance-prompt K/V included: a request with an adapter
+        and no negative prompt of its own gets its own unconditional slot, into which the engine-wide unconditional inputs are
+        projected under its adapter.  ValueError for a bad entry or scale and an adapter of another configuration or device.  The
+        request holds its adapter until it retires.  The request's draws start when it is admitted."""
         attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
@@ -447,8 +474,11 @@ class SamplingEngine:
         if attn_weights is not None:
             n_keys = self.model.max_attn_weights((self.H, self.W), self.model.conditioning_seq_len(model_inputs))
             attn_weights = ops.check_attn_weight_vector("attn_weights", attn_weights, min(n_keys, self.w_max))
+        if isinstance(lora, list):
+            raise ValueError("lora: a request takes one entry (got a list)")
+        lora = ops.lora_entries(ops.lora_table(lora, 1, self.model), 1)[0]
         if attention_source is not None:
-            self._check_attention_source(attention_source, model_inputs, steps, renoise_steps, cond_steps, prompt_regions)
+            self._check_attention_source(attention_source, model_inputs, steps, renoise_steps, cond_steps, prompt_regions, lora)
         cfgs = U._cfg_schedule(cfg, 1, steps)
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         mix_coef = None
@@ -462,14 +492,14 @@ class SamplingEngine:
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
                       sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap, regions,
-                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs), attention_source)
+                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs), attention_source, lora)
         if attention_source is not None:
             attention_source[0].edits.append(req)
         self._gens.add(id(generator))
         self._queue.append(req)
         return req
 
-    def _check_attention_source(self, attention_source, model_inputs, steps, renoise_steps, cond_steps, prompt_regions):
+    def _check_attention_source(self, attention_source, model_inputs, steps, renoise_steps, cond_steps, prompt_regions, lora=None):
         """submit's rules for ``attention_source`` (ValueError)."""
         if not isinstance(attention_source, (list, tuple)) or len(attention_source) != 2 or not isinstance(attention_source[0], Request) \
                 or isinstance(attention_source[1], bool) or not isinstance(attention_source[1], int):
@@ -490,11 +520,17 @@ class SamplingEngine:
             raise ValueError(f"attention_source: {k} injected steps; expected 0..{steps}")
         if len(src.edits) + 2 > self.max_batch:
             raise ValueError(f"attention_source: a source and its {len(src.edits) + 1} edits exceed max_batch={self.max_batch}")
+        if len(ops.distinct_adapters([q.lora for q in [src] + src.edits] + [lora])) > ops.MAX_LORA_ADAPTERS:
+            raise ValueError(f"attention_source: a source and its edits on more than {ops.MAX_LORA_ADAPTERS} distinct LoRA adapters "
+                             "cannot be admitted together")
 
     def _admit(self):
-        new = admit_from_queue(self._queue, len(self._free))
+        new = admit_from_queue(self._queue, len(self._free), self._active)
         for q in new:
             q.slot = self._free.pop(0)
+            # an adapter is part of the model: a request with one never reads the shared unconditional slot
+            if q.uncond is None and q.lora is not None and q.guided and self.shared_slot is not None:
+                q.uncond = self._uncond_inputs
             q.uncond_slot = self.max_batch + q.slot if q.uncond is not None else self.shared_slot
         if not new:
             return
@@ -524,7 +560,7 @@ class SamplingEngine:
                 masks[j] = q.regions[0]
                 for k, inputs in enumerate(q.regions[1]):
                     rslots[j, k] = self._region_slot(q.slot, k)
-                    region_writes.append((self._region_slot(q.slot, k), inputs))
+                    region_writes.append((self._region_slot(q.slot, k), inputs, q.lora))
         slots, w_lens_d, w_rows_d, regions_d, srcs_d, *regional_d = ops.to_device_packed(
             [torch.tensor([q.slot for q in new], dtype=torch.int32), w_lens, w_rows, regions, srcs] + ([masks, rslots] if R else []),
             self.dev)
@@ -556,11 +592,13 @@ class SamplingEngine:
         # that spans rows)
         for q in new:
             q.term_slot = [self._term_slot(q.slot, j) for j in range(q.n_terms)]
-        term_writes = [(s, inputs) for q in new for s, (inputs, _) in zip(q.term_slot, q.terms or [])]
-        writes = [(q.slot, q.inputs) for q in new] + [(q.uncond_slot, q.uncond) for q in new if q.uncond is not None] + region_writes \
-            + term_writes
-        for run in admission_runs([(slot, cond_layout(x)) for slot, x in writes]):
-            m.write_conditioning(self.cache, writes[run[0]][0], _cat_inputs([writes[i][1] for i in run], self.dev), (self.H, self.W))
+        term_writes = [(s, inputs, q.lora) for q in new for s, (inputs, _) in zip(q.term_slot, q.terms or [])]
+        writes = [(q.slot, q.inputs, q.lora) for q in new] + [(q.uncond_slot, q.uncond, q.lora) for q in new if q.uncond is not None] \
+            + region_writes + term_writes
+        for run in admission_runs([(slot, cond_layout(x)) for slot, x, _ in writes]):
+            entries = [writes[i][2] for i in run]
+            m.write_conditioning(self.cache, writes[run[0]][0], _cat_inputs([writes[i][1] for i in run], self.dev), (self.H, self.W),
+                                 lora=entries if any(e is not None for e in entries) else None)
         for q in new:
             q.inputs = q.uncond = q.init_x = q.region = q.regions = q.terms = None
         self._active += new
@@ -609,6 +647,8 @@ class SamplingEngine:
                 tail["maps"] = (part("map_row"), Bc, self.map_acc)
             if plan.injects:    # row b replays the attention of row inj_src[b]
                 tail["inject"] = part("inj_src")
+            if plan.loras:      # row b runs under adapter lora_id[b] (its tail rows under their source's)
+                tail["lora"] = (ops.lora_structs(plan.adapters), len(plan.adapters), part("lora_id"), part("lora_scale"))
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_tail, self.s_max, self.n_slots, kv_slot_d)
@@ -658,6 +698,7 @@ class SamplingEngine:
                     q.result = self.tokens[q.slot:q.slot + 1].clone()
                 self._free.append(q.slot)
                 self._gens.discard(id(q.generator))
+                q.lora = None
             self._free.sort()
             self._active = [q for q in self._active if q.k < q.steps]
             return done

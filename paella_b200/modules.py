@@ -521,18 +521,23 @@ class Paella(nn.Module):
     # -------------------------------------------------------------- conditioning
     def prepare_conditioning(self, groups: Sequence[Dict[str, torch.Tensor]], latent_hw=(32, 32),
                              share_uniform: bool = True, extra: Sequence[Dict[str, torch.Tensor]] = (),
-                             tail: Sequence[int] = ()) -> ConditioningCache:
+                             tail: Sequence[int] = (), lora=None, extra_lora=None) -> ConditioningCache:
         """gen_c_embeddings (ref/src/modules.py:223-232) + every AttnBlock's kv_mapper and K/V projection of the
         conditioning rows, for the concatenation of ``groups`` (e.g. [conditional, unconditional]).  A group whose
         samples all carry the same tensors (the usual unconditional group) is projected once and shared.  ``extra``: batch-1
         conditioning dicts (regional and guidance prompts) projected into slots of their own after the groups'
         (cache.extra_slot on), consecutive ones of one sequence layout in one projection.  ``tail``: indices into ``extra``; the
         cache then has len(tail) more samples after the groups', sample k of them attending to extra prompt tail[k] (the term
-        rows of features' ``tail_src``).  No other sample's slot_map entry names an extra slot."""
+        rows of features' ``tail_src``).  No other sample's slot_map entry names an extra slot.
+        ``lora``: None, or per group None or a list of its samples' LoRA entries (ops.lora_entries: None or (adapter, scale)), and
+        ``extra_lora``: None or one entry per ``extra`` prompt: each slot is projected under its entry's adapter
+        (pb200_paella_prepare_cond_lora), and a group is shared only when its samples also agree on the entry."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
         seq = self._cfg["clip_seq_len"]
+        glora = list(lora) if lora is not None else [None] * len(groups)
+        xlora = list(extra_lora) if extra_lora is not None else [None] * len(extra)
 
         def seqlen(g):
             n = (1 if g.get("clip") is not None else 0)
@@ -551,17 +556,20 @@ class Paella(nn.Module):
             ci = g.get("clip_image")
             ts += list(ci) if isinstance(ci, (list, tuple)) else [ci]
             return all(bool((t == t[:1]).all()) for t in ts if t is not None)
-        shared = [uniform(g) for g in groups]
+        shared = [uniform(g) and (ent is None or all(e == ent[0] for e in ent)) for g, ent in zip(groups, glora)]
         slots = sum(1 if sh else g["byt5"].shape[0] for g, sh in zip(groups, shared))
         extra_slot = slots
         if extra:
             from .engine import cond_layout
-            runs = []          # consecutive extra prompts of one layout: one projection, as groups of batch > 1
-            for g in extra:
+            runs, run_lora = [], []      # consecutive extra prompts of one layout: one projection, as groups of batch > 1
+            for g, e in zip(extra, xlora):
                 if runs and cond_layout(g) == cond_layout(runs[-1][0]):
                     runs[-1].append(g)
+                    run_lora[-1].append(e)
                 else:
                     runs.append([g])
+                    run_lora.append([e])
+            glora += [ent if any(e is not None for e in ent) else None for ent in run_lora]
             for run in runs:
                 ci = run[0].get("clip_image")
                 groups = list(groups) + [{
@@ -580,8 +588,10 @@ class Paella(nn.Module):
             off = 0
             keep = []
             slot_of = []
-            for g, sh in zip(groups, shared):
+            for g, sh, ent in zip(groups, shared, glora):
                 n_g = g["byt5"].shape[0]
+                if ent is not None and sh:
+                    ent = ent[:1]
                 if sh:
                     ci = g.get("clip_image")
                     g = {"byt5": g["byt5"][:1], "clip": g["clip"][:1] if g.get("clip") is not None else None,
@@ -604,8 +614,15 @@ class Paella(nn.Module):
                     ci = ci.contiguous()
                     cond.clip_image, cond.n_clip_image = ptr(ci).value, ci.shape[0]
                 keep += [byt5, clip, ci]
-                check(L.pb200_paella_prepare_cond(self._handle, ctypes.byref(cond), B, off, slots, s_max, ptr(cache), ptr(ws),
-                                                  ws.numel(), current_stream()), "pb200_paella_prepare_cond")
+                if ent is not None and any(e is not None for e in ent):
+                    adapters, ids_d, scales_d = ops.lora_rows_to_device(ent, dev)
+                    keep += [ids_d, scales_d]
+                    check(L.pb200_paella_prepare_cond_lora(self._handle, ctypes.byref(cond), B, off, slots, s_max, ptr(cache), ptr(ws),
+                                                           ws.numel(), ops.lora_structs(adapters), len(adapters), ptr(ids_d),
+                                                           ptr(scales_d), current_stream()), "pb200_paella_prepare_cond_lora")
+                else:
+                    check(L.pb200_paella_prepare_cond(self._handle, ctypes.byref(cond), B, off, slots, s_max, ptr(cache), ptr(ws),
+                                                      ws.numel(), current_stream()), "pb200_paella_prepare_cond")
                 off += B
             identity = slots == bt and not extra          # (extra slots: slots may equal bt with a shared group)
             slot_map = None if identity else torch.tensor(slot_of[:bt] + [extra_slot + k for k in tail], dtype=torch.int32, device=dev)
@@ -656,7 +673,7 @@ class Paella(nn.Module):
                  attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None,
                  w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None,
                  wrap: Optional[torch.Tensor] = None, regional=None, tail_src: Optional[torch.Tensor] = None,
-                 maps=None, inject: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 maps=None, inject: Optional[torch.Tensor] = None, lora=None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
@@ -686,7 +703,10 @@ class Paella(nn.Module):
         ``inject``: prompt-to-prompt injection, a device int32 [n] (n <= B): sample b < n of x with a = inject[b] >= 0 (-1: none)
         attends in every AttnBlock with sample a's attention probabilities and its own values and attn_weights
         (pb200_paella_features_inject).  Sample a and sample b must have the same conditioning length and no regions.  Every
-        other row is that of the call without it, bit for bit.  None launches exactly the kernels without it."""
+        other row is that of the call without it, bit for bit.  None launches exactly the kernels without it.
+        ``lora``: LoRA adapters (lora_device): sample b of x runs every AttnBlock's in_proj and out_proj under its adapter and
+        scale, and so does each tail row under its source's (pb200_paella_features_lora).  Rows without an adapter are those of
+        the call without it, bit for bit.  None launches exactly the kernels without it."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -729,10 +749,10 @@ class Paella(nn.Module):
                         or w_len.numel() != attn_weights.shape[0] or (w_row is not None and w_row.numel() < attn_weights_batch):
                     raise PaellaB200Error("features: a per-sample weight table is float32 [rows, w_ld] with int32 w_len [rows] "
                                           "and an optional int32 w_row [attn_weights_batch]")
-                if regional is not None or tail_src is not None or maps is not None or inject is not None:
+                if regional is not None or tail_src is not None or maps is not None or inject is not None or lora is not None:
                     self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(attn_weights), 0, attn_weights.shape[1], ptr(w_len),
                                                                             ptr(w_row)), attn_weights_batch, wrap, regional, feats, ws,
-                                            tail_src, maps, inject)
+                                            tail_src, maps, inject, lora)
                     return feats
                 if wrap is not None:
                     check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -746,9 +766,9 @@ class Paella(nn.Module):
                                                        current_stream()), "pb200_paella_features_weighted")
                 return feats
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
-            if regional is not None or tail_src is not None or maps is not None or inject is not None:
+            if regional is not None or tail_src is not None or maps is not None or inject is not None or lora is not None:
                 self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(aw), aw.numel() if aw is not None else 0, 0, None, None),
-                                        attn_weights_batch, wrap, regional, feats, ws, tail_src, maps, inject)
+                                        attn_weights_batch, wrap, regional, feats, ws, tail_src, maps, inject, lora)
                 return feats
             if wrap is not None:        # the single weight vector is the weighted call with w_ld = 0 and no w_len
                 check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -763,9 +783,10 @@ class Paella(nn.Module):
         return feats
 
     def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws, tail_src=None, maps=None,
-                           inject=None):
+                           inject=None, lora=None):
         """pb200_paella_features_regional, or with ``tail_src`` pb200_paella_features_tail, or with ``maps``
-        pb200_paella_features_maps, or with ``inject`` pb200_paella_features_inject (``regional`` may then be None)."""
+        pb200_paella_features_maps, or with ``inject`` pb200_paella_features_inject, or with ``lora`` pb200_paella_features_lora
+        (``regional`` may then be None)."""
         mask = region_slot = mask_row = None
         if regional is not None:
             mask, region_slot, mask_row = regional
@@ -778,6 +799,20 @@ class Paella(nn.Module):
         if w_batch > Bt - n_pairs:
             raise PaellaB200Error(f"features: {w_batch} weighted samples of {Bt - n_pairs}")
         n_regions = region_slot.shape[1] if region_slot is not None else 0
+        if lora is not None:
+            structs, n_adapters, ids, scales = lora
+            if ids.numel() != Bt - n_pairs or scales.numel() != Bt - n_pairs:
+                raise PaellaB200Error(f"features: LoRA tables of {ids.numel()} samples for {Bt - n_pairs}")
+            map_row, map_batch, acc = maps if maps is not None else (None, 0, None)
+            check(lib().pb200_paella_features_lora(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                   ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
+                                                   ptr(mask_row), ptr(region_slot), n_regions, ptr(tail_src), ptr(map_row), map_batch,
+                                                   ptr(acc), acc.shape[0] if acc is not None else 0,
+                                                   acc.shape[1] if acc is not None else 0, ptr(inject),
+                                                   inject.numel() if inject is not None else 0, structs, n_adapters, ptr(ids),
+                                                   ptr(scales), ptr(feats), ptr(ws), ws.numel(), current_stream()),
+                  "pb200_paella_features_lora")
+            return
         if inject is not None:
             map_row, map_batch, acc = maps if maps is not None else (None, 0, None)
             check(lib().pb200_paella_features_inject(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -1054,11 +1089,11 @@ class Paella(nn.Module):
         table, lens = ops.attn_weights_table(attn_weights, batch, [self.max_attn_weights(latent_hw, cond_len)] * batch)
         return ops.attn_weights_to_device(table, lens, self._device())
 
-    def write_conditioning(self, cache: ConditioningCache, slot: int, inputs: Dict[str, torch.Tensor], latent_hw) -> None:
+    def write_conditioning(self, cache: ConditioningCache, slot: int, inputs: Dict[str, torch.Tensor], latent_hw, lora=None) -> None:
         """Project the conditioning of B samples (``inputs`` with batch B, one sequence layout) into slots [slot, slot + B)
         of an existing cache, as prepare_conditioning projects a group; each slot's kv_len becomes this sequence's length, so
-        rows left over from a longer sequence are never attended to.  Host-to-device copies are asynchronous (no stream
-        synchronisation)."""
+        rows left over from a longer sequence are never attended to.  ``lora``: None or B entries (None or (adapter, scale)), the
+        adapter each slot is projected under.  Host-to-device copies are asynchronous (no stream synchronisation)."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -1077,6 +1112,12 @@ class Paella(nn.Module):
                 cond.clip_image, cond.n_clip_image = ptr(ci).value, ci.shape[0]
             B = byt5.shape[0]
             ws = self._ws(L.pb200_paella_workspace_bytes(self._handle, B, latent_hw[0], latent_hw[1], cache.s_max))
+            if lora is not None and any(e is not None for e in lora):
+                adapters, ids_d, scales_d = ops.lora_rows_to_device(lora, dev)
+                check(L.pb200_paella_prepare_cond_lora(self._handle, ctypes.byref(cond), B, slot, cache.slots, cache.s_max,
+                                                       ptr(cache.cache), ptr(ws), ws.numel(), ops.lora_structs(adapters), len(adapters),
+                                                       ptr(ids_d), ptr(scales_d), current_stream()), "pb200_paella_prepare_cond_lora")
+                return
             check(L.pb200_paella_prepare_cond(self._handle, ctypes.byref(cond), B, slot, cache.slots, cache.s_max, ptr(cache.cache),
                                               ptr(ws), ws.numel(), current_stream()), "pb200_paella_prepare_cond")
 
@@ -1103,7 +1144,12 @@ class Paella(nn.Module):
         probabilities over [self ; conditioning] keys (from a's queries and keys), times its own attn_weights, applied to its own
         values.  Every other sample's logits are those of the call without it, bit for bit.  ValueError, before anything is
         enqueued, for a bad entry, a source that is itself injected, and prompt_regions on an injected sample or its source
-        (ops.attention_source_table)."""
+        (ops.attention_source_table).
+        ``lora``: LoRA adapters (keyword only; paella_b200.lora.load_lora): None, an adapter or (adapter, scale) for every sample,
+        or a list or tuple of B entries, each None, an adapter or (adapter, scale).  Sample b is then the reference model with
+        W + scale * (alpha / r) * B A on its adapter's targets (every AttnBlock's in_proj, out_proj and kv_mapper), conditioning
+        included.  Samples without an adapter, or at scale 0, get the logits of the call without it, bit for bit.  ValueError,
+        before anything is enqueued, for a bad entry or scale and an adapter of another configuration or device (ops.lora_table)."""
         if x_cat is not None:
             x = torch.cat([x, x_cat], dim=1)
         attn_weights = kwargs.pop("attn_weights", None)
@@ -1111,6 +1157,7 @@ class Paella(nn.Module):
         prompt_regions = kwargs.pop("prompt_regions", None)
         attention_maps = ops.check_attention_maps(kwargs.pop("attention_maps", False), prompt_regions)
         attention_source = kwargs.pop("attention_source", None)
+        lora = kwargs.pop("lora", None)
         if kwargs:
             raise TypeError(f"unexpected keyword arguments {sorted(kwargs)}")
         B, H, W = x.shape
@@ -1118,29 +1165,35 @@ class Paella(nn.Module):
         regions = ops.regional_table(prompt_regions, B, (H, W), self._device())
         ops.check_regions_unweighted(regions, attn_weights)
         inject = ops.attention_source_table(attention_source, B, 1, regions, forward=True)
+        lora_t = ops.lora_table(lora, B, self)
         cond_len = self.conditioning_seq_len({"byt5": byt5, "clip": clip, "clip_image": clip_image})
         aw, w_len = self._attn_weights_table(attn_weights, B, (H, W), cond_len)
         regional = None
-        if regions is None:
+        if regions is None and lora_t is None:
             cond = self._cond_for_forward(byt5, clip, clip_image, (H, W))
         else:
+            entries = ops.lora_entries(lora_t, B)
             cond = self.prepare_conditioning([{"byt5": byt5, "clip": clip, "clip_image": clip_image}], (H, W), share_uniform=False,
-                                             extra=[g for own in regions[1] for g in own])
-            regional = self.regional_device(regions, cond)
+                                             extra=[g for own in regions[1] for g in own] if regions is not None else [],
+                                             lora=[entries] if lora_t is not None else None,
+                                             extra_lora=[entries[b] for b, own in enumerate(regions[1]) for _ in own]
+                                             if regions is not None else None)
+            regional = self.regional_device(regions, cond) if regions is not None else None
         if wrap is not None:
             wrap = ops.to_device_async(wrap, self._device())
         if inject is not None:
             inject = ops.to_device_async(inject[0], self._device())
         acc = self.map_accumulator(B, cond_len, (H, W)) if attention_maps else None
         feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len, wrap=wrap, regional=regional,
-                              maps=(None, B, acc) if attention_maps else None, inject=inject)
+                              maps=(None, B, acc) if attention_maps else None, inject=inject,
+                              lora=ops.lora_device(lora_t, self._device()))
         logits = self.logits_from_features(feats, B, H, W)
         if attention_maps:
             return logits, self.finalize_attention_maps(acc, (H, W), cond_len, 1)
         return logits
 
     def token_scores(self, x, r, targets, byt5, clip=None, clip_image=None, *, label_smoothing=0.0, cfg=None,
-                     unconditional_inputs=None, attn_weights=None, tiling=None, prompt_regions=None) -> TokenScores:
+                     unconditional_inputs=None, attn_weights=None, tiling=None, prompt_regions=None, lora=None) -> TokenScores:
         """How likely the denoiser finds ``targets`` given the noised tokens ``x`` at noise level ``r``: per token the statistics
         of train.py's objective (src/train.py:36,64,71), from one fused out_mapper + log-softmax kernel whose logits never reach
         HBM (pb200_paella_token_scores).  Returns TokenScores(nll, loss, argmax):
@@ -1152,14 +1205,15 @@ class Paella(nn.Module):
         only.  ``cfg``: None (the conditional logits), a number, or a CPU tensor [B] of per-sample scales: each sample is then
         scored under the guided logits u + cfg (c - u) of the CFG pair batch the sampling loop builds, the distribution sample()
         draws from at temperature 1, with ``unconditional_inputs`` (default: zeros like the conditioning, as in sample_notebook).
-        ``attn_weights``, ``tiling`` and ``prompt_regions`` mean what they mean in ``forward`` and apply to the conditional rows.
-        ValueError, before anything is enqueued, for bad targets, an eps outside [0, 1] and a bad cfg, attn_weights, tiling or
-        prompt_regions; TypeError for any other keyword argument."""
+        ``attn_weights``, ``tiling`` and ``prompt_regions`` mean what they mean in ``forward`` and apply to the conditional rows;
+        ``lora`` means what it means in ``forward`` and applies to the sample's conditional and unconditional rows.
+        ValueError, before anything is enqueued, for bad targets, an eps outside [0, 1] and a bad cfg, attn_weights, tiling,
+        prompt_regions or lora; TypeError for any other keyword argument."""
         B, H, W = x.shape
         eps = ops.check_label_smoothing(label_smoothing)
         self._check_score_targets(targets, x.shape)
         setup = self._score_setup(B, (H, W), {"byt5": byt5, "clip": clip, "clip_image": clip_image}, unconditional_inputs, cfg,
-                                  attn_weights, tiling, prompt_regions)
+                                  attn_weights, tiling, prompt_regions, lora)
         return self._score_tokens(setup, x, r, targets, eps)
 
     def _check_score_targets(self, targets, shape, name: str = "targets") -> None:
@@ -1168,7 +1222,8 @@ class Paella(nn.Module):
             got = f"{targets.dtype} {list(targets.shape)} on {targets.device}" if torch.is_tensor(targets) else type(targets).__name__
             raise ValueError(f"{name}: expected int64 codes of shape {list(shape)} on {self._device()} (got {got})")
 
-    def _score_setup(self, batch: int, latent_hw, model_inputs, unconditional_inputs, cfg, attn_weights, tiling, prompt_regions):
+    def _score_setup(self, batch: int, latent_hw, model_inputs, unconditional_inputs, cfg, attn_weights, tiling, prompt_regions,
+                     lora=None):
         """token_scores' per-call state, reused by every forward of utils.score: validates the arguments (ValueError before
         anything is enqueued), then builds the conditioning and the device tables of the conditional rows."""
         H, W = int(latent_hw[0]), int(latent_hw[1])
@@ -1176,6 +1231,7 @@ class Paella(nn.Module):
         wrap = ops.tiling_table(tiling, batch)
         regions = ops.regional_table(prompt_regions, batch, (H, W), self._device())
         ops.check_regions_unweighted(regions, attn_weights)
+        lora_t = ops.lora_table(lora, batch, self)
         cond_len = self.conditioning_seq_len(model_inputs)
         w_table = None
         if isinstance(attn_weights, (list, tuple)):
@@ -1189,13 +1245,17 @@ class Paella(nn.Module):
             aw, w_len = ops.attn_weights_to_device(*w_table, dev)
         extra = [g for own in regions[1] for g in own] if regions is not None else []
         regional = None
-        if params is None and regions is None:
+        if params is None and regions is None and lora_t is None:
             cond = self._cond_for_forward(model_inputs["byt5"], model_inputs.get("clip"), model_inputs.get("clip_image"), (H, W))
         else:
             groups = [model_inputs] + ([unconditional_inputs] if params is not None else [])
-            cond = self.prepare_conditioning(groups, (H, W), extra=extra)
+            entries = ops.lora_entries(lora_t, batch)
+            cond = self.prepare_conditioning(groups, (H, W), extra=extra, lora=[entries] * len(groups) if lora_t is not None else None,
+                                             extra_lora=[entries[b] for b, own in enumerate(regions[1]) for _ in own]
+                                             if regions is not None else None)
             regional = self.regional_device(regions, cond) if regions is not None else None
         return {"batch": batch, "hw": (H, W), "cond": cond, "aw": aw, "w_len": w_len, "regional": regional,
+                "lora": ops.lora_device(lora_t, dev),
                 "wrap": ops.to_device_async(wrap, dev) if wrap is not None else None,
                 "params": ops.to_device_async(params, dev) if params is not None else None}
 
@@ -1208,7 +1268,7 @@ class Paella(nn.Module):
         params, aw = setup["params"], setup["aw"]
         guided = params is not None
         feats = self.features(x, r, setup["cond"], aw, B if aw is not None else 0, cfg_pairs=guided, w_len=setup["w_len"],
-                              wrap=setup["wrap"], regional=setup["regional"])
+                              wrap=setup["wrap"], regional=setup["regional"], lora=setup.get("lora"))
         L, dev = lib(), self._device()
         with torch.cuda.device(dev):
             nll = torch.empty(B, H, W, dtype=torch.float32, device=dev)

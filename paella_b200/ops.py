@@ -441,6 +441,116 @@ def attention_source_table(attention_source, batch: int, steps: int, regions=Non
     return table
 
 
+# ------------------------------------------------------------------ LoRA adapters
+# Each sample may run under one LoRA adapter at a scale (paella_b200/lora.py): its rows get the adapter's deltas in every AttnBlock
+# (pb200_paella_features_lora) and its conditioning slots are projected under it (pb200_paella_prepare_cond_lora).
+MAX_LORA_ADAPTERS = 32
+
+
+def _lora_entry(name: str, entry, model):
+    """None, an adapter or (adapter, scale) -> None or (adapter, scale); a scale of 0 is None.  ValueError for anything else, a
+    non-finite scale, and an adapter packed for another configuration or on another device."""
+    from .lora import LoraAdapter
+    if entry is None:
+        return None
+    if isinstance(entry, LoraAdapter):
+        adapter, scale = entry, 1.0
+    elif isinstance(entry, (list, tuple)) and len(entry) == 2 and isinstance(entry[0], LoraAdapter):
+        adapter, scale = entry
+        if isinstance(scale, bool) or not isinstance(scale, (int, float)):
+            raise ValueError(f"{name}: the scale must be a real number (got {scale!r})")
+        scale = float(scale)
+        if not math.isfinite(scale):
+            raise ValueError(f"{name}: the scale must be finite (got {scale!r})")
+    else:
+        raise ValueError(f"{name}: expected None, a LoraAdapter or an (adapter, scale) pair (got {type(entry).__name__})")
+    if adapter.config != model._cfg:
+        raise ValueError(f"{name}: the adapter was loaded for another model configuration")
+    if adapter.device != model._device():
+        raise ValueError(f"{name}: the adapter is on {adapter.device}, the model on {model._device()}")
+    return None if scale == 0.0 else (adapter, scale)
+
+
+def _is_lora_entry(lora) -> bool:
+    from .lora import LoraAdapter
+    return isinstance(lora, LoraAdapter) or (isinstance(lora, tuple) and len(lora) == 2 and isinstance(lora[0], LoraAdapter))
+
+
+def lora_table(lora, batch: int, model):
+    """``lora`` (None; an adapter or (adapter, scale) for every sample; or a list or tuple of ``batch`` such entries, each also
+    possibly None) -> None when no sample runs under an adapter, otherwise (adapters, ids, scales): the distinct adapters in order
+    of first use, int32 CPU [batch] of each sample's index into them (-1: none) and float32 CPU [batch] scales (0 where none).
+    ValueError, before anything is enqueued, for the wrong length, a bad entry or scale, an adapter of another configuration or
+    device, and more than 32 distinct adapters."""
+    if lora is None:
+        return None
+    if _is_lora_entry(lora):
+        entries = [_lora_entry("lora", lora, model)] * batch
+    elif isinstance(lora, (list, tuple)):
+        if len(lora) != batch:
+            raise ValueError(f"lora: got {len(lora)} entries for a batch of {batch} (one per sample, None for none)")
+        entries = [_lora_entry(f"lora[{b}]", e, model) for b, e in enumerate(lora)]
+    else:
+        raise ValueError(f"lora: expected None, a LoraAdapter, an (adapter, scale) pair or a list of {batch} entries "
+                         f"(got {type(lora).__name__})")
+    table = lora_rows(entries)
+    return table if table[0] else None
+
+
+def distinct_adapters(entries) -> list:
+    """The distinct adapters of per-row entries (None or (adapter, scale)), in order of first use."""
+    adapters = []
+    for e in entries:
+        if e is not None and not any(a is e[0] for a in adapters):
+            adapters.append(e[0])
+    return adapters
+
+
+def lora_rows(entries):
+    """Per-row entries (None or (adapter, scale)) -> (adapters, ids, scales): the distinct adapters in order of first use, int32 CPU
+    [rows] of each row's index into them (-1: none) and float32 CPU [rows] scales (0 where none) -- the index space of one launch's
+    adapter array.  ValueError for more than MAX_LORA_ADAPTERS distinct adapters."""
+    adapters = distinct_adapters(entries)
+    if len(adapters) > MAX_LORA_ADAPTERS:
+        raise ValueError(f"lora: {len(adapters)} distinct adapters in one call (at most {MAX_LORA_ADAPTERS})")
+    ids = torch.tensor([-1 if e is None else next(i for i, a in enumerate(adapters) if a is e[0]) for e in entries], dtype=torch.int32)
+    scales = torch.tensor([0.0 if e is None else e[1] for e in entries], dtype=torch.float32)
+    return adapters, ids, scales
+
+
+def lora_entries(table, batch: int) -> list:
+    """lora_table's result -> per sample None or (adapter, scale)."""
+    if table is None:
+        return [None] * batch
+    adapters, ids, scales = table
+    return [None if i < 0 else (adapters[i], float(s)) for i, s in zip(ids.tolist(), scales.tolist())]
+
+
+def lora_rows_to_device(entries, device):
+    """lora_rows on per-row entries, the two tables in one asynchronous copy: (adapters, device int32 ids, device float32 scales)."""
+    adapters, ids, scales = lora_rows(entries)
+    ids_d, scales_d = to_device_packed([ids, scales], device)
+    return adapters, ids_d, scales_d
+
+
+def lora_device(table, device):
+    """lora_table's result -> Paella.features' ``lora``: (HOST adapter array, its length, device int32 ids, device float32 scales),
+    the two tables in one asynchronous copy; None stays None."""
+    if table is None:
+        return None
+    adapters, ids, scales = table
+    ids_d, scales_d = to_device_packed([ids, scales], device)
+    return lora_structs(adapters), len(adapters), ids_d, scales_d
+
+
+def lora_structs(adapters):
+    """The HOST pb200_lora_adapter array of a table's adapters."""
+    arr = (_lib.LoraAdapter * max(1, len(adapters)))()
+    for i, a in enumerate(adapters):
+        arr[i] = a._c
+    return arr
+
+
 # ------------------------------------------------------------------ guidance prompts
 # Each sample of a guided call may carry up to MAX_GUIDANCE_PROMPTS (inputs, weight) terms.  On a guided step with scale cfg its
 # logits are l_u + cfg * [(l_c - l_u) + sum_j w_j (l_j - l_u)], l_j being the conditional forward under term j's inputs.  The

@@ -91,6 +91,17 @@ before any generator advances, for the wrong length, a bad entry (a bool is not 
 sample, a source that is itself injected, k outside [0, steps], ``prompt_regions`` on an edit or its source, and ``exact=True``
 (ops.attention_source_table; pb200_paella_features_inject).
 
+LoRA adapters: ``lora`` (all three functions and ``score``; None, an adapter or (adapter, scale) for every sample, or a list or tuple
+of B entries, each None, an adapter or (adapter, scale)) runs sample i under its own fine-tuned adapter (paella_b200.lora.load_lora):
+sample i is the reference model with W + scale * (alpha / r) * B A on the adapter's targets, the in_proj, out_proj and kv_mapper of
+every AttnBlock, in every forward it takes part in -- its conditional, unconditional and guidance-prompt rows and the projections of
+its own, unconditional, regional and term prompts (an adapter is part of the model, not of the prompt).  Samples on different
+adapters share one denoiser batch: each row's delta comes from a segmented shrink + expand kernel after the shared GEMM
+(pb200_paella_features_lora).  Adapters draw no random numbers, so every generator ends at the same offset and the per-sample
+guarantees above hold for adapted rows too; rows without an adapter, or at scale 0, are those of the call without it, bit for bit.
+ValueError, before anything is enqueued and before any generator advances, for the wrong length, a bad entry or non-finite scale, and
+an adapter loaded for another configuration or on another device (ops.lora_table).
+
 Scoring: ``score`` asks the denoiser how likely a given token grid is under a prompt -- held-out evaluation of a checkpoint with
 train.py's objective, reranking of candidates, or picking the prompt that best explains an image.  It noises the tokens at each
 of a list of noise levels, as add_noise does, and scores each noised grid against the clean tokens with Paella.token_scores
@@ -203,13 +214,14 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
                  codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None,
-                 prompt_regions=None, guidance_prompts=None, attention_maps=False, attention_source=None):
+                 prompt_regions=None, guidance_prompts=None, attention_maps=False, attention_source=None, lora=None):
     """Returns (tokens, intermediates, maps or None).  ``modes``: None, or per step the list of B mode names (sampling_modes) --
     a step whose modes differ samples each row in its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the
     scalar path in that mode.  ``top_k`` / ``top_p``: the truncation of the multinomial draws (module docstring); a truncating
     call takes the per-sample table path, and so does a call with ``guidance_prompts`` (module docstring).  ``attention_maps``:
     the maps of the conditional rows (module docstring).  ``attention_source``: prompt-to-prompt injection (module docstring);
-    step i passes row i of the table to the denoiser, or nothing when no sample is injected there."""
+    step i passes row i of the table to the denoiser, or nothing when no sample is injected there.  ``lora``: per-sample LoRA
+    adapters (module docstring)."""
     B, H, W = latent_shape
     dev = model._device()
     attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
@@ -221,7 +233,10 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     terms = ops.guidance_table(guidance_prompts, B)
     inj = ops.attention_source_table(attention_source, B, steps, regions, exact)
     inj_steps = [bool((row >= 0).any()) for row in inj] if inj is not None else [False] * steps
+    lora_t = ops.lora_table(lora, B, model)
+    entries = ops.lora_entries(lora_t, B)
     extra = [g for own in regions[1] for g in own] if regions is not None else []
+    extra_lora = [entries[b] for b, own in enumerate(regions[1]) for _ in own] if regions is not None else []
     if exact and trunc is not None:
         raise ValueError("exact=True restates the reference op for op, which has no top_k / top_p truncation")
     use_cfg_any = cfgs is not None
@@ -243,6 +258,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             term_src += [b] * len(terms[b])
             k += len(terms[b])
         extra = extra + [inputs for b in comp for inputs, _ in terms[b]]
+        extra_lora = extra_lora + [entries[b] for b in comp for _ in terms[b]]
         n_guided = min(steps, sampling_conditional_steps)
         step_cfgs = [[(cfgs[b] if per_sample_cfg else cfgs)[i] for b in comp] for i in range(n_guided)]
         mix_rows, mix_coef = ops.guidance_mix_table([[w for _, w in terms[b]] for b in comp], comp, [B + b for b in comp], term_rows,
@@ -288,10 +304,15 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             t_list = torch.linspace(t_start, t_end, steps + 1)
             temperatures = torch.linspace(temperature[0], temperature[1], steps)
         groups = [model_inputs] + ([unconditional_inputs] if use_cfg_any else [])
+        # an adapter is part of the model: a sample's unconditional, regional and term prompts are projected under its adapter
+        glora = [entries] * len(groups) if lora_t is not None else None
+        xlora = extra_lora if lora_t is not None else None
         # with guidance prompts the guided batch is [B conditional; B unconditional; term rows by sample, then term]
-        cond_full = model.prepare_conditioning(groups, (H, W), extra=extra, tail=mix[1] if mix is not None else ())
+        cond_full = model.prepare_conditioning(groups, (H, W), extra=extra, tail=mix[1] if mix is not None else (), lora=glora,
+                                               extra_lora=xlora)
         regional_full = model.regional_device(regions, cond_full) if regions is not None else None
         extra_only = extra[:len(extra) - len(mix[1])] if mix is not None else extra
+        lora_d = ops.lora_device(lora_t, dev)
         cond_only = regional_only = None
         # attention maps: the conditional rows [0, B) accumulate into rows [0, B), finalized once after the loop
         maps_len = model.conditioning_seq_len(model_inputs) if attention_maps else 0
@@ -309,7 +330,8 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                 cond, tokens = cond_full, sampled          # one (tokens, r) per CFG pair, see Paella.features
             elif use_cfg_any:
                 if cond_only is None:
-                    cond_only = model.prepare_conditioning([model_inputs], (H, W), extra=extra_only)
+                    cond_only = model.prepare_conditioning([model_inputs], (H, W), extra=extra_only, lora=glora[:1] if glora else None,
+                                                           extra_lora=xlora[:len(extra_only)] if xlora is not None else None)
                     regional_only = model.regional_device(regions, cond_only) if regions is not None else None
                 cond, tokens = cond_only, sampled
             else:
@@ -323,7 +345,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided and not composed,
                                    w_len=w_len, wrap=wrap_d, regional=regional_only if cond is cond_only else regional_full,
                                    tail_src=tail_d if composed else None, maps=(None, B, acc) if attention_maps else None,
-                                   inject=inj_d[i] if inj_steps[i] else None)
+                                   inject=inj_d[i] if inj_steps[i] else None, lora=lora_d)
             if composed:
                 model.guidance_mix(feats, H * W, mix_rows_d, mix_coef_d[i])
             if step_modes is not None:
@@ -416,14 +438,14 @@ Scores = namedtuple("Scores", ["nll", "loss", "acc", "nll_map"])
 
 
 def score(model, tokens, model_inputs, unconditional_inputs=None, levels=None, cfg=None, label_smoothing=0.0, generator=None,
-          region=None, attn_weights=None, tiling=None, prompt_regions=None) -> Scores:
+          region=None, attn_weights=None, tiling=None, prompt_regions=None, lora=None) -> Scores:
     """The Monte-Carlo denoising score of ``tokens`` (int64 [B, H, W] on the model's device) under ``model_inputs``.
 
     For each noise level t_k of ``levels`` in order (default torch.linspace(1.0, 0.0, 9)[:8], the levels at which an 8-step
     sample() calls the model) the tokens are noised with exactly the draws of ``model.add_noise(tokens, t_k * ones(B),
     generator=generator)`` -- a mask, then the replacement codes, on the default CUDA generator, one generator, or per sample on
     a list of B -- and the noised grid is scored against ``tokens`` by ``model.token_scores`` at r = t_k, with ``cfg``,
-    ``unconditional_inputs``, ``label_smoothing``, ``attn_weights``, ``tiling`` and ``prompt_regions`` as there.  ``region`` (bool
+    ``unconditional_inputs``, ``label_smoothing``, ``attn_weights``, ``tiling``, ``prompt_regions`` and ``lora`` as there.  ``region`` (bool
     [B, H, W] on the CPU or the model's device) keeps the tokens outside it from ever being noised (add_noise's ``src=tokens,
     region=region``) and restricts the means to the tokens inside it.
 
@@ -433,7 +455,7 @@ def score(model, tokens, model_inputs, unconditional_inputs=None, levels=None, c
     tokens, prompt and seed get equal scores where the forward is batch-invariant (DESIGN.md §3), so per-sample generators
     seeded alike compare prompts on common noise.  ValueError, before anything is enqueued and before any generator advances,
     for tokens that are not int64 [B, H, W] on the model's device, bad levels, an eps outside [0, 1], and a bad cfg,
-    generator list, region, attn_weights, tiling or prompt_regions."""
+    generator list, region, attn_weights, tiling, prompt_regions or lora."""
     dev = model._device()
     if not torch.is_tensor(tokens) or tokens.dim() != 3:
         raise ValueError("tokens: expected int64 codes [B, H, W] on the model's device")
@@ -445,7 +467,7 @@ def score(model, tokens, model_inputs, unconditional_inputs=None, levels=None, c
         ops.check_generators(generator, B, dev)
         ops.check_per_sample_numel(H * W)
     check_region(region, tokens, tokens.shape, dev)
-    setup = model._score_setup(B, (H, W), model_inputs, unconditional_inputs, cfg, attn_weights, tiling, prompt_regions)
+    setup = model._score_setup(B, (H, W), model_inputs, unconditional_inputs, cfg, attn_weights, tiling, prompt_regions, lora)
     region_d = region.to(dev) if region is not None else None
     nll_sum = loss_sum = hits = None
     for t_k in levels:
@@ -507,7 +529,7 @@ def _decode_tail(tokens, decode, decode_output, tiling=None):
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
            cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
            top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None, attention_maps=False,
-           attention_source=None):
+           attention_source=None, lora=None):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -525,7 +547,8 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     wrong length or a tensor.  ``prompt_regions`` (module docstring): regional prompts per sample.  ``guidance_prompts`` (module
     docstring): weighted extra and negative prompts per sample in the guided mix; a sample with terms needs a cfg other than 0.
     ``attention_maps=True`` (module docstring): returns (tokens or images, maps).  ``attention_source`` (module docstring):
-    prompt-to-prompt edits of other samples of the call; give each edit its own generator seeded like its source's."""
+    prompt-to-prompt edits of other samples of the call; give each edit its own generator seeded like its source's.
+    ``lora`` (module docstring): a LoRA adapter per sample, or one for every sample."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     per_sample_cfg = torch.is_tensor(cfg)
     terms = ops.guidance_table(guidance_prompts, latent_shape[0])
@@ -545,7 +568,7 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
                                 temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
                                 per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling,
                                 prompt_regions=prompt_regions, guidance_prompts=guidance_prompts, attention_maps=attention_maps,
-                                attention_source=attention_source)
+                                attention_source=attention_source, lora=lora)
     out = _decode_tail(out, decode, decode_output, tiling)
     return (out, maps) if attention_maps else out
 
@@ -553,7 +576,7 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
                        exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None,
-                       guidance_prompts=None, attention_maps=False, attention_source=None):
+                       guidance_prompts=None, attention_maps=False, attention_source=None, lora=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
@@ -564,7 +587,9 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     what rows [lo, hi) compute.  ``prompt_regions`` (module docstring) likewise: a shard given ``prompt_regions[lo:hi]`` computes
     what rows [lo, hi) compute.  ``guidance_prompts`` (module docstring) likewise: a shard given ``guidance_prompts[lo:hi]``
     computes what rows [lo, hi) compute.  ``attention_maps=True`` (module docstring): returns (tokens, maps) for the shard's rows.
-    ``attention_source`` (module docstring): a source and its edits sit in the same shard, with indices relative to the shard."""
+    ``attention_source`` (module docstring): a source and its edits sit in the same shard, with indices relative to the shard.
+    ``lora`` (module docstring): a shard given ``lora[lo:hi]`` computes what rows [lo, hi) compute; each rank loads its adapters
+    itself (load_lora)."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -575,7 +600,7 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
                                 temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
                                 generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
                                 tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts,
-                                attention_maps=attention_maps, attention_source=attention_source)
+                                attention_maps=attention_maps, attention_source=attention_source, lora=lora)
     return (out, maps) if attention_maps else out
 
 
@@ -583,7 +608,7 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
                     generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
-                    attention_maps=False, attention_source=None):
+                    attention_maps=False, attention_source=None, lora=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -601,7 +626,7 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     have ``attn_weights``.  ``guidance_prompts`` as in ``sample``: the argmax and quant steps of a sample with terms see its mixed
     features, and ``attn_weights`` weight its conditional row only.  ``attention_maps=True`` (module docstring): returns
     (sampled, intermediate_images, maps).  ``attention_source`` (module docstring): prompt-to-prompt edits; an edit's
-    ``attn_weights`` reweight the replayed probabilities."""
+    ``attn_weights`` reweight the replayed probabilities.  ``lora`` (module docstring): a LoRA adapter per sample."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -622,5 +647,5 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                                                 per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes, top_k=top_k,
                                                 top_p=top_p, tiling=tiling, prompt_regions=prompt_regions,
                                                 guidance_prompts=guidance_prompts, attention_maps=attention_maps,
-                                                attention_source=attention_source)
+                                                attention_source=attention_source, lora=lora)
     return (sampled, intermediates, maps) if attention_maps else (sampled, intermediates)
