@@ -289,6 +289,18 @@ int pb200_attention_inject(const void* qkv16, const void* ckv16, const int* kv_l
                            const uint8_t* q_mask, const int* region_slot, const int* mask_row, int max_regions, int mask_batch,
                            float* scores, float* lse2, const int* map_row, int map_batch, const int* inj_src, int inj_batch,
                            void* stream);
+/* Perturbed-attention guidance: pb200_attention_inject where sample b < pag_batch with bit pag_block of pag_mask[b] set (DEVICE
+ * uint64 [pag_batch]) has the self part of its attention collapsed onto the diagonal:
+ *   P = softmax(scale * q_p [K_self ; K_cond]^T) * w_b,   out[b, p] = (sum_{j in self} P_pj) V_self,p + sum_{k in cond} P_pk V_cond,k
+ * The conditioning probabilities are unchanged; with no conditioning keys out[b, p] = V_self,p.  A perturbed sample is not
+ * regional, injected or a source.  Every other sample gets the bits of pb200_attention_inject.  pag_batch = 0 is
+ * pb200_attention_inject, the same launch.  [perturbed-attention guidance, Ahn et al. 2024, on ref/src/modules.py Attention2D] */
+int pb200_attention_perturb(const void* qkv16, const void* ckv16, const int* kv_len, const int* kv_slot, int n_slots, void* out16,
+                            int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
+                            int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
+                            const uint8_t* q_mask, const int* region_slot, const int* mask_row, int max_regions, int mask_batch,
+                            float* scores, float* lse2, const int* map_row, int map_batch, const int* inj_src, int inj_batch,
+                            const uint64_t* pag_mask, int pag_batch, int pag_block, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Denoiser (ref/src/modules.py:109-283, ref/utils/modules.py) as an opaque handle.
@@ -521,6 +533,19 @@ int pb200_paella_features_lora(pb200_paella* m, const int64_t* tokens, const flo
                                const int* inj_src, int inj_batch, const pb200_lora_adapter* adapters, int n_adapters,
                                const int* row_adapter, const float* row_scale, float* features, void* workspace,
                                int64_t workspace_bytes, void* stream);
+/* pb200_paella_features_lora with perturbed-attention guidance: row b < pag_batch (of all batch_total rows, tail rows included)
+ * runs AttnBlock i (plan order, at most 64 AttnBlocks) as pb200_attention_perturb when bit i of pag_mask[b] is set (DEVICE uint64
+ * [pag_batch]); every other block and every other part of its forward is the row's plain forward.  A perturbed row is not
+ * regional, injected or a source.  Rows whose mask is 0 get the bits of the call without it.  pag_batch = 0 is
+ * pb200_paella_features_lora, the same launches. */
+int pb200_paella_features_pag(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                              const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                              int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
+                              const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
+                              const int* tail_src, const int* map_row, int map_batch, float* map_acc, int map_rows, int map_len,
+                              const int* inj_src, int inj_batch, const pb200_lora_adapter* adapters, int n_adapters,
+                              const int* row_adapter, const float* row_scale, const uint64_t* pag_mask, int pag_batch,
+                              float* features, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* maps fp32 [rows][s][h][w] from rows consecutive accumulator rows of pb200_paella_features_maps accumulated over n_steps
  * forwards: maps[row][j][y][x] = (1 / (n_steps * n_attn)) * sum over levels l, ascending, of

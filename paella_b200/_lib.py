@@ -115,6 +115,9 @@ SIGNATURES = {
     "pb200_attention_inject": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                        c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                        c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "pb200_attention_perturb": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                        c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                        c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "pb200_paella_create": (c_int, [POINTER(PaellaConfig), POINTER(c_void_p)]),
     "pb200_paella_destroy": (None, [c_void_p]),
     "pb200_paella_weight_bytes": (c_int64, [c_void_p]),
@@ -164,6 +167,11 @@ SIGNATURES = {
                                            c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int,
                                            POINTER(LoraAdapter), c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "pb200_paella_features_pag": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                          c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int,
+                                          POINTER(LoraAdapter), c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64,
+                                          c_void_p]),
     "pb200_paella_attention_maps_finalize": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "pb200_paella_sample_tokens_pairs": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_int64, c_void_p]),

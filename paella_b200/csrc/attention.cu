@@ -48,9 +48,12 @@ constexpr float NEG_BIG = -1e30f;
 // row also stores the scaled scores of its own conditioning keys (prompt 0's) and, at the end, its rows' log2-sum-exp, and O takes
 // the same arithmetic as the instance without maps.  INJ (the _inject instances): prompt-to-prompt injection (AttnInject); Q and
 // the K rows come from the source sample's row (self keys) or slot (its prompt 0's conditioning keys), the V rows from the
-// sample's own, so ks and vs have separate bases.
-template <int HD, bool REG, bool MAPS, bool INJ>
-__device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRegion& rg, const AttnMapOut& mo, const AttnInject& inj) {
+// sample's own, so ks and vs have separate bases.  PERTURB (the _perturb instances): perturbed-attention guidance (AttnPerturb); a
+// perturbed sample's self keys (those before the chunk walk's first conditioning key) add their weighted P to a per-thread running
+// self mass and enter P V as zeros, and the store adds mass * V_self of the query's own row before the division.
+template <int HD, bool REG, bool MAPS, bool INJ, bool PERTURB = false>
+__device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRegion& rg, const AttnMapOut& mo, const AttnInject& inj,
+                                               const AttnPerturb& pt = AttnPerturb{}) {
     constexpr int LDS = HD + 8;           // padded row: (HD+8)*2 bytes is an odd multiple of 16 -> conflict-free ldmatrix
     constexpr int CPR = HD / 8;           // 16-byte chunks per row
     constexpr int QROWS = ATT_BM;
@@ -71,6 +74,7 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
     const int n_cond = p.kv_len ? p.kv_len[slot] : p.S_max;
     const int Nk = n_self + n_cond;
     const int mr = MAPS ? attn_map_row(mo, b) : -1;
+    const bool pert = PERTURB && attn_perturbed(pt, b);        // CTA-uniform
     const __half* qkv_b = p.qkv + (int64_t)b * p.P * ldq;
     const __half* ckv_b = p.ckv + (int64_t)slot * p.S_max * ldc;
     const int qb = INJ ? attn_inj_src(inj, b) : b;            // the sample whose Q and K this one uses
@@ -156,6 +160,7 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
 #pragma unroll
     for (int i = 0; i < HD / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
     float m_run[2] = {NEG_BIG, NEG_BIG}, l_run[2] = {0.f, 0.f};
+    float mass[2] = {0.f, 0.f};                               // PERTURB: this thread's share of the running self mass
 
     const float* w_row = nullptr;
     const int n_w = attn_weight_row(p, b, w_row);
@@ -266,6 +271,23 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
                 }
             }
         }
+        if constexpr (PERTURB) {
+            if (pert) {
+                mass[0] *= corr[0];
+                mass[1] *= corr[1];
+                const int self_end = REG ? from : n_self;      // keys before it are self keys
+                if (j0 < self_end) {
+#pragma unroll
+                    for (int nt = 0; nt < ATT_BN / 8; ++nt)
+#pragma unroll
+                        for (int e = 0; e < 4; ++e)
+                            if (j0 + nt * 8 + 2 * t + (e & 1) < self_end) {
+                                mass[e >> 1] += s[nt][e];
+                                s[nt][e] = 0.f;
+                            }
+                }
+            }
+        }
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
             rs[r] += __shfl_xor_sync(0xffffffffu, rs[r], 1);
@@ -325,12 +347,32 @@ __device__ __forceinline__ void attention_body(const AttnParams& p, const AttnRe
     }
     cp_async_wait<0>();
     // ---- normalise and store
+    if constexpr (PERTURB) {
+        if (pert) {
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                mass[r] += __shfl_xor_sync(0xffffffffu, mass[r], 1);
+                mass[r] += __shfl_xor_sync(0xffffffffu, mass[r], 2);
+            }
+        }
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         const int row = q0 + warp * 16 + g + r * 8;
         if (row < p.P) {
             const float inv = 1.0f / l_run[r];
             __half* dst = p.out + ((int64_t)b * p.P + row) * E + h * HD + 2 * t;
+            if constexpr (PERTURB) {
+                if (pert) {         // the diagonal: mass * V_self of the query's own row
+                    const __half* v = qkv_b + (int64_t)row * ldq + 2 * E + h * HD + 2 * t;
+#pragma unroll
+                    for (int nt = 0; nt < HD / 8; ++nt) {
+                        const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(v + nt * 8));
+                        o[nt][2 * r] = fmaf(mass[r], vf.x, o[nt][2 * r]);
+                        o[nt][2 * r + 1] = fmaf(mass[r], vf.y, o[nt][2 * r + 1]);
+                    }
+                }
+            }
 #pragma unroll
             for (int nt = 0; nt < HD / 8; ++nt)
                 *reinterpret_cast<uint32_t*>(dst + nt * 8) = pack_half2(o[nt][2 * r] * inv, o[nt][2 * r + 1] * inv);
@@ -375,13 +417,58 @@ __global__ void __launch_bounds__(128, 1) attention_kernel_regional_maps_inject(
     attention_body<HD, true, true, true>(p, rg, mo, inj);
 }
 
-int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo, const AttnInject* inj) {
+// every combination of the other flags, for the rows of the launch that are not perturbed (min blocks 1 with regions, as above)
+template <int HD, bool MAPS, bool INJ>
+__global__ void __launch_bounds__(128) attention_kernel_perturb(const AttnParams p, const AttnMapOut mo, const AttnInject inj,
+                                                                const AttnPerturb pt) {
+    attention_body<HD, false, MAPS, INJ, true>(p, AttnRegion{}, mo, inj, pt);
+}
+template <int HD, bool MAPS, bool INJ>
+__global__ void __launch_bounds__(128, 1) attention_kernel_regional_perturb(const AttnParams p, const AttnRegion rg, const AttnMapOut mo,
+                                                                            const AttnInject inj, const AttnPerturb pt) {
+    attention_body<HD, true, MAPS, INJ, true>(p, rg, mo, inj, pt);
+}
+
+template <int HD, bool REG, bool MAPS, bool INJ>
+static int launch_perturb(dim3 grid, size_t smem, cudaStream_t st, const AttnParams& p, const AttnRegion* rg, const AttnMapOut* mo,
+                          const AttnInject* inj, const AttnPerturb& pt) {
+    static DeviceOnce attr_once;
+    const AttnMapOut mo0 = mo ? *mo : AttnMapOut{};
+    const AttnInject inj0 = inj ? *inj : AttnInject{};
+    if constexpr (REG) {
+        if (attr_once.first())
+            PB_CUDA(cudaFuncSetAttribute(attention_kernel_regional_perturb<HD, MAPS, INJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attention_kernel_regional_perturb<HD, MAPS, INJ><<<grid, 128, smem, st>>>(p, *rg, mo0, inj0, pt);
+    } else {
+        if (attr_once.first())
+            PB_CUDA(cudaFuncSetAttribute(attention_kernel_perturb<HD, MAPS, INJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attention_kernel_perturb<HD, MAPS, INJ><<<grid, 128, smem, st>>>(p, mo0, inj0, pt);
+    }
+    return 0;
+}
+
+template <int HD>
+static int launch_perturb_hd(dim3 grid, size_t smem, cudaStream_t st, const AttnParams& p, const AttnRegion* rg, const AttnMapOut* mo,
+                             const AttnInject* inj, const AttnPerturb& pt) {
+    const bool r = rg != nullptr, mp = mo != nullptr, in = inj != nullptr;
+    if (r && mp && in) return launch_perturb<HD, true, true, true>(grid, smem, st, p, rg, mo, inj, pt);
+    if (r && mp) return launch_perturb<HD, true, true, false>(grid, smem, st, p, rg, mo, inj, pt);
+    if (r && in) return launch_perturb<HD, true, false, true>(grid, smem, st, p, rg, mo, inj, pt);
+    if (mp && in) return launch_perturb<HD, false, true, true>(grid, smem, st, p, rg, mo, inj, pt);
+    if (r) return launch_perturb<HD, true, false, false>(grid, smem, st, p, rg, mo, inj, pt);
+    if (mp) return launch_perturb<HD, false, true, false>(grid, smem, st, p, rg, mo, inj, pt);
+    if (in) return launch_perturb<HD, false, false, true>(grid, smem, st, p, rg, mo, inj, pt);
+    return launch_perturb<HD, false, false, false>(grid, smem, st, p, rg, mo, inj, pt);
+}
+
+int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo, const AttnInject* inj,
+                     const AttnPerturb* pt) {
     PB_CHECK(p.nhead > 0 && p.E % p.nhead == 0, "attention: E=%d not divisible by nhead=%d", p.E, p.nhead);
     const int hd = p.E / p.nhead;
     PB_CHECK(p.E % 8 == 0, "attention: E must be a multiple of 8");
     if (p.B == 0 || p.P == 0) return 0;
     {
-        const int rc = launch_attention_wgmma(p, st, rg, mo, inj);
+        const int rc = launch_attention_wgmma(p, st, rg, mo, inj, pt);
         if (rc >= 0) return rc;
     }
     // algorithmic bytes: q, self k/v, out once; conditioning k/v once per sample
@@ -400,6 +487,10 @@ int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg,
     switch (hd) {
 #define PB_ATT_CASE(H)                                                                                              \
     case H: {                                                                                                       \
+        if (pt != nullptr) {                                                                                        \
+            PB_TRY(launch_perturb_hd<H>(grid, smem, st, p, rg, mo, inj, *pt));                                      \
+            break;                                                                                                  \
+        }                                                                                                           \
         if (inj != nullptr && mo != nullptr && reg) PB_ATT_LAUNCH(attention_kernel_regional_maps_inject<H>, *rg, *mo, *inj) \
         if (inj != nullptr && mo != nullptr) PB_ATT_LAUNCH(attention_kernel_maps_inject<H>, *mo, *inj)              \
         if (inj != nullptr && reg) PB_ATT_LAUNCH(attention_kernel_regional_inject<H>, *rg, *inj)                    \

@@ -71,6 +71,21 @@ __device__ __forceinline__ int attn_inj_src(const AttnInject& inj, int b) {
     return a >= 0 ? a : b;
 }
 
+// Perturbed-attention guidance, for samples b < batch with bit `block` of block_mask[b] set (the launch's AttnBlock): the self
+// part of every query's attention collapses onto the diagonal.  The self keys enter S, the running max and the denominator as
+// usual, but their P (after attn_weights) is kept as a running self mass instead of entering P V, and mass * V_self[query] is
+// added to O before the division; the conditioning keys' P is unchanged.  A perturbed sample is never regional, injected or
+// a source.  A separate kernel argument, so the plain instances keep their code.
+struct AttnPerturb {
+    const uint64_t* block_mask;
+    int batch;
+    int block;
+};
+
+__device__ __forceinline__ bool attn_perturbed(const AttnPerturb& pt, int b) {
+    return b < pt.batch && ((pt.block_mask[b] >> pt.block) & 1ull);
+}
+
 constexpr int ATT_MAX_REGIONS = 7;      // prompts 1..7: the mask bits above prompt 0's
 
 // The key walk of a regional tile: segments of keys, each cut into 64-key chunks from its own first key.  Bit `bit` of a
@@ -143,10 +158,11 @@ __device__ __forceinline__ int attn_weight_row(const AttnParams& p, int b, const
 // (mo: the map outputs, or NULL.  With rg too, a map row's keys are its prompt 0's; its queries should all see prompt 0 alone.)
 // (inj: the injection table, or NULL.  With rg too, only samples whose queries all see prompt 0 alone may be injected or be
 // sources: an injected sample's prompt 0 keys come from its source's slot, further prompts' from their own.)
+// (pt: the perturbation table, or NULL: the _perturb instances, with every combination of rg, mo and inj for the other rows.)
 int launch_attention(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr, const AttnMapOut* mo = nullptr,
-                     const AttnInject* inj = nullptr);
+                     const AttnInject* inj = nullptr, const AttnPerturb* pt = nullptr);
 int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg = nullptr, const AttnMapOut* mo = nullptr,
-                           const AttnInject* inj = nullptr);      // 0 launched, 1 error, -1 shape not handled
+                           const AttnInject* inj = nullptr, const AttnPerturb* pt = nullptr);      // 0 launched, 1 error, -1 shape not handled
 // Attention maps (ops.cu): acc [rows][acc_ld][acc_pos] += (1/nhead) * sum over heads h in ascending order of
 // w_s * exp2(score - lse2) at columns [acc_off, acc_off + P), for every map row of p's batch and every conditioning key s < kv_len
 int launch_attention_maps_accumulate(const AttnParams& p, const AttnMapOut& mo, float* acc, int acc_ld, int acc_pos, int acc_off,

@@ -48,9 +48,13 @@ struct AttnMaps {
 // INJ (the _inject instances): prompt-to-prompt injection (AttnInject).  Q and the K boxes of every stage come from the source
 // sample's row (self keys) or slot (its prompt 0's conditioning keys), the V box from the sample's own; the bytes of a stage are
 // the same, so expect_tx is too.
-template <bool REG, bool MAPS, bool INJ>
+// PERTURB (the _perturb instances): perturbed-attention guidance (AttnPerturb).  A perturbed sample's self chunks add their
+// weighted P to a per-thread running self mass (rescaled like l_run, reduced over the quad at the end) and enter P V as zeros;
+// the store adds mass * V_self of the query's own row before the division.
+template <bool REG, bool MAPS, bool INJ, bool PERTURB = false>
 __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const AttnParams& p, const AttnRegion& rg,
-                                                     const AttnMapOut& mo, const AttnInject& inj) {
+                                                     const AttnMapOut& mo, const AttnInject& inj,
+                                                     const AttnPerturb& pt = AttnPerturb{}) {
     pdl_launch_dependents();
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -69,6 +73,7 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
     const int mr = MAPS ? attn_map_row(mo, b) : -1;
     const int qb = INJ ? attn_inj_src(inj, b) : b;                           // the sample whose Q and K this one uses
     const int kslot = INJ ? (p.kv_slot ? p.kv_slot[qb] : qb) : slot;
+    const bool pert = PERTURB && attn_perturbed(pt, b);                       // CTA-uniform
     int n_chunks = n_sc + (n_cond + AW_BN - 1) / AW_BN;
     AttnSegs* segs = reinterpret_cast<AttnSegs*>(gbase + AW_OFF_SEGS);
     auto seg_of = [&](int c) {
@@ -140,6 +145,7 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
 #pragma unroll
     for (int i = 0; i < AW_HD / 2; ++i) o[i] = 0.f;
     float m_run[2] = {-1e30f, -1e30f}, l_run[2] = {0.f, 0.f};
+    float mass[2] = {0.f, 0.f};             // PERTURB: this thread's share of the running self mass
     const uint64_t dq64 = ptx::wgmma_desc_kmajor_sw128(base);      // the warpgroup's 64 rows are the whole query tile
     const uint64_t dq16 = ptx::wgmma_desc_kmajor_sw32(base + AW_OFF_Q16);
     ptx::mbar_wait(q_bar, 0);
@@ -148,9 +154,11 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
         const int st = c & 1;
         int k0, valid, key0, lim[2];
         bool own_cond;                      // a chunk of the sample's own conditioning keys (the map's keys)
+        bool self_chunk;
         if constexpr (REG) {
             const int si = seg_of(c), bit = segs->bit[si];
             own_cond = bit == 0;
+            self_chunk = bit < 0;
             k0 = (c - segs->first[si]) * AW_BN;
             valid = min(AW_BN, segs->len[si] - k0);
             key0 = bit < 0 ? k0 : bit == 0 ? n_self + k0 : Nk;              // only [self ; prompt 0] is weighted
@@ -158,6 +166,7 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
         } else {
             const bool self = c < n_sc;
             own_cond = !self;
+            self_chunk = self;
             k0 = self ? c * AW_BN : (c - n_sc) * AW_BN;                      // first key of the chunk inside its source
             valid = min(AW_BN, (self ? n_self : n_cond) - k0);
             key0 = self ? k0 : n_self + k0;                                   // index in [self ; cond]
@@ -250,6 +259,19 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
             }
             s[i] = pv;
         }
+        if constexpr (PERTURB) {
+            if (pert) {
+                mass[0] *= corr[0];
+                mass[1] *= corr[1];
+                if (self_chunk) {
+#pragma unroll
+                    for (int i = 0; i < AW_BN / 2; ++i) {
+                        mass[(i >> 1) & 1] += s[i];
+                        s[i] = 0.f;
+                    }
+                }
+            }
+        }
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
             rs[r] += __shfl_xor_sync(0xffffffffu, rs[r], 1);
@@ -275,12 +297,32 @@ __device__ __forceinline__ void attention_wgmma_body(const AttnMaps& maps, const
     }
 
     // ---- normalise and store
+    if constexpr (PERTURB) {
+        if (pert) {
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                mass[r] += __shfl_xor_sync(0xffffffffu, mass[r], 1);
+                mass[r] += __shfl_xor_sync(0xffffffffu, mass[r], 2);
+            }
+        }
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         const int row = q0 + wq * 16 + (lane >> 2) + 8 * r;
         if (row < p.P) {
             const float inv = 1.0f / l_run[r];
             __half* dst = p.out + ((int64_t)b * p.P + row) * E + h * AW_HD + 2 * (lane & 3);
+            if constexpr (PERTURB) {
+                if (pert) {         // the diagonal: mass * V_self of the query's own row
+                    const __half* v = p.qkv + ((int64_t)b * p.P + row) * 3 * E + 2 * E + h * AW_HD + 2 * (lane & 3);
+#pragma unroll
+                    for (int n = 0; n < AW_HD / 8; ++n) {
+                        const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(v + n * 8));
+                        o[4 * n + 2 * r] = fmaf(mass[r], vf.x, o[4 * n + 2 * r]);
+                        o[4 * n + 2 * r + 1] = fmaf(mass[r], vf.y, o[4 * n + 2 * r + 1]);
+                    }
+                }
+            }
 #pragma unroll
             for (int n = 0; n < AW_HD / 8; ++n)
                 *reinterpret_cast<uint32_t*>(dst + n * 8) = pack_half2(o[4 * n + 2 * r] * inv, o[4 * n + 2 * r + 1] * inv);
@@ -323,8 +365,29 @@ __global__ void __launch_bounds__(128) attention_wgmma_kernel_regional_maps_inje
     attention_wgmma_body<true, true, true>(maps, p, rg, mo, inj);
 }
 
+// every combination of the other flags, for the rows of the launch that are not perturbed
+template <bool REG, bool MAPS, bool INJ>
+__global__ void __launch_bounds__(128) attention_wgmma_kernel_perturb(const __grid_constant__ AttnMaps maps, const AttnParams p,
+                                                                      const AttnRegion rg, const AttnMapOut mo, const AttnInject inj,
+                                                                      const AttnPerturb pt) {
+    attention_wgmma_body<REG, MAPS, INJ, true>(maps, p, rg, mo, inj, pt);
+}
+
+template <bool REG, bool MAPS, bool INJ>
+static int launch_wgmma_perturb(dim3 grid, cudaStream_t st, const AttnMaps& m, const AttnParams& p, const AttnRegion* rg,
+                                const AttnMapOut* mo, const AttnInject* inj, const AttnPerturb& pt) {
+    constexpr int smem = REG ? AW_SMEM_REG : AW_SMEM;
+    static DeviceOnce attr_once;
+    if (attr_once.first())
+        PB_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel_perturb<REG, MAPS, INJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attention_wgmma_kernel_perturb<REG, MAPS, INJ><<<grid, 128, smem, st>>>(m, p, rg ? *rg : AttnRegion{}, mo ? *mo : AttnMapOut{},
+                                                                             inj ? *inj : AttnInject{}, pt);
+    return 0;
+}
+
 // returns 0 = launched, 1 = error, -1 = shape not handled here (head_dim != 80: the caller runs the mma.sync kernel)
-int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo, const AttnInject* inj) {
+int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegion* rg, const AttnMapOut* mo, const AttnInject* inj,
+                           const AttnPerturb* pt) {
     static const bool off = getenv("PB200_ATTN_MMA_SYNC") != nullptr;      // A/B knob: the mma.sync kernel for every shape
     if (off || p.E != AW_HD * p.nhead) return -1;
     const int64_t q_rows = (int64_t)p.B * p.P;
@@ -349,7 +412,17 @@ int launch_attention_wgmma(const AttnParams& p, cudaStream_t st, const AttnRegio
         if (attr_once.first()) PB_CUDA(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM)); \
         KERNEL<<<grid, 128, SMEM, st>>>(m, p, __VA_ARGS__);                                             \
     }
-    if (inj != nullptr) {
+    if (pt != nullptr) {
+        const bool r = rg != nullptr, mp = mo != nullptr, in = inj != nullptr;
+        if (r && mp && in) PB_TRY((launch_wgmma_perturb<true, true, true>(grid, st, m, p, rg, mo, inj, *pt)));
+        else if (r && mp) PB_TRY((launch_wgmma_perturb<true, true, false>(grid, st, m, p, rg, mo, inj, *pt)));
+        else if (r && in) PB_TRY((launch_wgmma_perturb<true, false, true>(grid, st, m, p, rg, mo, inj, *pt)));
+        else if (mp && in) PB_TRY((launch_wgmma_perturb<false, true, true>(grid, st, m, p, rg, mo, inj, *pt)));
+        else if (r) PB_TRY((launch_wgmma_perturb<true, false, false>(grid, st, m, p, rg, mo, inj, *pt)));
+        else if (mp) PB_TRY((launch_wgmma_perturb<false, true, false>(grid, st, m, p, rg, mo, inj, *pt)));
+        else if (in) PB_TRY((launch_wgmma_perturb<false, false, true>(grid, st, m, p, rg, mo, inj, *pt)));
+        else PB_TRY((launch_wgmma_perturb<false, false, false>(grid, st, m, p, rg, mo, inj, *pt)));
+    } else if (inj != nullptr) {
         if (mo != nullptr && rg != nullptr) PB_AW_LAUNCH(attention_wgmma_kernel_regional_maps_inject, AW_SMEM_REG, *rg, *mo, *inj)
         else if (mo != nullptr) PB_AW_LAUNCH(attention_wgmma_kernel_maps_inject, AW_SMEM, *mo, *inj)
         else if (rg != nullptr) PB_AW_LAUNCH(attention_wgmma_kernel_regional_inject, AW_SMEM_REG, *rg, *inj)

@@ -250,4 +250,46 @@ int pb200_attention_inject(const void* qkv16, const void* ckv16, const int* kv_l
     return launch_attention(p, (cudaStream_t)stream, q_mask ? &rg : nullptr, map_batch > 0 ? &mo : nullptr, inj_batch > 0 ? &inj : nullptr);
 }
 
+int pb200_attention_perturb(const void* qkv16, const void* ckv16, const int* kv_len, const int* kv_slot, int n_slots, void* out16,
+                            int batch, int positions, int s_max, int embed, int nhead, int self_attn, const float* attn_weights,
+                            int n_weights, int weights_ld, const int* weights_len, const int* weights_row, int weighted_batch,
+                            const uint8_t* q_mask, const int* region_slot, const int* mask_row, int max_regions, int mask_batch,
+                            float* scores, float* lse2, const int* map_row, int map_batch, const int* inj_src, int inj_batch,
+                            const uint64_t* pag_mask, int pag_batch, int pag_block, void* stream) {
+    PB_CHECK(pag_batch >= 0 && pag_batch <= batch && (pag_batch == 0 || pag_mask) && pag_block >= 0 && pag_block < 64,
+             "attention: pag_batch=%d for %d samples, block %d", pag_batch, batch, pag_block);
+    if (pag_batch == 0)
+        return pb200_attention_inject(qkv16, ckv16, kv_len, kv_slot, n_slots, out16, batch, positions, s_max, embed, nhead, self_attn,
+                                      attn_weights, n_weights, weights_ld, weights_len, weights_row, weighted_batch, q_mask, region_slot,
+                                      mask_row, max_regions, mask_batch, scores, lse2, map_row, map_batch, inj_src, inj_batch, stream);
+    PB_CHECK(qkv16 && out16 && (ckv16 || s_max == 0), "attention: null pointer");
+    PB_CHECK(self_attn || s_max > 0, "attention: no keys");
+    PB_CHECK(n_slots >= 0 && weights_ld >= 0, "attention: negative slot count or weight stride");
+    PB_CHECK(q_mask == nullptr || (mask_batch >= 0 && mask_batch <= batch && max_regions >= 0 && max_regions <= ATT_MAX_REGIONS &&
+                                   (region_slot != nullptr || max_regions == 0)),
+             "attention: regional table (mask_batch=%d, max_regions=%d) for %d samples", mask_batch, max_regions, batch);
+    PB_CHECK(map_batch >= 0 && map_batch <= batch && (map_batch == 0 || (scores && lse2)), "attention: map_batch=%d for %d samples",
+             map_batch, batch);
+    PB_CHECK(inj_batch >= 0 && inj_batch <= batch && (inj_batch == 0 || inj_src), "attention: inj_batch=%d for %d samples", inj_batch,
+             batch);
+    AttnParams p{};
+    p.qkv = reinterpret_cast<const __half*>(qkv16);
+    p.ckv = reinterpret_cast<const __half*>(ckv16 ? ckv16 : qkv16);
+    p.kv_len = kv_len;
+    p.kv_slot = kv_slot;
+    p.n_slots = n_slots;
+    p.out = reinterpret_cast<__half*>(out16);
+    p.B = batch; p.P = positions; p.S_max = s_max; p.E = embed; p.nhead = nhead;
+    p.self_attn = self_attn;
+    p.scale_log2 = 1.4426950408889634f / sqrtf((float)(embed / (nhead > 0 ? nhead : 1)));
+    p.attn_w = attn_weights; p.n_w = attn_weights ? n_weights : 0; p.w_batch = weighted_batch;
+    p.w_ld = weights_ld; p.w_len = weights_len; p.w_row = weights_row;
+    const AttnRegion rg{q_mask, region_slot, mask_row, max_regions, mask_batch};
+    const AttnMapOut mo{scores, lse2, map_row, map_batch};
+    const AttnInject inj{inj_src, inj_batch};
+    const AttnPerturb pt{pag_mask, pag_batch, pag_block};
+    return launch_attention(p, (cudaStream_t)stream, q_mask ? &rg : nullptr, map_batch > 0 ? &mo : nullptr, inj_batch > 0 ? &inj : nullptr,
+                            &pt);
+}
+
 }  // extern "C"

@@ -796,7 +796,23 @@ int pb200_paella_features_lora(pb200_paella* m, const int64_t* tokens, const flo
                                const int* inj_src, int inj_batch, const pb200_lora_adapter* adapters, int n_adapters,
                                const int* row_adapter, const float* row_scale, float* features, void* workspace,
                                int64_t workspace_bytes, void* stream) {
+    return pb200_paella_features_pag(m, tokens, r, batch_total, n_tail, h, w, cond_cache, cache_slots, kv_slot, s_max, attn_w, n_w, w_ld,
+                                     w_len, w_row, w_batch, wrap, prompt_mask, mask_row, region_slot, max_regions, tail_src, map_row,
+                                     map_batch, map_acc, map_rows, map_len, inj_src, inj_batch, adapters, n_adapters, row_adapter,
+                                     row_scale, nullptr, 0, features, workspace, workspace_bytes, stream);
+}
+
+int pb200_paella_features_pag(pb200_paella* m, const int64_t* tokens, const float* r, int batch_total, int n_tail, int h, int w,
+                              const void* cond_cache, int cache_slots, const int* kv_slot, int s_max, const float* attn_w, int n_w,
+                              int w_ld, const int* w_len, const int* w_row, int w_batch, const uint8_t* wrap,
+                              const uint8_t* prompt_mask, const int* mask_row, const int* region_slot, int max_regions,
+                              const int* tail_src, const int* map_row, int map_batch, float* map_acc, int map_rows, int map_len,
+                              const int* inj_src, int inj_batch, const pb200_lora_adapter* adapters, int n_adapters,
+                              const int* row_adapter, const float* row_scale, const uint64_t* pag_mask, int pag_batch,
+                              float* features, void* workspace, int64_t workspace_bytes, void* stream) {
     PB_CHECK(m->blob != nullptr, "features: weights not bound");
+    PB_CHECK(pag_batch == 0 || (pag_mask != nullptr && pag_batch > 0 && pag_batch <= batch_total && m->n_attn <= 64),
+             "features: perturbation table of %d rows for %d rows and %d AttnBlocks (at most 64)", pag_batch, batch_total, m->n_attn);
     LoraPlan lp;
     PB_TRY(lora_plan(m, adapters, n_adapters, lp));
     PB_CHECK(!lp.any || (row_adapter != nullptr && row_scale != nullptr), "features: adapters need row_adapter and row_scale");
@@ -1011,7 +1027,9 @@ int pb200_paella_features_lora(pb200_paella* m, const int64_t* tokens, const flo
                 ap.w_ld = w_ld; ap.w_len = w_len; ap.w_row = w_row;
                 const AttnRegion rg{ws.qmask + qmask_off[l], region_slot, mask_row, max_regions, n_base};
                 const AttnInject inj{inj_src, inj_batch};
-                PB_TRY(launch_attention(ap, st, prompt_mask ? &rg : nullptr, map_batch > 0 ? &mo : nullptr, inj_batch > 0 ? &inj : nullptr));
+                const AttnPerturb pt{pag_mask, pag_batch, b.attn_index};
+                PB_TRY(launch_attention(ap, st, prompt_mask ? &rg : nullptr, map_batch > 0 ? &mo : nullptr, inj_batch > 0 ? &inj : nullptr,
+                                        pag_batch > 0 ? &pt : nullptr));
                 if (map_batch > 0) PB_TRY(launch_attention_maps_accumulate(ap, mo, map_acc, map_len, map_pos, map_off[l], st));
                 pb200_gemm_epilogue e2 = epi(PB200_EPI_RESID_F32, m->w<float>(b.outproj_b), x, ch);
                 e2.resid = x; e2.ldr = ch; e2.rows_per_sample = P;

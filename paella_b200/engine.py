@@ -47,6 +47,10 @@ K/V slots are projected under the adapter at admission, and a guided request wit
 unconditional slot, holding the engine-wide unconditional inputs projected under its adapter (the shared slot is the model's
 without an adapter); adapters draw nothing.  One step's launches take at most 32 distinct adapters (ops.MAX_LORA_ADAPTERS):
 admission holds a request whose adapter would be the 33rd in flight, and everything queued behind it, until a request retires.
+With ``pag=s`` or ``(s, blocks)`` a request gets perturbed-attention guidance as ``sample_notebook(..., pag=[entry])`` does: on each
+of its steps before sampling_conditional_steps, guided or not, one more denoiser row -- its perturbed forward, reading its own
+conditional slot, weight row, wrap byte and adapter -- follows the term rows, and its mix coefficients (c + s, ..., -s) ride in
+the step table with the row's AttnBlock mask; PAG draws nothing and needs no K/V slot.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -100,7 +104,7 @@ class Request:
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
                  region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
                  top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None, terms=None, mix_coef=None,
-                 attention_maps: bool = False, maps_len: int = 0, attention_source=None, lora=None):
+                 attention_maps: bool = False, maps_len: int = 0, attention_source=None, lora=None, pag=None):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -114,7 +118,9 @@ class Request:
         self.regional = regions is not None
         self.terms = terms                       # guidance prompts: [(inputs, weight), ...] until admission, or None
         self.n_terms = len(terms) if terms is not None else 0
-        self.mix_coef = mix_coef                 # CPU float32 [cond_steps, 2 + n_terms]: the guided steps' mix coefficients
+        self.mix_coef = mix_coef                 # CPU float32 [cond_steps, row width]: the mixed steps' coefficients (guided:
+        #                                          c, u, the terms, then -s with PAG; unguided with PAG: 1 + s, -s)
+        self.pag = pag                           # perturbed-attention guidance: (scale, int64 AttnBlock mask) or None
         self.term_slot: List[int] = []           # the K/V slots of the terms
         self.want_maps, self.maps_len = attention_maps, maps_len      # attention maps, over maps_len conditioning keys
         self.attention_maps: Optional[torch.Tensor] = None            # float32 [maps_len, H, W], set at retirement
@@ -139,24 +145,45 @@ class Request:
 
 
 class StepPlan:
-    """The host tables of one step (CPU tensors), rows in batch order: guided requests first."""
+    """The host tables of one step (CPU tensors), rows in batch order: guided requests first.  ``w_zero_row``: the weight-pool
+    row of length 0 that the unconditional and term rows of a perturbing step read."""
 
-    def __init__(self, order: List[Request]):
+    def __init__(self, order: List[Request], w_zero_row: int = -1):
         self.order = order
         self.n_pairs = sum(1 for q in order if q.guided and q.k < q.cond_steps)
-        # guidance prompts: the guided rows with terms (composed), their term rows after the unconditional rows
-        self.composed = [i for i, q in enumerate(order[:self.n_pairs]) if q.n_terms]
         Bc, n_pairs = len(order), self.n_pairs
-        J = max((order[i].n_terms for i in self.composed), default=0)
-        self.tail = torch.tensor(list(range(n_pairs)) + [i for i in self.composed for _ in range(order[i].n_terms)], dtype=torch.int32)
-        self.mix_rows = torch.full((len(self.composed), 2 + J), -1, dtype=torch.int32)
-        self.mix_coef = torch.zeros(len(self.composed), 2 + J, dtype=torch.float32)
+        # perturbed-attention guidance: the rows perturbed this step (guided or not, before their sampling_conditional_steps)
+        self.perturbed = [i for i, q in enumerate(order) if q.pag is not None and q.k < q.cond_steps]
+        pert = set(self.perturbed)
+        # guidance prompts and PAG: the composed rows -- guided rows with terms or PAG, unguided rows with PAG -- then their term
+        # rows after the unconditional rows, then their perturbed rows
+        self.composed = [i for i, q in enumerate(order) if (i < n_pairs and q.n_terms) or i in pert]
+        term_src = [i for i in self.composed if i < n_pairs for _ in range(order[i].n_terms)]
+        self.tail = torch.tensor(list(range(n_pairs)) + term_src + self.perturbed, dtype=torch.int32)
+        p_row = {i: Bc + n_pairs + len(term_src) + j for j, i in enumerate(self.perturbed)}
+        own = []
         t = Bc + n_pairs
-        for y, i in enumerate(self.composed):
+        for i in self.composed:
             q = order[i]
-            self.mix_rows[y, :2 + q.n_terms] = torch.tensor([i, Bc + i] + list(range(t, t + q.n_terms)), dtype=torch.int32)
-            self.mix_coef[y, :2 + q.n_terms] = q.mix_coef[q.k]
-            t += q.n_terms
+            if i < n_pairs:
+                own.append([i, Bc + i] + list(range(t, t + q.n_terms)) + ([p_row[i]] if i in pert else []))
+                t += q.n_terms
+            else:
+                own.append([i, p_row[i]])
+        width = max((len(o) for o in own), default=2)
+        self.mix_rows = torch.full((len(self.composed), width), -1, dtype=torch.int32)
+        self.mix_coef = torch.zeros(len(self.composed), width, dtype=torch.float32)
+        for y, (i, o) in enumerate(zip(self.composed, own)):
+            self.mix_rows[y, :len(o)] = torch.tensor(o, dtype=torch.int32)
+            self.mix_coef[y, :len(o)] = order[i].mix_coef[order[i].k]
+        n_rows = Bc + self.tail.numel()
+        self.pag_rows = torch.zeros(n_rows, dtype=torch.int64)     # each row's AttnBlock mask, 0 but on the perturbed rows
+        for i in self.perturbed:
+            self.pag_rows[p_row[i]] = order[i].pag[1]
+        # a perturbed row reads its request's weight row; the unconditional and term rows read the empty one
+        self.pag_w_row = torch.tensor([q.slot if q.slot is not None else -1 for q in order] +
+                                      [w_zero_row] * (n_rows - Bc - len(self.perturbed)) +
+                                      [order[i].slot if order[i].slot is not None else -1 for i in self.perturbed], dtype=torch.int32)
         self.r = torch.stack([q.r[q.k] for q in order])
         self.params = torch.stack([q.params[q.k] for q in order])
         self.renoise = [q.k < q.renoise_steps for q in order]
@@ -173,7 +200,8 @@ class StepPlan:
         self.t_next = torch.stack([q.r[q.k + 1] if rn else torch.tensor(-1.0) for q, rn in zip(order, self.renoise)])
         self.row_slot = torch.tensor([q.slot for q in order], dtype=torch.int32)
         self.kv_slot = torch.tensor([q.slot for q in order] + [q.uncond_slot for q in order[:self.n_pairs]] +
-                                    [s for i in self.composed for s in order[i].term_slot], dtype=torch.int32)
+                                    [s for i in self.composed if i < n_pairs for s in order[i].term_slot] +
+                                    [order[i].slot for i in self.perturbed], dtype=torch.int32)
         # attention maps: each row's accumulator row (its token slot), -1 for the rows without maps
         self.maps = any(q.want_maps for q in order)
         self.map_row = torch.tensor([q.slot if q.want_maps else -1 for q in order], dtype=torch.int32)
@@ -211,8 +239,9 @@ def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List
 def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tuple[torch.Tensor, Dict[str, Tuple[str, int, int]]]:
     """The step's one host-to-device buffer: int64 [(seed, offset) pairs of the sampler's draw, then of the mask draw], then the
     float32 part [r, params (3 per row), t_next, (top_p), (mix_coef), (lora_scale)], then the int32 part [row_slot, kv_slot, (mode
-    table), (top_k), (tail, mix_rows), (map_row), (inj_src), (lora_id)], then the uint8 part [(wrap)], each part padded to whole
-    int64 words.  top_p / top_k are present only when ``plan.truncates``, the mode table only when the step mixes modes, wrap (one
+    table), (top_k), (tail, mix_rows), (map_row), (inj_src), (lora_id), (w_row)], then the uint8 part [(wrap)], each part padded to
+    whole int64 words, then (pag): the int64 AttnBlock mask of every row, tail included, with w_row (each row's weight-pool row)
+    only when some row is perturbed this step (perturbed-attention guidance).  top_p / top_k are present only when ``plan.truncates``, the mode table only when the step mixes modes, wrap (one
     byte per row) only when ``plan.wraps``, the tail map and the mix table only when some row of the step is composed (guidance
     prompts), map_row only when some row wants attention maps, inj_src only when some edit is inside its window, lora_id and
     lora_scale only when some row has a LoRA adapter (the adapters' blob pointers travel as kernel arguments).  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
@@ -234,6 +263,8 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
     if plan.loras:
         f32_parts.append(("lora_scale", plan.lora_scale))
         i32_parts.append(("lora_id", plan.lora_id))
+    if plan.perturbed:
+        i32_parts.append(("w_row", plan.pag_w_row))
     u8_parts = [("wrap", plan.wrap)] if plan.wraps else []
     layout: Dict[str, Tuple[str, int, int]] = {}
     for dt, parts in (("f32", f32_parts), ("i32", i32_parts), ("u8", u8_parts)):
@@ -247,11 +278,14 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
     i32 = torch.cat([i32, torch.zeros(i32.numel() % 2, dtype=torch.int32)])
     u8 = torch.cat([v for _, v in u8_parts] + [torch.zeros(0, dtype=torch.uint8)])
     u8 = torch.cat([u8, torch.zeros(-u8.numel() % 8, dtype=torch.uint8)])
+    pag = plan.pag_rows if plan.perturbed else torch.zeros(0, dtype=torch.int64)
     host = torch.cat([torch.tensor(draw + renoise, dtype=torch.int64), f32.view(torch.int64), i32.view(torch.int64),
-                      u8.view(torch.int64)])
+                      u8.view(torch.int64), pag])
     layout["f32"] = ("i64", 4 * Bc, f32.numel() // 2)
     layout["i32"] = ("i64", 4 * Bc + f32.numel() // 2, i32.numel() // 2)
     layout["u8"] = ("i64", 4 * Bc + f32.numel() // 2 + i32.numel() // 2, u8.numel() // 8)
+    if plan.perturbed:
+        layout["pag"] = ("i64", 4 * Bc + f32.numel() // 2 + i32.numel() // 2 + u8.numel() // 8, pag.numel())
     return host, layout
 
 
@@ -290,11 +324,11 @@ def admit_from_queue(queue: "collections.deque[Request]", n_free: int, active: L
     return new
 
 
-def build_step_plan(active: List[Request]) -> StepPlan:
+def build_step_plan(active: List[Request], w_zero_row: int = -1) -> StepPlan:
     """Order the active requests for one step -- guided this step first, each group in admission order -- and build the
     step's tables from each request's own schedule rows at its own step index."""
     guided = [q for q in active if q.guided and q.k < q.cond_steps]
-    return StepPlan(guided + [q for q in active if not (q.guided and q.k < q.cond_steps)])
+    return StepPlan(guided + [q for q in active if not (q.guided and q.k < q.cond_steps)], w_zero_row)
 
 
 class SamplingEngine:
@@ -387,7 +421,7 @@ class SamplingEngine:
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
                sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
-               attention_maps=False, attention_source=None, lora=None) -> Request:
+               attention_maps=False, attention_source=None, lora=None, pag=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -416,7 +450,12 @@ class SamplingEngine:
         as in sample_notebook, its conditional, unconditional, regional and guidance-prompt K/V included: a request with an adapter
         and no negative prompt of its own gets its own unconditional slot, into which the engine-wide unconditional inputs are
         projected under its adapter.  ValueError for a bad entry or scale and an adapter of another configuration or device.  The
-        request holds its adapter until it retires.  The request's draws start when it is admitted."""
+        request holds its adapter until it retires.  ``pag`` (None, a scale s or (s, blocks)) adds perturbed-attention guidance
+        as in sample_notebook: on the request's steps before sampling_conditional_steps, one more denoiser row, its perturbed
+        forward, joins its mix (guided or not); it reads the request's conditional slot, weight row, wrap byte and adapter.
+        ValueError for a bad entry (ops.pag_table), with ``prompt_regions``, and on an edit or a source.  The engine allocates
+        nothing for PAG until a request uses it (then one empty row of its weight pool).  The request's draws start when it is
+        admitted."""
         attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
@@ -479,20 +518,36 @@ class SamplingEngine:
         lora = ops.lora_entries(ops.lora_table(lora, 1, self.model), 1)[0]
         if attention_source is not None:
             self._check_attention_source(attention_source, model_inputs, steps, renoise_steps, cond_steps, prompt_regions, lora)
+        pag_e = None
+        if pag is not None:
+            if isinstance(pag, list):
+                raise ValueError("pag: a request takes one entry (got a list)")
+            pag_t = ops.pag_table([pag], 1, self.model.n_attn_blocks, self.model.pag_default_blocks())
+            if pag_t is not None:
+                if prompt_regions:
+                    raise ValueError("pag: perturbed-attention guidance on a request with prompt_regions is not supported")
+                if attention_source is not None:
+                    raise ValueError("pag: perturbed-attention guidance on a prompt-to-prompt edit is not supported")
+                pag_e = (pag_t[0][0], int(pag_t[1][0]))
         cfgs = U._cfg_schedule(cfg, 1, steps)
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         mix_coef = None
-        if terms is not None:      # the guided steps' mix coefficients; their params rows become (1, 0, 1/T): f*1 + u*0 = f
-            n_guided = min(steps, cond_steps)
+        n_mix = min(steps, cond_steps)
+        s = pag_e[0] if pag_e is not None else 0.0
+        if terms is not None or (pag_e is not None and cfgs is not None):
+            # the guided steps' mix coefficients; their params rows become (1, 0, 1/T): f*1 + u*0 = f
             step_cfg = cfgs[0] if torch.is_tensor(cfg) else cfgs
-            mix_coef = torch.tensor([ops.guidance_coefficients(step_cfg[i], [w for _, w in terms]) for i in range(n_guided)],
-                                    dtype=torch.float32).view(n_guided, 2 + len(terms))
-            params[:n_guided, 0, 0] = 1.0
-            params[:n_guided, 0, 1] = 0.0
+            ws = [w for _, w in terms] if terms is not None else []
+            mix_coef = torch.tensor([ops.guidance_coefficients(step_cfg[i], ws, s) for i in range(n_mix)],
+                                    dtype=torch.float32).view(n_mix, 2 + len(ws) + (pag_e is not None))
+            params[:n_mix, 0, 0] = 1.0
+            params[:n_mix, 0, 1] = 0.0
+        elif pag_e is not None:    # unguided: l_c + s (l_c - l_p)
+            mix_coef = torch.tensor([ops.guidance_coefficients(None, [], s)] * n_mix, dtype=torch.float32).view(n_mix, 2)
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
                       sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap, regions,
-                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs), attention_source, lora)
+                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs), attention_source, lora, pag_e)
         if attention_source is not None:
             attention_source[0].edits.append(req)
         self._gens.add(id(generator))
@@ -511,6 +566,8 @@ class SamplingEngine:
             raise ValueError("attention_source: the source is itself an edit (no chains)")
         if src.regional or prompt_regions:
             raise ValueError("attention_source: prompt_regions on an edit or on its source are not supported")
+        if src.pag is not None:
+            raise ValueError("attention_source: perturbed-attention guidance on the source is not supported")
         if src.maps_len != self.model.conditioning_seq_len(model_inputs):
             raise ValueError(f"attention_source: the source's conditioning has {src.maps_len} rows, the edit's "
                              f"{self.model.conditioning_seq_len(model_inputs)}")
@@ -534,6 +591,11 @@ class SamplingEngine:
             q.uncond_slot = self.max_batch + q.slot if q.uncond is not None else self.shared_slot
         if not new:
             return
+        if any(q.pag is not None for q in new) and self.w_pool.shape[0] == self.max_batch:
+            # perturbed-attention guidance: one weight row of length 0 (row max_batch) for the unconditional and term rows of a
+            # perturbing step, whose w_row covers every row
+            self.w_pool = torch.cat([self.w_pool, torch.zeros(1, self.w_max, dtype=torch.float32, device=self.dev)])
+            self.w_len = torch.cat([self.w_len, torch.zeros(1, dtype=torch.int32, device=self.dev)])
         m = self.model
         hw = self.H * self.W
         table = ops.philox_table([q.generator for q in new], hw, self.dev)
@@ -618,7 +680,7 @@ class SamplingEngine:
             self._admit()
             if not self._active:
                 return []
-            plan = build_step_plan(self._active)
+            plan = build_step_plan(self._active, self.max_batch)
             m, dev, H, W = self.model, self.dev, self.H, self.W
             Bc, n_pairs = len(plan.order), plan.n_pairs
             hw = H * W
@@ -649,12 +711,18 @@ class SamplingEngine:
                 tail["inject"] = part("inj_src")
             if plan.loras:      # row b runs under adapter lora_id[b] (its tail rows under their source's)
                 tail["lora"] = (ops.lora_structs(plan.adapters), len(plan.adapters), part("lora_id"), part("lora_scale"))
+            if plan.perturbed:  # the perturbed rows' AttnBlock masks
+                tail["perturb"] = buf[lay["pag"][1]:lay["pag"][1] + lay["pag"][2]]
 
             x = ops.gather_rows(self.tokens, row_slot_d, self._x[:Bc])
             cond = ConditioningCache(self.cache.cache, Bc + n_tail, self.s_max, self.n_slots, kv_slot_d)
             # row b reads the regional prompts of its token slot
             regional = (self.prompt_mask, self.region_slot, row_slot_d) if any(q.regional for q in plan.order) else None
-            if any(q.attn_weights is not None for q in plan.order):       # row b reads the weights of its token slot
+            if any(q.attn_weights is not None for q in plan.order) and plan.perturbed:
+                # every row reads its weight row: a perturbed row its request's, the unconditional and term rows the empty one
+                feats = m.features(x, r_d, cond, self.w_pool, Bc + n_tail, w_len=self.w_len, w_row=part("w_row"), wrap=wrap_d,
+                                   regional=regional, **tail)
+            elif any(q.attn_weights is not None for q in plan.order):       # row b reads the weights of its token slot
                 feats = m.features(x, r_d, cond, self.w_pool, Bc, w_len=self.w_len, w_row=row_slot_d, wrap=wrap_d, regional=regional,
                                    **tail)
             else:

@@ -521,14 +521,16 @@ class Paella(nn.Module):
     # -------------------------------------------------------------- conditioning
     def prepare_conditioning(self, groups: Sequence[Dict[str, torch.Tensor]], latent_hw=(32, 32),
                              share_uniform: bool = True, extra: Sequence[Dict[str, torch.Tensor]] = (),
-                             tail: Sequence[int] = (), lora=None, extra_lora=None) -> ConditioningCache:
+                             tail: Sequence[int] = (), lora=None, extra_lora=None, pag_tail: Sequence[int] = ()) -> ConditioningCache:
         """gen_c_embeddings (ref/src/modules.py:223-232) + every AttnBlock's kv_mapper and K/V projection of the
         conditioning rows, for the concatenation of ``groups`` (e.g. [conditional, unconditional]).  A group whose
         samples all carry the same tensors (the usual unconditional group) is projected once and shared.  ``extra``: batch-1
         conditioning dicts (regional and guidance prompts) projected into slots of their own after the groups'
         (cache.extra_slot on), consecutive ones of one sequence layout in one projection.  ``tail``: indices into ``extra``; the
         cache then has len(tail) more samples after the groups', sample k of them attending to extra prompt tail[k] (the term
-        rows of features' ``tail_src``).  No other sample's slot_map entry names an extra slot.
+        rows of features' ``tail_src``).  No other sample's slot_map entry names an extra slot.  ``pag_tail``: samples of the groups;
+        the cache then has len(pag_tail) more samples after those, sample k of them attending to sample pag_tail[k]'s own slot (the
+        perturbed rows of perturbed-attention guidance).
         ``lora``: None, or per group None or a list of its samples' LoRA entries (ops.lora_entries: None or (adapter, scale)), and
         ``extra_lora``: None or one entry per ``extra`` prompt: each slot is projected under its entry's adapter
         (pb200_paella_prepare_cond_lora), and a group is shared only when its samples also agree on the entry."""
@@ -624,9 +626,10 @@ class Paella(nn.Module):
                     check(L.pb200_paella_prepare_cond(self._handle, ctypes.byref(cond), B, off, slots, s_max, ptr(cache), ptr(ws),
                                                       ws.numel(), current_stream()), "pb200_paella_prepare_cond")
                 off += B
-            identity = slots == bt and not extra          # (extra slots: slots may equal bt with a shared group)
-            slot_map = None if identity else torch.tensor(slot_of[:bt] + [extra_slot + k for k in tail], dtype=torch.int32, device=dev)
-        return ConditioningCache(cache, bt + len(tail), s_max, slots, slot_map, extra_slot)
+            identity = slots == bt and not extra and not pag_tail      # (extra slots: slots may equal bt with a shared group)
+            slot_map = None if identity else torch.tensor(slot_of[:bt] + [extra_slot + k for k in tail] + [slot_of[b] for b in pag_tail],
+                                                          dtype=torch.int32, device=dev)
+        return ConditioningCache(cache, bt + len(tail) + len(pag_tail), s_max, slots, slot_map, extra_slot)
 
     def gen_r_embedding(self, r, max_positions=10000):
         """ref/src/modules.py:212-221 -> [B, c_r]."""
@@ -673,7 +676,7 @@ class Paella(nn.Module):
                  attn_weights_batch: int = 0, cfg_pairs: bool = False, n_pairs: Optional[int] = None,
                  w_len: Optional[torch.Tensor] = None, w_row: Optional[torch.Tensor] = None,
                  wrap: Optional[torch.Tensor] = None, regional=None, tail_src: Optional[torch.Tensor] = None,
-                 maps=None, inject: Optional[torch.Tensor] = None, lora=None) -> torch.Tensor:
+                 maps=None, inject: Optional[torch.Tensor] = None, lora=None, perturb: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Everything up to out_mapper's LayerNorm: tokens [Bt,H,W] -> fp32 [Bt*H*W, c_out].
 
         ``cfg_pairs=True``: x [B,H,W] and r [B] are the classifier-free-guidance batch of ref/src/utils.py:42-45 —
@@ -706,7 +709,13 @@ class Paella(nn.Module):
         other row is that of the call without it, bit for bit.  None launches exactly the kernels without it.
         ``lora``: LoRA adapters (lora_device): sample b of x runs every AttnBlock's in_proj and out_proj under its adapter and
         scale, and so does each tail row under its source's (pb200_paella_features_lora).  Rows without an adapter are those of
-        the call without it, bit for bit.  None launches exactly the kernels without it."""
+        the call without it, bit for bit.  None launches exactly the kernels without it.
+        ``perturb``: perturbed-attention guidance, a device int64 [n] (n <= rows of the result, tail rows included; ops.pag_table's
+        masks, read as uint64): row b < n runs AttnBlock i (plan order) with the self part of its attention collapsed onto the
+        diagonal when bit i of perturb[b] is set (pb200_paella_features_pag).  A perturbed row is not regional, injected or a
+        source.  With it, ``attn_weights_batch`` may cover tail rows too (a per-sample table whose w_row gives each tail row its
+        row; a zero-length row leaves one unweighted).  Rows whose mask is 0 are those of the call without it, bit for bit.
+        None launches exactly the kernels without it."""
         self._ensure_packed()
         L = lib()
         dev = self._device()
@@ -726,6 +735,9 @@ class Paella(nn.Module):
         if inject is not None and (inject.dtype != torch.int32 or inject.dim() != 1 or not 0 < inject.numel() <= Bt
                                    or inject.device != dev or not inject.is_contiguous()):
             raise PaellaB200Error(f"features: inject must be a contiguous int32 vector of at most {Bt} entries on {dev}")
+        if perturb is not None and (perturb.dtype != torch.int64 or perturb.dim() != 1 or not 0 < perturb.numel() <= Bt + n_pairs
+                                    or perturb.device != dev or not perturb.is_contiguous()):
+            raise PaellaB200Error(f"features: perturb must be a contiguous int64 vector of at most {Bt + n_pairs} entries on {dev}")
         Bt += n_pairs
         if Bt != cond.batch_total:
             raise PaellaB200Error(f"batch {Bt} does not match the conditioning cache ({cond.batch_total})")
@@ -749,10 +761,11 @@ class Paella(nn.Module):
                         or w_len.numel() != attn_weights.shape[0] or (w_row is not None and w_row.numel() < attn_weights_batch):
                     raise PaellaB200Error("features: a per-sample weight table is float32 [rows, w_ld] with int32 w_len [rows] "
                                           "and an optional int32 w_row [attn_weights_batch]")
-                if regional is not None or tail_src is not None or maps is not None or inject is not None or lora is not None:
+                if regional is not None or tail_src is not None or maps is not None or inject is not None or lora is not None \
+                        or perturb is not None:
                     self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(attn_weights), 0, attn_weights.shape[1], ptr(w_len),
                                                                             ptr(w_row)), attn_weights_batch, wrap, regional, feats, ws,
-                                            tail_src, maps, inject, lora)
+                                            tail_src, maps, inject, lora, perturb)
                     return feats
                 if wrap is not None:
                     check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -766,9 +779,10 @@ class Paella(nn.Module):
                                                        current_stream()), "pb200_paella_features_weighted")
                 return feats
             aw = attn_weights.to(device=dev, dtype=torch.float32).contiguous() if attn_weights is not None else None
-            if regional is not None or tail_src is not None or maps is not None or inject is not None or lora is not None:
+            if regional is not None or tail_src is not None or maps is not None or inject is not None or lora is not None \
+                    or perturb is not None:
                 self._features_regional(x, r, Bt, n_pairs, H, W, cond, (ptr(aw), aw.numel() if aw is not None else 0, 0, None, None),
-                                        attn_weights_batch, wrap, regional, feats, ws, tail_src, maps, inject, lora)
+                                        attn_weights_batch, wrap, regional, feats, ws, tail_src, maps, inject, lora, perturb)
                 return feats
             if wrap is not None:        # the single weight vector is the weighted call with w_ld = 0 and no w_len
                 check(L.pb200_paella_features_tiled(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
@@ -783,10 +797,10 @@ class Paella(nn.Module):
         return feats
 
     def _features_regional(self, x, r, Bt, n_pairs, H, W, cond, weights, w_batch, wrap, regional, feats, ws, tail_src=None, maps=None,
-                           inject=None, lora=None):
+                           inject=None, lora=None, perturb=None):
         """pb200_paella_features_regional, or with ``tail_src`` pb200_paella_features_tail, or with ``maps``
-        pb200_paella_features_maps, or with ``inject`` pb200_paella_features_inject, or with ``lora`` pb200_paella_features_lora
-        (``regional`` may then be None)."""
+        pb200_paella_features_maps, or with ``inject`` pb200_paella_features_inject, or with ``lora`` pb200_paella_features_lora, or
+        with ``perturb`` pb200_paella_features_pag (``regional`` may then be None)."""
         mask = region_slot = mask_row = None
         if regional is not None:
             mask, region_slot, mask_row = regional
@@ -796,9 +810,23 @@ class Paella(nn.Module):
                     or (mask_row is None and rows < Bt - n_pairs) or (mask_row is not None and mask_row.numel() < Bt - n_pairs):
                 raise PaellaB200Error(f"features: regional prompts are uint8 masks [rows, {H}, {W}], int32 region_slot [rows, <= "
                                       f"{ops.MAX_PROMPT_REGIONS}] and an optional int32 mask_row [{Bt - n_pairs}]")
-        if w_batch > Bt - n_pairs:
+        if w_batch > (Bt if perturb is not None else Bt - n_pairs):
             raise PaellaB200Error(f"features: {w_batch} weighted samples of {Bt - n_pairs}")
         n_regions = region_slot.shape[1] if region_slot is not None else 0
+        if perturb is not None:
+            structs, n_adapters, ids, scales = lora if lora is not None else (None, 0, None, None)
+            if lora is not None and (ids.numel() != Bt - n_pairs or scales.numel() != Bt - n_pairs):
+                raise PaellaB200Error(f"features: LoRA tables of {ids.numel()} samples for {Bt - n_pairs}")
+            map_row, map_batch, acc = maps if maps is not None else (None, 0, None)
+            check(lib().pb200_paella_features_pag(self._handle, ptr(x), ptr(r), Bt, n_pairs, H, W, ptr(cond.cache), cond.slots,
+                                                  ptr(cond.slot_map), cond.s_max, *weights, w_batch, ptr(wrap), ptr(mask),
+                                                  ptr(mask_row), ptr(region_slot), n_regions, ptr(tail_src), ptr(map_row), map_batch,
+                                                  ptr(acc), acc.shape[0] if acc is not None else 0,
+                                                  acc.shape[1] if acc is not None else 0, ptr(inject),
+                                                  inject.numel() if inject is not None else 0, structs, n_adapters, ptr(ids),
+                                                  ptr(scales), ptr(perturb), perturb.numel(), ptr(feats), ptr(ws), ws.numel(),
+                                                  current_stream()), "pb200_paella_features_pag")
+            return
         if lora is not None:
             structs, n_adapters, ids, scales = lora
             if ids.numel() != Bt - n_pairs or scales.numel() != Bt - n_pairs:
@@ -1063,6 +1091,16 @@ class Paella(nn.Module):
                                                       current_stream()), "pb200_paella_resample_samples")
         return out
 
+    @property
+    def n_attn_blocks(self) -> int:
+        """The number of AttnBlocks, the index space of perturbed-attention guidance's blocks (paella_b200.lora.attn_blocks)."""
+        from .lora import attn_blocks
+        return len(attn_blocks(self._cfg))
+
+    def pag_default_blocks(self) -> list:
+        """The AttnBlocks a PAG entry given as a scale perturbs: those of the deepest level, down and up (ops.pag_default_blocks)."""
+        return ops.pag_default_blocks(self._cfg)
+
     def conditioning_seq_len(self, inputs: Dict[str, torch.Tensor]) -> int:
         """Length of the conditioning sequence of ``inputs`` (byt5 rows + clip_seq_len per clip / clip_image embedding)."""
         n = (1 if inputs.get("clip") is not None else 0)
@@ -1149,7 +1187,15 @@ class Paella(nn.Module):
         or a list or tuple of B entries, each None, an adapter or (adapter, scale).  Sample b is then the reference model with
         W + scale * (alpha / r) * B A on its adapter's targets (every AttnBlock's in_proj, out_proj and kv_mapper), conditioning
         included.  Samples without an adapter, or at scale 0, get the logits of the call without it, bit for bit.  ValueError,
-        before anything is enqueued, for a bad entry or scale and an adapter of another configuration or device (ops.lora_table)."""
+        before anything is enqueued, for a bad entry or scale and an adapter of another configuration or device (ops.lora_table).
+        ``pag_blocks``: perturbed-attention guidance (keyword only): None, or a list or tuple of B entries, each None or a non-empty
+        list of AttnBlock indices (plan order, paella_b200.lora.attn_blocks).  Sample b's logits are then its perturbed logits l_p,
+        with no mix: in every listed AttnBlock and head, each query's attention mass on the self keys (post-softmax, post
+        attn_weights) goes to its own value, and its conditioning probabilities are unchanged.  Every other sample's logits are
+        those of the call without it, bit for bit.  With ``attention_maps=True`` a perturbed sample's maps are those of its
+        perturbed forward, which are its conditioning probabilities as the plain forward's are (the perturbation changes only
+        where the self keys' mass goes), taken at that forward's queries.  ValueError, before anything is enqueued, for a bad
+        entry, and PAG on a sample with prompt_regions or on an injected sample or its source (ops.pag_table)."""
         if x_cat is not None:
             x = torch.cat([x, x_cat], dim=1)
         attn_weights = kwargs.pop("attn_weights", None)
@@ -1158,6 +1204,7 @@ class Paella(nn.Module):
         attention_maps = ops.check_attention_maps(kwargs.pop("attention_maps", False), prompt_regions)
         attention_source = kwargs.pop("attention_source", None)
         lora = kwargs.pop("lora", None)
+        pag_blocks = kwargs.pop("pag_blocks", None)
         if kwargs:
             raise TypeError(f"unexpected keyword arguments {sorted(kwargs)}")
         B, H, W = x.shape
@@ -1165,6 +1212,7 @@ class Paella(nn.Module):
         regions = ops.regional_table(prompt_regions, B, (H, W), self._device())
         ops.check_regions_unweighted(regions, attn_weights)
         inject = ops.attention_source_table(attention_source, B, 1, regions, forward=True)
+        pag_t = ops.pag_table(pag_blocks, B, self.n_attn_blocks, regions=regions, inject=inject, forward=True)
         lora_t = ops.lora_table(lora, B, self)
         cond_len = self.conditioning_seq_len({"byt5": byt5, "clip": clip, "clip_image": clip_image})
         aw, w_len = self._attn_weights_table(attn_weights, B, (H, W), cond_len)
@@ -1183,10 +1231,11 @@ class Paella(nn.Module):
             wrap = ops.to_device_async(wrap, self._device())
         if inject is not None:
             inject = ops.to_device_async(inject[0], self._device())
+        perturb = ops.to_device_async(pag_t[1], self._device()) if pag_t is not None else None
         acc = self.map_accumulator(B, cond_len, (H, W)) if attention_maps else None
         feats = self.features(x, r, cond, aw, B if aw is not None else 0, w_len=w_len, wrap=wrap, regional=regional,
                               maps=(None, B, acc) if attention_maps else None, inject=inject,
-                              lora=ops.lora_device(lora_t, self._device()))
+                              lora=ops.lora_device(lora_t, self._device()), perturb=perturb)
         logits = self.logits_from_features(feats, B, H, W)
         if attention_maps:
             return logits, self.finalize_attention_maps(acc, (H, W), cond_len, 1)

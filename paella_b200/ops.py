@@ -594,32 +594,134 @@ def guidance_table(guidance_prompts, batch: int):
     return terms
 
 
-def guidance_coefficients(cfg: float, weights) -> list:
-    """The mix coefficients of one guided step as fp32 values: (float)cfg, (float)(1 - cfg (1 + sum w)), then (float)(cfg w_j)
-    per term, from doubles.  With no terms they are (cfg, 1 - cfg) of sampling_params, bit for bit."""
-    c = float(cfg)
-    total = 0.0
-    for w in weights:
-        total += w
-    vals = [c, 1.0 - c * (1.0 + total)] + [c * w for w in weights]
+def guidance_coefficients(cfg: float, weights, pag: float = 0.0) -> list:
+    """The mix coefficients of one guided step as fp32 values: (float)(cfg + s), (float)(1 - cfg (1 + sum w)), then (float)(cfg w_j)
+    per term, then (float)(-s) for a perturbed row (pag = s != 0), from doubles.  With no terms and no PAG they are (cfg, 1 - cfg)
+    of sampling_params, bit for bit.  ``cfg`` None (an unguided sample): (1 + s, -s), the mix l_c + s (l_c - l_p)."""
+    s = float(pag)
+    if cfg is None:
+        vals = [1.0 + s, -s]
+    else:
+        c = float(cfg)
+        total = 0.0
+        for w in weights:
+            total += w
+        vals = [c + s, 1.0 - c * (1.0 + total)] + [c * w for w in weights] + ([-s] if s != 0.0 else [])
     return torch.tensor(vals, dtype=torch.float64).float().tolist()
 
 
-def guidance_mix_table(terms, cond_row, uncond_row, term_rows, cfgs) -> Tuple[torch.Tensor, torch.Tensor]:
-    """The per-call mix table of the composed samples (those with terms, in ``terms`` order of the samples given): int32
-    [n_composed, 2 + J] row indices [c, u, t_1 .. t_J] (-1 after a sample's last term) and float32 [steps, n_composed, 2 + J]
-    coefficients (guidance_coefficients, 0 after the last term).  ``terms``: each composed sample's weights; ``cond_row``,
-    ``uncond_row``: its rows; ``term_rows``: its term rows; ``cfgs``: per step, each composed sample's cfg."""
+def guidance_mix_table(terms, cond_row, uncond_row, term_rows, cfgs, pag=None, pag_row=None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The per-call mix table of the composed samples (those with terms or PAG, in ``terms`` order of the samples given): int32
+    [n_composed, 2 + J] row indices [c, u, t_1 .. t_J, p] (-1 after a sample's last row) and float32 [steps, n_composed, 2 + J]
+    coefficients (guidance_coefficients, 0 after the last row).  ``terms``: each composed sample's weights; ``cond_row``,
+    ``uncond_row``: its rows (uncond_row None: an unguided call, rows [c, p]); ``term_rows``: its term rows; ``cfgs``: per step, each
+    composed sample's cfg (None entries in an unguided call); ``pag``: None or each composed sample's PAG scale (0: none), with
+    ``pag_row`` its perturbed row."""
     n = len(terms)
-    J = max(len(w) for w in terms)
-    rows = torch.full((n, 2 + J), -1, dtype=torch.int32)
-    coef = torch.zeros(len(cfgs), n, 2 + J, dtype=torch.float32)
-    for y, ws in enumerate(terms):
-        rows[y, 0], rows[y, 1] = cond_row[y], uncond_row[y]
-        rows[y, 2:2 + len(ws)] = torch.tensor(term_rows[y], dtype=torch.int32)
+    pag = pag if pag is not None else [0.0] * n
+    ld = max((1 if uncond_row is None else 2) + len(w) + (s != 0.0) for w, s in zip(terms, pag))
+    rows = torch.full((n, ld), -1, dtype=torch.int32)
+    coef = torch.zeros(len(cfgs), n, ld, dtype=torch.float32)
+    for y, (ws, s) in enumerate(zip(terms, pag)):
+        own = [cond_row[y]] + ([uncond_row[y]] if uncond_row is not None else []) + list(term_rows[y]) + ([pag_row[y]] if s != 0.0 else [])
+        rows[y, :len(own)] = torch.tensor(own, dtype=torch.int32)
         for i, step_cfgs in enumerate(cfgs):
-            coef[i, y, :2 + len(ws)] = torch.tensor(guidance_coefficients(step_cfgs[y], ws))
+            coef[i, y, :len(own)] = torch.tensor(guidance_coefficients(step_cfgs[y], ws, s))
     return rows, coef
+
+
+# ------------------------------------------------------------------ perturbed-attention guidance
+# A sample may carry a PAG entry (s, blocks): its perturbed forward is its conditional forward with the self part of every
+# attention map of the AttnBlocks in ``blocks`` (plan order, paella_b200.lora.attn_blocks) collapsed onto the diagonal
+# (pb200_attention_perturb), and its guided logits gain s (l_c - l_p) (Ahn et al. 2024, "Self-Rectifying Diffusion Sampling with
+# Perturbed-Attention Guidance").  The perturbed forward is one more tail row that reads its sample's own conditioning slot; the
+# per-row table of AttnBlock bit masks rides in the call's single packed copy (pb200_paella_features_pag).
+MAX_PAG_BLOCKS = 64
+
+
+def pag_default_blocks(cfg: dict) -> list:
+    """The default perturbed AttnBlocks of a Paella configuration: those of the deepest level, down and up, in plan order."""
+    from .lora import attn_blocks
+    deepest = len(cfg["c_hidden"]) - 1
+    return [i for i, (path, _) in enumerate(attn_blocks(cfg)) if path.startswith(f"down_blocks.{deepest}.") or path.startswith("up_blocks.0.")]
+
+
+def _pag_blocks(name: str, blocks, n_blocks: int) -> int:
+    """A non-empty list, tuple or set of distinct int AttnBlock indices in [0, n_blocks) -> its bit mask."""
+    if not isinstance(blocks, (list, tuple, set, frozenset)) or len(blocks) == 0:
+        raise ValueError(f"{name}: the blocks must be a non-empty list of AttnBlock indices (got {blocks!r})")
+    mask = 0
+    for i in blocks:
+        if not _is_int(i):
+            raise ValueError(f"{name}: AttnBlock index {i!r} is not an int")
+        if not 0 <= i < n_blocks:
+            raise ValueError(f"{name}: AttnBlock index {i} out of range (the model has {n_blocks} AttnBlocks)")
+        if (mask >> i) & 1:
+            raise ValueError(f"{name}: AttnBlock index {i} given twice")
+        mask |= 1 << i
+    return mask
+
+
+def _pag_entry(name: str, entry, n_blocks: int, default_blocks):
+    """None, a scale or (scale, blocks) -> (float scale, bit mask); a scale of 0 is no entry, (0.0, 0)."""
+    if entry is None:
+        return 0.0, 0
+    if isinstance(entry, (list, tuple)):
+        if len(entry) != 2:
+            raise ValueError(f"{name}: expected None, a scale or a (scale, blocks) pair (got {entry!r})")
+        scale, blocks = entry
+    else:
+        scale, blocks = entry, default_blocks
+    if isinstance(scale, bool) or not isinstance(scale, (int, float)) or not math.isfinite(scale):
+        raise ValueError(f"{name}: the scale must be a finite real number (got {scale!r})")
+    mask = _pag_blocks(name, blocks, n_blocks)
+    return (0.0, 0) if float(scale) == 0.0 else (float(scale), mask)
+
+
+def _mask_i64(m: int) -> int:
+    return m - (1 << 64) if m >= 1 << 63 else m
+
+
+def pag_table(pag, batch: int, n_blocks: int, default_blocks=None, regions=None, inject=None, exact: bool = False,
+              forward: bool = False):
+    """``pag`` (None, or a list or tuple of ``batch`` entries, each None, a scale or a (scale, blocks) pair; with ``forward`` each
+    None or a blocks list, perturbed in that single forward) -> None when no sample is perturbed, otherwise (scales, masks): the
+    float scale of every sample (0: none; 1.0 with ``forward``) and the int64 CPU [batch] AttnBlock bit masks the kernels read as
+    uint64 (0: none).  ``default_blocks``: the blocks of an entry given as a scale (pag_default_blocks).  ``regions``:
+    regional_table's result; ``inject``: attention_source_table's result.  ValueError, before anything is enqueued, for the wrong
+    length, a non-finite or bool scale, empty, duplicated, non-int or out-of-range blocks, more than 64 AttnBlocks, PAG on a sample
+    with prompt_regions or on a prompt-to-prompt edit or source, and ``exact=True``."""
+    if pag is None:
+        return None
+    if not isinstance(pag, (list, tuple)):
+        raise ValueError(f"pag: expected None or a list of {batch} entries (got {type(pag).__name__})")
+    if len(pag) != batch:
+        raise ValueError(f"pag: got {len(pag)} entries for a batch of {batch} (one per sample, None for none)")
+    if n_blocks > MAX_PAG_BLOCKS:
+        raise ValueError(f"pag: the model has {n_blocks} AttnBlocks; the perturbation masks hold {MAX_PAG_BLOCKS}")
+    if forward:
+        entries = [(0.0, 0) if e is None else (1.0, _pag_blocks(f"pag_blocks[{b}]", e, n_blocks)) for b, e in enumerate(pag)]
+    else:
+        entries = [_pag_entry(f"pag[{b}]", e, n_blocks, default_blocks) for b, e in enumerate(pag)]
+    edits = set()
+    if inject is not None:
+        for b in range(batch):
+            col = inject[:, b]
+            if bool((col >= 0).any()):
+                edits.add(b)
+                edits.update(int(a) for a in col[col >= 0].tolist())
+    for b, (s, _) in enumerate(entries):
+        if s == 0.0:
+            continue
+        if regions is not None and regions[1][b]:
+            raise ValueError(f"pag[{b}]: perturbed-attention guidance on a sample with prompt_regions is not supported")
+        if b in edits:
+            raise ValueError(f"pag[{b}]: perturbed-attention guidance on a prompt-to-prompt edit or source is not supported")
+    if all(s == 0.0 for s, _ in entries):
+        return None
+    if exact:
+        raise ValueError("exact=True restates the reference op for op, which has no perturbed-attention guidance")
+    return [s for s, _ in entries], torch.tensor([_mask_i64(m) for _, m in entries], dtype=torch.int64)
 
 
 # The notebook's sampling modes (paella_inference.ipynb cell 3).  'multinomial' draws H*W*num_labels exponentials per step; 'argmax'

@@ -102,6 +102,21 @@ guarantees above hold for adapted rows too; rows without an adapter, or at scale
 ValueError, before anything is enqueued and before any generator advances, for the wrong length, a bad entry or non-finite scale, and
 an adapter loaded for another configuration or on another device (ops.lora_table).
 
+Perturbed-attention guidance: ``pag`` (all three functions; None, or a list or tuple of B entries, each None, a scale s or an (s,
+blocks) pair) guides sample i away from its perturbed forward (Ahn et al. 2024, "Self-Rectifying Diffusion Sampling with
+Perturbed-Attention Guidance"): its conditional forward in which, in every AttnBlock listed in ``blocks`` (indices in plan order,
+paella_b200.lora.attn_blocks; default: the deepest level's, down and up, Paella.pag_default_blocks), each query's attention mass on the
+image's own tokens goes to its own value, while its probabilities on the prompt stay as they are.  On a step s <
+sampling_conditional_steps a guided sample's logits are l_u + cfg * [(l_c - l_u) + sum_j w_j (l_j - l_u)] + s (l_c - l_p), an
+unguided one's (cfg None, or a per-sample cfg of 1.0) l_c + s (l_c - l_p); later steps have no perturbed row.  The perturbed forward is
+one more tail row after the term rows, which reads its sample's own conditioning slot, wrap byte, adapter and ``attn_weights``
+(pb200_paella_features_pag), and its coefficients join the guided mix as guidance prompts' do.  The default blocks follow PAG's choice
+of the mid-block by analogy; their effect on images is unmeasured here (there are no trained weights).  PAG draws no random numbers,
+so every generator ends at the same offset and the per-sample guarantees above hold; a sample with no entry or s = 0 gets the tokens
+of the call without it, bit for bit.  ValueError, before anything is enqueued and before any generator advances, for the wrong length,
+a non-finite or bool scale, empty, duplicated, non-int or out-of-range blocks, PAG on a sample with ``prompt_regions`` or on a
+prompt-to-prompt edit or source, and ``exact=True`` (ops.pag_table).
+
 Scoring: ``score`` asks the denoiser how likely a given token grid is under a prompt -- held-out evaluation of a checkpoint with
 train.py's objective, reranking of candidates, or picking the prompt that best explains an image.  It noises the tokens at each
 of a list of noise levels, as add_noise does, and scores each noised grid against the clean tokens with Paella.token_scores
@@ -115,7 +130,7 @@ from typing import Dict, Optional, Sequence, Tuple
 import torch
 
 from . import ops
-from .modules import Paella
+from .modules import ConditioningCache, Paella
 
 
 def _zeros_like_inputs(inputs: Dict[str, torch.Tensor]):
@@ -214,14 +229,15 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
                  codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None,
-                 prompt_regions=None, guidance_prompts=None, attention_maps=False, attention_source=None, lora=None):
+                 prompt_regions=None, guidance_prompts=None, attention_maps=False, attention_source=None, lora=None, pag=None):
     """Returns (tokens, intermediates, maps or None).  ``modes``: None, or per step the list of B mode names (sampling_modes) --
     a step whose modes differ samples each row in its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the
     scalar path in that mode.  ``top_k`` / ``top_p``: the truncation of the multinomial draws (module docstring); a truncating
     call takes the per-sample table path, and so does a call with ``guidance_prompts`` (module docstring).  ``attention_maps``:
     the maps of the conditional rows (module docstring).  ``attention_source``: prompt-to-prompt injection (module docstring);
     step i passes row i of the table to the denoiser, or nothing when no sample is injected there.  ``lora``: per-sample LoRA
-    adapters (module docstring)."""
+    adapters (module docstring).  ``pag``: perturbed-attention guidance (module docstring): on steps i < sampling_conditional_steps
+    each perturbed sample has one more tail row, after the term rows, and joins the composed samples of the guided mix."""
     B, H, W = latent_shape
     dev = model._device()
     attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
@@ -233,6 +249,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     terms = ops.guidance_table(guidance_prompts, B)
     inj = ops.attention_source_table(attention_source, B, steps, regions, exact)
     inj_steps = [bool((row >= 0).any()) for row in inj] if inj is not None else [False] * steps
+    pag_t = ops.pag_table(pag, B, model.n_attn_blocks, model.pag_default_blocks(), regions, inj, exact) if pag is not None else None
     lora_t = ops.lora_table(lora, B, model)
     entries = ops.lora_entries(lora_t, B)
     extra = [g for own in regions[1] for g in own] if regions is not None else []
@@ -246,29 +263,46 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         raise ValueError("guidance_prompts need a guided call (cfg is None or 0)")
     mixed_steps = modes is not None and any(len(set(ms)) > 1 for ms in modes)
     sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg,
-                              always=mixed_steps or trunc is not None or terms is not None)
+                              always=mixed_steps or trunc is not None or terms is not None or pag_t is not None)
     mix = None
-    if terms is not None:
-        # the composed samples' mix table over the guided steps; their params rows there become (1, 0, 1/T): f*1 + u*0 = f
-        comp = [b for b in range(B) if terms[b]]
+    pag_src = []
+    n_mix = min(steps, sampling_conditional_steps)
+    if terms is not None or pag_t is not None:
+        # the composed samples' mix table over the guided steps; their params rows there become (1, 0, 1/T): f*1 + u*0 = f.  The
+        # batch is [B conditional; B unconditional (guided calls); term rows by sample, then term; perturbed rows by sample]
+        tl = terms if terms is not None else [[] for _ in range(B)]
+        pag_s = pag_t[0] if pag_t is not None else [0.0] * B
+        comp = [b for b in range(B) if tl[b] or pag_s[b] != 0.0]
         n_reg = len(extra)
-        term_src, term_rows, k = [], [], 2 * B
+        term_src, term_rows, k = [], [], 2 * B if use_cfg_any else B
         for b in comp:
-            term_rows.append(list(range(k, k + len(terms[b]))))
-            term_src += [b] * len(terms[b])
-            k += len(terms[b])
-        extra = extra + [inputs for b in comp for inputs, _ in terms[b]]
-        extra_lora = extra_lora + [entries[b] for b in comp for _ in terms[b]]
-        n_guided = min(steps, sampling_conditional_steps)
-        step_cfgs = [[(cfgs[b] if per_sample_cfg else cfgs)[i] for b in comp] for i in range(n_guided)]
-        mix_rows, mix_coef = ops.guidance_mix_table([[w for _, w in terms[b]] for b in comp], comp, [B + b for b in comp], term_rows,
-                                                    step_cfgs)
-        sched[0][:n_guided, comp, 0] = 1.0
-        sched[0][:n_guided, comp, 1] = 0.0
-        mix = (list(range(B)) + term_src, [n_reg + j for j in range(len(term_src))], mix_rows, mix_coef)
+            term_rows.append(list(range(k, k + len(tl[b]))))
+            term_src += [b] * len(tl[b])
+            k += len(tl[b])
+        pag_src = [b for b in comp if pag_s[b] != 0.0]
+        pag_row = {b: k + j for j, b in enumerate(pag_src)}
+        extra = extra + [inputs for b in comp for inputs, _ in tl[b]]
+        extra_lora = extra_lora + [entries[b] for b in comp for _ in tl[b]]
+        step_cfgs = [[(cfgs[b] if per_sample_cfg else cfgs)[i] if use_cfg_any else None for b in comp] for i in range(n_mix)]
+        mix_rows, mix_coef = ops.guidance_mix_table([[w for _, w in tl[b]] for b in comp], comp,
+                                                    [B + b for b in comp] if use_cfg_any else None, term_rows, step_cfgs,
+                                                    [pag_s[b] for b in comp], [pag_row.get(b, -1) for b in comp])
+        if use_cfg_any:
+            sched[0][:n_mix, comp, 0] = 1.0
+            sched[0][:n_mix, comp, 1] = 0.0
+        mix = ((list(range(B)) if use_cfg_any else []) + term_src + pag_src, [n_reg + j for j in range(len(term_src))], mix_rows,
+               mix_coef)
+    n_rows = (2 * B if use_cfg_any else B) + (len(mix[0]) - (B if use_cfg_any else 0) if mix is not None else 0)
     w_table = None
+    if pag_src and torch.is_tensor(attn_weights):      # perturbed rows read their sample's row of a per-sample table
+        attn_weights = [attn_weights] * B
     if isinstance(attn_weights, (list, tuple)):       # per-sample vectors, for the conditional rows only
         w_table = ops.attn_weights_table(attn_weights, B, [model.max_attn_weights((H, W), model.conditioning_seq_len(model_inputs))] * B)
+    w_row = None
+    if w_table is not None and pag_src:
+        # one zero-length row (B) for the unconditional and term rows; perturbed row k reads row pag_src[k]
+        w_table = (torch.cat([w_table[0], torch.zeros(1, w_table[0].shape[1])]), torch.cat([w_table[1], torch.zeros(1, dtype=torch.int32)]))
+        w_row = torch.tensor(list(range(B)) + [B] * (n_rows - B - len(pag_src)) + pag_src, dtype=torch.int32)
     if ops.per_sample(generator):
         ops.check_generators(generator, B, dev)
         ops.check_per_sample_numel(H * W * model.num_labels)
@@ -279,7 +313,13 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         parts += [wrap] if wrap is not None else []
         parts += [torch.tensor(mix[0], dtype=torch.int32), mix[2], mix[3]] if mix is not None else []
         parts += [inj] if any(inj_steps) else []
+        if pag_src:     # the per-row AttnBlock masks: zero before the perturbed rows, each perturbed row its sample's
+            pag_rows = torch.zeros(n_rows, dtype=torch.int64)
+            pag_rows[n_rows - len(pag_src):] = pag_t[1][pag_src]
+            parts += [pag_rows] + ([w_row] if w_row is not None else [])
         parts_d = ops.to_device_packed(parts, dev) if parts else []
+        w_row_d = parts_d.pop() if w_row is not None else None
+        pag_rows_d = parts_d.pop() if pag_src else None
         inj_d = parts_d.pop() if any(inj_steps) else None
         if mix is not None:
             mix_coef_d, mix_rows_d, tail_d = parts_d.pop(), parts_d.pop(), parts_d.pop()
@@ -309,7 +349,10 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         xlora = extra_lora if lora_t is not None else None
         # with guidance prompts the guided batch is [B conditional; B unconditional; term rows by sample, then term]
         cond_full = model.prepare_conditioning(groups, (H, W), extra=extra, tail=mix[1] if mix is not None else (), lora=glora,
-                                               extra_lora=xlora)
+                                               extra_lora=xlora, pag_tail=pag_src)
+        if pag_src and not use_cfg_any:     # the steps without PAG: the conditional rows alone, on the same cache
+            cond_plain = ConditioningCache(cond_full.cache, B, cond_full.s_max, cond_full.slots, cond_full.slot_map[:B],
+                                           cond_full.extra_slot)
         regional_full = model.regional_device(regions, cond_full) if regions is not None else None
         extra_only = extra[:len(extra) - len(mix[1])] if mix is not None else extra
         lora_d = ops.lora_device(lora_t, dev)
@@ -335,17 +378,19 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                     regional_only = model.regional_device(regions, cond_only) if regions is not None else None
                 cond, tokens = cond_only, sampled
             else:
-                cond, tokens = cond_full, sampled
+                cond, tokens = (cond_full if not pag_src or i < n_mix else cond_plain), sampled
             if sched is None:
                 r = torch.full((tokens.shape[0],), float(t_list[i]), dtype=torch.float32, device=dev)
                 cfg_i, temp_i = (float(cfgs[i]) if guided else None), float(temperatures[i])
             else:
                 r, params_i = r_d[i], params_d[i]
-            composed = guided and mix is not None
-            feats = model.features(tokens, r, cond, attn_weights, B if attn_weights is not None else 0, cfg_pairs=guided and not composed,
-                                   w_len=w_len, wrap=wrap_d, regional=regional_only if cond is cond_only else regional_full,
+            composed = mix is not None and i < n_mix and (guided or not use_cfg_any)
+            perturbed = composed and bool(pag_src)
+            feats = model.features(tokens, r, cond, attn_weights, (n_rows if perturbed and w_row is not None else B)
+                                   if attn_weights is not None else 0, cfg_pairs=guided and not composed, w_len=w_len,
+                                   w_row=w_row_d if perturbed else None, wrap=wrap_d, regional=regional_only if cond is cond_only else regional_full,
                                    tail_src=tail_d if composed else None, maps=(None, B, acc) if attention_maps else None,
-                                   inject=inj_d[i] if inj_steps[i] else None, lora=lora_d)
+                                   inject=inj_d[i] if inj_steps[i] else None, lora=lora_d, perturb=pag_rows_d if perturbed else None)
             if composed:
                 model.guidance_mix(feats, H * W, mix_rows_d, mix_coef_d[i])
             if step_modes is not None:
@@ -529,7 +574,7 @@ def _decode_tail(tokens, decode, decode_output, tiling=None):
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
            cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
            top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None, attention_maps=False,
-           attention_source=None, lora=None):
+           attention_source=None, lora=None, pag=None):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -548,7 +593,8 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     docstring): weighted extra and negative prompts per sample in the guided mix; a sample with terms needs a cfg other than 0.
     ``attention_maps=True`` (module docstring): returns (tokens or images, maps).  ``attention_source`` (module docstring):
     prompt-to-prompt edits of other samples of the call; give each edit its own generator seeded like its source's.
-    ``lora`` (module docstring): a LoRA adapter per sample, or one for every sample."""
+    ``lora`` (module docstring): a LoRA adapter per sample, or one for every sample.  ``pag`` (module docstring):
+    perturbed-attention guidance per sample, with CFG or without it."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     per_sample_cfg = torch.is_tensor(cfg)
     terms = ops.guidance_table(guidance_prompts, latent_shape[0])
@@ -568,7 +614,7 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
                                 temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
                                 per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling,
                                 prompt_regions=prompt_regions, guidance_prompts=guidance_prompts, attention_maps=attention_maps,
-                                attention_source=attention_source, lora=lora)
+                                attention_source=attention_source, lora=lora, pag=pag)
     out = _decode_tail(out, decode, decode_output, tiling)
     return (out, maps) if attention_maps else out
 
@@ -576,7 +622,7 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
                        exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None,
-                       guidance_prompts=None, attention_maps=False, attention_source=None, lora=None):
+                       guidance_prompts=None, attention_maps=False, attention_source=None, lora=None, pag=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
@@ -589,7 +635,7 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     computes what rows [lo, hi) compute.  ``attention_maps=True`` (module docstring): returns (tokens, maps) for the shard's rows.
     ``attention_source`` (module docstring): a source and its edits sit in the same shard, with indices relative to the shard.
     ``lora`` (module docstring): a shard given ``lora[lo:hi]`` computes what rows [lo, hi) compute; each rank loads its adapters
-    itself (load_lora)."""
+    itself (load_lora).  ``pag`` (module docstring) likewise: a shard given ``pag[lo:hi]`` computes what rows [lo, hi) compute."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -600,7 +646,7 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
                                 temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
                                 generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
                                 tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts,
-                                attention_maps=attention_maps, attention_source=attention_source, lora=lora)
+                                attention_maps=attention_maps, attention_source=attention_source, lora=lora, pag=pag)
     return (out, maps) if attention_maps else out
 
 
@@ -608,7 +654,7 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
                     generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
-                    attention_maps=False, attention_source=None, lora=None):
+                    attention_maps=False, attention_source=None, lora=None, pag=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -626,7 +672,9 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     have ``attn_weights``.  ``guidance_prompts`` as in ``sample``: the argmax and quant steps of a sample with terms see its mixed
     features, and ``attn_weights`` weight its conditional row only.  ``attention_maps=True`` (module docstring): returns
     (sampled, intermediate_images, maps).  ``attention_source`` (module docstring): prompt-to-prompt edits; an edit's
-    ``attn_weights`` reweight the replayed probabilities.  ``lora`` (module docstring): a LoRA adapter per sample."""
+    ``attn_weights`` reweight the replayed probabilities.  ``lora`` (module docstring): a LoRA adapter per sample.  ``pag``
+    (module docstring): perturbed-attention guidance per sample; its perturbed row carries the sample's ``attn_weights``, and the
+    argmax and quant steps see the mixed features."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -647,5 +695,5 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                                                 per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes, top_k=top_k,
                                                 top_p=top_p, tiling=tiling, prompt_regions=prompt_regions,
                                                 guidance_prompts=guidance_prompts, attention_maps=attention_maps,
-                                                attention_source=attention_source, lora=lora)
+                                                attention_source=attention_source, lora=lora, pag=pag)
     return (sampled, intermediates, maps) if attention_maps else (sampled, intermediates)
