@@ -144,7 +144,7 @@ def conv_k4s2p1(x: Tensor, w: Tensor, b: Tensor, mm=mm_fp32) -> Tensor:
     """Conv2d(k=4,s=2,p=1) channels-last as 16 shifted GEMMs.  w [Cout,Cin,4,4]."""
     B, H, W, C = x.shape
     xp = F.pad(x, (0, 0, 1, 1, 1, 1))
-    out = torch.zeros(B, H // 2, W // 2, w.shape[0]) + b
+    out = torch.zeros(B, H // 2, W // 2, w.shape[0], dtype=x.dtype) + b
     for ky in range(4):
         for kx in range(4):
             out = out + mm(xp[:, ky:ky + H:2, kx:kx + W:2, :], w[:, :, ky, kx])
@@ -158,10 +158,10 @@ def convT_k4s2p1(x: Tensor, w: Tensor, b: Tensor, mm=mm_fp32) -> Tensor:
     B, H, W, C = x.shape
     cout = w.shape[1]
     xp = F.pad(x, (0, 0, 1, 1, 1, 1))
-    out = torch.zeros(B, 2 * H, 2 * W, cout)
+    out = torch.zeros(B, 2 * H, 2 * W, cout, dtype=x.dtype)
     for py in range(2):
         for px in range(2):
-            acc = torch.zeros(B, H, W, cout) + b
+            acc = torch.zeros(B, H, W, cout, dtype=x.dtype) + b
             for ky in range(4):
                 if (py + 1 - ky) % 2:
                     continue

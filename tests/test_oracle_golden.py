@@ -79,6 +79,29 @@ def test_vqgan_conv_stacks():
     torch.testing.assert_close(dec2, t(g["dec"]), **TOL)
 
 
+def test_vqgan_oracle_fp64_stays_fp64():
+    """An fp64 run of the codec oracle is fp64 throughout: both k4s2 convolutions match torch's own fp64 convolutions to
+    fp64 rounding (an fp32 intermediate would leave ~1e-7 relative error), and encode / decode return fp64."""
+    import torch.nn.functional as F
+    cfg, sd, g = load_golden("vqgan_tiny.npz")
+    sd64 = {k: v.double() if v.is_floating_point() else v for k, v in sd.items()}
+    gen = torch.Generator().manual_seed(5)
+    x = torch.randn(2, 6, 10, 8, dtype=torch.float64, generator=gen)                          # NHWC
+    w = torch.randn(5, 8, 4, 4, dtype=torch.float64, generator=gen)
+    b = torch.randn(5, dtype=torch.float64, generator=gen)
+    got = vo.conv_k4s2p1(x, w, b)
+    want = F.conv2d(x.permute(0, 3, 1, 2), w, b, stride=2, padding=1).permute(0, 2, 3, 1)
+    assert got.dtype == torch.float64 and float((got - want).abs().max()) < 1e-12
+    wt = torch.randn(8, 5, 4, 4, dtype=torch.float64, generator=gen)
+    got = vo.convT_k4s2p1(x, wt, b)
+    want = F.conv_transpose2d(x.permute(0, 3, 1, 2), wt, b, stride=2, padding=1).permute(0, 2, 3, 1)
+    assert got.dtype == torch.float64 and float((got - want).abs().max()) < 1e-12
+    lat = vo.encode_latents(sd64, t(g["img"]).double())
+    dec = vo.decode_latents(sd64, sd64["vquantizer.codebook.weight"][t(g["idx_rand"])], n_bottleneck=cfg["bottleneck_blocks"])
+    assert lat.dtype == torch.float64 and dec.dtype == torch.float64
+    torch.testing.assert_close(lat.permute(0, 3, 1, 2).float(), t(g["latents"]), **TOL)
+
+
 def test_vq_nearest_definitions_agree():
     """C oracle (exact fmaf) == fp64 emulation == brute force argmin on well-separated data."""
     g = torch.Generator().manual_seed(0)
