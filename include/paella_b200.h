@@ -121,6 +121,24 @@ int pb200_add_noise_per_sample(const int64_t* x, const int64_t* random_x, const 
 int pb200_add_noise_region_per_sample(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region,
                                       const int* slot, const float* t, int64_t batch, int64_t hw, int64_t num_labels,
                                       const uint64_t* seed_offset, int64_t* out, int64_t* mask_out, void* stream);
+/* Confidence-guided renoise: replaces pb200_add_noise_region's random mask [ref/src/modules.py:277-283] by each sample's
+ * least likely tokens.  logp: fp32 [batch, hw], the step's log-probability of each drawn token (pb200_paella_token_logprob);
+ * t: fp32 [batch] next noise levels; tau: fp32 [batch] choice temperatures.  For sample b with tau[b] >= 0 and N candidate tokens
+ * (those inside region, all without one): u_j is the uniform pb200_add_noise_region draws for the token (same stream and element,
+ * so the offset consumed is the same), k_j = logp_j + (tau t) g_j with g_j = -logf(-logf(u_j)) (each operation rounded in fp32),
+ * and the n = floor(fp32(t * N)) candidates with the smallest keys are renoised, ties to the lower token index; a NaN key ranks
+ * below every other.  A sample with tau[b] < 0 is pb200_add_noise_region's own rule (u <= t), bit for bit, and one with t < 0
+ * keeps its tokens.  out = where(region, where(mask, random_x, x), src); mask_out (or NULL) = the renoised tokens.  random_x is
+ * required; src and region are both NULL or both set.  hw <= 32768 (the selection keeps a sample's keys in shared memory). */
+int pb200_renoise_confidence(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region, const float* logp,
+                             const float* t, const float* tau, int64_t batch, int64_t hw, uint64_t seed, uint64_t offset,
+                             int64_t* out, int64_t* mask_out, void* stream);
+/* pb200_renoise_confidence on per-sample streams, replacing pb200_add_noise_region_per_sample: sample b draws on
+ * seed_offset[b]; slot (int32 [batch] or NULL = identity) places its rows of random_x, src, region and out at slot[b]; x, logp
+ * and mask_out are by sample. */
+int pb200_renoise_confidence_per_sample(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region,
+                                        const int* slot, const float* logp, const float* t, const float* tau, int64_t batch,
+                                        int64_t hw, const uint64_t* seed_offset, int64_t* out, int64_t* mask_out, void* stream);
 /* out[b] = pool[slot[b]] for rows of hw int64 tokens (b < batch): a step batch gathered from a token pool. */
 int pb200_gather_rows(const int64_t* pool, const int* slot, int64_t batch, int64_t hw, int64_t* out, void* stream);
 
@@ -666,6 +684,14 @@ int64_t pb200_paella_token_scores_workspace_bytes(const pb200_paella* m, int bat
 int pb200_paella_token_scores(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
                               const int64_t* targets, float* nll_out, float* smooth_out, int64_t* argmax_out, void* workspace,
                               int64_t workspace_bytes, void* stream);
+/* The log-probability of each drawn token under the distribution the fused sampler drew it from, for confidence-guided
+ * renoising: replaces the log_softmax(logits / T) the reference would materialise.  The rows and the n_pairs mix are
+ * pb200_paella_token_scores's (the A operand pb200_paella_sample_tokens_pairs feeds the sampler; with n_pairs = 0 that of
+ * pb200_paella_sample_tokens_params with cfg_on = 0), and params (fp32 [batch][3], required) also gives each sample's 1/T
+ * (column 2).  logp_out fp32 [batch*hw] = s_y - logsumexp(s), s = l * (1/T) rounded once per logit, y = tokens[row]; at 1/T = 1
+ * this is -nll of pb200_paella_token_scores bit for bit.  workspace: pb200_paella_token_scores_workspace_bytes(batch, hw). */
+int pb200_paella_token_logprob(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                               const int64_t* tokens, float* logp_out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * VQGAN (ref/src/vqgan.py:45-107).

@@ -187,6 +187,12 @@ SIGNATURES = {
     "pb200_paella_token_scores_workspace_bytes": (c_int64, [c_void_p, c_int, c_int]),
     "pb200_paella_token_scores": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p, c_int64, c_void_p]),
+    "pb200_paella_token_logprob": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+                                           c_void_p]),
+    "pb200_renoise_confidence": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
+                                         c_uint64, c_uint64, c_void_p, c_void_p, c_void_p]),
+    "pb200_renoise_confidence_per_sample": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                    c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pb200_paella_logits":(c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p]),
     "pb200_paella_sample_tokens": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_double, c_uint64,
                                            c_uint64, c_void_p, c_void_p, c_int64, c_void_p]),

@@ -17,6 +17,7 @@
 #include "lora.cuh"
 #include "ops.cuh"
 #include "sampler.cuh"
+#include "confidence/confidence.h"
 #include "score.cuh"
 
 namespace pb {
@@ -1246,6 +1247,34 @@ int pb200_paella_token_scores(pb200_paella* m, const float* features, int batch,
     PB_TRY(launch_mix_cast_rows_f16(features, features + rows * c.c_out, params, (int64_t)hw * c.c_out, mixed, a16, st));
     PB_TRY(launch_cast_f16(features + mixed, rows * c.c_out - mixed, a16 + mixed, st));
     return launch_token_scores(a16, rows, c.c_out, m->w<__half>(m->out_w), c.num_labels, targets, nll_out, smooth_out, argmax_out, st);
+}
+
+int pb200_paella_token_logprob(pb200_paella* m, const float* features, int batch, int n_pairs, int hw, const float* params,
+                               const int64_t* tokens, float* logp_out, void* workspace, int64_t workspace_bytes, void* stream) {
+    PB_CHECK(m != nullptr && m->blob != nullptr, "token_logprob: weights not bound");
+    PB_CHECK(batch >= 0 && hw >= 0 && n_pairs >= 0 && n_pairs <= batch, "token_logprob: %d pairs among %d samples", n_pairs, batch);
+    PB_CHECK(params != nullptr, "token_logprob: params (the per-sample 1/T) is required");
+    const pb200_paella_config& c = m->cfg;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t rows = (int64_t)batch * hw;
+    if (rows == 0) return 0;
+    PB_CHECK(features != nullptr && tokens != nullptr && logp_out != nullptr, "token_logprob: features, tokens and logp_out are required");
+    PB_CHECK(rows * c.c_out * 2 <= workspace_bytes, "token_logprob: workspace too small (use pb200_paella_token_scores_workspace_bytes)");
+    __half* a16 = reinterpret_cast<__half*>(workspace);
+    // the A operand pb200_paella_sample_tokens_pairs (and _params) feeds the sampler, as in pb200_paella_token_scores
+    const int64_t mixed = (int64_t)n_pairs * hw * c.c_out;
+    PB_TRY(launch_mix_cast_rows_f16(features, features + rows * c.c_out, params, (int64_t)hw * c.c_out, mixed, a16, st));
+    PB_TRY(launch_cast_f16(features + mixed, rows * c.c_out - mixed, a16 + mixed, st));
+    // token_logprob_kernel (libpaella_b200_confidence.so) shares token_score_kernel's layout: c_out <= 256, 128-row / 128-label boxes
+    PB_CHECK(c.c_out % 8 == 0 && c.c_out <= 256, "token_logprob: c_out=%d unsupported (<= 256, multiple of 8)", c.c_out);
+    PB_CHECK(rows < (1ll << 31), "token_logprob: %lld rows", (long long)rows);
+    CUtensorMap ta, tw;
+    PB_TRY(make_tmap_f16_2d(&ta, a16, rows, c.c_out, c.c_out, 128));
+    PB_TRY(make_tmap_f16_2d(&tw, m->w<__half>(m->out_w), c.num_labels, c.c_out, c.c_out, 128));
+    ProfScope prof("token_logprob", 2.0 * (double)rows * (double)c.num_labels * (double)c.c_out, st);
+    PB_CUDA(pbc_token_logprob_launch(&ta, &tw, (int)rows, c.num_labels, c.c_out, hw, params, tokens, logp_out, st));
+    prof_count_launch();
+    return 0;
 }
 
 // scratch of pb200_paella_resample_samples: fp16 features and fp32 logits of 2 * chunk sample blocks

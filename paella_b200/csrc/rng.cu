@@ -6,6 +6,7 @@
 //   Paella.add_noise     ref/src/modules.py:277-283  (and its explicit-mask form, the region sampling of utils._sample_core)
 // PyTorch-side arithmetic: ATen/native/cuda/DistributionTemplates.h, ATen/core/TransformationHelper.h.
 #include "common.cuh"
+#include "confidence/confidence.h"
 #include "ops.cuh"
 #include "paella_b200.h"
 
@@ -530,6 +531,41 @@ int pb200_gather_rows(const int64_t* pool, const int* slot, int64_t batch, int64
     gather_rows_kernel<<<dim3(ceil_div(hw, 256), (unsigned)batch), 256, 0, (cudaStream_t)stream>>>(pool, slot, hw, out);
     PB_LAUNCH_CHECK();
     return 0;
+}
+
+// confidence-guided renoise: validation, the Philox stream and launch bookkeeping here; renoise_confidence_kernel lives in
+// libpaella_b200_confidence.so (confidence/renoise.cu)
+static int renoise_confidence(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region, const int* slot,
+                              const float* logp, const float* t, const float* tau, int64_t batch, int64_t hw, TorchPhilox s,
+                              const uint64_t* seed_off, int64_t* out, int64_t* mask_out, cudaStream_t st) {
+    PB_CHECK(x != nullptr && random_x != nullptr && logp != nullptr && t != nullptr && tau != nullptr && out != nullptr,
+             "renoise_confidence: x, random_x, logp, t, tau and out are required");
+    PB_CHECK((src == nullptr) == (region == nullptr), "renoise_confidence: src and region must both be set or both be NULL");
+    PB_CHECK(hw >= 0 && hw <= PBC_RENOISE_MAX_HW, "renoise_confidence: %lld tokens per sample; the selection holds at most %d (a "
+             "181x181 grid) in shared memory", (long long)hw, PBC_RENOISE_MAX_HW);
+    PB_CHECK(batch >= 0 && batch < (1ll << 31), "renoise_confidence: batch %lld", (long long)batch);
+    if (batch == 0 || hw == 0) return 0;
+    PB_CUDA(pbc_renoise_confidence_launch(x, random_x, src, region, slot, logp, t, tau, batch, hw, s, seed_off, out, mask_out, st));
+    prof_count_launch();
+    return 0;
+}
+
+int pb200_renoise_confidence(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region, const float* logp,
+                             const float* t, const float* tau, int64_t batch, int64_t hw, uint64_t seed, uint64_t offset,
+                             int64_t* out, int64_t* mask_out, void* stream) {
+    PB_CHECK(offset % 4 == 0, "philox offset must be a multiple of 4");
+    if (batch * hw == 0) return 0;
+    return renoise_confidence(x, random_x, src, region, nullptr, logp, t, tau, batch, hw, make_torch_philox(seed, offset, batch * hw),
+                              nullptr, out, mask_out, (cudaStream_t)stream);
+}
+
+int pb200_renoise_confidence_per_sample(const int64_t* x, const int64_t* random_x, const int64_t* src, const uint8_t* region,
+                                        const int* slot, const float* logp, const float* t, const float* tau, int64_t batch,
+                                        int64_t hw, const uint64_t* seed_offset, int64_t* out, int64_t* mask_out, void* stream) {
+    PB_CHECK(seed_offset != nullptr, "renoise_confidence_per_sample: per-sample (seed, offset) table is NULL");
+    if (batch == 0 || hw == 0) return 0;
+    return renoise_confidence(x, random_x, src, region, slot, logp, t, tau, batch, hw, make_torch_philox(0, 0, hw), seed_offset, out,
+                              mask_out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -50,7 +50,10 @@ admission holds a request whose adapter would be the 33rd in flight, and everyth
 With ``pag=s`` or ``(s, blocks)`` a request gets perturbed-attention guidance as ``sample_notebook(..., pag=[entry])`` does: on each
 of its steps before sampling_conditional_steps, guided or not, one more denoiser row -- its perturbed forward, reading its own
 conditional slot, weight row, wrap byte and adapter -- follows the term rows, and its mix coefficients (c + s, ..., -s) ride in
-the step table with the row's AttnBlock mask; PAG draws nothing and needs no K/V slot.
+the step table with the row's AttnBlock mask; PAG draws nothing and needs no K/V slot.  With ``confidence_renoise=tau`` a request
+renoises its least likely tokens as ``sample_notebook(..., confidence_renoise=[tau])`` does (utils module docstring): on the
+request's renoising steps its tokens' log-probabilities come from the step's sampler operand (Paella.token_logprob) and its
+mask from the uniforms of its own mask draw; it draws nothing more.
 
 Each step orders its batch with the guided requests first: rows [0, n_pairs) are guided, [n_pairs, Bc) are not, and the
 unconditional rows of the guided ones follow as [Bc, Bc + n_pairs) (Paella.features with ``n_pairs``).  Per step the host
@@ -75,7 +78,10 @@ retires.  A step with no such row launches exactly as without maps.  A step in w
 row's source row in this step's order (-1 for the other rows) to the table and runs the injecting denoiser
 (pb200_paella_features_inject); a step with no such row launches exactly as without edits.  A step in which some row has a LoRA
 adapter adds each row's adapter index and scale to the table and runs the adapted denoiser (pb200_paella_features_lora); a step
-with no such row launches exactly as without adapters.  No adapter memory is reserved: an adapter lives in its LoraAdapter.
+with no such row launches exactly as without adapters.  No adapter memory is reserved: an adapter lives in its LoraAdapter.  A
+step in which some renoising row has a choice temperature adds each row's (-1 for the others) to the table, scores the step's drawn
+tokens (pb200_paella_token_logprob) and renoises every row in one pb200_renoise_confidence_per_sample launch in place of the
+add-noise launch, the other rows by add_noise's rule; a step with no such row launches exactly as without it.
 The host knows which
 requests finish at which step, so ``step()`` never synchronises.  Admission projects the conditioning of the requests admitted
 in one step together: one prepare_cond per run of contiguous slots with one sequence layout (``admission_runs``), conditional
@@ -104,7 +110,7 @@ class Request:
                  attn_weights: Optional[torch.Tensor] = None, keep_intermediates: bool = False,
                  region: Optional[torch.Tensor] = None, mode: str = "multinomial", quant_steps: Optional[int] = None,
                  top_k: int = 0, top_p: float = 1.0, wrap: int = 0, regions=None, terms=None, mix_coef=None,
-                 attention_maps: bool = False, maps_len: int = 0, attention_source=None, lora=None, pag=None):
+                 attention_maps: bool = False, maps_len: int = 0, attention_source=None, lora=None, pag=None, confidence: float = -1.0):
         self.steps, self.renoise_steps, self.cond_steps, self.guided = steps, renoise_steps, cond_steps, guided
         self.params, self.r = params, r          # CPU float32 [steps, 3] and [steps + 1]: rows of utils.sampling_schedule
         self.generator, self.inputs, self.uncond, self.init_x, self.decode = generator, inputs, uncond, init_x, decode
@@ -121,6 +127,7 @@ class Request:
         self.mix_coef = mix_coef                 # CPU float32 [cond_steps, row width]: the mixed steps' coefficients (guided:
         #                                          c, u, the terms, then -s with PAG; unguided with PAG: 1 + s, -s)
         self.pag = pag                           # perturbed-attention guidance: (scale, int64 AttnBlock mask) or None
+        self.confidence = confidence             # confidence-guided renoising: the choice temperature, -1 for none
         self.term_slot: List[int] = []           # the K/V slots of the terms
         self.want_maps, self.maps_len = attention_maps, maps_len      # attention maps, over maps_len conditioning keys
         self.attention_maps: Optional[torch.Tensor] = None            # float32 [maps_len, H, W], set at retirement
@@ -213,6 +220,9 @@ class StepPlan:
         # LoRA: each row's index into the step's distinct adapters (-1: none) and its scale, when some row has an adapter
         self.adapters, self.lora_id, self.lora_scale = ops.lora_rows([q.lora for q in order])
         self.loras = bool(self.adapters)
+        # confidence-guided renoising: each row's choice temperature (-1: add_noise's rule), when some renoising row has one
+        self.confident = any(rn and q.confidence >= 0 for q, rn in zip(order, self.renoise))
+        self.tau = torch.tensor([q.confidence for q in order], dtype=torch.float32)
 
 
 def cond_layout(inputs: Dict[str, torch.Tensor]) -> Tuple[int, bool, int]:
@@ -238,13 +248,14 @@ def admission_runs(writes: List[Tuple[int, Tuple[int, bool, int]]]) -> List[List
 
 def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tuple[torch.Tensor, Dict[str, Tuple[str, int, int]]]:
     """The step's one host-to-device buffer: int64 [(seed, offset) pairs of the sampler's draw, then of the mask draw], then the
-    float32 part [r, params (3 per row), t_next, (top_p), (mix_coef), (lora_scale)], then the int32 part [row_slot, kv_slot, (mode
+    float32 part [r, params (3 per row), t_next, (top_p), (mix_coef), (lora_scale), (tau)], then the int32 part [row_slot, kv_slot, (mode
     table), (top_k), (tail, mix_rows), (map_row), (inj_src), (lora_id), (w_row)], then the uint8 part [(wrap)], each part padded to
     whole int64 words, then (pag): the int64 AttnBlock mask of every row, tail included, with w_row (each row's weight-pool row)
     only when some row is perturbed this step (perturbed-attention guidance).  top_p / top_k are present only when ``plan.truncates``, the mode table only when the step mixes modes, wrap (one
     byte per row) only when ``plan.wraps``, the tail map and the mix table only when some row of the step is composed (guidance
     prompts), map_row only when some row wants attention maps, inj_src only when some edit is inside its window, lora_id and
-    lora_scale only when some row has a LoRA adapter (the adapters' blob pointers travel as kernel arguments).  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
+    lora_scale only when some row has a LoRA adapter (the adapters' blob pointers travel as kernel arguments), tau only when some
+    renoising row has a choice temperature (confidence-guided renoising).  Returns (buffer, {name: (dtype, start, length)}), start and length in elements of that dtype within its part."""
     Bc, n_pairs = len(plan.order), plan.n_pairs
     mixed = not all(plan.draws)
     modes = ops.mode_table(plan.modes) if mixed else torch.zeros(0, dtype=torch.int32)
@@ -265,6 +276,8 @@ def step_host_table(plan: StepPlan, draw: List[int], renoise: List[int]) -> Tupl
         i32_parts.append(("lora_id", plan.lora_id))
     if plan.perturbed:
         i32_parts.append(("w_row", plan.pag_w_row))
+    if plan.confident:
+        f32_parts.append(("tau", plan.tau))
     u8_parts = [("wrap", plan.wrap)] if plan.wraps else []
     layout: Dict[str, Tuple[str, int, int]] = {}
     for dt, parts in (("f32", f32_parts), ("i32", i32_parts), ("u8", u8_parts)):
@@ -421,7 +434,7 @@ class SamplingEngine:
                temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None, init_x=None,
                decode=False, attn_weights=None, keep_intermediates=False, region=None, mode="multinomial",
                sampling_quant_steps=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
-               attention_maps=False, attention_source=None, lora=None, pag=None) -> Request:
+               attention_maps=False, attention_source=None, lora=None, pag=None, confidence_renoise=None) -> Request:
         """Queue one request: the arguments of ``sample_distributed`` with batch 1, plus its own CUDA generator, which no other
         request in flight may use.  Raises ValueError, before anything is enqueued and before any generator advances, for a
         missing or wrong generator, conditioning longer than max_cond_len, an init_x of the wrong shape, a temperature <= 0,
@@ -454,8 +467,10 @@ class SamplingEngine:
         as in sample_notebook: on the request's steps before sampling_conditional_steps, one more denoiser row, its perturbed
         forward, joins its mix (guided or not); it reads the request's conditional slot, weight row, wrap byte and adapter.
         ValueError for a bad entry (ops.pag_table), with ``prompt_regions``, and on an edit or a source.  The engine allocates
-        nothing for PAG until a request uses it (then one empty row of its weight pool).  The request's draws start when it is
-        admitted."""
+        nothing for PAG until a request uses it (then one empty row of its weight pool).  ``confidence_renoise`` (None or a choice
+        temperature tau, a finite float >= 0) renoises the request's least likely tokens as in sample_notebook; ValueError for any
+        other value and for a latent grid larger than the selection kernel takes (ops.confidence_table).  The request's draws
+        start when it is admitted."""
         attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
         if not isinstance(generator, torch.Generator) or generator.device.type != "cuda":
             raise ValueError(f"generator: one CUDA torch.Generator per request is required (got {type(generator).__name__})")
@@ -529,6 +544,9 @@ class SamplingEngine:
                 if attention_source is not None:
                     raise ValueError("pag: perturbed-attention guidance on a prompt-to-prompt edit is not supported")
                 pag_e = (pag_t[0][0], int(pag_t[1][0]))
+        if isinstance(confidence_renoise, (list, tuple)):
+            raise ValueError("confidence_renoise: a request takes one value (got a list)")
+        conf = ops.confidence_table(confidence_renoise, 1, self.H * self.W)
         cfgs = U._cfg_schedule(cfg, 1, steps)
         params, r = U.sampling_schedule(1, steps, temperature, cfgs, t_start, t_end, torch.is_tensor(cfg), always=True)
         mix_coef = None
@@ -547,7 +565,8 @@ class SamplingEngine:
         req = Request(steps, renoise_steps, cond_steps, cfgs is not None, params[:, 0], r[:, 0], generator, model_inputs,
                       unconditional_inputs, init_x, bool(decode), attn_weights, bool(keep_intermediates), region, mode,
                       sampling_quant_steps, *((int(trunc[0][0]), float(trunc[1][0])) if trunc is not None else (0, 1.0)), wrap, regions,
-                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs), attention_source, lora, pag_e)
+                      terms, mix_coef, attention_maps, self.model.conditioning_seq_len(model_inputs), attention_source, lora, pag_e,
+                      float(conf[0]) if conf is not None else -1.0)
         if attention_source is not None:
             attention_source[0].edits.append(req)
         self._gens.add(id(generator))
@@ -742,8 +761,13 @@ class SamplingEngine:
                                            if q.has_region else sampled[i:i + 1].clone())
             # every row back into its slot, renoised or not; with a region in the batch, each row's source tokens outside it
             regions = any(q.has_region for q in plan.order)
-            ops.add_noise_per_sample(sampled, t_next_d, self.noise, m.num_labels, renoise_d, self.tokens, slot=row_slot_d,
-                                     src=self.src if regions else None, region=self.region if regions else None)
+            if plan.confident:      # the rows' confidence from the operand the step's sampler read
+                logp = m.token_logprob(feats, Bc, n_pairs, hw, params_d, sampled)
+                ops.renoise_confidence_per_sample(sampled, t_next_d, part("tau"), logp, self.noise, renoise_d, self.tokens, slot=row_slot_d,
+                                                  src=self.src if regions else None, region=self.region if regions else None)
+            else:
+                ops.add_noise_per_sample(sampled, t_next_d, self.noise, m.num_labels, renoise_d, self.tokens, slot=row_slot_d,
+                                         src=self.src if regions else None, region=self.region if regions else None)
             for q, rn in zip(plan.order, plan.renoise):
                 if q.intermediates is not None and rn:
                     q.intermediates.append(self.tokens[q.slot:q.slot + 1].clone())

@@ -1356,10 +1356,42 @@ class Paella(nn.Module):
             self._cond_single = memos
         return cond
 
-    def add_noise(self, x, t, mask=None, random_x=None, generator=None, src=None, region=None):
+    def token_logprob(self, feats: torch.Tensor, batch: int, n_pairs: int, hw: int, params: torch.Tensor,
+                      tokens: torch.Tensor) -> torch.Tensor:
+        """fp32 log_softmax(l * (1/T))[token] per token, shaped like ``tokens`` (int64, batch * hw codes on the device): l the logits
+        of the fp16 operand the fused sampler reads from ``feats`` (sample_tokens_pairs' rows: samples b < n_pairs mixed with their
+        unconditional rows by ``params`` [batch, 3], the others cast) and 1/T params column 2 (pb200_paella_token_logprob, whose
+        logits never reach HBM).  The confidence of confidence-guided renoising (utils module docstring)."""
+        self._ensure_packed()
+        L = lib()
+        dev = self._device()
+        with torch.cuda.device(dev):
+            out = torch.empty(tokens.shape, dtype=torch.float32, device=dev)
+            ws = self._ws(L.pb200_paella_token_scores_workspace_bytes(self._handle, batch, hw))
+            check(L.pb200_paella_token_logprob(self._handle, ptr(feats), batch, n_pairs, hw, ptr(params), ptr(tokens.contiguous()),
+                                               ptr(out), ptr(ws), ws.numel(), current_stream()), "pb200_paella_token_logprob")
+        return out
+
+    def add_noise(self, x, t, mask=None, random_x=None, generator=None, src=None, region=None, confidence=None,
+                  choice_temperature=0.0):
         """ref/src/modules.py:277-283 on torch's random stream (``generator``: as in ``sample_tokens``).  ``src`` and ``region``
         (device tensors shaped like x, with mask=None): the tokens outside the region are src's and are never renoised
-        (ops.add_noise)."""
+        (ops.add_noise).  ``confidence`` (fp32 like x, with mask=None: each token's log-probability, token_logprob) renoises each
+        sample's floor(t N) least likely tokens instead, ranked by confidence + tau t Gumbel(u) on the uniforms this call draws
+        anyway (utils module docstring; ops.renoise_confidence): ``choice_temperature`` is tau, one value >= 0, a list of B entries
+        each None (add_noise's rule) or tau, or a device float32 [B] table (ops.confidence_table's encoding).  ``random_x`` (the
+        replacement codes, e.g. the loop's initial noise) is required with confidence."""
+        if confidence is not None:
+            if mask is not None or random_x is None:
+                raise ValueError("add_noise: confidence picks the mask itself and needs random_x (the replacement codes)")
+            B = x.shape[0]
+            if torch.is_tensor(choice_temperature):
+                tau = choice_temperature
+            else:
+                tau = ops.confidence_table(choice_temperature, B, x[0].numel())
+                tau = torch.full((B,), -1.0) if tau is None else tau
+                tau = ops.to_device_async(tau, x.device)
+            return ops.renoise_confidence(x, t, tau, confidence, random_x, generator, src=src, region=region)
         if mask is None:
             return ops.add_noise(x, t, random_x, self.num_labels, generator, src=src, region=region)
         if region is not None:

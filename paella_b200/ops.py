@@ -724,6 +724,38 @@ def pag_table(pag, batch: int, n_blocks: int, default_blocks=None, regions=None,
     return [s for s, _ in entries], torch.tensor([_mask_i64(m) for _, m in entries], dtype=torch.int64)
 
 
+# ------------------------------------------------------------------ confidence-guided renoising
+MAX_CONFIDENCE_TOKENS = 32768       # pb200_renoise_confidence keeps a sample's keys (4 bytes per token) in shared memory
+
+
+def _confidence_tau(name: str, v) -> float:
+    if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or v < 0:
+        raise ValueError(f"{name}: the choice temperature must be a finite real number >= 0 (got {v!r})")
+    return float(v)
+
+
+def confidence_table(confidence_renoise, batch: int, hw: Optional[int] = None) -> Optional[torch.Tensor]:
+    """``confidence_renoise`` (None, one choice temperature tau for every sample, or a list or tuple of ``batch`` entries, each
+    None or tau) -> None when no sample has an entry, otherwise the CPU float32 [batch] table pb200_renoise_confidence reads:
+    tau, or -1 for a sample renoised at random as add_noise does.  ValueError, before anything is enqueued, for the wrong
+    length, a bool, negative or non-finite tau, and (``hw``: tokens per sample) a grid of more than MAX_CONFIDENCE_TOKENS tokens."""
+    if confidence_renoise is None:
+        return None
+    if isinstance(confidence_renoise, (list, tuple)):
+        if len(confidence_renoise) != batch:
+            raise ValueError(f"confidence_renoise: got {len(confidence_renoise)} entries for a batch of {batch} (one per sample, "
+                             "None for none)")
+        taus = [-1.0 if v is None else _confidence_tau(f"confidence_renoise[{b}]", v) for b, v in enumerate(confidence_renoise)]
+    else:
+        taus = [_confidence_tau("confidence_renoise", confidence_renoise)] * batch
+    if all(v < 0 for v in taus):
+        return None
+    if hw is not None and hw > MAX_CONFIDENCE_TOKENS:
+        raise ValueError(f"confidence_renoise: a latent grid of {hw} tokens; the selection kernel takes at most "
+                         f"{MAX_CONFIDENCE_TOKENS} per sample (e.g. 128 x 256)")
+    return torch.tensor(taus, dtype=torch.float32)
+
+
 # The notebook's sampling modes (paella_inference.ipynb cell 3).  'multinomial' draws H*W*num_labels exponentials per step; 'argmax'
 # and 'quant' draw nothing.  A step with several modes sends one int32 table to the device: the mode code of every sample, then
 # the samples in argmax mode, then the samples in quant mode, each list ascending.
@@ -991,6 +1023,42 @@ def add_noise_per_sample(x: torch.Tensor, t: torch.Tensor, random_x: Optional[to
     check(lib().pb200_add_noise_region_per_sample(ptr(x), ptr(random_x), ptr(src), ptr(_region_u8(region)), ptr(slot), ptr(t), B, hw,
                                                   num_labels, ptr(table), ptr(out), ptr(mask), current_stream()),
           "pb200_add_noise_region_per_sample")
+
+
+def renoise_confidence(x: torch.Tensor, t: torch.Tensor, tau: torch.Tensor, logp: torch.Tensor, random_x: torch.Tensor, generator=None,
+                       src: Optional[torch.Tensor] = None, region: Optional[torch.Tensor] = None):
+    """add_noise with the confidence rule (pb200_renoise_confidence): sample b (tau fp32 [B] on the device, >= 0) renoises its
+    floor(t_b N) tokens of smallest key logp + tau t g(u), u being the uniforms add_noise draws; a sample with tau < 0 is
+    add_noise's.  ``logp``: fp32, x's log-probabilities (Paella.token_logprob).  Takes exactly add_noise's draws from ``generator``
+    (None, one, or a list of B).  ``random_x`` is required.  Returns (out, mask) like add_noise."""
+    x = x.contiguous()
+    B, hw = x.shape[0], x[0].numel()
+    out, mask = torch.empty_like(x), torch.empty_like(x)
+    src = src.contiguous() if src is not None else None
+    args = (ptr(x), ptr(random_x.contiguous()), ptr(src), ptr(_region_u8(region)))
+    rest = (ptr(logp.contiguous()), ptr(t.contiguous().float()), ptr(tau.contiguous()), B, hw)
+    if per_sample(generator):
+        check_generators(generator, B, x.device)
+        check_per_sample_numel(hw)
+        table = philox_table(generator, hw, x.device)
+        check(lib().pb200_renoise_confidence_per_sample(*args, None, *rest, ptr(table), ptr(out), ptr(mask), current_stream()),
+              "pb200_renoise_confidence_per_sample")
+        return out, mask
+    seed, off = take_philox(x.numel(), x.device, generator)
+    check(lib().pb200_renoise_confidence(*args, *rest, seed, off, ptr(out), ptr(mask), current_stream()), "pb200_renoise_confidence")
+    return out, mask
+
+
+def renoise_confidence_per_sample(x: torch.Tensor, t: torch.Tensor, tau: torch.Tensor, logp: torch.Tensor, random_x: torch.Tensor,
+                                  table: torch.Tensor, out: torch.Tensor, mask: Optional[torch.Tensor] = None,
+                                  slot: Optional[torch.Tensor] = None, src: Optional[torch.Tensor] = None,
+                                  region: Optional[torch.Tensor] = None) -> None:
+    """add_noise_per_sample with the confidence rule of renoise_confidence, in one launch: the same (seed, offset) ``table``, slot
+    map, src and region; ``logp`` fp32 by sample like x, ``tau`` fp32 [B] (< 0: add_noise_per_sample's rule)."""
+    B, hw = x.shape[0], x[0].numel()
+    check(lib().pb200_renoise_confidence_per_sample(ptr(x), ptr(random_x), ptr(src), ptr(_region_u8(region)), ptr(slot), ptr(logp),
+                                                    ptr(t), ptr(tau), B, hw, ptr(table), ptr(out), ptr(mask), current_stream()),
+          "pb200_renoise_confidence_per_sample")
 
 
 def gather_rows(pool: torch.Tensor, slot: torch.Tensor, out: torch.Tensor) -> torch.Tensor:

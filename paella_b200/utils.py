@@ -117,6 +117,29 @@ of the call without it, bit for bit.  ValueError, before anything is enqueued an
 a non-finite or bool scale, empty, duplicated, non-int or out-of-range blocks, PAG on a sample with ``prompt_regions`` or on a
 prompt-to-prompt edit or source, and ``exact=True`` (ops.pag_table).
 
+Confidence-guided renoising: ``confidence_renoise`` (all three functions; None, one choice temperature tau for every sample, or a
+list or tuple of B entries, each None or tau, a finite float >= 0) renoises sample i's least likely tokens instead of a random set,
+as MaskGIT and Muse do (Chang et al. 2022, "MaskGIT", section 3.2).  On every renoising step s < renoise_steps a sample with an
+entry is renoised as follows, x being the step's drawn token grid:
+  1. confidence: c_j = log_softmax(l * (1/T_s))[x_j] per token, l the out_mapper product of the same fp16 operand the step's
+     sampler consumed (CFG pre-mixed; guidance prompts and PAG mixed in place), T_s the sample's temperature at the step, the
+     product rounded once.  It is computed so whatever drew the tokens (multinomial, argmax, quant, truncated), always under the
+     untruncated tempered distribution (Paella.token_logprob; pb200_paella_token_logprob).
+  2. count: n = floor(t * N) in fp32, t = t_{s+1} the sample's next noise level (the level add_noise renoises to) and N = H*W, or
+     the number of tokens in the sample's ``region`` when inpainting.
+  3. key: k_j = c_j + (tau * t) * g_j in fp32, g_j = -logf(-logf(u_j)), u_j exactly the uniform add_noise would draw for token j:
+     same generator, same offset, same Philox element, so the generator's draws and final offset are unchanged.  A u of 0 gives
+     g = -inf; a NaN key ranks lowest (renoised first).
+  4. renoise: the n tokens with the smallest keys are renoised, ties broken by ascending token index; a renoised token becomes the
+     initial noise's code, as with add_noise.  Tokens outside a ``region`` are never candidates and stay init_x's.
+With the default schedule t_{s+1} = 1 - (s+1)/steps, tau * t is MaskGIT's annealed choice temperature tau (1 - ratio).  Samples
+without an entry are, bit for bit, those of the call without the argument, and a call with no entries launches exactly what it
+launches without it.  No extra random numbers are drawn, so every generator ends at the same offset and the per-sample guarantees
+above hold for confidence rows too.  A call with an entry takes the per-sample table path.  ValueError, before anything is enqueued
+and before any generator advances, for the wrong length, a bool, negative or non-finite tau, ``exact=True``, and a latent grid of more
+than 32768 tokens (the selection kernel keeps a sample's keys in shared memory; ops.confidence_table, pb200_renoise_confidence).  Its
+effect on image quality is not measured here (there are no trained weights).
+
 Scoring: ``score`` asks the denoiser how likely a given token grid is under a prompt -- held-out evaluation of a checkpoint with
 train.py's objective, reranking of candidates, or picking the prompt that best explains an image.  It noises the tokens at each
 of a list of noise levels, as add_noise does, and scores each noised grid against the clean tokens with Paella.token_scores
@@ -229,7 +252,8 @@ def outpaint_canvas(tokens: torch.Tensor, canvas_hw, top: int, left: int) -> Tup
 def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs, init_x, steps, renoise_steps, temperature,
                  cfgs, t_start, t_end, sampling_conditional_steps, mode, attn_weights, exact, collect, sampling_quant_steps=None,
                  codebook=None, generator=None, per_sample_cfg=False, region=None, modes=None, top_k=None, top_p=None, tiling=None,
-                 prompt_regions=None, guidance_prompts=None, attention_maps=False, attention_source=None, lora=None, pag=None):
+                 prompt_regions=None, guidance_prompts=None, attention_maps=False, attention_source=None, lora=None, pag=None,
+                 confidence_renoise=None):
     """Returns (tokens, intermediates, maps or None).  ``modes``: None, or per step the list of B mode names (sampling_modes) --
     a step whose modes differ samples each row in its own mode (Paella.sample_tokens_modes), a step whose modes agree takes the
     scalar path in that mode.  ``top_k`` / ``top_p``: the truncation of the multinomial draws (module docstring); a truncating
@@ -237,7 +261,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     the maps of the conditional rows (module docstring).  ``attention_source``: prompt-to-prompt injection (module docstring);
     step i passes row i of the table to the denoiser, or nothing when no sample is injected there.  ``lora``: per-sample LoRA
     adapters (module docstring).  ``pag``: perturbed-attention guidance (module docstring): on steps i < sampling_conditional_steps
-    each perturbed sample has one more tail row, after the term rows, and joins the composed samples of the guided mix."""
+    each perturbed sample has one more tail row, after the term rows, and joins the composed samples of the guided mix.
+    ``confidence_renoise``: confidence-guided renoising (module docstring): each renoising step scores the drawn tokens on the
+    step's own sampler operand and renoises with pb200_renoise_confidence in place of add_noise."""
     B, H, W = latent_shape
     dev = model._device()
     attention_maps = ops.check_attention_maps(attention_maps, prompt_regions)
@@ -256,6 +282,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
     extra_lora = [entries[b] for b, own in enumerate(regions[1]) for _ in own] if regions is not None else []
     if exact and trunc is not None:
         raise ValueError("exact=True restates the reference op for op, which has no top_k / top_p truncation")
+    conf = ops.confidence_table(confidence_renoise, B, H * W)
+    if exact and conf is not None:
+        raise ValueError("exact=True restates the reference op for op, which has no confidence-guided renoising")
     use_cfg_any = cfgs is not None
     if terms is not None and exact:
         raise ValueError("exact=True restates the reference op for op, which has no guidance prompts")
@@ -263,7 +292,7 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
         raise ValueError("guidance_prompts need a guided call (cfg is None or 0)")
     mixed_steps = modes is not None and any(len(set(ms)) > 1 for ms in modes)
     sched = sampling_schedule(B, steps, temperature, cfgs, t_start, t_end, per_sample_cfg,
-                              always=mixed_steps or trunc is not None or terms is not None or pag_t is not None)
+                              always=mixed_steps or trunc is not None or terms is not None or pag_t is not None or conf is not None)
     mix = None
     pag_src = []
     n_mix = min(steps, sampling_conditional_steps)
@@ -317,7 +346,9 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
             pag_rows = torch.zeros(n_rows, dtype=torch.int64)
             pag_rows[n_rows - len(pag_src):] = pag_t[1][pag_src]
             parts += [pag_rows] + ([w_row] if w_row is not None else [])
+        parts += [conf] if conf is not None else []
         parts_d = ops.to_device_packed(parts, dev) if parts else []
+        conf_d = parts_d.pop() if conf is not None else None
         w_row_d = parts_d.pop() if w_row is not None else None
         pag_rows_d = parts_d.pop() if pag_src else None
         inj_d = parts_d.pop() if any(inj_steps) else None
@@ -426,7 +457,11 @@ def _sample_core(model: Paella, model_inputs, latent_shape, unconditional_inputs
                     t_next = torch.full((B,), float(t_list[i + 1]), dtype=torch.float32, device=dev)
                 else:
                     t_next = r_d[i + 1]
-                if region_d is None:
+                if conf_d is not None:      # confidence from the operand the step's sampler read
+                    logp = model.token_logprob(feats, B, B if guided else 0, H * W, params_i, sampled)
+                    sampled = model.add_noise(sampled, t_next, random_x=init_noise, generator=generator, src=src_d if region_d is not None
+                                              else None, region=region_d, confidence=logp, choice_temperature=conf_d)[0]
+                elif region_d is None:
                     sampled = model.add_noise(sampled, t_next, random_x=init_noise, generator=generator)[0]
                 else:
                     sampled = model.add_noise(sampled, t_next, random_x=init_noise, generator=generator, src=src_d, region=region_d)[0]
@@ -574,7 +609,7 @@ def _decode_tail(tokens, decode, decode_output, tiling=None):
 def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=12, renoise_steps=11, temperature=(1.0, 0.2),
            cfg=8.0, t_start=1.0, t_end=0.0, device="cuda", exact=False, decode=None, decode_output="uint8", generator=None,
            top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None, attention_maps=False,
-           attention_source=None, lora=None, pag=None):
+           attention_source=None, lora=None, pag=None, confidence_renoise=None):
     """ref/src/utils.py:35-55 (same positional/keyword arguments; ``device`` is accepted and must be the model's).
     ``exact=True`` materialises the logits and uses the op-for-op torch arithmetic (parity path).
     ``decode=vqmodel`` appends the reference callers' next step, ``vqmodel.decode_indices(tokens).clamp(0, 1)``, fused on the
@@ -594,7 +629,8 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
     ``attention_maps=True`` (module docstring): returns (tokens or images, maps).  ``attention_source`` (module docstring):
     prompt-to-prompt edits of other samples of the call; give each edit its own generator seeded like its source's.
     ``lora`` (module docstring): a LoRA adapter per sample, or one for every sample.  ``pag`` (module docstring):
-    perturbed-attention guidance per sample, with CFG or without it."""
+    perturbed-attention guidance per sample, with CFG or without it.  ``confidence_renoise`` (module docstring): renoise each
+    sample's least likely tokens, one choice temperature for every sample or one entry per sample."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     per_sample_cfg = torch.is_tensor(cfg)
     terms = ops.guidance_table(guidance_prompts, latent_shape[0])
@@ -614,7 +650,7 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
                                 temperature, cfgs, t_start, t_end, steps, "multinomial", None, exact, False, generator=generator,
                                 per_sample_cfg=per_sample_cfg, top_k=top_k, top_p=top_p, tiling=tiling,
                                 prompt_regions=prompt_regions, guidance_prompts=guidance_prompts, attention_maps=attention_maps,
-                                attention_source=attention_source, lora=lora, pag=pag)
+                                attention_source=attention_source, lora=lora, pag=pag, confidence_renoise=confidence_renoise)
     out = _decode_tail(out, decode, decode_output, tiling)
     return (out, maps) if attention_maps else out
 
@@ -622,7 +658,8 @@ def sample(model, model_inputs, latent_shape, unconditional_inputs=None, steps=1
 def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, init_x=None, steps=12, renoise_steps=None,
                        temperature=(0.7, 0.3), cfg=(8.0, 8.0), t_start=1.0, t_end=0.0, sampling_conditional_steps=None,
                        exact=False, generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None,
-                       guidance_prompts=None, attention_maps=False, attention_source=None, lora=None, pag=None):
+                       guidance_prompts=None, attention_maps=False, attention_source=None, lora=None, pag=None,
+                       confidence_renoise=None):
     """ref/src_distributed/utils.py:97-126.  ``generator`` as in ``sample``: a shard given ``generators[lo:hi]`` draws what
     rows [lo, hi) of the single-GPU call draw.  Per-sample settings (module docstring): ``cfg`` and ``temperature`` [B, 2],
     ``t_start`` / ``t_end`` [B]; a shard given ``settings[lo:hi]`` computes what rows [lo, hi) compute.  ``region`` (module
@@ -635,7 +672,9 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
     computes what rows [lo, hi) compute.  ``attention_maps=True`` (module docstring): returns (tokens, maps) for the shard's rows.
     ``attention_source`` (module docstring): a source and its edits sit in the same shard, with indices relative to the shard.
     ``lora`` (module docstring): a shard given ``lora[lo:hi]`` computes what rows [lo, hi) compute; each rank loads its adapters
-    itself (load_lora).  ``pag`` (module docstring) likewise: a shard given ``pag[lo:hi]`` computes what rows [lo, hi) compute."""
+    itself (load_lora).  ``pag`` (module docstring) likewise: a shard given ``pag[lo:hi]`` computes what rows [lo, hi) compute.
+    ``confidence_renoise`` (module docstring) likewise: a shard given ``confidence_renoise[lo:hi]`` computes what rows [lo, hi)
+    compute."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -646,7 +685,8 @@ def sample_distributed(model, model_inputs, unconditional_inputs, latent_shape, 
                                 temperature, cfgs, t_start, t_end, sampling_conditional_steps, "multinomial", None, exact, False,
                                 generator=generator, per_sample_cfg=torch.is_tensor(cfg), region=region, top_k=top_k, top_p=top_p,
                                 tiling=tiling, prompt_regions=prompt_regions, guidance_prompts=guidance_prompts,
-                                attention_maps=attention_maps, attention_source=attention_source, lora=lora, pag=pag)
+                                attention_maps=attention_maps, attention_source=attention_source, lora=lora, pag=pag,
+                                confidence_renoise=confidence_renoise)
     return (out, maps) if attention_maps else out
 
 
@@ -654,7 +694,7 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                     temperature=(0.7, 0.3), cfg=(8.0, 8.0), mode='multinomial', t_start=1.0, t_end=0.0,
                     sampling_conditional_steps=None, sampling_quant_steps=None, attn_weights=None, exact=False, vqmodel=None,
                     generator=None, region=None, top_k=None, top_p=None, tiling=None, prompt_regions=None, guidance_prompts=None,
-                    attention_maps=False, attention_source=None, lora=None, pag=None):
+                    attention_maps=False, attention_source=None, lora=None, pag=None, confidence_renoise=None):
     """paella_inference.ipynb cell 3: returns (sampled, intermediate_images).  ``vqmodel`` replaces the notebook's global
     of the same name for ``mode='quant'`` / ``sampling_quant_steps`` (softmax @ codebook -> nearest code).  ``generator`` as
     in ``sample``; per-sample settings as in ``sample_distributed``.  ``attn_weights``: one 1-D tensor for every sample, or a
@@ -674,7 +714,8 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
     (sampled, intermediate_images, maps).  ``attention_source`` (module docstring): prompt-to-prompt edits; an edit's
     ``attn_weights`` reweight the replayed probabilities.  ``lora`` (module docstring): a LoRA adapter per sample.  ``pag``
     (module docstring): perturbed-attention guidance per sample; its perturbed row carries the sample's ``attn_weights``, and the
-    argmax and quant steps see the mixed features."""
+    argmax and quant steps see the mixed features.  ``confidence_renoise`` (module docstring): renoise each sample's least likely
+    tokens; the intermediates show the renoised grids."""
     ops.check_attention_maps(attention_maps, prompt_regions)
     if sampling_conditional_steps is None:
         sampling_conditional_steps = steps
@@ -695,5 +736,6 @@ def sample_notebook(model, model_inputs, latent_shape, unconditional_inputs=None
                                                 per_sample_cfg=torch.is_tensor(cfg), region=region, modes=modes, top_k=top_k,
                                                 top_p=top_p, tiling=tiling, prompt_regions=prompt_regions,
                                                 guidance_prompts=guidance_prompts, attention_maps=attention_maps,
-                                                attention_source=attention_source, lora=lora, pag=pag)
+                                                attention_source=attention_source, lora=lora, pag=pag,
+                                                confidence_renoise=confidence_renoise)
     return (sampled, intermediates, maps) if attention_maps else (sampled, intermediates)
