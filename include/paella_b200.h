@@ -248,6 +248,50 @@ int pb200_grn_f32(const float* x, int batch, int rows_per_sample, int n, const f
  * [ref/src/modules.py:104-106] */
 int pb200_film_apply(float* x, int64_t rows, int n, int rows_per_sample, const float* film, int64_t film_ld, int64_t film_off,
                      void* stream);
+/* ------------------------------------------------------------------------------------------
+ * Executor kernels exposed for testing: the launchers the model executor below runs from its plan,
+ * with every argument it passes them, so that each kernel can be checked on its own against a
+ * high-precision reference.  A refusal returns nonzero (pb200_last_error) with nothing enqueued.
+ * ------------------------------------------------------------------------------------------ */
+/* in_mapper (Embedding + LayerNorm, eps 1e-6) + PixelUnshuffle(patch): tokens int64 [batch, h, w] (clamped to
+ * [0, num_labels)), emb fp32 [num_labels, c_in] -> fp16 [batch*(h/patch)*(w/patch), c_in*patch^2], column c*patch^2 +
+ * dy*patch + dx; c_in*patch^2 <= 3072   [ref/src/modules.py:126-131,271] */
+int pb200_embed_tokens(const int64_t* tokens, const float* emb, int num_labels, int c_in, int batch, int h, int w, int patch,
+                       void* out16, void* stream);
+/* LayerNorm over rows of c % 4 == 0 fp32 values (eps 1e-6) with a scalar affine: y = (x-mean)*rstd*scale + shift into exactly
+ * one of out16 / out32 (out32 may be x: in place); mean_out (optional) fp32 [rows] = the row means */
+int pb200_ln_rows(const float* x, int64_t rows, int c, float scale, float shift, void* out16, float* out32, float* mean_out,
+                  void* stream);
+/* LayerNorm2d + the im2col of Conv2d(k=2, s=2): x fp32 NHWC [batch, h, w, c] (h, w even, c % 4 == 0) -> fp16
+ * [batch*(h/2)*(w/2), 4c], column (dy*2 + dx)*c + ch   [ref/src/modules.py:153-156] */
+int pb200_ln_patchify2(const float* x, int batch, int h, int w, int c, void* out16, void* stream);
+/* every TimestepBlock mapper at once: out[b, j] = bias[j] + sum_i r_embed[b, i] * weight[j, i]; weight fp32 [total, c_r]
+ * [ref/src/modules.py:99-106] */
+int pb200_film_table(const float* r_embed, int batch, int c_r, const float* weight, const float* bias, int total, float* out,
+                     void* stream);
+/* out16[i] = fp16(a[i]*wa + b[i]*wb) (b NULL: a[i]*wa), i < n */
+int pb200_mix_cast_f16(const float* a, const float* b, float wa, float wb, int64_t n, void* out16, void* stream);
+/* the same mix with per-sample weights: element e of sample s = e / per uses (w[3s], w[3s+1]) (w DEVICE fp32 [samples][3]) */
+int pb200_mix_cast_rows_f16(const float* a, const float* b, const float* w, int64_t per, int64_t n, void* out16, void* stream);
+/* fp32 NHWC [batch, h, w, c] -> fp16 [batch, h+2, w+2, c] with a one-position border: circular copies on the axes wrap[b]
+ * (DEVICE uint8 [batch]; bit 0 x, bit 1 y) wraps, zeros on the others; c % 4 == 0 */
+int pb200_pad_cast_f16(const float* x, int batch, int h, int w, int c, const uint8_t* wrap, void* out16, void* stream);
+/* fp16 cast of whole samples of `per` fp32 elements into n_blocks packed blocks: block j < n_list is sample samples[j] of a,
+ * block j >= n_list is sample batch + samples[j - n_list] (samples DEVICE int32 [n_list]); per % 4 == 0, n_blocks <= 2*n_list */
+int pb200_gather_cast_f16(const float* a, const int* samples, int n_list, int n_blocks, int batch, int64_t per, void* out16,
+                          void* stream);
+/* sample n_base + i of base (per bytes per sample, base 16-byte aligned) becomes a copy of sample src[i] (DEVICE int32 [n_tail]) */
+int pb200_replicate_rows(void* base, int64_t per, int n_base, const int* src, int n_tail, void* stream);
+/* per-level regional masks: level l of out holds uint8 [batch][(h/s)*(w/s)], s = patch << l, at offset batch * (sum of the
+ * earlier levels' sizes); each value is the OR of its s x s footprint of token-mask row mask_row[b] (NULL: b) of tok_mask
+ * (DEVICE uint8 [rows, h*w]) */
+int pb200_regional_masks(const uint8_t* tok_mask, const int* mask_row, int batch, int h, int w, int patch, int n_levels, uint8_t* out,
+                         void* stream);
+/* pb200_paella_guidance_mix on `per` fp32 elements per sample (per % 4 == 0, features 16-byte aligned), without a model */
+int pb200_guidance_mix(float* features, int64_t per, const int* rows, const float* coef, int n_composed, int ld, void* stream);
+/* pb200_dwconv_ln_tiled on a CFG batch: sample b reads wrap[b < n_base ? b : b - n_base] (n_base <= batch <= 2*n_base) */
+int pb200_dwconv_ln_pairs(const float* x, const float* skip, const float* w_packed, const float* bias, int batch, int h, int w,
+                          int c, int k, const uint8_t* wrap, int n_base, void* out16, void* stream);
 /* Attention core of nn.MultiheadAttention / CustomMultiheadAttention after the in-projection:
  * qkv16 [batch*positions, 3*embed] = q | k_self | v_self, ckv16 [batch, s_max, 2*embed] = k_cond | v_cond
  * (kv_len[batch] valid rows, NULL = s_max); keys = [self ; cond] if self_attn else cond; optional post-softmax

@@ -102,6 +102,19 @@ SIGNATURES = {
     "pb200_grn_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pb200_grn_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pb200_film_apply": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_int64, c_int64, c_void_p]),
+    "pb200_embed_tokens": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pb200_ln_rows": (c_int, [c_void_p, c_int64, c_int, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pb200_ln_patchify2": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pb200_film_table": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "pb200_mix_cast_f16": (c_int, [c_void_p, c_void_p, c_float, c_float, c_int64, c_void_p, c_void_p]),
+    "pb200_mix_cast_rows_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
+    "pb200_pad_cast_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "pb200_gather_cast_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p]),
+    "pb200_replicate_rows": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_int, c_void_p]),
+    "pb200_regional_masks": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "pb200_guidance_mix": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "pb200_dwconv_ln_pairs": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                                      c_void_p, c_void_p]),
     "pb200_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                 c_int, c_int, c_void_p]),
     "pb200_attention_slots": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,

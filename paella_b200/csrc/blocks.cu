@@ -147,6 +147,90 @@ int pb200_film_apply(float* x, int64_t rows, int n, int rows_per_sample, const f
     return launch_film_apply(x, rows, n, rows_per_sample, film, film_ld, film_off, (cudaStream_t)stream);
 }
 
+// ---- executor kernels exposed for testing: thin forwards to the launchers paella_model.cu runs from its plan.  Every
+// refusal happens before anything is enqueued.
+int pb200_embed_tokens(const int64_t* tokens, const float* emb, int num_labels, int c_in, int batch, int h, int w, int patch,
+                       void* out16, void* stream) {
+    PB_CHECK(tokens && emb && out16, "embed_tokens: null pointer");
+    PB_CHECK(num_labels > 0 && c_in > 0 && patch > 0 && batch >= 0 && h >= 0 && w >= 0, "embed_tokens: bad arguments");
+    if ((int64_t)batch * h * w == 0) return 0;
+    return launch_embed_tokens(tokens, emb, num_labels, c_in, batch, h, w, patch, reinterpret_cast<__half*>(out16),
+                               (cudaStream_t)stream);
+}
+
+int pb200_ln_rows(const float* x, int64_t rows, int c, float scale, float shift, void* out16, float* out32, float* mean_out,
+                  void* stream) {
+    PB_CHECK(x != nullptr && rows >= 0 && c > 0, "ln_rows: bad arguments");
+    return launch_ln_rows(x, rows, c, scale, shift, reinterpret_cast<__half*>(out16), out32, (cudaStream_t)stream, mean_out);
+}
+
+int pb200_ln_patchify2(const float* x, int batch, int h, int w, int c, void* out16, void* stream) {
+    PB_CHECK(x && out16, "ln_patchify2: null pointer");
+    PB_CHECK(batch >= 0 && h >= 0 && w >= 0 && c > 0, "ln_patchify2: bad arguments");
+    if ((int64_t)batch * h * w == 0) return 0;
+    return launch_ln_patchify2(x, batch, h, w, c, reinterpret_cast<__half*>(out16), (cudaStream_t)stream);
+}
+
+int pb200_film_table(const float* r_embed, int batch, int c_r, const float* weight, const float* bias, int total, float* out,
+                     void* stream) {
+    PB_CHECK(r_embed && weight && bias && out, "film_table: null pointer");
+    PB_CHECK(batch >= 0 && c_r > 0 && total >= 0, "film_table: bad arguments");
+    if (batch == 0) return 0;
+    return launch_film_table(r_embed, batch, c_r, weight, bias, total, out, (cudaStream_t)stream);
+}
+
+int pb200_mix_cast_f16(const float* a, const float* b, float wa, float wb, int64_t n, void* out16, void* stream) {
+    PB_CHECK(a && out16 && n >= 0, "mix_cast: bad arguments");
+    return launch_mix_cast_f16(a, b, wa, wb, n, reinterpret_cast<__half*>(out16), (cudaStream_t)stream);
+}
+
+int pb200_mix_cast_rows_f16(const float* a, const float* b, const float* w, int64_t per, int64_t n, void* out16, void* stream) {
+    PB_CHECK(a && b && w && out16 && n >= 0, "mix_cast_rows: bad arguments");
+    return launch_mix_cast_rows_f16(a, b, w, per, n, reinterpret_cast<__half*>(out16), (cudaStream_t)stream);
+}
+
+int pb200_pad_cast_f16(const float* x, int batch, int h, int w, int c, const uint8_t* wrap, void* out16, void* stream) {
+    PB_CHECK(x && out16, "pad_cast: null pointer");
+    PB_CHECK(batch >= 0 && h > 0 && w > 0 && c > 0, "pad_cast: bad arguments");
+    return launch_pad_cast_f16(x, batch, h, w, c, wrap, reinterpret_cast<__half*>(out16), (cudaStream_t)stream);
+}
+
+int pb200_gather_cast_f16(const float* a, const int* samples, int n_list, int n_blocks, int batch, int64_t per, void* out16,
+                          void* stream) {
+    PB_CHECK(a && samples && out16, "gather_cast: null pointer");
+    PB_CHECK(n_list >= 0 && n_blocks >= 0 && batch >= 0 && per >= 0, "gather_cast: bad arguments");
+    return launch_gather_cast_f16(a, samples, n_list, n_blocks, batch, per, reinterpret_cast<__half*>(out16), (cudaStream_t)stream);
+}
+
+int pb200_replicate_rows(void* base, int64_t per, int n_base, const int* src, int n_tail, void* stream) {
+    PB_CHECK(base && src, "replicate_rows: null pointer");
+    PB_CHECK(per >= 0 && n_base >= 0 && n_tail >= 0, "replicate_rows: bad arguments");
+    return launch_replicate_rows(base, per, n_base, src, n_tail, (cudaStream_t)stream);
+}
+
+int pb200_regional_masks(const uint8_t* tok_mask, const int* mask_row, int batch, int h, int w, int patch, int n_levels, uint8_t* out,
+                         void* stream) {
+    PB_CHECK(tok_mask && out, "regional_masks: null pointer");
+    PB_CHECK(batch >= 0 && patch > 0 && n_levels > 0 && n_levels <= PB200_MAX_LEVELS && h >= (patch << (n_levels - 1)) &&
+                 w >= (patch << (n_levels - 1)),
+             "regional_masks: %d levels of patch %d on a %dx%d grid", n_levels, patch, h, w);
+    return launch_regional_masks(tok_mask, mask_row, batch, h, w, patch, n_levels, out, (cudaStream_t)stream);
+}
+
+int pb200_guidance_mix(float* features, int64_t per, const int* rows, const float* coef, int n_composed, int ld, void* stream) {
+    PB_CHECK(features && rows && coef, "guidance_mix: null pointer");
+    PB_CHECK(per >= 0 && n_composed >= 0, "guidance_mix: bad arguments");
+    return launch_guidance_mix(features, per, rows, coef, n_composed, ld, (cudaStream_t)stream);
+}
+
+int pb200_dwconv_ln_pairs(const float* x, const float* skip, const float* w_packed, const float* bias, int batch, int h, int w,
+                          int c, int k, const uint8_t* wrap, int n_base, void* out16, void* stream) {
+    PB_CHECK(x && w_packed && bias && out16 && wrap, "dwconv_ln: null pointer");
+    PB_CHECK(n_base > 0 && n_base <= batch && batch <= 2 * n_base, "dwconv_ln: %d samples with %d wrap codes", batch, n_base);
+    return launch_dwconv_ln(x, skip, w_packed, bias, batch, h, w, c, k, reinterpret_cast<__half*>(out16), (cudaStream_t)stream,
+                            wrap, n_base);
+}
+
 int pb200_attention(const void* qkv16, const void* ckv16, const int* kv_len, void* out16, int batch, int positions, int s_max,
                     int embed, int nhead, int self_attn, const float* attn_weights, int n_weights, int weighted_batch,
                     void* stream) {
